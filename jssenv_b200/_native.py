@@ -11,7 +11,7 @@ from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_uint8,
 import numpy as np
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("JSS_B200_LIB") or os.path.join(_PKG_DIR, "libjss_b200.so")   # override: kernel-variant experiments only
+LIB_PATH = os.path.join(_PKG_DIR, "libjss_b200.so")
 
 JSS_ABI_VERSION = 2
 ACTION_SKIP, ACTION_ADVANCE = -1, -2

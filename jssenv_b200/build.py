@@ -26,20 +26,10 @@ def needs_build():
     return os.path.getmtime(OUT) < max(os.path.getmtime(d) for d in deps)
 
 
-def build_variant(name, extra_flags):
-    """Experiment builds (occupancy sweeps etc.): jssenv_b200/variants/libjss_b200_<name>.so, selected with JSS_B200_LIB."""
-    d = os.path.join(PKG, "variants")
-    os.makedirs(d, exist_ok=True)
-    out = os.path.join(d, f"libjss_b200_{name}.so")
-    subprocess.check_call([find_nvcc()] + NVCC_FLAGS + list(extra_flags) + ["-o", out] + SRCS)
-    return out
-
-
 def build(force=False, verbose=False):
     if not force and not needs_build():
         return OUT
-    extra = os.environ.get("JSS_NVCC_EXTRA", "").split()   # experiments only (e.g. -DJSS_MIN_CTAS=4)
-    cmd = [find_nvcc()] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT] + SRCS
+    cmd = [find_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT] + SRCS
     subprocess.check_call(cmd)
     return OUT
 

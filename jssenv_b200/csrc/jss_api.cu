@@ -78,9 +78,8 @@ struct jss_handle {
     JssParams p{};
     JssSmemLayout sl_env{}, sl_step{}, sl_step_rem{};   // shared-memory layouts of the generic / step kernels (step: without / with the suffix-sum table)
     int class_tile_begin[4] = {0, 0, 0, 0}, class_tile_end[4] = {0, 0, 0, 0};  // KJ = 1, 2, 4, 8
-    int step_grid[24] = {0};
-    int env_grid[16] = {0};                         // resident CTAs per SM of the generic kernel variants (filled lazily)                        // resident-CTA grids of the step kernel variants (filled lazily)
-    bool use_pdl = true;
+    int step_grid[24] = {0};                        // resident-CTA grids of the step kernel variants (filled lazily)
+    int env_grid[16] = {0};                         // resident CTAs per SM of the generic kernel variants (filled lazily)
     std::vector<int32_t> env_inst;
 
     // host-buffer stepping
@@ -149,47 +148,41 @@ int step_grid_for(jss_t *h, Kern kern, int slot, size_t smem) {
     return JSS_OK;
 }
 
-// uniform batch: one instance, static strided tiles
+// one fused step launch (PDL).  A uniform batch runs min(tiles, resident CTAs) persistent CTAs over static strided
+// tiles; a mixed batch runs one CTA per JssCtaRange (all resident: SMs x 3).
+template <typename Kern>
+int launch_step_kernel(jss_t *h, Kern kern, int slot, const JssLaunch &a, bool want_rem, cudaStream_t st) {
+    const JssSmemLayout &sl = want_rem ? h->sl_step_rem : h->sl_step;
+    const size_t smem = smem_bytes(sl);
+    int rc = step_grid_for(h, kern, slot, smem);
+    if (rc) return rc;
+    const int grid = h->p.uniform_inst >= 0 ? std::min(a.tile_end, h->step_grid[slot]) : h->p.n_cta_ranges;
+    JSS_CUDA(h, JSS_LAUNCH_PDL(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl));
+    JSS_CUDA(h, cudaGetLastError());
+    h->launches += 1;
+    return JSS_OK;
+}
+
+// uniform batch: one instance, its scalars in the kernel parameters
 template <int KJ, int SAMPLE>
 int launch_step_uniform(jss_t *h, const JssLaunch &a_in, bool want_rem, cudaStream_t st) {
     JssLaunch a = a_in;
     fill_uni(h->descs[h->p.uniform_inst], a.uni);
     a.tile_begin = 0;
     a.tile_end = (h->n_envs + JSS_WARPS_PER_CTA - 1) / JSS_WARPS_PER_CTA;
-    const JssSmemLayout &sl = want_rem ? h->sl_step_rem : h->sl_step;
-    const size_t smem = smem_bytes(sl);
-    auto kern = jss_step_kernel<KJ, SAMPLE>;
-    const int slot = class_of(KJ) * 4 + SAMPLE + (want_rem ? 1 : 0);
-    int rc = step_grid_for(h, kern, slot, smem);
-    if (rc) return rc;
-    const int grid = std::min(a.tile_end, h->step_grid[slot]);
-    if (h->use_pdl) JSS_CUDA(h, JSS_LAUNCH_PDL(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl));
-    else JSS_LAUNCH(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
-    JSS_CUDA(h, cudaGetLastError());
-    h->launches += 1;
-    return JSS_OK;
+    return launch_step_kernel(h, jss_step_kernel<KJ, SAMPLE>, class_of(KJ) * 4 + SAMPLE + (want_rem ? 1 : 0), a,
+                              want_rem, st);
 }
 
-// mixed batch: ONE launch over all lane classes, chunks handed out by ticket
+// mixed batch: ONE launch over all lane classes, every CTA an equal slice of each class (jss_assign)
 template <int SAMPLE, bool BIG>
-int launch_step_mixed(jss_t *h, const JssLaunch &a_in, bool want_rem, cudaStream_t st) {
-    JssLaunch a = a_in;
-    const JssSmemLayout &sl = want_rem ? h->sl_step_rem : h->sl_step;
-    const size_t smem = smem_bytes(sl);
-    auto kern = jss_step_mixed_kernel<SAMPLE, BIG>;
-    const int slot = (BIG ? 20 : 16) + SAMPLE + (want_rem ? 1 : 0);
-    int rc = step_grid_for(h, kern, slot, smem);
-    if (rc) return rc;
-    const int grid = h->p.n_cta_ranges;                   // one CTA per range (all resident: SMs x 3)
-    if (h->use_pdl) JSS_CUDA(h, JSS_LAUNCH_PDL(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl));
-    else JSS_LAUNCH(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
-    JSS_CUDA(h, cudaGetLastError());
-    h->launches += 1;
-    return JSS_OK;
+int launch_step_mixed(jss_t *h, const JssLaunch &a, bool want_rem, cudaStream_t st) {
+    return launch_step_kernel(h, jss_step_mixed_kernel<SAMPLE, BIG>, (BIG ? 20 : 16) + SAMPLE + (want_rem ? 1 : 0), a,
+                              want_rem, st);
 }
 
 int launch_step(jss_t *h, const JssLaunch &a, cudaStream_t st) {
-    const bool rem = a.rule == JSS_RULE_MWR || a.rule == JSS_RULE_LWR || a.rule == JSS_RULE_CR;
+    const bool rem = jss_rule_wants_rem(a.rule);
     const int sample = a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
     if (h->p.uniform_inst < 0) {
         const bool big = h->class_tile_end[3] > h->class_tile_begin[3];     // instances with 129..256 jobs in the batch
@@ -248,9 +241,8 @@ int launch_class(jss_t *h, const JssLaunch &a, const JssSmemLayout &sl, cudaStre
     }
 }
 
-int launch_all(jss_t *h, JssLaunch a, bool want_rem, cudaStream_t st) {
+int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
-    (void)want_rem;
     const JssSmemLayout &sl = h->sl_env;
     for (int c = 0; c < 4; c++) {
         a.tile_begin = h->class_tile_begin[c];
@@ -264,8 +256,6 @@ int launch_all(jss_t *h, JssLaunch a, bool want_rem, cudaStream_t st) {
     }
     return JSS_OK;
 }
-
-bool rule_wants_rem(int rule) { return rule == JSS_RULE_MWR || rule == JSS_RULE_LWR || rule == JSS_RULE_CR; }
 
 int check_ready(jss_t *h) {
     if (!h) return JSS_ERR_INVALID;
@@ -440,9 +430,8 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
         ops_max = std::max(ops_max, h->insts[k].J * h->insts[k].M);
         rem_max = std::max(rem_max, h->insts[k].J * (h->insts[k].M + 1));
     }
-    // group envs by (KJ class, instance) -> tiles of <= JSS_WARPS_PER_CTA envs of one instance.  The most
-    // expensive lane class (KJ = 4) comes first: the mixed-batch step kernel hands the tile list out front to
-    // back, so the cheap 15..30-job envs fill the tail (longest processing time first).
+    // group envs by (KJ class, instance) -> tiles of <= JSS_WARPS_PER_CTA envs of one instance, the largest lane class
+    // first (the order in which the mixed-batch step kernel walks its slices)
     std::vector<int32_t> order(N);
     for (int e = 0; e < N; e++) order[e] = e;
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
@@ -453,7 +442,6 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     });
     std::vector<JssTile> tiles;
     std::vector<uint32_t> state_off16((size_t)N), hdr_off16((size_t)N);
-    std::vector<double> tile_cost;
     for (int c = 0; c < 4; c++) h->class_tile_begin[c] = h->class_tile_end[c] = 0;
     int pos = 0;
     int cur_class = -1;
@@ -483,9 +471,6 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
             }
             off16 += (uint64_t)cnt * block16;
             tiles.push_back(t);
-            // relative cost of an env-step: ~linear in J, like the bytes it moves (the uniform ta80 step is
-            // bandwidth-bound: packing the state block, -28 % bytes, made it 22 % faster; DESIGN.md section 4)
-            tile_cost.push_back(cnt * (40.0 + h->insts[k].J));
         }
         pos = end;
     }
@@ -517,12 +502,6 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     p.n_envs = N;
     p.jobs_max = jmax;
     p.machines_max = mmax;
-    {
-        const JssBlockGeom g = jss_block_geom(jmax, mmax);   // the geometry grows with J and M: batch maxima
-        p.Jcap = g.Jcap;
-        p.Mcap = g.Mcap;
-        p.block_words = g.words;                          // sizes the shared-memory staging buffers
-    }
     p.mask_stride = round_up(jmax + 1, jmax > 128 ? 8 : 4);   // the 8-jobs-per-lane class stores 8 mask bytes per lane
     p.create_flags = (int32_t)h->create_flags;
     p.env_id_base = h->env_id_base;
@@ -534,19 +513,20 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     p.inst = h->d_inst; p.ops_pool = h->d_ops; p.len_pool = h->d_len; p.rem_pool = h->d_rem;
 
     {   // shared-memory layouts: [SmInst][ops u16][len i32][rem u16][per-warp regions], 16-byte aligned regions
+        const JssBlockGeom g = jss_block_geom(jmax, mmax);   // the geometry grows with J and M: batch maxima
         JssSmemLayout sl{};
         sl.off_len = (int32_t)sizeof(SmInst) + round_up(ops_max, 8) * 2;
         sl.off_rem = sl.off_len + round_up(jmax, 4) * 4;
         sl.off_warp0 = sl.off_rem + round_up(rem_max, 8) * 2;
         // observation staging (7 floats per job slot); env_check_no_op (general instances) also keeps its 32-int
         // per-warp machine-horizon table here, so never less than 32 words (tiny instances: 7 * Jcap < 32)
-        sl.scratch_words = std::max(7 * p.Jcap, 32);
+        sl.scratch_words = std::max(7 * g.Jcap, 32);
         h->sl_env = sl;
         h->sl_env.warp_stride = sl.scratch_words * 4;
         h->sl_env.off_scratch = 0;
         h->sl_step_rem = sl;
-        h->sl_step_rem.off_scratch = 16 + p.block_words * 4;                               // [mbarrier][state-in]
-        h->sl_step_rem.warp_stride = h->sl_step_rem.off_scratch + sl.scratch_words * 4 + p.block_words * 4;   // [scratch][state-out]
+        h->sl_step_rem.off_scratch = 16 + g.words * 4;                                     // [mbarrier][state-in]
+        h->sl_step_rem.warp_stride = h->sl_step_rem.off_scratch + sl.scratch_words * 4 + g.words * 4;   // [scratch][state-out]
         h->sl_step = h->sl_step_rem;                      // launches that stage no suffix sums leave their room to the L1
         h->sl_step.off_warp0 = h->sl_step.off_rem;
     }
@@ -652,7 +632,7 @@ int jss_reset(jss_t *h, const uint8_t *env_mask_dev, void *stream) {
     JssLaunch a{};
     a.mode = JSS_MODE_RESET;
     a.env_mask = env_mask_dev;
-    return launch_all(h, a, false, (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_step(jss_t *h, const int32_t *actions_dev, void *stream) {
@@ -662,7 +642,7 @@ int jss_step(jss_t *h, const int32_t *actions_dev, void *stream) {
     JssLaunch a{};
     a.mode = JSS_MODE_STEP;
     a.actions = actions_dev;
-    return launch_all(h, a, false, (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_step_export(jss_t *h, const int32_t *actions_dev, void *stream) {
@@ -673,7 +653,7 @@ int jss_step_export(jss_t *h, const int32_t *actions_dev, void *stream) {
     a.mode = JSS_MODE_STEP;
     a.actions = actions_dev;
     a.export_after = 1;
-    return launch_all(h, a, false, (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mode, uint64_t seed,
@@ -689,7 +669,7 @@ int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mod
     a.actions_out = next_actions_dev;
     a.rule = rule; a.coin_mode = coin_mode; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
     a.hash_key = jss_hash_key(seed, step_index);
-    return launch_all(h, a, false, (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_policy(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_index, int32_t *actions_dev,
@@ -702,7 +682,7 @@ int jss_policy(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_i
     a.mode = JSS_MODE_POLICY;
     a.rule = rule; a.coin_mode = coin_mode; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
     a.actions_out = actions_dev;
-    return launch_all(h, a, rule_wants_rem(rule), (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_rollout(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_steps, int write_obs, void *stream) {
@@ -714,7 +694,7 @@ int jss_rollout(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_st
     a.mode = JSS_MODE_ROLLOUT;
     a.rule = rule; a.coin_mode = JSS_COIN_DEVICE; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
     a.n_steps = n_steps; a.write_obs = write_obs;
-    return launch_all(h, a, rule_wants_rem(rule), (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_steps, float *traj_obs,
@@ -730,7 +710,7 @@ int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int
     a.rule = rule; a.coin_mode = JSS_COIN_DEVICE; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
     a.n_steps = n_steps; a.write_obs = 1;
     a.traj_obs = traj_obs; a.traj_mask = traj_mask; a.traj_scalars = traj_scalars; a.traj_actions = traj_actions;
-    return launch_all(h, a, rule_wants_rem(rule), (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_step_host(jss_t *h, const int32_t *actions_host, uint8_t *mask_host, float *obs_host,
@@ -781,8 +761,7 @@ int host_step_begin_impl(jss_t *h, const int32_t *actions_host, uint8_t *mask_ho
     }
     if (obs_host && !h->obs_staging && (rc = dev_alloc(h, &h->obs_staging, N * p.jobs_max * 7, false))) return rc;
     if (wire_host && !h->wire[0]) {
-        // 16-byte multiple with >= 6 bytes of slack behind the last record (the host expansion loads 16 bytes per job)
-        h->wire_stride = round_up(JSS_WIRE_JOB_BYTES * p.jobs_max + 6, 16);
+        h->wire_stride = jss_host_wire_stride(h);
         for (int k = 0; k < 2; k++)
             if ((rc = dev_alloc(h, &h->wire[k], N * (size_t)h->wire_stride))) return rc;
     }
@@ -828,7 +807,7 @@ int host_step_begin_impl(jss_t *h, const int32_t *actions_host, uint8_t *mask_ho
         a.mode = JSS_MODE_PACK;
         a.wire = h->wire[h->pipe_cur];
         a.wire_stride = (int32_t)h->wire_stride;
-        if ((rc = launch_all(h, a, false, sc))) return rc;
+        if ((rc = launch_all(h, a, sc))) return rc;
     }
     // the copy stream never runs ahead of the step (also when nothing large is copied: JSS_WAIT_OBS is the barrier
     // callers take before going back to the stream-ordered entry points)
@@ -868,6 +847,7 @@ int jss_host_step_begin_hybrid(jss_t *h, const int32_t *actions_host, uint8_t *m
 
 int64_t jss_host_wire_stride(jss_t *h) {
     if (!h || !h->assigned) return JSS_ERR_STATE;
+    // 16-byte multiple with >= 6 bytes of slack behind the last record (the host expansion loads 16 bytes per job)
     return round_up(JSS_WIRE_JOB_BYTES * h->p.jobs_max + 6, 16);
 }
 
@@ -970,7 +950,7 @@ int jss_export_state(jss_t *h, void *stream) {
     if (rc) return rc;
     JssLaunch a{};
     a.mode = JSS_MODE_EXPORT;
-    return launch_all(h, a, false, (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_import_state(jss_t *h, const uint8_t *env_mask_dev, void *stream) {
@@ -979,7 +959,7 @@ int jss_import_state(jss_t *h, const uint8_t *env_mask_dev, void *stream) {
     JssLaunch a{};
     a.mode = JSS_MODE_IMPORT;
     a.env_mask = env_mask_dev;
-    return launch_all(h, a, false, (cudaStream_t)stream);
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_host_masked_random(const uint8_t *mask_host, int n, int width, int64_t row_stride, uint64_t seed,

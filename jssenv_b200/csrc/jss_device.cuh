@@ -70,28 +70,16 @@ struct EnvRegs {
 // collective, BSSY/BSYNC around each branch, nothing kept in uniform registers.  The few truly uniform inputs of an
 // env-step go through a lane-0 shuffle.  ptxas for sm_90a still guards the collectives with BRA.DIV, but the hinted
 // code is faster where it matters: measured on an H100 SXM (80 GB HBM3, 400 W power limit), the mixed-batch step
-// kernel (cfg5, N = 65 536) takes 126.8 / 131.5 us per launch with FIFO / MWR instead of 134.9 / 139.0 us without
-// the hints; uniform ta80 batches are unchanged (195 us either way).
+// kernel (cfg5, N = 65 536) takes 126.8 / 131.5 us per launch with FIFO / MWR instead of 134.9 / 139.0 us with the
+// shuffle left out (6 %); uniform ta80 batches are unchanged (195 us either way).
 // The value MUST be the same in every lane -- the shuffle is a hint, not a broadcast of lane 0's opinion.
-JSS_DEV int jss_uniform(int v) {
-#ifdef JSS_NO_UNIFORM_HINTS
-    return v;
-#else
-    return __shfl_sync(JSS_FULL, v, 0);
-#endif
-}
+JSS_DEV int jss_uniform(int v) { return __shfl_sync(JSS_FULL, v, 0); }
 JSS_DEV uint32_t jss_uniform(uint32_t v) { return (uint32_t)jss_uniform((int)v); }
 JSS_DEV int jss_warp_index() { return jss_uniform((int)(threadIdx.x >> 5)); }
 // Where the flags word gets the hint: everywhere except the uniform 4-jobs-per-lane step kernel (the ta71..80 shape),
-// which keeps the conservative code (not re-measured on H100 in isolation; JSS_EXP_HINT_ALL builds the other variant).
+// which keeps the conservative code (hinting it too has not been measured on H100 in isolation).
 template <int KJ, bool UNI>
-JSS_DEV constexpr bool jss_hint_flags() {
-#ifdef JSS_EXP_HINT_ALL
-    return true;
-#else
-    return !(UNI && KJ == 4);
-#endif
-}
+JSS_DEV constexpr bool jss_hint_flags() { return !(UNI && KJ == 4); }
 
 // ---- small helpers --------------------------------------------------------------
 template <int KJ, typename T>
@@ -131,12 +119,6 @@ JSS_DEV float jss_div(float x, float y, float ry) {
     return __fmaf_rn(r, ry, q);
 }
 
-// two quotients of an observation column pair (ny = -divisor, host-negated); sm_90 has no packed-fp32 pipe, so this
-// is two independent jss_div sequences (the compiler interleaves them)
-JSS_DEV float2 jss_div2(float2 x, const float (&ny)[2], const float (&ry)[2]) {
-    return make_float2(jss_div(x.x, -ny[0], ry[0]), jss_div(x.y, -ny[1], ry[1]));
-}
-
 // ---- TMA (cp.async.bulk) + mbarrier helpers -----------------------------------------------
 // The state block of the NEXT env of a warp is prefetched into the warp's shared-memory
 // buffer by one bulk copy (global -> shared, completion on an mbarrier) while the current env
@@ -159,30 +141,18 @@ JSS_DEV void jss_bulk_load(jss_saddr_t smem_dst, const void *gmem_src, uint32_t 
 JSS_DEV void jss_mbar_wait(jss_saddr_t mbar, uint32_t phase) {
     uint32_t ok;
     do {
-        // non-blocking poll: test_wait returns at once, try_wait may park the warp for a scheduler time slice when the
-        // block has not landed yet (JSS_MBAR_TRY_WAIT builds the other variant)
-#ifdef JSS_MBAR_TRY_WAIT
-        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok) : "r"(mbar), "r"(phase) : "memory");
-#else
+        // non-blocking poll: test_wait returns at once, where try_wait may park the warp for a scheduler time slice
+        // when the block has not landed yet
         asm volatile("{\n .reg .pred p;\n mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
                      : "=r"(ok) : "r"(mbar), "r"(phase) : "memory");
-#endif
     } while (!ok);
 }
 JSS_DEV void jss_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 JSS_DEV void jss_bulk_store(void *gmem_dst, jss_saddr_t smem_src, uint32_t bytes) {   // joins the open bulk group
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
                  ::"l"(gmem_dst), "r"(smem_src), "r"(bytes) : "memory");
-#ifdef JSS_EXP_TWO_COMMITS
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-#endif
 }
-JSS_DEV void jss_bulk_commit() {
-#ifndef JSS_EXP_TWO_COMMITS
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-#endif
-}
+JSS_DEV void jss_bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 JSS_DEV void jss_bulk_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 JSS_DEV void jss_bulk_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 #else   // host emulation (tests/emu): synchronous copies; the waits are warp rendezvous points
@@ -309,7 +279,7 @@ JSS_DEV void env_clear_jobs(const InstView &iv, EnvRegs<KJ> &s) {
     for (int i = 0; i < KJ; i++) { s.todo[i] = jss_M(iv); s.tufco[i] = 0; s.idle_last[i] = 0; s.total_idle[i] = 0; s.col4[i] = 0; }
 }
 
-// The per-job words of the block (w0, w1, w2; jss_types.h) are decoded into the five EnvRegs arrays on load and
+// The job records of the block (w0, w1, w2; jss_types.h) are decoded into the five EnvRegs arrays on load and
 // encoded on store: everything between works on plain ints.
 template <int KJ>
 JSS_DEV void env_load_jobs(const int32_t *blk, int Jc, int lane, EnvRegs<KJ> &s) {
@@ -321,12 +291,20 @@ JSS_DEV void env_load_jobs(const int32_t *blk, int Jc, int lane, EnvRegs<KJ> &s)
 #pragma unroll
     for (int i = 0; i < KJ; i++) {
         const uint32_t a = (uint32_t)w0[i], b = (uint32_t)w1[i];
-        s.todo[i] = (int)(a & ((1u << JSS_PACK_TODO_BITS) - 1u));
-        s.tufco[i] = (int)((a >> JSS_PACK_TODO_BITS) & JSS_OP_DMASK);
-        s.col4[i] = (int)(a >> (JSS_PACK_TODO_BITS + JSS_PACK_DUR_BITS));
-        s.idle_last[i] = (int)(b & (uint32_t)JSS_PACK_IDLE_MAX);
-        s.total_idle[i] = (int)((b >> 24) | (w2[i] << 8));
+        s.todo[i] = jss_job_todo(a);
+        s.tufco[i] = jss_job_tufco(a);
+        s.col4[i] = jss_job_col4(a);
+        s.idle_last[i] = jss_job_idle_last(b);
+        s.total_idle[i] = jss_job_total_idle(b, w2[i]);
     }
+}
+
+// a lane's legal / blocked bits and the env's header, behind the tuam words of the block
+template <int KJ>
+JSS_DEV void env_load_bits_hdr(const int32_t *tail, int Mc, int lane, EnvRegs<KJ> &s) {
+    s.lb = jss_ld_bits<KJ>(tail + Mc, lane);
+    const int4 h4 = *reinterpret_cast<const int4 *>(tail + Mc + jss_bits_words<KJ>());
+    s.t = h4.x; s.flags = (uint32_t)h4.y; s.ep_steps = h4.z; s.ep_return = h4.w;
 }
 
 template <int KJ>
@@ -336,9 +314,7 @@ JSS_DEV void env_load_from(const JssParams &p, const InstView &iv, const int32_t
     else env_clear_jobs<KJ>(iv, s);
     const int32_t *tail = blk + iv.si->tail;
     s.tuam = (lane < jss_M(iv)) ? tail[lane] : 0;
-    s.lb = jss_ld_bits<KJ>(tail + Mc, lane);
-    const int4 h4 = *reinterpret_cast<const int4 *>(tail + Mc + jss_bits_words<KJ>());
-    s.t = h4.x; s.flags = (uint32_t)h4.y; s.ep_steps = h4.z; s.ep_return = h4.w;
+    env_load_bits_hdr<KJ>(tail, Mc, lane, s);
     env_derive_ops<KJ>(iv, s, lane);
 }
 // start of env's state block (blocks are stored in tile order with per-instance sizes, see JssTile)
@@ -357,20 +333,17 @@ JSS_DEV void env_load_for_policy(const JssParams &p, const InstView &iv, int env
     const int Jc = iv.si->Jcap, Mc = iv.si->Mcap;
     env_clear_jobs<KJ>(iv, s);
     if (rule != JSS_RULE_RANDOM && KJ * lane < jss_J(iv)) {
-        jss_ld<KJ>(blk + KJ * lane, s.todo);          // w0: todo in the low bits
+        jss_ld<KJ>(blk + KJ * lane, s.todo);          // w0 (todo)
 #pragma unroll
-        for (int i = 0; i < KJ; i++) s.todo[i] &= (1 << JSS_PACK_TODO_BITS) - 1;
-        if (rule == JSS_RULE_FIFO) {                  // w1: idle_last in the low 24 bits
+        for (int i = 0; i < KJ; i++) s.todo[i] = jss_job_todo((uint32_t)s.todo[i]);
+        if (rule == JSS_RULE_FIFO) {                  // w1 (idle_last)
             jss_ld<KJ>(blk + Jc + KJ * lane, s.idle_last);
 #pragma unroll
-            for (int i = 0; i < KJ; i++) s.idle_last[i] &= JSS_PACK_IDLE_MAX;
+            for (int i = 0; i < KJ; i++) s.idle_last[i] = jss_job_idle_last((uint32_t)s.idle_last[i]);
         }
     }
     s.tuam = 0;
-    const int32_t *tail = blk + iv.si->tail;
-    s.lb = jss_ld_bits<KJ>(tail + Mc, lane);
-    const int4 h4 = *reinterpret_cast<const int4 *>(tail + Mc + jss_bits_words<KJ>());
-    s.t = h4.x; s.flags = (uint32_t)h4.y; s.ep_steps = h4.z; s.ep_return = h4.w;
+    env_load_bits_hdr<KJ>(blk + iv.si->tail, Mc, lane, s);
     if (rule != JSS_RULE_RANDOM) env_derive_ops<KJ>(iv, s, lane);
     else {
 #pragma unroll
@@ -388,11 +361,8 @@ JSS_DEV void env_store_to(const JssParams &p, const InstView &iv, int32_t *blk, 
         uint32_t w2[KJ];
 #pragma unroll
         for (int i = 0; i < KJ; i++) {
-            const uint32_t ti = (uint32_t)s.total_idle[i];
-            w0[i] = (int)((uint32_t)s.todo[i] | ((uint32_t)s.tufco[i] << JSS_PACK_TODO_BITS) |
-                          ((uint32_t)s.col4[i] << (JSS_PACK_TODO_BITS + JSS_PACK_DUR_BITS)));
-            w1[i] = (int)((uint32_t)s.idle_last[i] | (ti << 24));
-            w2[i] = ti >> 8;
+            const JssJobWords r = jss_pack_job(s.todo[i], s.tufco[i], s.col4[i], s.idle_last[i], s.total_idle[i]);
+            w0[i] = (int)r.w0; w1[i] = (int)r.w1; w2[i] = r.w2;
         }
         if (KJ * lane < Jc) {
             jss_st<KJ>(blk + KJ * lane, w0);
@@ -622,14 +592,14 @@ JSS_DEV void env_emit_obs(const JssParams &p, const JssOut &out, const InstView 
             // the two counters until the job completes)
             const int len = iv.len[KJ * lane + i];        // unconditional (in-bounds) load + select
             const int perf = (s.todo[i] < jss_M(iv)) ? s.t - s.total_idle[i] : len;
+            const SmInst &si = *iv.si;
             v[7 * i + 0] = (s.lb & (1u << i)) ? 1.0f : 0.0f;
-            // columns that share a divisor (or sit next to each other) go through the packed-fp32 pipe in pairs
-            const float2 q14 = jss_div2(make_float2((float)s.tufco[i], (float)s.col4[i]), iv.si->n14, iv.si->r14);
-            const float2 q23 = jss_div2(make_float2((float)s.todo[i], (float)perf), iv.si->n23, iv.si->r23);
-            const float2 q56 = jss_div2(make_float2((float)s.idle_last[i], (float)s.total_idle[i]), iv.si->n56, iv.si->r56);
-            v[7 * i + 1] = q14.x; v[7 * i + 4] = q14.y;
-            v[7 * i + 2] = q23.x; v[7 * i + 3] = q23.y;
-            v[7 * i + 5] = q56.x; v[7 * i + 6] = q56.y;
+            v[7 * i + 1] = jss_div((float)s.tufco[i], si.f_mto, si.r_mto);
+            v[7 * i + 2] = jss_div((float)s.todo[i], si.f_M, si.r_M);
+            v[7 * i + 3] = jss_div((float)perf, si.f_mtj, si.r_mtj);
+            v[7 * i + 4] = jss_div((float)s.col4[i], si.f_mto, si.r_mto);
+            v[7 * i + 5] = jss_div((float)s.idle_last[i], si.f_sop, si.r_sop);
+            v[7 * i + 6] = jss_div((float)s.total_idle[i], si.f_sop, si.r_sop);
         }
         // stage the lane's 7*KJ floats (one contiguous, bank-conflict-free run per lane) ...
         float *mine = scratch + 7 * KJ * lane;
@@ -731,6 +701,14 @@ JSS_DEV void env_episode_end(const JssParams &p, const EnvRegs<KJ> &s, int env, 
     }
 }
 
+// a reset env's solution row (JSS_CREATE_RECORD_SOLUTION) holds -1 everywhere
+JSS_DEV void env_clear_solution(const JssParams &p, int env, int lane) {
+    if (p.solution) {
+        int32_t *sol = p.solution + (size_t)env * p.jobs_max * p.machines_max;
+        for (int k = lane; k < p.jobs_max * p.machines_max; k += 32) sol[k] = -1;
+    }
+}
+
 // ---- step (jss_env.py:403-481) ---------------------------------------------------------
 // Returns true if the env changed (outputs must be re-emitted).
 template <int KJ>
@@ -741,10 +719,7 @@ JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, in
     if (s.flags & JSS_FLAG_DONE) {
         if (p.create_flags & JSS_CREATE_AUTO_RESET) {
             env_reset_regs<KJ>(iv, s, lane);
-            if (p.solution) {
-                int32_t *sol = p.solution + (size_t)env * p.jobs_max * p.machines_max;
-                for (int k = lane; k < p.jobs_max * p.machines_max; k += 32) sol[k] = -1;
-            }
+            env_clear_solution(p, env, lane);
             return true;
         }
         return false;  // frozen until reset
@@ -913,8 +888,10 @@ JSS_DEV void env_export(const JssParams &p, const InstView &iv, const EnvRegs<KJ
     }
 }
 
-// The state block keeps todo in [0, M], tufco and col4 in [0, 2047], idle_last and total_idle in [0, 2^24)
+// The job records keep todo in [0, M], tufco and col4 in [0, 2047], idle_last and total_idle in [0, 2^24)
 // (jss_types.h).  An imported value outside its range is clamped into it and the env gets the sticky error bit.
+static_assert(JSS_MAX_MACHINES <= (int)JSS_PACK_TODO_MASK && JSS_MAX_DURATION <= (int)JSS_PACK_DUR_MASK,
+              "the job record must hold every todo and duration the kernels accept");
 template <int KJ>
 JSS_DEV void env_import(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, int env, int lane) {
     const size_t jb = (size_t)env * p.jobs_max;
@@ -926,10 +903,10 @@ JSS_DEV void env_import(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, 
         const int j = KJ * lane + i;
         const bool valid = j < jss_J(iv);
         s.todo[i] = valid ? take(p.x_todo[jb + j], jss_M(iv)) : jss_M(iv);
-        s.tufco[i] = valid ? take(p.x_tufco[jb + j], JSS_MAX_DURATION) : 0;
+        s.tufco[i] = valid ? take(p.x_tufco[jb + j], (int)JSS_PACK_DUR_MASK) : 0;
         s.idle_last[i] = valid ? take(p.x_idle_last[jb + j], JSS_PACK_IDLE_MAX) : 0;
         s.total_idle[i] = valid ? take(p.x_total_idle[jb + j], JSS_PACK_IDLE_MAX) : 0;
-        s.col4[i] = valid ? take(p.x_col4[jb + j], JSS_MAX_DURATION) : 0;
+        s.col4[i] = valid ? take(p.x_col4[jb + j], (int)JSS_PACK_DUR_MASK) : 0;
         if (valid && p.x_legal[jb + j] != 0) s.lb |= 1u << i;
         if (valid && p.x_blocked[jb + j] != 0) s.lb |= (1u << jss_bs<KJ>()) << i;
     }
@@ -941,23 +918,21 @@ JSS_DEV void env_import(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, 
 }
 
 // ---- packed observation row (host-buffer path) ---------------------------------------------------------
-// 10 bytes per job: w0 = legal | tufco << 1 | todo << 12 | col4 << 18, then idle_last and total_idle as 24-bit
-// little-endian integers (the makespan bound J*M*2047 < 2^24).  Column 3 (total_perform) is derivable on the host
-// from total_idle, todo, t and jobs_length.  jss_host_expand_obs() turns a row back into the exact real_obs floats.
+// One job record per job (jss_types.h, 10 bytes), with the legal bit in w0.  Column 3 (total_perform) is derivable
+// on the host from total_idle, todo, t and jobs_length.  jss_host_expand_obs() turns a row back into the exact
+// real_obs floats.
 template <int KJ>
 JSS_DEV void env_pack(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane, float *scratch) {
     uint16_t *st = reinterpret_cast<uint16_t *>(scratch);
     if (KJ * lane < jss_J(iv)) {
 #pragma unroll
         for (int i = 0; i < KJ; i++) {
-            const uint32_t w0 = ((s.lb >> i) & 1u) | ((uint32_t)s.tufco[i] << 1) | ((uint32_t)s.todo[i] << 12) |
-                                ((uint32_t)s.col4[i] << 18);
-            const uint32_t il = (uint32_t)s.idle_last[i], ti = (uint32_t)s.total_idle[i];
-            uint16_t *r = st + 5 * (KJ * lane + i);
+            const JssJobWords w = jss_pack_job(s.todo[i], s.tufco[i], s.col4[i], s.idle_last[i], s.total_idle[i]);
+            const uint32_t w0 = w.w0 | (((s.lb >> i) & 1u) << JSS_PACK_LEGAL_SHIFT);
+            uint16_t *r = st + 5 * (KJ * lane + i);   // 2-byte aligned: stored as five u16
             r[0] = (uint16_t)w0; r[1] = (uint16_t)(w0 >> 16);
-            r[2] = (uint16_t)il;                                      // bytes 4,5
-            r[3] = (uint16_t)(((il >> 16) & 255u) | ((ti & 255u) << 8));   // byte 6 = idle[23:16], byte 7 = total[7:0]
-            r[4] = (uint16_t)(ti >> 8);                               // bytes 8,9
+            r[2] = (uint16_t)w.w1; r[3] = (uint16_t)(w.w1 >> 16);
+            r[4] = (uint16_t)w.w2;
         }
     }
     __syncwarp();
@@ -1002,7 +977,9 @@ JSS_DEV void jss_iv_shape(InstView &iv) {
 #define JSS_STAGE_REM 2     // suffix sums (rules MWR / LWR / CR)
 #define JSS_STAGE_ALL 3
 // the rules that read the suffix sums; the host sizes the shared-memory layout with the same predicate
-JSS_DEV bool jss_rule_wants_rem(int rule) { return rule == JSS_RULE_MWR || rule == JSS_RULE_LWR || rule == JSS_RULE_CR; }
+JSS_HD static inline bool jss_rule_wants_rem(int rule) {
+    return rule == JSS_RULE_MWR || rule == JSS_RULE_LWR || rule == JSS_RULE_CR;
+}
 
 // per-instance scalars: staged in shared memory by the kernels, and filled on the host for the kernel parameters of
 // uniform batches
@@ -1014,9 +991,6 @@ JSS_HD static inline void jss_fill_sminst(const JssInstDesc &d, SmInst *si) {
     si->r_mto = d.r_mto; si->r_mtj = d.r_mtj; si->r_sop = d.r_sop; si->r_M = d.r_M;
     const JssBlockGeom g = jss_block_geom(d.J, d.M);
     si->Jcap = g.Jcap; si->Mcap = g.Mcap; si->block_words = g.words; si->tail = g.tail;
-    si->n14[0] = si->n14[1] = -si->f_mto; si->r14[0] = si->r14[1] = d.r_mto;
-    si->n23[0] = -si->f_M; si->n23[1] = -si->f_mtj; si->r23[0] = d.r_M; si->r23[1] = d.r_mtj;
-    si->n56[0] = si->n56[1] = -si->f_sop; si->r56[0] = si->r56[1] = d.r_sop;
 }
 
 JSS_DEV void jss_stage_instance(const JssParams &p, const JssInstDesc &d, const JssCtaSmem &c, int what) {
@@ -1055,6 +1029,16 @@ JSS_DEV void env_emit_all(const JssParams &p, const InstView &iv, const EnvRegs<
     env_emit_scalars<KJ>(out, iv, s, env, lane, raw);
 }
 
+// a step that changed nothing but the sticky error bit: store the new flags word and a zero-reward scalar record
+template <int KJ>
+JSS_DEV void env_store_flags_only(const JssParams &p, const EnvRegs<KJ> &s, int env, int lane) {
+    if (lane == 0) {
+        p.state[(size_t)p.hdr_off16[env] * 4 + JSS_HDR_FLAGS] = (int32_t)s.flags;
+        reinterpret_cast<int4 *>(p.scalars)[env] =
+            make_int4(0, 0, s.t, (int)((s.flags << 8) | (s.flags & JSS_FLAG_DONE)));
+    }
+}
+
 template <int KJ, int MODE>
 JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int lane,
                              float *scratch) {
@@ -1066,10 +1050,7 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
     if (mode == JSS_MODE_RESET) {
         if (a.env_mask && a.env_mask[env] == 0) return;
         env_reset_regs<KJ>(iv, s, lane);
-        if (p.solution) {
-            int32_t *sol = p.solution + (size_t)env * p.jobs_max * p.machines_max;
-            for (int k = lane; k < p.jobs_max * p.machines_max; k += 32) sol[k] = -1;
-        }
+        env_clear_solution(p, env, lane);
         env_store<KJ>(p, iv, env, lane, s);
         env_emit_all<KJ>(p, iv, s, env, lane, scratch, 0);
         return;
@@ -1105,12 +1086,8 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         if (changed) {
             env_store<KJ>(p, iv, env, lane, s);
             env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
-        } else if (s.flags != flags_in) {                // only the sticky error bit changed
-            if (lane == 0) {
-                p.state[(size_t)p.hdr_off16[env] * 4 + JSS_HDR_FLAGS] = (int32_t)s.flags;
-                reinterpret_cast<int4 *>(p.scalars)[env] =
-                    make_int4(0, 0, s.t, (int)((s.flags << 8) | (s.flags & JSS_FLAG_DONE)));
-            }
+        } else if (s.flags != flags_in) {
+            env_store_flags_only<KJ>(p, s, env, lane);
         }
         if (a.export_after) env_export<KJ>(p, iv, s, env, lane);   // single-env facade: one launch per transition
         return;
@@ -1155,14 +1132,10 @@ JSS_DEV void jss_tile_desc(const JssParams &p, int tile, int &first, int &inst, 
     }
 }
 
-#ifndef JSS_MIN_CTAS
 // 80 registers -> 3 CTAs = 24 warps per SM; 3 x ~45 KB of shared memory (ta80) fit the 228 KB of an sm_90 SM.  4 CTAs
 // would fit in shared memory, but at 64 registers the 4-jobs-per-lane step kernel spills (DESIGN.md section 4).
 #define JSS_MIN_CTAS 3
-#endif
-#ifndef JSS_MIN_CTAS_SMALL
 #define JSS_MIN_CTAS_SMALL 4   // uniform batches with <= 32 jobs (KJ = 1) are latency-bound: 4 CTAs = 32 warps per SM at 64 registers
-#endif
 
 template <int KJ, int MODE>
 __global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, 1)
@@ -1224,37 +1197,36 @@ struct JssWarpSmem {        // per-warp shared-memory regions of the step kernel
     jss_saddr_t mbar, state_sa, scratch_sa, state_out_sa;
 };
 
-// env handled by `warp` in `tile` (-1: none) and where its state block lives (16-byte units)
+// where the state block of warp `warp` of `tile` (env `env`) lives, in 16-byte units: a uniform batch stores env e's
+// block at e * block16 (nothing to load), any other batch at the tile's base in tile order (JssTile).  The step
+// recomputes it after the env is simulated instead of carrying it in registers across the step.
 template <bool UNI>
-JSS_DEV int jss_tile_env(const JssParams &p, const JssLaunch &a, int tile, int tile_end, int warp, int lane,
-                         uint32_t &off16, uint32_t &blk16) {
-    if (UNI) {                           // env = 8 * tile + warp, block = env * block_words: nothing to load
-        const int e = tile * JSS_WARPS_PER_CTA + warp;
-        blk16 = (uint32_t)a.uni.block_words >> 2;
-        off16 = (uint32_t)e * blk16;
-        return (tile < tile_end && e < p.n_envs) ? e : -1;
-    }
-    if (tile >= tile_end) return -1;
-    const int4 td = *reinterpret_cast<const int4 *>(p.tiles + tile);     // JssTile, one 16-byte load
-    if (warp >= (td.y & 255)) return -1;
-    blk16 = (uint32_t)td.w;
-    off16 = (uint32_t)td.z + (uint32_t)warp * blk16;
-    return p.order[td.x + warp];
-}
-
-// where the state block of warp `warp` of `tile` lives (16-byte units); recomputed after the step instead of
-// being carried in registers across it
-template <bool UNI>
-JSS_DEV void jss_tile_state(const JssParams &p, const SmInst *uni, int tile, int warp, int env, uint32_t &off16,
+JSS_DEV void jss_tile_block(const JssParams &p, const SmInst &uni, int tile, int warp, int env, uint32_t &off16,
                             uint32_t &blk16) {
     if (UNI) {
-        blk16 = (uint32_t)uni->block_words >> 2;
+        blk16 = (uint32_t)uni.block_words >> 2;
         off16 = (uint32_t)env * blk16;
     } else {
-        const int4 td = *reinterpret_cast<const int4 *>(p.tiles + tile);
+        const int4 td = *reinterpret_cast<const int4 *>(p.tiles + tile);   // JssTile, one 16-byte load
         blk16 = (uint32_t)td.w;
         off16 = (uint32_t)td.z + (uint32_t)warp * blk16;
     }
+}
+
+// env handled by `warp` in `tile` (-1: none) and where its state block lives
+template <bool UNI>
+JSS_DEV int jss_tile_env(const JssParams &p, const JssLaunch &a, int tile, int tile_end, int warp, uint32_t &off16,
+                         uint32_t &blk16) {
+    if (UNI) {                           // env = 8 * tile + warp
+        const int e = tile * JSS_WARPS_PER_CTA + warp;
+        jss_tile_block<UNI>(p, a.uni, tile, warp, e, off16, blk16);
+        return (tile < tile_end && e < p.n_envs) ? e : -1;
+    }
+    if (tile >= tile_end) return -1;
+    const int4 td = *reinterpret_cast<const int4 *>(p.tiles + tile);
+    if (warp >= (td.y & 255)) return -1;
+    jss_tile_block<UNI>(p, a.uni, tile, warp, -1, off16, blk16);
+    return p.order[td.x + warp];
 }
 
 // tiles tile, tile + tile_step, ... < tile_end of ONE lane class through the prefetch pipeline
@@ -1265,7 +1237,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
     int env_next, act_next = 0;
     {
         uint32_t off16, blk16;
-        env_next = jss_tile_env<UNI>(p, a, tile, tile_end, warp, lane, off16, blk16);
+        env_next = jss_tile_env<UNI>(p, a, tile, tile_end, warp, off16, blk16);
         if (env_next >= 0) {
             if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)off16 * 4, blk16 * 16u, w.mbar);
             act_next = a.actions[env_next];
@@ -1292,7 +1264,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
         }
         {   // prefetch the next env's block + action
             uint32_t off16, blk16;
-            env_next = jss_tile_env<UNI>(p, a, tile + tile_step, tile_end, warp, lane, off16, blk16);
+            env_next = jss_tile_env<UNI>(p, a, tile + tile_step, tile_end, warp, off16, blk16);
             if (env_next >= 0) {
                 if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)off16 * 4, blk16 * 16u, w.mbar);
                 act_next = a.actions[env_next];
@@ -1318,22 +1290,18 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
             // new state -> shared staging -> one bulk store (every word of the block is rewritten)
             env_store_to<KJ>(p, iv, w.state_out, lane, s);
             uint32_t off16, blk16;
-            jss_tile_state<UNI>(p, &a.uni, tile, warp, env, off16, blk16);
+            jss_tile_block<UNI>(p, a.uni, tile, warp, env, off16, blk16);
             env_emit_all<KJ, true>(p, iv, s, env, lane, w.scratch, raw, w.scratch_sa,
                                    p.state + (size_t)off16 * 4, w.state_out_sa, blk16 * 16u);
-        } else if (s.flags != flags_in) {                // only the sticky error bit changed
-            if (lane == 0) {
-                p.state[(size_t)p.hdr_off16[env] * 4 + JSS_HDR_FLAGS] = (int32_t)s.flags;
-                reinterpret_cast<int4 *>(p.scalars)[env] =
-                    make_int4(0, 0, s.t, (int)((s.flags << 8) | (s.flags & JSS_FLAG_DONE)));
-            }
+        } else if (s.flags != flags_in) {
+            env_store_flags_only<KJ>(p, s, env, lane);
         }
     }
 }
 
 JSS_DEV void jss_step_carve(const JssSmemLayout &sl, char *sm, int warp, JssWarpSmem &w) {
     int woff = sl.off_warp0 + warp * sl.warp_stride;
-#if !defined(JSS_NO_OPAQUE_WBASE) && !defined(JSS_EMU)
+#ifndef JSS_EMU
     // keep the warp's region offset in ONE register instead of letting the optimiser recompute it from threadIdx
     // (S2R + shift + multiply-add) at every use: -1 % on the uniform ta80 step (94.0 -> 93.2 us)
     asm volatile("" : "+r"(woff));

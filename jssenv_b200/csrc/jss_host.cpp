@@ -30,6 +30,7 @@
 #endif
 
 #include "jss_rng.h"
+#include "jss_types.h"
 
 namespace {
 
@@ -159,12 +160,9 @@ class Pool {
 };
 
 // ---- packed observation -> float rows ----------------------------------------------------------------
-// Wire record of one job (JSS_WIRE_JOB_BYTES = 10, little endian):
-//   bytes 0..3  w0 = legal | tufco << 1 | todo << 12 | col4 << 18      (1 + 11 + 6 + 11 bits)
-//   bytes 4..6  idle_time_jobs_last_op   (24 bits; the makespan bound J*M*2047 < 2^24)
-//   bytes 7..9  total_idle_time_jobs     (24 bits)
-// total_perform_op_time_jobs (column 3) is not shipped: it equals t - total_idle while the job is unfinished and
-// jobs_length[j] afterwards; t travels in the env's scalar record.
+// A wire row holds one job record per job (jss_types.h; JSS_WIRE_JOB_BYTES = 10, little endian) with the legal bit
+// in w0.  total_perform_op_time_jobs (column 3) is not shipped: it equals t - total_idle while the job is unfinished
+// and jobs_length[j] afterwards; t travels in the env's scalar record.
 struct Cols {                  // per output column: divisor 1, max_time_op, M, max_time_jobs, max_time_op, sum_op, sum_op
     float d[16], r[16];        // d = divisor, r = RN(1 / divisor); the 7-column pattern twice (two jobs per 512-bit vector)
 };
@@ -178,19 +176,28 @@ inline float markstein(float x, float d, float r) {
 }
 
 inline void expand_job_scalar(const uint8_t *rec, int t, int M, int len, const Cols &c, float *out) {
-    uint32_t w0;
-    memcpy(&w0, rec, 4);
-    const int idle = rec[4] | (rec[5] << 8) | (rec[6] << 16), total = rec[7] | (rec[8] << 8) | (rec[9] << 16);
-    const int todo = (int)((w0 >> 12) & 63u);
+    uint32_t w0, w1;
+    uint16_t w2;
+    memcpy(&w0, rec, 4); memcpy(&w1, rec + 4, 4); memcpy(&w2, rec + 8, 2);
+    const int todo = jss_job_todo(w0), total = jss_job_total_idle(w1, w2);
     const int perf = todo < M ? t - total : len;
-    out[0] = (float)(w0 & 1u);
-    out[1] = markstein((float)((w0 >> 1) & 2047u), c.d[1], c.r[1]);
+    out[0] = (float)jss_job_legal(w0);
+    out[1] = markstein((float)jss_job_tufco(w0), c.d[1], c.r[1]);
     out[2] = markstein((float)todo, c.d[2], c.r[2]);
     out[3] = markstein((float)perf, c.d[3], c.r[3]);
-    out[4] = markstein((float)((w0 >> 18) & 2047u), c.d[4], c.r[4]);
-    out[5] = markstein((float)idle, c.d[5], c.r[5]);
+    out[4] = markstein((float)jss_job_col4(w0 & JSS_PACK_W0_MASK), c.d[4], c.r[4]);
+    out[5] = markstein((float)jss_job_idle_last(w1), c.d[5], c.r[5]);
     out[6] = markstein((float)total, c.d[6], c.r[6]);
 }
+
+// The SIMD paths shuffle a record's bytes to the dwords [w0, idle_last (bytes 4..6), total_idle (bytes 7..9), 0],
+// pick one dword per output column and shift and mask it: columns 0..6 of one job, twice for two jobs per vector.
+#define JSS_REC_SHIFTS JSS_PACK_LEGAL_SHIFT, JSS_PACK_TUFCO_SHIFT, 0, 0, JSS_PACK_COL4_SHIFT, 0, 0
+#define JSS_REC_MASKS 1, (int)JSS_PACK_DUR_MASK, (int)JSS_PACK_TODO_MASK, -1, (int)JSS_PACK_DUR_MASK, JSS_PACK_IDLE_MAX, \
+                      JSS_PACK_IDLE_MAX
+alignas(64) const int32_t k_rec_shift[16] = {JSS_REC_SHIFTS, JSS_REC_SHIFTS, 0, 0};
+alignas(64) const int32_t k_rec_mask[16] = {JSS_REC_MASKS, JSS_REC_MASKS, 0, 0};
+alignas(16) const uint8_t k_rec_shuffle[16] = {0, 1, 2, 3, 4, 5, 6, 0x80, 7, 8, 9, 0x80, 0x80, 0x80, 0x80, 0x80};
 
 void expand_env_scalar(const uint8_t *row, int J, int M, int t, const int32_t *len, const Cols &c, float *out) {
     for (int j = 0; j < J; j++) expand_job_scalar(row + (size_t)j * JSS_WIRE_JOB_BYTES, t, M, len[j], c, out + 7 * j);
@@ -200,11 +207,10 @@ void expand_env_scalar(const uint8_t *row, int J, int M, int t, const int32_t *l
 // one job per iteration: 16-byte load, byte shuffle to dwords, per-lane shift + mask, convert, divide
 __attribute__((target("avx2,fma"))) void expand_env_avx2(const uint8_t *row, int J, int M, int t, const int32_t *len,
                                                     const Cols &c, float *out) {
-    const __m128i shuf = _mm_setr_epi8(0, 1, 2, 3, 4, 5, 6, (char)0x80, 7, 8, 9, (char)0x80, (char)0x80, (char)0x80,
-                                       (char)0x80, (char)0x80);                    // -> [w0, idle, total, 0]
+    const __m128i shuf = _mm_load_si128(reinterpret_cast<const __m128i *>(k_rec_shuffle));
     const __m256i pick = _mm256_setr_epi32(0, 0, 0, 3, 0, 1, 2, 3);                // lane 3 (perf) is patched in below
-    const __m256i shift = _mm256_setr_epi32(0, 1, 12, 0, 18, 0, 0, 0);
-    const __m256i mask = _mm256_setr_epi32(1, 2047, 63, -1, 2047, 0xFFFFFF, 0xFFFFFF, 0);
+    const __m256i shift = _mm256_load_si256(reinterpret_cast<const __m256i *>(k_rec_shift));   // lane 7 is not stored
+    const __m256i mask = _mm256_load_si256(reinterpret_cast<const __m256i *>(k_rec_mask));
     const __m256 div = _mm256_loadu_ps(c.d), rcp = _mm256_loadu_ps(c.r);
     const __m256i store7 = _mm256_setr_epi32(-1, -1, -1, -1, -1, -1, -1, 0);
     for (int j = 0; j < J; j++) {
@@ -212,7 +218,7 @@ __attribute__((target("avx2,fma"))) void expand_env_avx2(const uint8_t *row, int
         __m128i d4 = _mm_shuffle_epi8(raw, shuf);
         const uint32_t w0 = (uint32_t)_mm_cvtsi128_si32(d4);
         const int total = _mm_extract_epi32(d4, 2);
-        const int todo = (int)((w0 >> 12) & 63u);
+        const int todo = jss_job_todo(w0);
         d4 = _mm_insert_epi32(d4, todo < M ? t - total : len[j], 3);
         __m256i v = _mm256_permutevar8x32_epi32(_mm256_castsi128_si256(d4), pick);
         v = _mm256_and_si256(_mm256_srlv_epi32(v, shift), mask);
@@ -226,13 +232,10 @@ __attribute__((target("avx2,fma"))) void expand_env_avx2(const uint8_t *row, int
 // two jobs (14 floats) per 512-bit vector
 __attribute__((target("avx512f,avx512bw,avx512vl,avx512dq"))) void expand_env_avx512(const uint8_t *row, int J, int M, int t,
                                                                                    const int32_t *len, const Cols &c, float *out) {
-    const __m128i shuf = _mm_setr_epi8(0, 1, 2, 3, 4, 5, 6, (char)0x80, 7, 8, 9, (char)0x80, (char)0x80, (char)0x80,
-                                       (char)0x80, (char)0x80);                    // -> [w0, idle, total, 0]
-    // source dwords: job A = 0..2, job B = 4..6.  Output lanes: A = 0..6, B = 7..13.
+    const __m128i shuf = _mm_load_si128(reinterpret_cast<const __m128i *>(k_rec_shuffle));
+    // source dwords: job A = 0..2, job B = 4..6.  Output lanes: A = 0..6, B = 7..13 (lanes 3 and 10 are replaced below)
     const __m512i pick = _mm512_setr_epi32(0, 0, 0, 2, 0, 1, 2, 4, 4, 4, 6, 4, 5, 6, 0, 0);
-    const __m512i shift = _mm512_setr_epi32(0, 1, 12, 0, 18, 0, 0, 0, 1, 12, 0, 18, 0, 0, 0, 0);
-    const __m512i mask = _mm512_setr_epi32(1, 2047, 63, 0xFFFFFF, 2047, 0xFFFFFF, 0xFFFFFF, 1, 2047, 63, 0xFFFFFF, 2047,
-                                           0xFFFFFF, 0xFFFFFF, 0, 0);
+    const __m512i shift = _mm512_load_si512(k_rec_shift), mask = _mm512_load_si512(k_rec_mask);
     const __m512i lenpick = _mm512_setr_epi32(0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0);   // lane 3 <- len[j], lane 10 <- len[j+1]
     const __m512 div = _mm512_loadu_ps(c.d), rcp = _mm512_loadu_ps(c.r);
     const __m512i tv = _mm512_set1_epi32(t), mv = _mm512_set1_epi32(M);
@@ -266,8 +269,6 @@ bool have_avx512() {
 // dst and n need no alignment; cache-bypassing stores for the 64-byte-aligned body (the expanded batch is
 // far larger than the caches and is consumed by somebody else)
 __attribute__((target("avx2"))) void stream_copy(float *dst, const float *src, size_t n) {
-    static const bool nt = !(getenv("JSS_HOST_NT") && getenv("JSS_HOST_NT")[0] == '0');   // experiments: regular stores
-    if (!nt) { memcpy(dst, src, n * sizeof(float)); return; }
     size_t i = 0;
     while (i < n && (reinterpret_cast<uintptr_t>(dst + i) & 63u)) { dst[i] = src[i]; i++; }
     for (; i + 16 <= n; i += 16) {

@@ -20,17 +20,59 @@ struct JssInstDesc {
     float r_mto, r_mtj, r_sop, r_M;
 };
 
-// ---- per-env state block in HBM (every region 16-byte aligned) -------------------
-// The five per-job integers carry 76 bits, packed into 10 bytes per job:
-//   w0  u32[Jcap]  todo | tufco << 6 | col4 << 17          (28 bits used)
-//   w1  u32[Jcap]  idle_last | (total_idle & 0xff) << 24
-//   w2  u16[Jcap]  total_idle >> 8                        (region padded to a multiple of 16 bytes)
+#ifndef JSS_HD   // as in jss_rng.h
+#if defined(__CUDACC__)
+#define JSS_HD __host__ __device__
+#else
+#define JSS_HD
+#endif
+#endif
+
+// ---- packed record of one job: the state block and the host wire rows both use it ------------------
+// The five per-job integers carry 76 bits, packed into three words (10 bytes):
+//   w0  u32  todo | tufco << 6 | col4 << 17          (bits 28..31: the legal bit in a wire record, 0 in the state block)
+//   w1  u32  idle_last | (total_idle & 0xff) << 24
+//   w2  u16  total_idle >> 8
 // todo = todo_time_step_job in [0, M], M <= 32 (padding slots hold M): 6 bits; tufco =
 // time_until_finish_current_op_jobs and col4 = the numerator of real_obs[:,4] (stale by design,
 // jss_env.py:569-586) are at most one duration, <= 2047: 11 bits each; idle_last = idle_time_jobs_last_op and
 // total_idle = total_idle_time_jobs are at most current_time_step, and time only advances to a pending
-// machine completion, so t <= sum_op <= 256 * 32 * 2047 < 2^24: 24 bits each (the packed host wire rows,
-// env_pack, rely on the same bound).  jss_import_state checks these ranges.
+// machine completion, so t <= sum_op <= 256 * 32 * 2047 < 2^24: 24 bits each.  jss_import_state checks these
+// ranges.  Read as little-endian bytes, w1 and w2 are idle_last (bytes 4..6) and total_idle (bytes 7..9).
+#define JSS_PACK_TODO_BITS 6
+#define JSS_PACK_DUR_BITS 11
+#define JSS_PACK_IDLE_BITS 24
+#define JSS_PACK_TUFCO_SHIFT JSS_PACK_TODO_BITS
+#define JSS_PACK_COL4_SHIFT (JSS_PACK_TUFCO_SHIFT + JSS_PACK_DUR_BITS)
+#define JSS_PACK_LEGAL_SHIFT (JSS_PACK_COL4_SHIFT + JSS_PACK_DUR_BITS)   // wire records only
+#define JSS_PACK_W0_MASK ((1u << JSS_PACK_LEGAL_SHIFT) - 1u)   // w0 without a wire record's legal bit
+#define JSS_PACK_TODO_MASK ((1u << JSS_PACK_TODO_BITS) - 1u)
+#define JSS_PACK_DUR_MASK ((1u << JSS_PACK_DUR_BITS) - 1u)
+#define JSS_PACK_IDLE_MAX ((1 << JSS_PACK_IDLE_BITS) - 1)   // largest idle_last / total_idle a record holds
+
+struct JssJobWords {
+    uint32_t w0, w1, w2;
+};
+JSS_HD static inline JssJobWords jss_pack_job(int todo, int tufco, int col4, int idle_last, int total_idle) {
+    const uint32_t ti = (uint32_t)total_idle;
+    JssJobWords r;
+    r.w0 = (uint32_t)todo | ((uint32_t)tufco << JSS_PACK_TUFCO_SHIFT) | ((uint32_t)col4 << JSS_PACK_COL4_SHIFT);
+    r.w1 = (uint32_t)idle_last | (ti << JSS_PACK_IDLE_BITS);
+    r.w2 = ti >> (32 - JSS_PACK_IDLE_BITS);
+    return r;
+}
+JSS_HD static inline int jss_job_todo(uint32_t w0) { return (int)(w0 & JSS_PACK_TODO_MASK); }
+JSS_HD static inline int jss_job_tufco(uint32_t w0) { return (int)((w0 >> JSS_PACK_TUFCO_SHIFT) & JSS_PACK_DUR_MASK); }
+// col4 is the top field of a state-block w0; a wire record's w0 goes through JSS_PACK_W0_MASK first
+JSS_HD static inline int jss_job_col4(uint32_t w0) { return (int)(w0 >> JSS_PACK_COL4_SHIFT); }
+JSS_HD static inline uint32_t jss_job_legal(uint32_t w0) { return w0 >> JSS_PACK_LEGAL_SHIFT; }
+JSS_HD static inline int jss_job_idle_last(uint32_t w1) { return (int)(w1 & (uint32_t)JSS_PACK_IDLE_MAX); }
+JSS_HD static inline int jss_job_total_idle(uint32_t w1, uint32_t w2) {
+    return (int)((w1 >> JSS_PACK_IDLE_BITS) | (w2 << (32 - JSS_PACK_IDLE_BITS)));
+}
+
+// ---- per-env state block in HBM (every region 16-byte aligned) -------------------
+//   w0  u32[Jcap], w1  u32[Jcap], w2  u16[Jcap] (region padded to a multiple of 16 bytes): the job records
 //   tail:  [0, Mcap)  time_until_available_machine (int32)
 //   then 8 words  = 32 bytes, byte l = lane l's job bits: bit i legal(job KJ*l+i),
 //                   bit 4+i blocked by a no-op (action_illegal_no_op)
@@ -43,17 +85,6 @@ struct JssInstDesc {
 #define JSS_HDR_FLAGS 1
 #define JSS_HDR_EP_STEPS 2
 #define JSS_HDR_EP_RETURN 3
-#define JSS_PACK_TODO_BITS 6
-#define JSS_PACK_DUR_BITS 11
-#define JSS_PACK_IDLE_MAX 0xffffff   // largest idle_last / total_idle the block holds (2^24 - 1)
-
-#ifndef JSS_HD   // as in jss_rng.h
-#if defined(__CUDACC__)
-#define JSS_HD __host__ __device__
-#else
-#define JSS_HD
-#endif
-#endif
 
 // State-block geometry of an instance in int32 words: the ONE definition the host (block offsets, shared-memory
 // sizing) and the kernels (SmInst) use.  Per-lane slices are whole vectors: J rounded up to 4 (to 8 for the
@@ -90,7 +121,11 @@ struct JssCtaRange {   // mixed batches: the tiles of one persistent CTA -- an e
 };
 
 struct JssParams {
-    int32_t n_envs, Jcap, Mcap, block_words;   // Jcap / Mcap / block_words: batch maxima (shared-memory sizing only)
+    int32_t n_envs;
+    // Unused: keeps the kernel-parameter offsets.  Without it ptxas allocates the 80-register mixed-batch step
+    // kernels differently and the masked-random one spills; a build with that spill ran cfg5's masked-random step
+    // 1.6 % slower on an H100 SXM (400 W power limit).
+    int32_t pad0_[3];
     int32_t jobs_max, machines_max, mask_stride, create_flags;
     int32_t uniform_inst;    // >= 0: every env runs this instance and `order` is the identity
     uint64_t env_id_base;
@@ -127,9 +162,7 @@ struct SmInst {
     float r_mto, r_mtj, r_sop, r_M;       // ... and their correctly rounded reciprocals
     int Jcap, Mcap, block_words;          // state-block geometry of THIS instance (jss_block_geom) ...
     int tail;                             // ... and the word where tuam starts
-    // NEGATED divisor / reciprocal PAIRS for the packed (f32x2) observation quotients: columns (1,4), (2,3), (5,6)
-    float n14[2], r14[2], n23[2], r23[2], n56[2], r56[2];
-    int pad_[3];                          // 32 words: the tables behind it in shared memory stay 16-byte aligned
+    int pad_[3];                          // 20 words: the tables behind it in shared memory stay 16-byte aligned
 };
 static_assert(sizeof(SmInst) % 16 == 0, "SmInst must keep the shared-memory tables 16-byte aligned");
 struct JssLaunch {           // per-launch arguments
@@ -159,6 +192,4 @@ struct JssLaunch {           // per-launch arguments
 #define JSS_MODE_IMPORT 5
 #define JSS_MODE_PACK 6     // packed observation wire rows for the host-buffer path (jss_host_step_begin_packed)
 
-#ifndef JSS_WARPS_PER_CTA
 #define JSS_WARPS_PER_CTA 8
-#endif
