@@ -35,6 +35,8 @@ static cudaError_t jss_launch_pdl(void (*kern)(KArgs...), int grid, int block, s
 #include <string>
 #include <sched.h>
 #include <cctype>
+#include <map>
+#include <utility>
 #include <vector>
 
 #include "jss_device.cuh"
@@ -43,12 +45,6 @@ static cudaError_t jss_launch_pdl(void (*kern)(KArgs...), int grid, int block, s
 namespace {
 
 std::string g_create_error;
-
-struct HostInst {
-    int J, M;
-    int64_t max_time_op, max_time_jobs, sum_op;
-    std::vector<int32_t> len;      // jobs_length (host copy: the packed-observation expansion needs it)
-};
 
 }  // namespace
 
@@ -62,15 +58,15 @@ struct jss_handle {
     int64_t launches = 0;
     double cr_factor = 1.5;                        // CriticalRatio(due_date_factor), dispatching.py:337
 
-    std::vector<HostInst> insts;
-    std::vector<JssInstDesc> descs;
+    std::vector<JssInst> insts;
+    std::vector<int32_t> len;                      // the jobs_length pool (the packed-observation expansion reads it)
     bool loaded = false, assigned = false;
 
     // device allocations
     std::vector<void *> allocs;
     void *host_block = nullptr;                    // JSS_CREATE_HOST_MIRROR: pinned + mapped block behind the outputs
     int32_t *mirror_actions = nullptr;
-    JssInstDesc *d_inst = nullptr;
+    JssInst *d_inst = nullptr;
     uint16_t *d_ops = nullptr, *d_rem = nullptr;
     int32_t *d_len = nullptr;
     unsigned long long *d_stats = nullptr;
@@ -78,8 +74,9 @@ struct jss_handle {
     JssParams p{};
     JssSmemLayout sl_env{}, sl_step{}, sl_step_rem{};   // shared-memory layouts of the generic / step kernels (step: without / with the suffix-sum table)
     int class_tile_begin[4] = {0, 0, 0, 0}, class_tile_end[4] = {0, 0, 0, 0};  // KJ = 1, 2, 4, 8
-    int step_grid[24] = {0};                        // resident-CTA grids of the step kernel variants (filled lazily)
-    int env_grid[16] = {0};                         // resident CTAs per SM of the generic kernel variants (filled lazily)
+    int n_tiles = 0;
+    std::map<std::pair<const void *, size_t>, int> ctas_per_sm;   // by kernel and dynamic shared memory (filled lazily)
+    std::map<const void *, size_t> smem_optin;     // by kernel: the largest dynamic shared memory it was opted in to
     std::vector<int32_t> env_inst;
 
     // host-buffer stepping
@@ -129,130 +126,94 @@ inline int kj_of(int J) { return J <= 32 ? 1 : (J <= 64 ? 2 : (J <= 128 ? 4 : 8)
 inline int class_of(int kj) { return kj == 1 ? 0 : (kj == 2 ? 1 : (kj == 4 ? 2 : 3)); }
 size_t smem_bytes(const JssSmemLayout &sl) { return (size_t)sl.off_warp0 + (size_t)JSS_WARPS_PER_CTA * sl.warp_stride; }
 
-void fill_uni(const JssInstDesc &d, SmInst &u) {
-    u = SmInst{};
-    jss_fill_sminst(d, &u);
+// resident CTAs per SM of `kern` at `smem` bytes of dynamic shared memory; the first call per kernel and size also
+// opts the kernel in to more than 48 KB.  Keyed by size too: the rule-sampling step kernels run with and without the
+// suffix-sum table.  The opt-in is one limit per kernel, so it only ever grows: lowering it for the smaller layout
+// would make the next launch with the larger one fail.
+template <typename Kern>
+int ctas_per_sm(jss_t *h, Kern kern, size_t smem, int &per_sm) {
+    const void *key = reinterpret_cast<const void *>(kern);
+    int &n = h->ctas_per_sm[{key, smem}];
+    if (n == 0) {
+        size_t &optin = h->smem_optin[key];
+        if (smem > 48 * 1024 && smem > optin) {
+            JSS_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            optin = smem;
+        }
+        JSS_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, JSS_WARPS_PER_CTA * 32, smem));
+        if (n < 1) { n = 0; return fail(h, JSS_ERR_CUDA, "kernel does not fit on an SM (smem %zu B)", smem); }
+    }
+    per_sm = n;
+    return JSS_OK;
 }
 
-template <typename Kern>
-int step_grid_for(jss_t *h, Kern kern, int slot, size_t smem) {
-    int &grid = h->step_grid[slot];
-    if (grid == 0) {                                     // once per handle: opt-in smem + occupancy
-        if (smem > 48 * 1024)
-            JSS_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 0;
-        JSS_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, JSS_WARPS_PER_CTA * 32, smem));
-        if (per_sm < 1) return fail(h, JSS_ERR_CUDA, "step kernel does not fit on an SM (smem %zu B)", smem);
-        grid = h->sm_count * per_sm;
+typedef void (*JssKernel)(JssParams, JssLaunch, JssSmemLayout);
+
+// the fused step kernel: uniform batches by lane class, mixed batches by whether they hold instances with 129..256 jobs
+template <int SAMPLE>
+JssKernel step_kernel(const jss_t *h) {
+    if (h->p.uniform_inst < 0)
+        return h->class_tile_end[3] > h->class_tile_begin[3] ? jss_step_mixed_kernel<SAMPLE, true>
+                                                               : jss_step_mixed_kernel<SAMPLE, false>;
+    switch (kj_of(h->insts[h->p.uniform_inst].J)) {
+    case 1: return jss_step_kernel<1, SAMPLE>;
+    case 2: return jss_step_kernel<2, SAMPLE>;
+    case 4: return jss_step_kernel<4, SAMPLE>;
+    default: return jss_step_kernel<8, SAMPLE>;
     }
-    return JSS_OK;
 }
 
 // one fused step launch (PDL).  A uniform batch runs min(tiles, resident CTAs) persistent CTAs over static strided
 // tiles; a mixed batch runs one CTA per JssCtaRange (all resident: SMs x 3).
-template <typename Kern>
-int launch_step_kernel(jss_t *h, Kern kern, int slot, const JssLaunch &a, bool want_rem, cudaStream_t st) {
-    const JssSmemLayout &sl = want_rem ? h->sl_step_rem : h->sl_step;
+int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
+    // SAMPLE: 0 none, 1 masked-uniform sampler, 2 dispatching rule
+    const int sample = a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
+    const JssKernel kern = sample == 0 ? step_kernel<0>(h) : sample == 1 ? step_kernel<1>(h) : step_kernel<2>(h);
+    // only the rules that read the suffix sums stage them; the other launches leave their room to the L1
+    const JssSmemLayout &sl = sample == 2 && jss_rule_wants_rem(a.rule) ? h->sl_step_rem : h->sl_step;
     const size_t smem = smem_bytes(sl);
-    int rc = step_grid_for(h, kern, slot, smem);
+    int per_sm = 0, rc = ctas_per_sm(h, kern, smem, per_sm);
     if (rc) return rc;
-    const int grid = h->p.uniform_inst >= 0 ? std::min(a.tile_end, h->step_grid[slot]) : h->p.n_cta_ranges;
+    int grid = h->p.n_cta_ranges;
+    if (h->p.uniform_inst >= 0) {
+        a.tile_begin = 0;
+        a.tile_end = (h->n_envs + JSS_WARPS_PER_CTA - 1) / JSS_WARPS_PER_CTA;
+        grid = std::min(a.tile_end, h->sm_count * per_sm);
+    }
     JSS_CUDA(h, JSS_LAUNCH_PDL(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl));
     JSS_CUDA(h, cudaGetLastError());
     h->launches += 1;
     return JSS_OK;
 }
 
-// uniform batch: one instance, its scalars in the kernel parameters
-template <int KJ, int SAMPLE>
-int launch_step_uniform(jss_t *h, const JssLaunch &a_in, bool want_rem, cudaStream_t st) {
-    JssLaunch a = a_in;
-    fill_uni(h->descs[h->p.uniform_inst], a.uni);
-    a.tile_begin = 0;
-    a.tile_end = (h->n_envs + JSS_WARPS_PER_CTA - 1) / JSS_WARPS_PER_CTA;
-    return launch_step_kernel(h, jss_step_kernel<KJ, SAMPLE>, class_of(KJ) * 4 + SAMPLE + (want_rem ? 1 : 0), a,
-                              want_rem, st);
-}
-
-// mixed batch: ONE launch over all lane classes, every CTA an equal slice of each class (jss_assign)
-template <int SAMPLE, bool BIG>
-int launch_step_mixed(jss_t *h, const JssLaunch &a, bool want_rem, cudaStream_t st) {
-    return launch_step_kernel(h, jss_step_mixed_kernel<SAMPLE, BIG>, (BIG ? 20 : 16) + SAMPLE + (want_rem ? 1 : 0), a,
-                              want_rem, st);
-}
-
-int launch_step(jss_t *h, const JssLaunch &a, cudaStream_t st) {
-    const bool rem = jss_rule_wants_rem(a.rule);
-    const int sample = a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
-    if (h->p.uniform_inst < 0) {
-        const bool big = h->class_tile_end[3] > h->class_tile_begin[3];     // instances with 129..256 jobs in the batch
-        if (big) {
-            if (sample == 0) return launch_step_mixed<0, true>(h, a, false, st);
-            if (sample == 1) return launch_step_mixed<1, true>(h, a, false, st);
-            return launch_step_mixed<2, true>(h, a, rem, st);
-        }
-        if (sample == 0) return launch_step_mixed<0, false>(h, a, false, st);
-        if (sample == 1) return launch_step_mixed<1, false>(h, a, false, st);
-        return launch_step_mixed<2, false>(h, a, rem, st);
-    }
-    const int kj = kj_of(h->insts[h->p.uniform_inst].J);
-#define JSS_STEP_UNI(KJ_)                                                               \
-    do {                                                                                \
-        if (sample == 0) return launch_step_uniform<KJ_, 0>(h, a, false, st);           \
-        if (sample == 1) return launch_step_uniform<KJ_, 1>(h, a, false, st);           \
-        return launch_step_uniform<KJ_, 2>(h, a, rem, st);                              \
-    } while (0)
-    if (kj == 1) JSS_STEP_UNI(1);
-    if (kj == 2) JSS_STEP_UNI(2);
-    if (kj == 4) JSS_STEP_UNI(4);
-    JSS_STEP_UNI(8);
-#undef JSS_STEP_UNI
-}
-
-template <int KJ, int MODE>
-int launch_variant(jss_t *h, const JssLaunch &a, const JssSmemLayout &sl, cudaStream_t st) {
-    const int n_tiles = a.tile_end - a.tile_begin;
-    const size_t smem = smem_bytes(sl);
-    auto kern = jss_env_kernel<KJ, MODE>;
-    // once per handle and kernel variant: opt-in to > 48 KB of dynamic shared memory, resident CTAs per SM
-    int &per_sm = h->env_grid[class_of(KJ) * 4 + (MODE == JSS_MODE_RESET ? 0 : MODE == JSS_MODE_ROLLOUT ? 1 : 2)];
-    if (per_sm == 0) {
-        if (smem > 48 * 1024)
-            JSS_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        JSS_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, JSS_WARPS_PER_CTA * 32, smem));
-        if (per_sm < 1) { per_sm = 0; return fail(h, JSS_ERR_CUDA, "kernel does not fit on an SM (smem %zu B)", smem); }
-    }
-    // policy kernels touch ~50 B per env: latency-bound, so give every tile its own CTA
-    // instead of a persistent loop with a dependent load per iteration
-    const int grid = (MODE == JSS_MODE_POLICY) ? n_tiles : std::min(n_tiles, h->sm_count * per_sm);
-    JSS_LAUNCH(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
-    JSS_CUDA(h, cudaGetLastError());
-    h->launches += 1;
-    return JSS_OK;
-}
-
+// the generic kernel of lane class KJ: MODE = JSS_MODE_RESET also serves export, import, pack and exporting steps
 template <int KJ>
-int launch_class(jss_t *h, const JssLaunch &a, const JssSmemLayout &sl, cudaStream_t st) {
-    if (a.tile_end - a.tile_begin <= 0) return JSS_OK;
-    switch (a.mode) {
-    case JSS_MODE_POLICY: return launch_variant<KJ, JSS_MODE_POLICY>(h, a, sl, st);
-    case JSS_MODE_ROLLOUT: return launch_variant<KJ, JSS_MODE_ROLLOUT>(h, a, sl, st);
-    default: return launch_variant<KJ, JSS_MODE_RESET>(h, a, sl, st);   // reset / export / import
-    }
+JssKernel env_kernel(int mode) {
+    if (mode == JSS_MODE_POLICY) return jss_env_kernel<KJ, JSS_MODE_POLICY>;
+    if (mode == JSS_MODE_ROLLOUT) return jss_env_kernel<KJ, JSS_MODE_ROLLOUT>;
+    return jss_env_kernel<KJ, JSS_MODE_RESET>;
 }
 
 int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
+    if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
     const JssSmemLayout &sl = h->sl_env;
-    for (int c = 0; c < 4; c++) {
+    const size_t smem = smem_bytes(sl);
+    for (int c = 0; c < 4; c++) {               // one launch per lane class present
         a.tile_begin = h->class_tile_begin[c];
         a.tile_end = h->class_tile_end[c];
-        int rc = JSS_OK;
-        if (c == 0) rc = launch_class<1>(h, a, sl, st);
-        else if (c == 1) rc = launch_class<2>(h, a, sl, st);
-        else if (c == 2) rc = launch_class<4>(h, a, sl, st);
-        else rc = launch_class<8>(h, a, sl, st);
-        if (rc != JSS_OK) return rc;
+        const int n_tiles = a.tile_end - a.tile_begin;
+        if (n_tiles <= 0) continue;
+        const JssKernel kern = c == 0 ? env_kernel<1>(a.mode) : c == 1 ? env_kernel<2>(a.mode)
+                             : c == 2 ? env_kernel<4>(a.mode) : env_kernel<8>(a.mode);
+        int per_sm = 0, rc = ctas_per_sm(h, kern, smem, per_sm);
+        if (rc) return rc;
+        // policy kernels touch ~50 B per env: latency-bound, so give every tile its own CTA
+        // instead of a persistent loop with a dependent load per iteration
+        const int grid = (a.mode == JSS_MODE_POLICY) ? n_tiles : std::min(n_tiles, h->sm_count * per_sm);
+        JSS_LAUNCH(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
+        JSS_CUDA(h, cudaGetLastError());
+        h->launches += 1;
     }
     return JSS_OK;
 }
@@ -333,7 +294,6 @@ int jss_load_instances(jss_t *h, int n_inst, const int32_t *jobs, const int32_t 
     std::vector<uint16_t> ops, rem;
     std::vector<int32_t> len;
     h->insts.resize(n_inst);
-    h->descs.resize(n_inst);
     for (int k = 0; k < n_inst; k++) {
         const int J = jobs[k], M = machines[k];
         if (J <= 0 || M <= 1)  // asserts at jss_env.py:93-94
@@ -342,8 +302,8 @@ int jss_load_instances(jss_t *h, int n_inst, const int32_t *jobs, const int32_t 
             return fail(h, JSS_ERR_UNSUPPORTED, "instance %d: %dx%d exceeds the %dx%d kernel limit", k, J, M,
                         JSS_MAX_JOBS, JSS_MAX_MACHINES);
         const int32_t *mm = machine + offsets[k], *dd = duration + offsets[k];
-        HostInst hi{J, M, 0, 0, 0, std::vector<int32_t>((size_t)J)};
-        JssInstDesc d{};
+        int64_t max_time_op = 0, max_time_jobs = 0, sum_op = 0;
+        JssInst d{};
         d.J = J; d.M = M;
         d.ops_off = (int32_t)ops.size();
         d.len_off = (int32_t)len.size();
@@ -364,12 +324,11 @@ int jss_load_instances(jss_t *h, int n_inst, const int32_t *jobs, const int32_t 
                                 JSS_MAX_DURATION);
                 ops[d.ops_off + j * M + i] = (uint16_t)((m << JSS_OP_SHIFT) | t);
                 total += t;
-                hi.max_time_op = std::max<int64_t>(hi.max_time_op, t);  // jss_env.py:86
+                max_time_op = std::max<int64_t>(max_time_op, t);        // jss_env.py:86
             }
             len[d.len_off + j] = (int32_t)total;                        // jss_env.py:87
-            hi.len[j] = (int32_t)total;
-            hi.sum_op += total;                                         // jss_env.py:88
-            hi.max_time_jobs = std::max(hi.max_time_jobs, total);       // jss_env.py:89
+            sum_op += total;                                            // jss_env.py:88
+            max_time_jobs = std::max(max_time_jobs, total);             // jss_env.py:89
             int64_t suffix = 0;
             rem[d.rem_off + j * (M + 1) + M] = 0;
             for (int i = M - 1; i >= 0; i--) {
@@ -377,25 +336,28 @@ int jss_load_instances(jss_t *h, int n_inst, const int32_t *jobs, const int32_t 
                 rem[d.rem_off + j * (M + 1) + i] = (uint16_t)suffix;    // <= 32 * 2047 < 65536
             }
         }
-        d.max_time_op = (int32_t)hi.max_time_op;
-        d.max_time_jobs = (int32_t)hi.max_time_jobs;
-        d.sum_op = (int32_t)hi.sum_op;
+        d.max_time_op = (int32_t)max_time_op;
+        d.max_time_jobs = (int32_t)max_time_jobs;
+        d.sum_op = (int32_t)sum_op;
+        d.f_mto = (float)d.max_time_op; d.f_mtj = (float)d.max_time_jobs; d.f_sop = (float)d.sum_op; d.f_M = (float)d.M;
         d.r_mto = 1.0f / (float)d.max_time_op;
         d.r_mtj = 1.0f / (float)d.max_time_jobs;
         d.r_sop = 1.0f / (float)d.sum_op;
         d.r_M = 1.0f / (float)d.M;
-        h->insts[k] = hi;
-        h->descs[k] = d;
+        const JssBlockGeom g = jss_block_geom(J, M);
+        d.Jcap = g.Jcap; d.Mcap = g.Mcap; d.block_words = g.words; d.tail = g.tail;
+        h->insts[k] = d;
     }
     int rc;
     if ((rc = dev_alloc(h, &h->d_inst, (size_t)n_inst))) return rc;
     if ((rc = dev_alloc(h, &h->d_ops, ops.size()))) return rc;
     if ((rc = dev_alloc(h, &h->d_len, len.size()))) return rc;
     if ((rc = dev_alloc(h, &h->d_rem, rem.size()))) return rc;
-    JSS_CUDA(h, cudaMemcpy(h->d_inst, h->descs.data(), sizeof(JssInstDesc) * n_inst, cudaMemcpyHostToDevice));
+    JSS_CUDA(h, cudaMemcpy(h->d_inst, h->insts.data(), sizeof(JssInst) * n_inst, cudaMemcpyHostToDevice));
     JSS_CUDA(h, cudaMemcpy(h->d_ops, ops.data(), ops.size() * 2, cudaMemcpyHostToDevice));
     JSS_CUDA(h, cudaMemcpy(h->d_len, len.data(), len.size() * 4, cudaMemcpyHostToDevice));
     JSS_CUDA(h, cudaMemcpy(h->d_rem, rem.data(), rem.size() * 2, cudaMemcpyHostToDevice));
+    h->len = std::move(len);
     h->loaded = true;
     return JSS_OK;
 }
@@ -441,7 +403,6 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
         return ka < kb;
     });
     std::vector<JssTile> tiles;
-    std::vector<uint32_t> state_off16((size_t)N), hdr_off16((size_t)N);
     for (int c = 0; c < 4; c++) h->class_tile_begin[c] = h->class_tile_end[c] = 0;
     int pos = 0;
     int cur_class = -1;
@@ -449,8 +410,7 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     while (pos < N) {
         const int k = env_to_inst[order[pos]];
         const int c = class_of(kj_of(h->insts[k].J));
-        const JssBlockGeom g = jss_block_geom(h->insts[k].J, h->insts[k].M);
-        const uint32_t block16 = (uint32_t)g.words / 4, hdr16 = (uint32_t)g.hdr / 4;
+        const uint32_t block16 = (uint32_t)h->insts[k].block_words / 4;
         int end = pos;
         while (end < N && env_to_inst[order[end]] == k) end++;
         if (c != cur_class) {
@@ -465,16 +425,13 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
             t.inst_count = (k << 8) | cnt;
             t.state_off16 = (uint32_t)off16;
             t.block16 = block16;
-            for (int w = 0; w < cnt; w++) {
-                state_off16[order[f + w]] = (uint32_t)(off16 + (uint64_t)w * block16);
-                hdr_off16[order[f + w]] = (uint32_t)(off16 + (uint64_t)w * block16) + hdr16;
-            }
             off16 += (uint64_t)cnt * block16;
             tiles.push_back(t);
         }
         pos = end;
     }
     if (cur_class >= 0) h->class_tile_end[cur_class] = (int)tiles.size();
+    h->n_tiles = (int)tiles.size();
     if (off16 >= (1ull << 32)) return fail(h, JSS_ERR_UNSUPPORTED, "state exceeds 64 GiB");
     const size_t state_words = (size_t)off16 * 4;
 
@@ -512,10 +469,10 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     }
     p.inst = h->d_inst; p.ops_pool = h->d_ops; p.len_pool = h->d_len; p.rem_pool = h->d_rem;
 
-    {   // shared-memory layouts: [SmInst][ops u16][len i32][rem u16][per-warp regions], 16-byte aligned regions
+    {   // shared-memory layouts: [JssInst][ops u16][len i32][rem u16][per-warp regions], 16-byte aligned regions
         const JssBlockGeom g = jss_block_geom(jmax, mmax);   // the geometry grows with J and M: batch maxima
         JssSmemLayout sl{};
-        sl.off_len = (int32_t)sizeof(SmInst) + round_up(ops_max, 8) * 2;
+        sl.off_len = (int32_t)sizeof(JssInst) + round_up(ops_max, 8) * 2;
         sl.off_rem = sl.off_len + round_up(jmax, 4) * 4;
         sl.off_warp0 = sl.off_rem + round_up(rem_max, 8) * 2;
         // observation staging (7 floats per job slot); env_check_no_op (general instances) also keeps its 32-int
@@ -535,23 +492,16 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     int32_t *d_order = nullptr;
     JssTile *d_tiles = nullptr;
     JssCtaRange *d_ranges = nullptr;
-    uint32_t *d_soff = nullptr, *d_hoff = nullptr;
     if ((rc = dev_alloc(h, &d_order, (size_t)N))) return rc;
     if ((rc = dev_alloc(h, &d_tiles, tiles.size()))) return rc;
     if ((rc = dev_alloc(h, &d_ranges, ranges.size()))) return rc;
-    if ((rc = dev_alloc(h, &d_soff, (size_t)N))) return rc;
-    if ((rc = dev_alloc(h, &d_hoff, (size_t)N))) return rc;
     JSS_CUDA(h, cudaMemcpy(d_order, order.data(), (size_t)N * 4, cudaMemcpyHostToDevice));
     JSS_CUDA(h, cudaMemcpy(d_tiles, tiles.data(), tiles.size() * sizeof(JssTile), cudaMemcpyHostToDevice));
     JSS_CUDA(h, cudaMemcpy(d_ranges, ranges.data(), ranges.size() * sizeof(JssCtaRange), cudaMemcpyHostToDevice));
-    JSS_CUDA(h, cudaMemcpy(d_soff, state_off16.data(), (size_t)N * 4, cudaMemcpyHostToDevice));
-    JSS_CUDA(h, cudaMemcpy(d_hoff, hdr_off16.data(), (size_t)N * 4, cudaMemcpyHostToDevice));
     p.order = d_order;
     p.tiles = d_tiles;
     p.cta_ranges = d_ranges;
     p.n_cta_ranges = (int32_t)ranges.size();
-    p.state_off16 = d_soff;
-    p.hdr_off16 = d_hoff;
     const size_t NJ = (size_t)N * jmax, NM = (size_t)N * mmax;
     if ((rc = dev_alloc(h, &p.state, state_words))) return rc;
     if (h->create_flags & JSS_CREATE_HOST_MIRROR) {
@@ -860,12 +810,8 @@ int jss_host_expand_obs_range(jss_t *h, const uint8_t *wire_host, const int32_t 
     if (!h || !h->assigned) return fail(h, JSS_ERR_STATE, "jss_host_expand_obs: jss_assign must be called first");
     if (!wire_host || !scalars_host || !obs_host || env_begin < 0 || env_end > h->n_envs || env_begin > env_end)
         return fail(h, JSS_ERR_INVALID, "jss_host_expand_obs: bad arguments");
-    std::vector<JssHostInst> hi(h->insts.size());
-    for (size_t k = 0; k < h->insts.size(); k++)
-        hi[k] = JssHostInst{h->insts[k].J, h->insts[k].M, h->insts[k].max_time_op, h->insts[k].max_time_jobs,
-                            h->insts[k].sum_op, h->insts[k].len.data()};
-    JssHostExpandArgs a{wire_host, jss_host_wire_stride(h), scalars_host, h->env_inst.data(), hi.data(), obs_host,
-                        h->p.jobs_max, env_begin, env_end};
+    JssHostExpandArgs a{wire_host, jss_host_wire_stride(h), scalars_host, h->env_inst.data(), h->insts.data(),
+                        h->len.data(), obs_host, h->p.jobs_max, env_begin, env_end};
     jss_host_expand_impl(&a);
     return JSS_OK;
 }
@@ -934,7 +880,10 @@ int jss_stats(jss_t *h, int64_t *out_host, void *stream) {
     JSS_CUDA(h, cudaMemcpyAsync(h->d_stats, init, sizeof init, cudaMemcpyHostToDevice, st));
     const int threads = 256;
     const int blocks = std::min((h->n_envs + threads - 1) / threads, h->sm_count * 4);
-    JSS_LAUNCH(jss_stats_kernel, blocks, threads, 0, st, h->p, h->d_stats);
+    JssLaunch a{};                       // every tile of the batch
+    a.tile_end = h->n_tiles;
+    if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
+    JSS_LAUNCH(jss_stats_kernel, blocks, threads, 0, st, h->p, a, h->d_stats);
     JSS_CUDA(h, cudaGetLastError());
     h->launches += 1;
     unsigned long long res[JSS_STATS_LEN];

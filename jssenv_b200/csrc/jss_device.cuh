@@ -41,7 +41,7 @@ struct InstView {  // instance tables staged in shared memory
     const uint16_t *ops;
     const int32_t *len;
     const uint16_t *rem;
-    const SmInst *si;
+    const JssInst *si;
     // Shape of the instance for branch conditions and loop bounds.  Uniform-batch kernels point `si` at the kernel
     // parameters (constant bank: ptxas knows those are warp-uniform) and read it there; kernels that stage the instance
     // in shared memory keep register copies that went through jss_uniform (jss_iv_shape).
@@ -307,8 +307,9 @@ JSS_DEV void env_load_bits_hdr(const int32_t *tail, int Mc, int lane, EnvRegs<KJ
     s.t = h4.x; s.flags = (uint32_t)h4.y; s.ep_steps = h4.z; s.ep_return = h4.w;
 }
 
+// `blk`: the env's state block (in global memory, or the step kernels' shared-memory copy)
 template <int KJ>
-JSS_DEV void env_load_from(const JssParams &p, const InstView &iv, const int32_t *blk, int lane, EnvRegs<KJ> &s) {
+JSS_DEV void env_load(const JssParams &p, const InstView &iv, const int32_t *blk, int lane, EnvRegs<KJ> &s) {
     const int Jc = iv.si->Jcap, Mc = iv.si->Mcap;   // geometry of the env's own instance
     if (KJ * lane < jss_J(iv)) env_load_jobs<KJ>(blk, Jc, lane, s);
     else env_clear_jobs<KJ>(iv, s);
@@ -317,19 +318,12 @@ JSS_DEV void env_load_from(const JssParams &p, const InstView &iv, const int32_t
     env_load_bits_hdr<KJ>(tail, Mc, lane, s);
     env_derive_ops<KJ>(iv, s, lane);
 }
-// start of env's state block (blocks are stored in tile order with per-instance sizes, see JssTile)
-JSS_DEV int32_t *env_block(const JssParams &p, int env) { return p.state + (size_t)p.state_off16[env] * 4; }
-template <int KJ>
-JSS_DEV void env_load(const JssParams &p, const InstView &iv, int env, int lane, EnvRegs<KJ> &s) {
-    env_load_from<KJ>(p, iv, env_block(p, env), lane, s);
-}
 
 // policy kernels read only what the rule looks at: bits + header always, todo for every
 // rule (current op / remaining work / remaining ops), idle_last for FIFO
 template <int KJ>
-JSS_DEV void env_load_for_policy(const JssParams &p, const InstView &iv, int env, int lane, EnvRegs<KJ> &s,
+JSS_DEV void env_load_for_policy(const JssParams &p, const InstView &iv, const int32_t *blk, int lane, EnvRegs<KJ> &s,
                                  int rule) {
-    const int32_t *blk = env_block(p, env);
     const int Jc = iv.si->Jcap, Mc = iv.si->Mcap;
     env_clear_jobs<KJ>(iv, s);
     if (rule != JSS_RULE_RANDOM && KJ * lane < jss_J(iv)) {
@@ -378,12 +372,12 @@ JSS_DEV void env_store_to(const JssParams &p, const InstView &iv, int32_t *blk, 
 }
 
 template <int KJ>
-JSS_DEV void env_store(const JssParams &p, const InstView &iv, int env, int lane, const EnvRegs<KJ> &s) {
+JSS_DEV void env_store(const JssParams &p, const InstView &iv, int32_t *blk, int lane, const EnvRegs<KJ> &s) {
     // all lanes must have finished env_load (every lane reads the shared header words)
     // before any lane overwrites the block: paths such as the auto-reset have no
     // collective between load and store
     __syncwarp();
-    env_store_to<KJ>(p, iv, env_block(p, env), lane, s);
+    env_store_to<KJ>(p, iv, blk, lane, s);
 }
 
 // jss_env.py:145-181
@@ -592,7 +586,7 @@ JSS_DEV void env_emit_obs(const JssParams &p, const JssOut &out, const InstView 
             // the two counters until the job completes)
             const int len = iv.len[KJ * lane + i];        // unconditional (in-bounds) load + select
             const int perf = (s.todo[i] < jss_M(iv)) ? s.t - s.total_idle[i] : len;
-            const SmInst &si = *iv.si;
+            const JssInst &si = *iv.si;
             v[7 * i + 0] = (s.lb & (1u << i)) ? 1.0f : 0.0f;
             v[7 * i + 1] = jss_div((float)s.tufco[i], si.f_mto, si.r_mto);
             v[7 * i + 2] = jss_div((float)s.todo[i], si.f_M, si.r_M);
@@ -945,7 +939,7 @@ JSS_DEV void env_pack(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> 
 // ---- CTA-level driver -----------------------------------------------------------------------
 struct JssSmemLayout {
     // byte offsets from the start of dynamic shared memory, precomputed on the host so the kernels derive every
-    // pointer with one add (each region 16-byte aligned): [SmInst][ops u16][len i32][rem u16][per-warp regions]
+    // pointer with one add (each region 16-byte aligned): [JssInst][ops u16][len i32][rem u16][per-warp regions]
     int32_t off_len, off_rem, off_warp0, pad0_;
     int32_t warp_stride;    // bytes per warp region
     int32_t scratch_words;  // observation staging (7 floats per job slot), >= 32 words
@@ -954,14 +948,14 @@ struct JssSmemLayout {
 };
 
 struct JssCtaSmem {         // the CTA-shared part
-    SmInst *si;
+    JssInst *si;
     uint16_t *ops;
     int32_t *len;
     uint16_t *rem;
 };
 JSS_DEV void jss_cta_carve(const JssSmemLayout &sl, char *sm, JssCtaSmem &c, InstView &iv) {
-    c.si = reinterpret_cast<SmInst *>(sm);
-    c.ops = reinterpret_cast<uint16_t *>(sm + sizeof(SmInst));
+    c.si = reinterpret_cast<JssInst *>(sm);
+    c.ops = reinterpret_cast<uint16_t *>(sm + sizeof(JssInst));
     c.len = reinterpret_cast<int32_t *>(sm + sl.off_len);
     c.rem = reinterpret_cast<uint16_t *>(sm + sl.off_rem);
     iv.ops = c.ops; iv.len = c.len; iv.rem = c.rem; iv.si = c.si; iv.staged = true; iv.Ju = iv.Mu = 0;
@@ -981,21 +975,10 @@ JSS_HD static inline bool jss_rule_wants_rem(int rule) {
     return rule == JSS_RULE_MWR || rule == JSS_RULE_LWR || rule == JSS_RULE_CR;
 }
 
-// per-instance scalars: staged in shared memory by the kernels, and filled on the host for the kernel parameters of
-// uniform batches
-JSS_HD static inline void jss_fill_sminst(const JssInstDesc &d, SmInst *si) {
-    si->J = d.J; si->M = d.M; si->max_time_op = d.max_time_op; si->max_time_jobs = d.max_time_jobs;
-    si->sum_op = d.sum_op;
-    si->f_mto = (float)d.max_time_op; si->f_mtj = (float)d.max_time_jobs; si->f_sop = (float)d.sum_op;
-    si->f_M = (float)d.M;
-    si->r_mto = d.r_mto; si->r_mtj = d.r_mtj; si->r_sop = d.r_sop; si->r_M = d.r_M;
-    const JssBlockGeom g = jss_block_geom(d.J, d.M);
-    si->Jcap = g.Jcap; si->Mcap = g.Mcap; si->block_words = g.words; si->tail = g.tail;
-}
-
-JSS_DEV void jss_stage_instance(const JssParams &p, const JssInstDesc &d, const JssCtaSmem &c, int what) {
+JSS_DEV void jss_stage_instance(const JssParams &p, const JssInst &d, const JssCtaSmem &c, int what) {
     const int tid = threadIdx.x, nt = blockDim.x;
-    if (tid == 0) jss_fill_sminst(d, c.si);
+    if (tid < (int)(sizeof(JssInst) / 16))
+        reinterpret_cast<uint4 *>(c.si)[tid] = reinterpret_cast<const uint4 *>(&d)[tid];
     // pools are padded so whole uint4 copies stay in-bounds
     if (what & JSS_STAGE_OPS) {
         {
@@ -1029,20 +1012,52 @@ JSS_DEV void env_emit_all(const JssParams &p, const InstView &iv, const EnvRegs<
     env_emit_scalars<KJ>(out, iv, s, env, lane, raw);
 }
 
-// a step that changed nothing but the sticky error bit: store the new flags word and a zero-reward scalar record
+// a step that changed nothing but the sticky error bit: store the new flags word (in the header, the last 4 words of
+// the block) and a zero-reward scalar record
 template <int KJ>
-JSS_DEV void env_store_flags_only(const JssParams &p, const EnvRegs<KJ> &s, int env, int lane) {
+JSS_DEV void env_store_flags_only(const JssParams &p, const InstView &iv, int32_t *blk, const EnvRegs<KJ> &s, int env,
+                                  int lane) {
     if (lane == 0) {
-        p.state[(size_t)p.hdr_off16[env] * 4 + JSS_HDR_FLAGS] = (int32_t)s.flags;
+        blk[iv.si->block_words - 4 + JSS_HDR_FLAGS] = (int32_t)s.flags;
         reinterpret_cast<int4 *>(p.scalars)[env] =
             make_int4(0, 0, s.t, (int)((s.flags << 8) | (s.flags & JSS_FLAG_DONE)));
     }
 }
 
+// What warp `warp` of `tile` works on, and where that env's state block lives.  The kernels recompute it where they
+// store the block instead of carrying it in registers across a step or a rollout.
+struct JssTileWarp {
+    int env;                 // -1: the tile has fewer envs than warp + 1
+    int inst;                // the tile's instance
+    uint32_t off16, blk16;   // the env's state block: offset and size in 16-byte units
+};
+// uni: every env runs the instance `a.uni` (a compile-time constant in the step kernels).  Then env = 8 * tile + warp
+// and its block lies at env * block16: no descriptor load.  Otherwise one 16-byte JssTile load (blocks in tile order).
+JSS_DEV JssTileWarp jss_tile(const JssParams &p, const JssLaunch &a, bool uni, int tile, int warp) {
+    JssTileWarp t;
+    if (uni) {
+        const int e = tile * JSS_WARPS_PER_CTA + warp;
+        t.env = e < p.n_envs ? e : -1;
+        t.inst = p.uniform_inst;
+        t.blk16 = (uint32_t)a.uni.block_words >> 2;
+        t.off16 = (uint32_t)e * t.blk16;
+    } else {
+        const int4 td = *reinterpret_cast<const int4 *>(p.tiles + tile);
+        t.inst = td.y >> 8;
+        t.env = warp < (td.y & 255) ? p.order[td.x + warp] : -1;
+        t.blk16 = (uint32_t)td.w;
+        t.off16 = (uint32_t)td.z + (uint32_t)warp * t.blk16;
+    }
+    return t;
+}
+
 template <int KJ, int MODE>
-JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int lane,
-                             float *scratch) {
+JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
+                             int lane, float *scratch) {
     EnvRegs<KJ> s;
+    // the env's state block, derived at each use: with the pointer carried across the rollout loop, bench.py's cfg2
+    // recording rollout took 3.88 instead of 3.83 us per transition (median of 3, H100 SXM, 400 W power limit)
+    const auto blk = [&]() { return p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4; };
     // MODE is a compile-time kernel variant (the hot step kernel carries no policy /
     // rollout / export code); JSS_MODE_RESET instantiates the rarely used rest
     const int mode = (MODE == JSS_MODE_RESET) ? a.mode : MODE;
@@ -1051,7 +1066,7 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         if (a.env_mask && a.env_mask[env] == 0) return;
         env_reset_regs<KJ>(iv, s, lane);
         env_clear_solution(p, env, lane);
-        env_store<KJ>(p, iv, env, lane, s);
+        env_store<KJ>(p, iv, blk(), lane, s);
         env_emit_all<KJ>(p, iv, s, env, lane, scratch, 0);
         return;
     }
@@ -1059,15 +1074,15 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         if (a.env_mask && a.env_mask[env] == 0) return;
         env_import<KJ>(p, iv, s, env, lane);
         s.ep_steps = 0; s.ep_return = 0;
-        env_store<KJ>(p, iv, env, lane, s);
+        env_store<KJ>(p, iv, blk(), lane, s);
         env_emit_obs<KJ>(p, jss_out_default(p), iv, s, env, lane, scratch);
         env_emit_mask<KJ>(p, jss_out_default(p), iv, s, env, lane, (s.flags & JSS_FLAG_NOOP_LEGAL) != 0u);
         if (lane == 0) p.scalars[4 * (size_t)env + 3] = (int32_t)((s.flags << 8) | (s.flags & JSS_FLAG_DONE));
         return;
     }
     const uint64_t genv = p.env_id_base + (uint64_t)env;
-    if (mode == JSS_MODE_POLICY) env_load_for_policy<KJ>(p, iv, env, lane, s, a.rule);
-    else env_load<KJ>(p, iv, env, lane, s);
+    if (mode == JSS_MODE_POLICY) env_load_for_policy<KJ>(p, iv, blk(), lane, s, a.rule);
+    else env_load<KJ>(p, iv, blk(), lane, s);
     s.flags = jss_uniform(s.flags);                      // one word read by every lane (see jss_uniform)
     if (mode == JSS_MODE_EXPORT) { env_export<KJ>(p, iv, s, env, lane); return; }
     if (mode == JSS_MODE_PACK) { env_pack<KJ>(a, iv, s, env, lane, scratch); return; }
@@ -1084,10 +1099,10 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         const bool changed = env_step<KJ>(p, iv, s, env, lane, action, raw, hz);
         s.flags = jss_uniform(s.flags);
         if (changed) {
-            env_store<KJ>(p, iv, env, lane, s);
+            env_store<KJ>(p, iv, blk(), lane, s);
             env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
         } else if (s.flags != flags_in) {
-            env_store_flags_only<KJ>(p, s, env, lane);
+            env_store_flags_only<KJ>(p, iv, blk(), s, env, lane);
         }
         if (a.export_after) env_export<KJ>(p, iv, s, env, lane);   // single-env facade: one launch per transition
         return;
@@ -1116,19 +1131,8 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         }
     }
     if (dirty) {
-        env_store<KJ>(p, iv, env, lane, s);
+        env_store<KJ>(p, iv, blk(), lane, s);
         if (!a.write_obs || record) env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
-    }
-}
-
-JSS_DEV void jss_tile_desc(const JssParams &p, int tile, int &first, int &inst, int &count) {
-    if (p.uniform_inst >= 0) {           // one instance, identity order: no descriptor loads
-        first = tile * JSS_WARPS_PER_CTA;
-        inst = p.uniform_inst;
-        count = min(JSS_WARPS_PER_CTA, p.n_envs - first);
-    } else {
-        const JssTile td = p.tiles[tile];
-        first = td.first; inst = td.inst_count >> 8; count = td.inst_count & 255;
     }
 }
 
@@ -1155,9 +1159,8 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
         what = a.rule == JSS_RULE_RANDOM ? 0 : jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
     int staged = -1;
     for (int tile = a.tile_begin + (int)blockIdx.x; tile < a.tile_end; tile += (int)gridDim.x) {
-        int first, inst, count;
-        jss_tile_desc(p, tile, first, inst, count);
-        first = jss_uniform(first); inst = jss_uniform(inst); count = jss_uniform(count);
+        const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, tile, warp);
+        const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
         if (inst != staged) {                            // CTA-uniform
             __syncthreads();
             jss_stage_instance(p, p.inst[inst], c, what);
@@ -1165,9 +1168,7 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
             __syncthreads();
         }
         jss_iv_shape(iv);
-        if (warp < count)
-            jss_process_env<KJ, MODE>(p, a, iv, p.uniform_inst >= 0 ? first + warp : jss_uniform(p.order[first + warp]),
-                                      lane, scratch);
+        if (env >= 0) jss_process_env<KJ, MODE>(p, a, iv, env, tile, warp, lane, scratch);
     }
 }
 
@@ -1197,55 +1198,27 @@ struct JssWarpSmem {        // per-warp shared-memory regions of the step kernel
     jss_saddr_t mbar, state_sa, scratch_sa, state_out_sa;
 };
 
-// where the state block of warp `warp` of `tile` (env `env`) lives, in 16-byte units: a uniform batch stores env e's
-// block at e * block16 (nothing to load), any other batch at the tile's base in tile order (JssTile).  The step
-// recomputes it after the env is simulated instead of carrying it in registers across the step.
-template <bool UNI>
-JSS_DEV void jss_tile_block(const JssParams &p, const SmInst &uni, int tile, int warp, int env, uint32_t &off16,
-                            uint32_t &blk16) {
-    if (UNI) {
-        blk16 = (uint32_t)uni.block_words >> 2;
-        off16 = (uint32_t)env * blk16;
-    } else {
-        const int4 td = *reinterpret_cast<const int4 *>(p.tiles + tile);   // JssTile, one 16-byte load
-        blk16 = (uint32_t)td.w;
-        off16 = (uint32_t)td.z + (uint32_t)warp * blk16;
-    }
-}
-
-// env handled by `warp` in `tile` (-1: none) and where its state block lives
-template <bool UNI>
-JSS_DEV int jss_tile_env(const JssParams &p, const JssLaunch &a, int tile, int tile_end, int warp, uint32_t &off16,
-                         uint32_t &blk16) {
-    if (UNI) {                           // env = 8 * tile + warp
-        const int e = tile * JSS_WARPS_PER_CTA + warp;
-        jss_tile_block<UNI>(p, a.uni, tile, warp, e, off16, blk16);
-        return (tile < tile_end && e < p.n_envs) ? e : -1;
-    }
-    if (tile >= tile_end) return -1;
-    const int4 td = *reinterpret_cast<const int4 *>(p.tiles + tile);
-    if (warp >= (td.y & 255)) return -1;
-    jss_tile_block<UNI>(p, a.uni, tile, warp, -1, off16, blk16);
-    return p.order[td.x + warp];
-}
-
 // tiles tile, tile + tile_step, ... < tile_end of ONE lane class through the prefetch pipeline
 template <int KJ, int SAMPLE, bool UNI>
 JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSmemLayout &sl, InstView &iv,
                             const JssCtaSmem &c, const JssWarpSmem &w, int warp, int lane, int tile, int tile_end,
                             int tile_step, int &staged, uint32_t &phase) {
-    int env_next, act_next = 0;
-    {
-        uint32_t off16, blk16;
-        env_next = jss_tile_env<UNI>(p, a, tile, tile_end, warp, off16, blk16);
+    int env_next = -1, act_next = 0;
+    // start the bulk load of the state block of this warp's env of tile `next` and fetch its action
+    const auto prefetch = [&](int next) {
+        env_next = -1;
+        if (next >= tile_end) return;
+        const JssTileWarp t = jss_tile(p, a, UNI, next, warp);
+        env_next = t.env;
         if (env_next >= 0) {
-            if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)off16 * 4, blk16 * 16u, w.mbar);
+            if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)t.off16 * 4, t.blk16 * 16u, w.mbar);
             act_next = a.actions[env_next];
         }
-    }
+    };
+    prefetch(tile);
     for (; tile < tile_end; tile += tile_step) {
         if (!UNI) {
-            const int inst = p.tiles[tile].inst_count >> 8;
+            const int inst = jss_tile(p, a, UNI, tile, warp).inst;
             if (inst != staged) {                        // CTA-uniform
                 __syncthreads();
                 jss_stage_instance(p, p.inst[inst], c, (SAMPLE == 2 && jss_rule_wants_rem(a.rule)) ? JSS_STAGE_ALL : JSS_STAGE_OPS);
@@ -1259,17 +1232,10 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
         if (env >= 0) {
             jss_mbar_wait(w.mbar, phase);                // this env's block has landed in shared memory
             phase ^= 1u;
-            env_load_from<KJ>(p, iv, w.state_in, lane, s);
+            env_load<KJ>(p, iv, w.state_in, lane, s);
             __syncwarp();                                // every lane has read the buffer
         }
-        {   // prefetch the next env's block + action
-            uint32_t off16, blk16;
-            env_next = jss_tile_env<UNI>(p, a, tile + tile_step, tile_end, warp, off16, blk16);
-            if (env_next >= 0) {
-                if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)off16 * 4, blk16 * 16u, w.mbar);
-                act_next = a.actions[env_next];
-            }
-        }
+        prefetch(tile + tile_step);
         if (env < 0) continue;
         int raw = 0;
         // the previous env's observation must have left the staging buffer (also aliased by hz)
@@ -1289,12 +1255,11 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
         if (changed) {
             // new state -> shared staging -> one bulk store (every word of the block is rewritten)
             env_store_to<KJ>(p, iv, w.state_out, lane, s);
-            uint32_t off16, blk16;
-            jss_tile_block<UNI>(p, a.uni, tile, warp, env, off16, blk16);
+            const JssTileWarp t = jss_tile(p, a, UNI, tile, warp);
             env_emit_all<KJ, true>(p, iv, s, env, lane, w.scratch, raw, w.scratch_sa,
-                                   p.state + (size_t)off16 * 4, w.state_out_sa, blk16 * 16u);
+                                   p.state + (size_t)t.off16 * 4, w.state_out_sa, t.blk16 * 16u);
         } else if (s.flags != flags_in) {
-            env_store_flags_only<KJ>(p, s, env, lane);
+            env_store_flags_only<KJ>(p, iv, p.state + (size_t)jss_tile(p, a, UNI, tile, warp).off16 * 4, s, env, lane);
         }
     }
 }
@@ -1386,14 +1351,19 @@ __global__ void jss_copy16_kernel(uint4 *dst, const uint4 *src, size_t n16) {
 }
 
 // ---- per-shard statistics ------------------------------------------------------------------
-__global__ void jss_stats_kernel(const JssParams p, unsigned long long *out) {
+// one thread per warp slot of the tiles [a.tile_begin, a.tile_end); slots past a tile's count hold no env
+__global__ void jss_stats_kernel(const JssParams p, const JssLaunch a, unsigned long long *out) {
     // out[0..7] pre-initialised by the host: sums 0, min = ~0ull
     unsigned long long ep = 0, steps = 0, smk = 0, ndone = 0, nerr = 0;
     long long sret = 0;
     unsigned long long mn = ~0ull, mx = 0;
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < p.n_envs; e += gridDim.x * blockDim.x) {
+    for (int slot = a.tile_begin * JSS_WARPS_PER_CTA + blockIdx.x * blockDim.x + threadIdx.x;
+         slot < a.tile_end * JSS_WARPS_PER_CTA; slot += gridDim.x * blockDim.x) {
+        const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, slot / JSS_WARPS_PER_CTA, slot % JSS_WARPS_PER_CTA);
+        const int e = t.env;
+        if (e < 0) continue;
         const int64_t *acc = p.acc + (size_t)e * 4;
-        const int32_t *hdr = p.state + (size_t)p.hdr_off16[e] * 4;
+        const int32_t *hdr = p.state + (size_t)(t.off16 + t.blk16) * 4 - 4;   // the block's last 4 words
         ep += (unsigned long long)p.episode_count[e];
         steps += (unsigned long long)acc[0] + (unsigned long long)(((uint32_t)hdr[JSS_HDR_FLAGS] & JSS_FLAG_DONE) ? 0 : hdr[JSS_HDR_EP_STEPS]);
         smk += (unsigned long long)acc[1];

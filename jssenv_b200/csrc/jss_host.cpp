@@ -367,24 +367,25 @@ void jss_host_expand_impl(const JssHostExpandArgs *a) {
     auto work = [&](int64_t lo, int64_t hi) {
         std::vector<float> stage((size_t)a->jobs_max * 7 + 8);
         for (int64_t e = lo; e < hi; e++) {
-            const JssHostInst &hi_ = a->insts[a->env_inst[e]];
+            const JssInst &in = a->insts[a->env_inst[e]];
+            const int32_t *len = a->len_pool + in.len_off;
             Cols c;
-            const float d7[7] = {1.0f, (float)hi_.max_time_op, (float)hi_.M, (float)hi_.max_time_jobs,
-                                 (float)hi_.max_time_op, (float)hi_.sum_op, (float)hi_.sum_op};
-            for (int k = 0; k < 16; k++) { c.d[k] = k < 14 ? d7[k % 7] : 1.0f; c.r[k] = 1.0f / c.d[k]; }
+            const float d7[7] = {1.0f, in.f_mto, in.f_M, in.f_mtj, in.f_mto, in.f_sop, in.f_sop};
+            const float r7[7] = {1.0f, in.r_mto, in.r_M, in.r_mtj, in.r_mto, in.r_sop, in.r_sop};
+            for (int k = 0; k < 16; k++) { c.d[k] = k < 14 ? d7[k % 7] : 1.0f; c.r[k] = k < 14 ? r7[k % 7] : 1.0f; }
             const uint8_t *row = a->wire + (size_t)e * a->wire_stride;
             const int t = a->scalars[4 * (size_t)e + 2];
             float *dst = a->obs + (size_t)e * a->jobs_max * 7;
-            const size_t n = (size_t)hi_.J * 7;
+            const size_t n = (size_t)in.J * 7;
 #ifdef JSS_HAVE_AVX2_TARGET
             if (have_avx512() || have_avx2()) {
-                if (have_avx512()) expand_env_avx512(row, hi_.J, hi_.M, t, hi_.len, c, stage.data());
-                else expand_env_avx2(row, hi_.J, hi_.M, t, hi_.len, c, stage.data());
+                if (have_avx512()) expand_env_avx512(row, in.J, in.M, t, len, c, stage.data());
+                else expand_env_avx2(row, in.J, in.M, t, len, c, stage.data());
                 stream_copy(dst, stage.data(), n);
                 continue;
             }
 #endif
-            expand_env_scalar(row, hi_.J, hi_.M, t, hi_.len, c, dst);
+            expand_env_scalar(row, in.J, in.M, t, len, c, dst);
         }
 #ifdef JSS_HAVE_AVX2_TARGET
         if (have_avx2()) _mm_sfence();

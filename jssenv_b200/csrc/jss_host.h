@@ -2,20 +2,17 @@
 #pragma once
 #include <stdint.h>
 
-#define JSS_WIRE_JOB_BYTES 10   // packed observation record of one job (layout: jss_host.cpp / env_pack in jss_device.cuh)
+#include "jss_types.h"
 
-struct JssHostInst {            // what the expansion needs of an instance (host copies)
-    int J, M;
-    int64_t max_time_op, max_time_jobs, sum_op;
-    const int32_t *len;         // jobs_length[J]
-};
+#define JSS_WIRE_JOB_BYTES 10   // packed observation record of one job (layout: jss_host.cpp / env_pack in jss_device.cuh)
 
 struct JssHostExpandArgs {
     const uint8_t *wire;        // [N][wire_stride] packed rows
     int64_t wire_stride;
     const int32_t *scalars;     // [N][4] scalar records (current_time_step at index 2)
     const int32_t *env_inst;    // [N]
-    const JssHostInst *insts;
+    const JssInst *insts;       // the records jss_load_instances filled
+    const int32_t *len_pool;    // jobs_length of instance k at insts[k].len_off
     float *obs;                 // [N][jobs_max][7]
     int jobs_max;
     int64_t env_begin, env_end;

@@ -10,16 +10,6 @@
 #define JSS_OP_DMASK 2047u
 #define JSS_OP_NONE 0xFFFFFFFFu  // register-only marker "job has no current op" (finished / padding): machine field >= 32
 
-struct JssInstDesc {
-    int32_t J, M;
-    int32_t max_time_op, max_time_jobs, sum_op;  // jss_env.py:86-89
-    int32_t ops_off;                              // offsets into the pools, in elements
-    int32_t len_off;
-    int32_t rem_off;
-    // correctly rounded fp32 reciprocals of the four observation divisors (jss_div)
-    float r_mto, r_mtj, r_sop, r_M;
-};
-
 #ifndef JSS_HD   // as in jss_rng.h
 #if defined(__CUDACC__)
 #define JSS_HD __host__ __device__
@@ -87,7 +77,7 @@ JSS_HD static inline int jss_job_total_idle(uint32_t w1, uint32_t w2) {
 #define JSS_HDR_EP_RETURN 3
 
 // State-block geometry of an instance in int32 words: the ONE definition the host (block offsets, shared-memory
-// sizing) and the kernels (SmInst) use.  Per-lane slices are whole vectors: J rounded up to 4 (to 8 for the
+// sizing, JssInst) and the kernels use.  Per-lane slices are whole vectors: J rounded up to 4 (to 8 for the
 // 8-jobs-per-lane class, which also keeps 16 bits per lane in the bits region).
 struct JssBlockGeom {
     int32_t Jcap, Mcap;
@@ -104,6 +94,20 @@ JSS_HD static inline JssBlockGeom jss_block_geom(int J, int M) {
     g.words = g.hdr + 4;
     return g;
 }
+
+// One instance, filled once by jss_load_instances: the kernels stage it in shared memory next to the tables
+// (CTA-uniform, re-read with cheap broadcast LDS instead of pinning ~14 registers per thread), or -- uniform batches
+// -- read it from the kernel parameters so its fields become constant-bank operands.  The host's packed-row expansion
+// divides by the same divisors and reciprocals, so its observation equals the device's bit for bit.
+struct JssInst {
+    int J, M, max_time_op, max_time_jobs, sum_op;   // jss_env.py:86-89
+    float f_mto, f_mtj, f_sop, f_M;       // the divisors as floats ...
+    float r_mto, r_mtj, r_sop, r_M;       // ... and their correctly rounded reciprocals (jss_div)
+    int Jcap, Mcap, block_words;          // state-block geometry of THIS instance (jss_block_geom) ...
+    int tail;                             // ... and the word where tuam starts
+    int ops_off, len_off, rem_off;        // offsets into the pools, in elements
+};
+static_assert(sizeof(JssInst) % 16 == 0, "JssInst is staged with 16-byte copies and keeps the tables behind it aligned");
 
 struct JssTile {       // one CTA work item: up to `count` envs of ONE instance (one 16-byte load)
     int32_t first;     // index into `order`
@@ -129,7 +133,7 @@ struct JssParams {
     int32_t jobs_max, machines_max, mask_stride, create_flags;
     int32_t uniform_inst;    // >= 0: every env runs this instance and `order` is the identity
     uint64_t env_id_base;
-    const JssInstDesc *inst;
+    const JssInst *inst;
     const uint16_t *ops_pool;
     const int32_t *len_pool;
     const uint16_t *rem_pool;
@@ -137,8 +141,6 @@ struct JssParams {
     const JssTile *tiles;
     const JssCtaRange *cta_ranges;   // mixed-batch step kernel: per CTA an equal slice of every lane class
     int32_t n_cta_ranges;
-    const uint32_t *state_off16;   // per env: start of its state block, in 16-byte units (tile order, see JssTile)
-    const uint32_t *hdr_off16;     // per env: start of its 4-word header (t, flags, episode steps / return), 16-byte units
     int32_t *state;          // per-env blocks of jss_block_geom(J_i, M_i).words words (the env's own instance)
     uint8_t *mask;           // [N][mask_stride]
     float *obs;              // [N][jobs_max][7]
@@ -153,18 +155,6 @@ struct JssParams {
     uint8_t *x_legal, *x_blocked;
 };
 
-// Per-instance scalars: staged in shared memory next to the tables (CTA-uniform, re-read with cheap
-// broadcast LDS instead of pinning ~14 registers per thread), or -- uniform batches -- passed in the
-// kernel parameters so they become constant-bank operands.
-struct SmInst {
-    int J, M, max_time_op, max_time_jobs, sum_op;
-    float f_mto, f_mtj, f_sop, f_M;       // the divisors as floats ...
-    float r_mto, r_mtj, r_sop, r_M;       // ... and their correctly rounded reciprocals
-    int Jcap, Mcap, block_words;          // state-block geometry of THIS instance (jss_block_geom) ...
-    int tail;                             // ... and the word where tuam starts
-    int pad_[3];                          // 20 words: the tables behind it in shared memory stay 16-byte aligned
-};
-static_assert(sizeof(SmInst) % 16 == 0, "SmInst must keep the shared-memory tables 16-byte aligned");
 struct JssLaunch {           // per-launch arguments
     int32_t tile_begin, tile_end;
     int32_t mode;            // JSS_MODE_*
@@ -181,7 +171,7 @@ struct JssLaunch {           // per-launch arguments
     float *traj_obs; uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
     uint8_t *wire;           // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
     int32_t wire_stride;
-    SmInst uni;              // scalars of the single instance of a uniform batch (step kernel, UNI = true)
+    JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
 };
 
 #define JSS_MODE_RESET 0

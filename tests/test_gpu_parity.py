@@ -79,6 +79,29 @@ def test_gpu_step_sample_fused(rule):
     pc.check_step_sample(make_env, ["ta01", "ta31", "ta51", "ta80", "ta80"], rule, n_steps=2600, seed=12)
 
 
+def test_gpu_step_sample_alternating_rules_big_instances():
+    """MWR stages the suffix-sum table and FIFO does not, so the fused step kernel runs with two shared-memory layouts.
+    With 256-job instances both need more than 48 KB: switching rules back and forth must keep launching, and must
+    equal the policy kernel + step kernel (uniform and mixed batches)."""
+    big = pc.synthetic_instance(256, 32, seed=31)
+    for insts, e2i in (([big], [0] * 16), ([big, "ta01"], [0, 1] * 8)):
+        cfg = {"instance_paths": insts, "env_to_instance": e2i}
+        a_env = make_env(16, cfg, seed=4, auto_reset=True)
+        b_env = make_env(16, cfg, seed=4, auto_reset=True)
+        a_env.reset(); b_env.reset()
+        act_a = a_env.policy("MWR").clone()
+        b_env._step_index = 0
+        prev = "MWR"
+        for k, rule in enumerate(["MWR", "FIFO"] * 12):
+            act_b = b_env.policy(prev)
+            assert np.array_equal(pc._np(act_a), pc._np(act_b)), (len(insts), k)
+            b_env.step(act_b)
+            *_, act_a = a_env.step_sample(act_a, rule)
+            for name in ("action_mask", "real_obs", "reward", "done"):
+                assert np.array_equal(pc._np(getattr(a_env, name)), pc._np(getattr(b_env, name))), (len(insts), k, name)
+            prev = rule
+
+
 def test_gpu_errors_freeze_reset():
     pc.check_errors_and_freeze(make_env)
 
