@@ -194,6 +194,28 @@ int jss_set_cr_due_date_factor(jss_t *h, double factor);
 int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mode, uint64_t seed,
                     uint64_t step_index, int32_t *next_actions_dev, void *stream);
 
+/* Step a batch from policy logits (the action_mask-restricted categorical draw of README.md:84-97, driven by a
+ * network instead of np.random.choice): chooses every env's action from its logits row, then applies it exactly as
+ * jss_step() would, in one launch, and writes the chosen actions and their log-probabilities.
+ *   logits_dev: device fp32 [N][ld], ld >= jobs_max + 1, unit column stride.  Columns 0..J_i-1 of env i's row are
+ *     its jobs, column J_i its no-op (the columns of its action_mask row); columns past J_i are never read.
+ *   Candidates: the actions legal in the env's current state (the action_mask the caller's network saw).  Logits of
+ *     illegal actions are ignored whatever their value, NaN and +-inf included.
+ *   Draw: Gumbel-max, a = argmax over legal a of logit[a] + g[a], g = -log(-log u[a]), ties to the lowest index, with
+ *     u[a] = ((H(h_env, a) >> 8) + 0.5) * 2^-24, H = jss_hash_env and h_env = jss_hash3 of (seed, env_id_base + i,
+ *     step_index) (jss_rng.h): replayable on the host and independent of sharding.  Computed in fp32.
+ *   log_prob_out_dev[i] = logit[a] - logsumexp(legal logits), fp32, max-subtracted.
+ *   Special cases (as env_select_action / jss_step):
+ *     done env: frozen, or reset under JSS_CREATE_AUTO_RESET, as by jss_step(); writes action 0, log_prob 0;
+ *     only the no-op legal: action J_i, log_prob 0 (its logit is not read);
+ *     bad logits (a legal logit NaN or +inf, or every legal logit -inf): the env gets the sticky JSS_FLAG_ERROR bit
+ *       and is left unchanged, like an illegal action; writes action JSS_ACTION_SKIP, log_prob NaN;
+ *     no legal action at all (not reachable from reset; an imported state): env untouched, JSS_ACTION_SKIP, NaN.
+ *   actions_out_dev: device int32[N] (required); log_prob_out_dev: device fp32[N], NULL skips that store.
+ *   Returns JSS_ERR_INVALID for a NULL logits_dev / actions_out_dev or ld < jobs_max + 1. */
+int jss_step_logits(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
+                    int32_t *actions_out_dev, float *log_prob_out_dev, void *stream);
+
 /* Replaces DispatchingRule.run_episode (dispatching.py:55-75) for the whole
  * batch: n_steps x (policy -> step) fused in one launch, state kept on chip
  * between steps; observations are written every step iff write_obs != 0. */

@@ -29,6 +29,7 @@ EXPORTED_SYMBOLS = (
     "jss_step_host", "jss_host_step_begin", "jss_host_wait", "jss_step_sample", "jss_stats", "jss_export_state", "jss_import_state", "jss_host_masked_random",
     "jss_launch_count", "jss_set_cr_due_date_factor", "jss_host_step_begin_packed", "jss_host_wire_stride",
     "jss_host_expand_obs", "jss_host_configure", "jss_host_threads", "jss_host_set_simd", "jss_rollout_traj", "jss_step_export", "jss_host_step_begin_hybrid", "jss_host_expand_obs_range",
+    "jss_step_logits",
 )
 
 
@@ -65,6 +66,8 @@ def _declare(L):
     L.jss_step.argtypes = [c_void_p, c_void_p, c_void_p]
     L.jss_policy.argtypes = [c_void_p, c_int, c_int, c_uint64, c_uint64, c_void_p, c_void_p]
     L.jss_step_sample.argtypes = [c_void_p, c_void_p, c_int, c_int, c_uint64, c_uint64, c_void_p, c_void_p]
+    L.jss_step_logits.argtypes = [c_void_p, c_void_p, c_int64, c_uint64, c_uint64, c_void_p, c_void_p, c_void_p]
+    L.jss_step_logits.restype = c_int
     L.jss_rollout.argtypes = [c_void_p, c_int, c_uint64, c_uint64, c_int, c_int, c_void_p]
     L.jss_step_host.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     L.jss_host_step_begin.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]

@@ -73,6 +73,7 @@ struct jss_handle {
 
     JssParams p{};
     JssSmemLayout sl_env{}, sl_step{}, sl_step_rem{};   // shared-memory layouts of the generic / step kernels (step: without / with the suffix-sum table)
+    JssSmemLayout sl_step_logits{};                // step kernels drawing the action from policy logits (a logits row per warp)
     int class_tile_begin[4] = {0, 0, 0, 0}, class_tile_end[4] = {0, 0, 0, 0};  // KJ = 1, 2, 4, 8
     int n_tiles = 0;
     std::map<std::pair<const void *, size_t>, int> ctas_per_sm;   // by kernel and dynamic shared memory (filled lazily)
@@ -166,11 +167,13 @@ JssKernel step_kernel(const jss_t *h) {
 // one fused step launch (PDL).  A uniform batch runs min(tiles, resident CTAs) persistent CTAs over static strided
 // tiles; a mixed batch runs one CTA per JssCtaRange (all resident: SMs x 3).
 int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
-    // SAMPLE: 0 none, 1 masked-uniform sampler, 2 dispatching rule
-    const int sample = a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
-    const JssKernel kern = sample == 0 ? step_kernel<0>(h) : sample == 1 ? step_kernel<1>(h) : step_kernel<2>(h);
+    // SAMPLE: 0 none, 1 masked-uniform sampler, 2 dispatching rule, 3 action drawn from policy logits before the step
+    const int sample = a.logits ? 3 : a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
+    const JssKernel kern = sample == 0 ? step_kernel<0>(h) : sample == 1 ? step_kernel<1>(h)
+                         : sample == 2 ? step_kernel<2>(h) : step_kernel<3>(h);
     // only the rules that read the suffix sums stage them; the other launches leave their room to the L1
-    const JssSmemLayout &sl = sample == 2 && jss_rule_wants_rem(a.rule) ? h->sl_step_rem : h->sl_step;
+    const JssSmemLayout &sl = sample == 3 ? h->sl_step_logits
+                            : sample == 2 && jss_rule_wants_rem(a.rule) ? h->sl_step_rem : h->sl_step;
     const size_t smem = smem_bytes(sl);
     int per_sm = 0, rc = ctas_per_sm(h, kern, smem, per_sm);
     if (rc) return rc;
@@ -486,6 +489,9 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
         h->sl_step_rem.warp_stride = h->sl_step_rem.off_scratch + sl.scratch_words * 4 + g.words * 4;   // [scratch][state-out]
         h->sl_step = h->sl_step_rem;                      // launches that stage no suffix sums leave their room to the L1
         h->sl_step.off_warp0 = h->sl_step.off_rem;
+        h->sl_step_logits = h->sl_step;                   // + [logits row: jobs_max + 1 floats]
+        h->sl_step_logits.off_logits = h->sl_step.warp_stride;
+        h->sl_step_logits.warp_stride += round_up(4 * (jmax + 1), 16);
     }
 
     int rc;
@@ -618,6 +624,23 @@ int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mod
     a.actions = actions_dev;
     a.actions_out = next_actions_dev;
     a.rule = rule; a.coin_mode = coin_mode; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
+    a.hash_key = jss_hash_key(seed, step_index);
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_step_logits(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
+                    int32_t *actions_out_dev, float *log_prob_out_dev, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    if (!logits_dev || !actions_out_dev || ld < (int64_t)h->p.jobs_max + 1)
+        return fail(h, JSS_ERR_INVALID, "jss_step_logits: bad arguments (logits %p, actions_out %p, ld %lld < jobs_max + 1 = %d)",
+                    (const void *)logits_dev, (void *)actions_out_dev, (long long)ld, h->p.jobs_max + 1);
+    JssLaunch a{};
+    a.mode = JSS_MODE_STEP;
+    a.logits = logits_dev;
+    a.logits_ld = ld;
+    a.actions_out = actions_out_dev;
+    a.log_prob_out = log_prob_out_dev;
     a.hash_key = jss_hash_key(seed, step_index);
     return launch_all(h, a, (cudaStream_t)stream);
 }

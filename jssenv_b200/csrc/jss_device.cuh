@@ -155,6 +155,13 @@ JSS_DEV void jss_bulk_store(void *gmem_dst, jss_saddr_t smem_src, uint32_t bytes
 JSS_DEV void jss_bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 JSS_DEV void jss_bulk_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 JSS_DEV void jss_bulk_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// 4-byte asynchronous copies global -> shared (LDGSTS), per-thread groups: the policy-logits rows of jss_step_logits are
+// only 4-byte aligned (an (N, J+1) fp32 tensor has 404-byte rows for ta80), which rules out the bulk copy
+JSS_DEV void jss_cp_async4(jss_saddr_t smem_dst, const void *gmem_src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_dst), "l"(gmem_src) : "memory");
+}
+JSS_DEV void jss_cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+JSS_DEV void jss_cp_async_wait() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 #else   // host emulation (tests/emu): synchronous copies; the waits are warp rendezvous points
 typedef char *jss_saddr_t;
 JSS_DEV jss_saddr_t jss_saddr(const void *generic_ptr) { return (char *)generic_ptr; }
@@ -166,6 +173,9 @@ JSS_DEV void jss_bulk_store(void *gmem_dst, jss_saddr_t smem_src, uint32_t bytes
 JSS_DEV void jss_bulk_commit() {}
 JSS_DEV void jss_bulk_store_wait_read() {}
 JSS_DEV void jss_bulk_store_wait_all() {}
+JSS_DEV void jss_cp_async4(jss_saddr_t smem_dst, const void *gmem_src) { memcpy(smem_dst, gmem_src, 4); }
+JSS_DEV void jss_cp_async_commit() {}
+JSS_DEV void jss_cp_async_wait() {}
 #endif
 
 // vector access to a lane's KJ-word slice
@@ -860,6 +870,91 @@ JSS_DEV int env_select_action(const InstView &iv, const EnvRegs<KJ> &s, int lane
     return best;
 }
 
+// ---- masked categorical draw from policy logits (jss_step_logits, jss_b200.h) ----------------------------------
+#define JSS_F32_INF __int_as_float(0x7f800000)
+#define JSS_F32_NAN __int_as_float(0x7fffffff)
+// unsigned key with the order of the floats (NaN aside), so one REDUX.MAX finds a warp maximum
+JSS_DEV uint32_t jss_f32_key(float x) {
+    const uint32_t b = (uint32_t)__float_as_int(x);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+JSS_DEV float jss_key_f32(uint32_t k) { return __int_as_float((int)((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k)); }
+// The draw's log / exp: the MUFU approximations (a few ulp, absolute error 2^-21.4 near 1) are well inside what a
+// sampler needs, and they are shorter: a build with libm's logf / expf spilled 28 bytes in the uniform 1-job-per-lane
+// kernel at 64 registers, this one spills nothing.  log1pf stays, for -log u close to 0.  The host emulation uses libm.
+#ifndef JSS_EMU
+JSS_DEV float jss_fast_log(float x) { return __logf(x); }
+JSS_DEV float jss_fast_exp(float x) { return __expf(x); }
+#else
+JSS_DEV float jss_fast_log(float x) { return logf(x); }
+JSS_DEV float jss_fast_exp(float x) { return expf(x); }
+#endif
+
+// Gumbel noise g = -log(-log u) of u = ((bits >> 8) + 0.5) * 2^-24.  fp32 cannot hold every u close to 1
+// (u = 1 - 2^-25 would round to 1 and give g = +inf), so the upper half works with 1 - u, which it holds exactly.
+JSS_DEV float jss_gumbel(uint32_t bits) {
+    const uint32_t k = bits >> 8;
+    const float e = k < (1u << 23) ? -jss_fast_log(((float)k + 0.5f) * 0x1p-24f)
+                                   : -log1pf(-(((float)((1u << 24) - 1u - k) + 0.5f) * 0x1p-24f));
+    return -jss_fast_log(e);
+}
+
+// Gumbel-max over the actions legal in the env's current state: a = argmax(logit[a] + g[a]) (lowest index on ties),
+// g[a] from jss_hash_env(h, a) with h = jss_hash3(seed, global env id, step_index), and
+// log_prob = logit[a] - logsumexp(legal logits).  `row` holds the env's logits, columns 0..J; only legal columns are
+// read.  Writes what the call reports to act / logp and returns the action to apply: the drawn one, 0 for a done env,
+// or, for bad logits, an out-of-range action, so that env_step sets the sticky error bit and changes nothing else.
+template <int KJ>
+JSS_DEV int env_sample_logits(const InstView &iv, const EnvRegs<KJ> &s, int lane, const float *row, uint32_t h,
+                              int &act, float &logp) {
+    constexpr uint32_t LM = jss_legal_mask<KJ>();
+    const uint32_t flags = jss_uniform(s.flags);
+    const int J = jss_J(iv);
+    const bool noop = (flags & JSS_FLAG_NOOP_LEGAL) != 0u;
+    act = 0;
+    logp = 0.0f;
+    if (flags & JSS_FLAG_DONE) return 0;                 // reset or frozen by env_step, as with any action
+    if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u)) {      // only the no-op is legal (its logit is not read)
+        act = noop ? J : JSS_ACTION_SKIP;
+        logp = noop ? 0.0f : JSS_F32_NAN;
+        return act;
+    }
+    // candidates: this lane's legal jobs in ascending order, then (lane 0) the legal no-op
+    bool bad = false;                                    // a legal logit is NaN or +inf
+    uint32_t xkey = 0u, skey = 0u;                       // 0: below every candidate's key
+    int sidx = 1 << 20;
+#pragma unroll
+    for (int i = 0; i <= KJ; i++) {
+        const bool cand = i < KJ ? ((s.lb >> i) & 1u) != 0u : (lane == 0 && noop);
+        const int j = i < KJ ? KJ * lane + i : J;
+        if (cand) {
+            const float x = row[j];
+            bad = bad || !(x < JSS_F32_INF);
+            xkey = max(xkey, jss_f32_key(x));
+            const uint32_t k = jss_f32_key(x + jss_gumbel(jss_hash_env(h, (uint64_t)j)));
+            if (k > skey) { skey = k; sidx = j; }
+        }
+    }
+    const float mx = jss_key_f32(__reduce_max_sync(JSS_FULL, xkey));
+    if (__any_sync(JSS_FULL, bad) || mx == -JSS_F32_INF) {   // bad logits, or every legal logit is -inf
+        act = JSS_ACTION_SKIP;
+        logp = JSS_F32_NAN;
+        return JSS_INF;
+    }
+    const uint32_t best = __reduce_max_sync(JSS_FULL, skey);
+    act = (int)__reduce_min_sync(JSS_FULL, (unsigned)(skey == best ? sidx : 1 << 20));
+    float sum = 0.0f;
+#pragma unroll
+    for (int i = 0; i <= KJ; i++) {
+        const bool cand = i < KJ ? ((s.lb >> i) & 1u) != 0u : (lane == 0 && noop);
+        if (cand) sum += jss_fast_exp(row[i < KJ ? KJ * lane + i : J] - mx);
+    }
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) sum += __shfl_xor_sync(JSS_FULL, sum, off);   // the same sum in every lane
+    logp = (row[act] - mx) - jss_fast_log(sum);
+    return act;
+}
+
 // ---- canonical export / import (snapshot & restore; host attribute views) -------------
 template <int KJ>
 JSS_DEV void env_export(const JssParams &p, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane) {
@@ -944,7 +1039,7 @@ struct JssSmemLayout {
     int32_t warp_stride;    // bytes per warp region
     int32_t scratch_words;  // observation staging (7 floats per job slot), >= 32 words
     int32_t off_scratch;    // step kernels: [mbarrier 16 B][state-in block][scratch][state-out block]; else 0
-    int32_t pad_;
+    int32_t off_logits;     // step kernels with SAMPLE = 3: [logits row, J + 1 floats] behind state-out; else 0
 };
 
 struct JssCtaSmem {         // the CTA-shared part
@@ -1192,10 +1287,12 @@ JSS_DEV void jss_pdl_wait() {}
 // that leave by bulk store.
 // SAMPLE = 1 / 2 additionally picks every env's NEXT action (masked-uniform sampler / any dispatching
 // rule) from the freshly computed state, so a policy-driven loop is one launch per step.
+// SAMPLE = 3 takes the env's action from the caller's policy logits BEFORE the step (jss_step_logits): the next env's
+// logits row is prefetched like its state block, by 4-byte cp.async into the warp's logits slot.
 struct JssWarpSmem {        // per-warp shared-memory regions of the step kernels
     int32_t *state_in, *state_out;
-    float *scratch;
-    jss_saddr_t mbar, state_sa, scratch_sa, state_out_sa;
+    float *scratch, *logits;
+    jss_saddr_t mbar, state_sa, scratch_sa, state_out_sa, logits_sa;
 };
 
 // tiles tile, tile + tile_step, ... < tile_end of ONE lane class through the prefetch pipeline
@@ -1204,7 +1301,8 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
                             const JssCtaSmem &c, const JssWarpSmem &w, int warp, int lane, int tile, int tile_end,
                             int tile_step, int &staged, uint32_t &phase) {
     int env_next = -1, act_next = 0;
-    // start the bulk load of the state block of this warp's env of tile `next` and fetch its action
+    // start the bulk load of the state block of this warp's env of tile `next` and fetch its action (SAMPLE = 3: start
+    // the copy of its logits row, columns 0..J, one 4-byte cp.async per column)
     const auto prefetch = [&](int next) {
         env_next = -1;
         if (next >= tile_end) return;
@@ -1212,7 +1310,14 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
         env_next = t.env;
         if (env_next >= 0) {
             if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)t.off16 * 4, t.blk16 * 16u, w.mbar);
-            act_next = a.actions[env_next];
+            if (SAMPLE == 3) {
+                const int J = UNI ? a.uni.J : p.inst[t.inst].J;
+                const float *src = a.logits + (size_t)env_next * (size_t)a.logits_ld;
+                for (int k = lane; k <= J; k += 32) jss_cp_async4(w.logits_sa + 4u * (uint32_t)k, src + k);
+                jss_cp_async_commit();
+            } else {
+                act_next = a.actions[env_next];
+            }
         }
     };
     prefetch(tile);
@@ -1227,13 +1332,27 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
             }
             jss_iv_shape(iv);
         }
-        const int env = UNI ? env_next : jss_uniform(env_next), action = act_next;
+        const int env = UNI ? env_next : jss_uniform(env_next);
+        int action = act_next;
         EnvRegs<KJ> s;
         if (env >= 0) {
             jss_mbar_wait(w.mbar, phase);                // this env's block has landed in shared memory
             phase ^= 1u;
             env_load<KJ>(p, iv, w.state_in, lane, s);
             __syncwarp();                                // every lane has read the buffer
+            if (SAMPLE == 3) {
+                jss_cp_async_wait();
+                __syncwarp();                            // every lane's columns of the logits row have landed
+                int act;
+                float logp;
+                action = env_sample_logits<KJ>(iv, s, lane, w.logits, jss_hash_env(a.hash_key, p.env_id_base + (uint64_t)env),
+                                               act, logp);
+                if (lane == 0) {
+                    a.actions_out[env] = act;
+                    if (a.log_prob_out) a.log_prob_out[env] = logp;
+                }
+                __syncwarp();                            // every lane has read the row before the next one is copied in
+            }
         }
         prefetch(tile + tile_step);
         if (env < 0) continue;
@@ -1247,7 +1366,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
         const uint32_t flags_in = s.flags;
         const bool changed = env_step<KJ>(p, iv, s, env, lane, action, raw, reinterpret_cast<int *>(w.scratch));
         if (jss_hint_flags<KJ, UNI>()) s.flags = jss_uniform(s.flags);   // the no-op test returns from inside lane-dependent code
-        if (SAMPLE) {
+        if (SAMPLE == 1 || SAMPLE == 2) {
             const uint32_t h = jss_hash_env(a.hash_key, p.env_id_base + (uint64_t)env);   // == jss_hash3(seed, genv, step_index)
             const int nxt = env_select_action<KJ, SAMPLE == 1>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor);
             if (lane == 0) a.actions_out[env] = nxt;
@@ -1280,6 +1399,8 @@ JSS_DEV void jss_step_carve(const JssSmemLayout &sl, char *sm, int warp, JssWarp
     // state-out staging sits right behind the observation staging (both leave by bulk store)
     w.state_out = reinterpret_cast<int32_t *>(w.scratch + sl.scratch_words);
     w.state_out_sa = w.scratch_sa + sl.scratch_words * 4;
+    w.logits = reinterpret_cast<float *>(wbase + sl.off_logits);   // behind state-out (SAMPLE = 3 layouts only)
+    w.logits_sa = w.mbar + sl.off_logits;
 }
 
 // Uniform batch (every env runs the same instance): static strided tiles, the per-instance scalars are

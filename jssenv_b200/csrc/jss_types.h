@@ -172,6 +172,11 @@ struct JssLaunch {           // per-launch arguments
     uint8_t *wire;           // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
     int32_t wire_stride;
     JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
+    // jss_step_logits: env i's logits at logits + i * logits_ld; the drawn actions go to actions_out, their
+    // log-probabilities to log_prob_out (may be NULL)
+    const float *logits;
+    float *log_prob_out;
+    int64_t logits_ld;
 };
 
 #define JSS_MODE_RESET 0

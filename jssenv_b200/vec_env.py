@@ -191,6 +191,35 @@ class JssVecEnv:
         self._step_index += 1
         return self._obs(), self.reward, self.done, self._truncated, {}, out
 
+    def step_logits(self, logits, actions_out=None, log_prob_out=None):
+        """Step every env with an action drawn from policy logits (jss_step_logits, one launch): a masked categorical
+        draw (Gumbel-max over the legal actions, RNG counter ``self._step_index``), then the step.  `logits`: (N, >= J+1)
+        tensor on the env's device whose columns line up with ``action_mask``; converted to float32 with unit column
+        stride only if needed.  Returns the step tuple with ``{"actions": int32 (N,), "log_prob": float32 (N,)}`` as info.
+        A done env gets action 0 and log_prob 0, an env whose only legal action is the no-op gets J_i and 0, and an env
+        whose legal logits are bad (NaN / +inf, or all -inf) gets the error bit, action JSS_ACTION_SKIP and NaN."""
+        import torch
+        n, J = self.num_envs, self.jobs
+        x = torch.as_tensor(logits, device=self.device)
+        if x.dim() != 2 or x.shape[0] != n or x.shape[1] < J + 1:
+            raise ValueError(f"step_logits: logits must have shape ({n}, >= {J + 1}), got {tuple(x.shape)}")
+        if x.dtype != torch.float32 or x.stride(1) != 1 or (n > 1 and x.stride(0) < J + 1):
+            x = x.to(torch.float32).contiguous()
+        ld = x.stride(0) if n > 1 else max(x.stride(0), J + 1)
+        if actions_out is None:
+            actions_out = torch.empty(n, dtype=torch.int32, device=self.device)
+        if log_prob_out is None:
+            log_prob_out = torch.empty(n, dtype=torch.float32, device=self.device)
+        for t, dt in ((actions_out, torch.int32), (log_prob_out, torch.float32)):
+            if t.dtype != dt or t.shape != (n,) or not t.is_contiguous() or t.device != x.device:
+                raise ValueError(f"step_logits: outputs must be contiguous {dt} tensors of shape ({n},) on {x.device}")
+        rc = self._L.jss_step_logits(self._h, ctypes.c_void_p(x.data_ptr()), int(ld), self.seed, self._step_index,
+                                     ctypes.c_void_p(actions_out.data_ptr()), ctypes.c_void_p(log_prob_out.data_ptr()),
+                                     self._stream())
+        N.check(self._h, rc, "jss_step_logits")
+        self._step_index += 1
+        return self._obs(), self.reward, self.done, self._truncated, {"actions": actions_out, "log_prob": log_prob_out}
+
     def get_legal_actions(self):
         return self.action_mask
 
