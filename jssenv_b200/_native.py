@@ -6,7 +6,7 @@ H100 (compute capability 9.0) is present, construction fails loudly.
 """
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_uint8, c_uint32, c_uint64, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_int, c_int32, c_int64, c_uint8, c_uint32, c_uint64, c_void_p
 
 import numpy as np
 
@@ -22,15 +22,6 @@ WAIT_MASK, WAIT_OBS, WAIT_OBS_PREV = 1, 2, 3
 RULES = {"RANDOM": 0, "SPT": 1, "FIFO": 2, "MWR": 3, "LWR": 4, "MOR": 5, "LOR": 6, "CR": 7}
 STATS_KEYS = ("episodes", "steps", "sum_makespan", "min_makespan", "max_makespan", "sum_return",
               "envs_done", "envs_error")
-
-EXPORTED_SYMBOLS = (
-    "jss_abi_version", "jss_create", "jss_destroy", "jss_last_error", "jss_load_instances", "jss_assign",
-    "jss_get_buffers", "jss_instance_scalars", "jss_reset", "jss_step", "jss_policy", "jss_rollout",
-    "jss_step_host", "jss_host_step_begin", "jss_host_wait", "jss_step_sample", "jss_stats", "jss_export_state", "jss_import_state", "jss_host_masked_random",
-    "jss_launch_count", "jss_set_cr_due_date_factor", "jss_host_step_begin_packed", "jss_host_wire_stride",
-    "jss_host_expand_obs", "jss_host_configure", "jss_host_threads", "jss_host_set_simd", "jss_rollout_traj", "jss_step_export", "jss_host_step_begin_hybrid", "jss_host_expand_obs_range",
-    "jss_step_logits",
-)
 
 
 class JssBuffers(ctypes.Structure):
@@ -50,60 +41,51 @@ class NativeError(RuntimeError):
     pass
 
 
+_VP, _I32P, _I64P = c_void_p, POINTER(c_int32), POINTER(c_int64)
+
+# every entry point of include/jss_b200.h: symbol -> (restype, argtypes), in the header's order
+SIGNATURES = {
+    "jss_create": (c_int, [POINTER(c_void_p), c_int, c_int, c_uint32, c_uint64]),
+    "jss_destroy": (None, [_VP]),
+    "jss_last_error": (c_char_p, [_VP]),
+    "jss_abi_version": (c_int, []),
+    "jss_load_instances": (c_int, [_VP, c_int, _I32P, _I32P, _I64P, _I32P, _I32P]),
+    "jss_assign": (c_int, [_VP, _I32P]),
+    "jss_get_buffers": (c_int, [_VP, POINTER(JssBuffers)]),
+    "jss_instance_scalars": (c_int, [_VP, c_int, _I64P]),
+    "jss_reset": (c_int, [_VP, _VP, _VP]),
+    "jss_step": (c_int, [_VP, _VP, _VP]),
+    "jss_step_export": (c_int, [_VP, _VP, _VP]),
+    "jss_policy": (c_int, [_VP, c_int, c_int, c_uint64, c_uint64, _VP, _VP]),
+    "jss_set_cr_due_date_factor": (c_int, [_VP, c_double]),
+    "jss_step_sample": (c_int, [_VP, _VP, c_int, c_int, c_uint64, c_uint64, _VP, _VP]),
+    "jss_step_logits": (c_int, [_VP, _VP, c_int64, c_uint64, c_uint64, _VP, _VP, _VP]),
+    "jss_rollout": (c_int, [_VP, c_int, c_uint64, c_uint64, c_int, c_int, _VP]),
+    "jss_rollout_traj": (c_int, [_VP, c_int, c_uint64, c_uint64, c_int, _VP, _VP, _VP, _VP, _VP]),
+    "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
+    "jss_host_step_begin": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
+    "jss_host_wait": (c_int, [_VP, c_int]),
+    "jss_host_step_begin_packed": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
+    "jss_host_step_begin_hybrid": (c_int, [_VP, _VP, _VP, _VP, _VP, c_int, _VP, _VP]),
+    "jss_host_expand_obs_range": (c_int, [_VP, _VP, _VP, _VP, c_int, c_int]),
+    "jss_host_wire_stride": (c_int64, [_VP]),
+    "jss_host_expand_obs": (c_int, [_VP, _VP, _VP, _VP]),
+    "jss_host_configure": (c_int, [c_int, c_int]),
+    "jss_host_threads": (c_int, []),
+    "jss_host_set_simd": (c_int, [c_int]),
+    "jss_stats": (c_int, [_VP, _I64P, _VP]),
+    "jss_export_state": (c_int, [_VP, _VP]),
+    "jss_import_state": (c_int, [_VP, _VP, _VP]),
+    "jss_host_masked_random": (c_int, [_VP, c_int, c_int, c_int64, c_uint64, c_uint64, c_uint64, _VP]),
+    "jss_launch_count": (c_int64, [_VP]),
+}
+EXPORTED_SYMBOLS = tuple(SIGNATURES)
+
+
 def _declare(L):
-    L.jss_abi_version.restype = c_int
-    L.jss_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_uint32, c_uint64]
-    L.jss_destroy.argtypes = [c_void_p]
-    L.jss_destroy.restype = None
-    L.jss_last_error.argtypes = [c_void_p]
-    L.jss_last_error.restype = c_char_p
-    L.jss_load_instances.argtypes = [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int64),
-                                     POINTER(c_int32), POINTER(c_int32)]
-    L.jss_assign.argtypes = [c_void_p, POINTER(c_int32)]
-    L.jss_get_buffers.argtypes = [c_void_p, POINTER(JssBuffers)]
-    L.jss_instance_scalars.argtypes = [c_void_p, c_int, POINTER(c_int64)]
-    L.jss_reset.argtypes = [c_void_p, c_void_p, c_void_p]
-    L.jss_step.argtypes = [c_void_p, c_void_p, c_void_p]
-    L.jss_policy.argtypes = [c_void_p, c_int, c_int, c_uint64, c_uint64, c_void_p, c_void_p]
-    L.jss_step_sample.argtypes = [c_void_p, c_void_p, c_int, c_int, c_uint64, c_uint64, c_void_p, c_void_p]
-    L.jss_step_logits.argtypes = [c_void_p, c_void_p, c_int64, c_uint64, c_uint64, c_void_p, c_void_p, c_void_p]
-    L.jss_step_logits.restype = c_int
-    L.jss_rollout.argtypes = [c_void_p, c_int, c_uint64, c_uint64, c_int, c_int, c_void_p]
-    L.jss_step_host.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    L.jss_host_step_begin.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    L.jss_host_wait.argtypes = [c_void_p, c_int]
-    L.jss_host_step_begin_packed.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    L.jss_host_step_begin_packed.restype = c_int
-    L.jss_host_step_begin_hybrid.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
-    L.jss_host_step_begin_hybrid.restype = c_int
-    L.jss_host_expand_obs_range.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int]
-    L.jss_host_expand_obs_range.restype = c_int
-    L.jss_host_wire_stride.argtypes = [c_void_p]
-    L.jss_host_wire_stride.restype = c_int64
-    L.jss_host_expand_obs.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p]
-    L.jss_host_expand_obs.restype = c_int
-    L.jss_host_configure.argtypes = [c_int, c_int]
-    L.jss_host_configure.restype = c_int
-    L.jss_rollout_traj.argtypes = [c_void_p, c_int, c_uint64, c_uint64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    L.jss_rollout_traj.restype = c_int
-    L.jss_step_export.argtypes = [c_void_p, c_void_p, c_void_p]
-    L.jss_step_export.restype = c_int
-    L.jss_host_set_simd.argtypes = [c_int]
-    L.jss_host_set_simd.restype = c_int
-    L.jss_host_threads.argtypes = []
-    L.jss_host_threads.restype = c_int
-    L.jss_stats.argtypes = [c_void_p, POINTER(c_int64), c_void_p]
-    L.jss_export_state.argtypes = [c_void_p, c_void_p]
-    L.jss_import_state.argtypes = [c_void_p, c_void_p, c_void_p]
-    L.jss_host_masked_random.argtypes = [c_void_p, c_int, c_int, c_int64, c_uint64, c_uint64, c_uint64, c_void_p]
-    L.jss_set_cr_due_date_factor.argtypes = [c_void_p, ctypes.c_double]
-    L.jss_set_cr_due_date_factor.restype = c_int
-    L.jss_launch_count.argtypes = [c_void_p]
-    L.jss_launch_count.restype = c_int64
-    for name in ("jss_create", "jss_load_instances", "jss_assign", "jss_get_buffers", "jss_instance_scalars",
-                 "jss_reset", "jss_step", "jss_policy", "jss_rollout", "jss_step_host", "jss_host_step_begin", "jss_host_wait", "jss_step_sample", "jss_stats",
-                 "jss_export_state", "jss_import_state", "jss_host_masked_random"):
-        getattr(L, name).restype = c_int
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     return L
 
 
@@ -111,6 +93,7 @@ class CudaBackend:
     """Device memory / stream plumbing through torch (plumbing only: every kernel is ours)."""
 
     name = "cuda"
+    pin_memory = True        # host staging buffers are page-locked: DMA targets, device-mapped by the kernels
 
     def __init__(self):
         self._lib = None
@@ -166,3 +149,13 @@ def check(handle, rc, what):
 
 def as_i32p(a):
     return a.ctypes.data_as(POINTER(c_int32))
+
+
+def host_view(ptr, shape, dtype, strides=None):
+    """Zero-copy numpy view of host memory at address `ptr` (byte `strides`; default: C-contiguous)."""
+    dt = np.dtype(dtype)
+    shape = tuple(int(s) for s in shape)
+    nbytes = (int(np.prod(shape)) * dt.itemsize if strides is None
+              else sum((sh - 1) * int(st) for sh, st in zip(shape, strides)) + dt.itemsize)
+    buf = (ctypes.c_char * max(nbytes, 1)).from_address(int(ptr))
+    return np.ndarray(shape, dt, buffer=buf, strides=None if strides is None else tuple(int(s) for s in strides))

@@ -221,10 +221,136 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     return JSS_OK;
 }
 
+// the action choice of jss_policy / jss_step_sample / jss_rollout / jss_rollout_traj
+bool valid_rule_coin(int rule, int coin_mode) {
+    return rule >= 0 && rule < JSS_NUM_RULES && (coin_mode == JSS_COIN_DEVICE || coin_mode == JSS_COIN_NEVER);
+}
+
 int check_ready(jss_t *h) {
     if (!h) return JSS_ERR_INVALID;
     if (!h->assigned) return fail(h, JSS_ERR_STATE, "jss_load_instances + jss_assign must be called first");
     JSS_CUDA(h, cudaSetDevice(h->device));
+    return JSS_OK;
+}
+
+// group envs by (KJ class, instance) -> tiles of <= JSS_WARPS_PER_CTA envs of one instance, the largest lane class
+// first (the order in which the mixed-batch step kernel walks its slices); sets the class tile ranges of `h`
+int plan_tiles(jss_t *h, const int32_t *env_to_inst, std::vector<int32_t> &order, std::vector<JssTile> &tiles,
+               size_t &state_words) {
+    const int N = h->n_envs;
+    order.resize(N);
+    for (int e = 0; e < N; e++) order[e] = e;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
+        const int ka = env_to_inst[a], kb = env_to_inst[b];
+        const int ca = class_of(kj_of(h->insts[ka].J)), cb = class_of(kj_of(h->insts[kb].J));
+        if (ca != cb) return ca > cb;
+        return ka < kb;
+    });
+    for (int c = 0; c < 4; c++) h->class_tile_begin[c] = h->class_tile_end[c] = 0;
+    int pos = 0;
+    int cur_class = -1;
+    uint64_t off16 = 0;                                  // running state offset in 16-byte units
+    while (pos < N) {
+        const int k = env_to_inst[order[pos]];
+        const int c = class_of(kj_of(h->insts[k].J));
+        const uint32_t block16 = (uint32_t)h->insts[k].block_words / 4;
+        int end = pos;
+        while (end < N && env_to_inst[order[end]] == k) end++;
+        if (c != cur_class) {
+            if (cur_class >= 0) h->class_tile_end[cur_class] = (int)tiles.size();
+            h->class_tile_begin[c] = (int)tiles.size();
+            cur_class = c;
+        }
+        for (int f = pos; f < end; f += JSS_WARPS_PER_CTA) {
+            JssTile t;
+            const int cnt = std::min(JSS_WARPS_PER_CTA, end - f);
+            t.first = f;
+            t.inst_count = (k << 8) | cnt;
+            t.state_off16 = (uint32_t)off16;
+            t.block16 = block16;
+            off16 += (uint64_t)cnt * block16;
+            tiles.push_back(t);
+        }
+        pos = end;
+    }
+    if (cur_class >= 0) h->class_tile_end[cur_class] = (int)tiles.size();
+    h->n_tiles = (int)tiles.size();
+    if (off16 >= (1ull << 32)) return fail(h, JSS_ERR_UNSUPPORTED, "state exceeds 64 GiB");
+    state_words = (size_t)off16 * 4;
+    return JSS_OK;
+}
+
+// mixed-batch step kernel: every persistent CTA gets an equal slice of EVERY lane class (tile counts differ by at
+// most one per class; the extras are dithered with a different phase per class so that no CTA collects them all)
+std::vector<JssCtaRange> plan_cta_ranges(const jss_t *h) {
+    const int n_cta = std::max(1, std::min(h->n_tiles, h->sm_count * JSS_MIN_CTAS));
+    std::vector<JssCtaRange> ranges((size_t)n_cta);
+    for (int c = 0; c < 4; c++) {                     // c = 3: KJ = 8, c = 2: KJ = 4, c = 1: KJ = 2, c = 0: KJ = 1
+        const int tb = h->class_tile_begin[c], n = h->class_tile_end[c] - tb;
+        const int shift = (c * n_cta) / 4;            // CTA that starts this class's Bresenham sequence
+        int given = 0;
+        for (int k = 0; k < n_cta; k++) {
+            const int b = (k + shift) % n_cta;
+            const int upto = (int)(((int64_t)(k + 1) * n) / n_cta);
+            int32_t *lo = c == 3 ? &ranges[b].a8 : (c == 2 ? &ranges[b].a4 : (c == 1 ? &ranges[b].a2 : &ranges[b].a1));
+            lo[0] = tb + given; lo[1] = tb + upto;
+            given = upto;
+        }
+    }
+    return ranges;
+}
+
+// shared-memory layouts: [JssInst][ops u16][len i32][rem u16][per-warp regions], 16-byte aligned regions; ops_max and
+// rem_max are the largest ops / suffix-sum tables of the batch's instances
+void plan_smem_layouts(jss_t *h, int jmax, int mmax, int ops_max, int rem_max) {
+    const JssBlockGeom g = jss_block_geom(jmax, mmax);   // the geometry grows with J and M: batch maxima
+    JssSmemLayout sl{};
+    sl.off_len = (int32_t)sizeof(JssInst) + round_up(ops_max, 8) * 2;
+    sl.off_rem = sl.off_len + round_up(jmax, 4) * 4;
+    sl.off_warp0 = sl.off_rem + round_up(rem_max, 8) * 2;
+    // observation staging (7 floats per job slot); env_check_no_op (general instances) also keeps its 32-int
+    // per-warp machine-horizon table here, so never less than 32 words (tiny instances: 7 * Jcap < 32)
+    sl.scratch_words = std::max(7 * g.Jcap, 32);
+    h->sl_env = sl;
+    h->sl_env.warp_stride = sl.scratch_words * 4;
+    h->sl_env.off_scratch = 0;
+    h->sl_step_rem = sl;
+    h->sl_step_rem.off_scratch = 16 + g.words * 4;                                     // [mbarrier][state-in]
+    h->sl_step_rem.warp_stride = h->sl_step_rem.off_scratch + sl.scratch_words * 4 + g.words * 4;   // [scratch][state-out]
+    h->sl_step = h->sl_step_rem;                      // launches that stage no suffix sums leave their room to the L1
+    h->sl_step.off_warp0 = h->sl_step.off_rem;
+    h->sl_step_logits = h->sl_step;                   // + [logits row: jobs_max + 1 floats]
+    h->sl_step_logits.off_logits = h->sl_step.warp_stride;
+    h->sl_step_logits.warp_stride += round_up(4 * (jmax + 1), 16);
+}
+
+// the per-transition outputs, one device allocation each; with JSS_CREATE_HOST_MIRROR all of them (and an action slot)
+// in one pinned, device-mapped host block instead (unified addressing: the device pointer equals the host pointer),
+// meant for small batches -- the kernels write over PCIe
+int alloc_outputs(jss_t *h) {
+    JssParams &p = h->p;
+    const size_t N = (size_t)p.n_envs, NJ = N * p.jobs_max, NM = N * p.machines_max;
+    struct Output { char **slot; size_t bytes; bool mirror_only = false; };
+    const Output outputs[] = {
+        {(char **)&p.mask, N * p.mask_stride}, {(char **)&p.obs, NJ * 7 * 4}, {(char **)&p.scalars, N * 16},
+        {(char **)&p.x_todo, NJ * 4}, {(char **)&p.x_tufco, NJ * 4}, {(char **)&p.x_idle_last, NJ * 4},
+        {(char **)&p.x_total_idle, NJ * 4}, {(char **)&p.x_col4, NJ * 4}, {(char **)&p.x_tuam, NM * 4},
+        {(char **)&p.x_legal, NJ}, {(char **)&p.x_blocked, NJ}, {(char **)&h->mirror_actions, N * 4, true}};
+    if (!(h->create_flags & JSS_CREATE_HOST_MIRROR)) {
+        for (const Output &o : outputs)
+            if (int rc = o.mirror_only ? JSS_OK : dev_alloc(h, o.slot, o.bytes)) return rc;
+        return JSS_OK;
+    }
+    auto padded = [](size_t bytes) { return (bytes + 255) / 256 * 256; };
+    size_t total = 0;
+    for (const Output &o : outputs) total += padded(o.bytes);
+    JSS_CUDA(h, cudaHostAlloc(&h->host_block, total, cudaHostAllocMapped | cudaHostAllocPortable));
+    memset(h->host_block, 0, total);
+    void *dev = nullptr;
+    JSS_CUDA(h, cudaHostGetDevicePointer(&dev, h->host_block, 0));
+    if (dev != h->host_block) return fail(h, JSS_ERR_CUDA, "host mirror needs unified addressing");
+    char *b = static_cast<char *>(h->host_block);
+    for (const Output &o : outputs) { *o.slot = b; b += padded(o.bytes); }
     return JSS_OK;
 }
 
@@ -395,68 +521,12 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
         ops_max = std::max(ops_max, h->insts[k].J * h->insts[k].M);
         rem_max = std::max(rem_max, h->insts[k].J * (h->insts[k].M + 1));
     }
-    // group envs by (KJ class, instance) -> tiles of <= JSS_WARPS_PER_CTA envs of one instance, the largest lane class
-    // first (the order in which the mixed-batch step kernel walks its slices)
-    std::vector<int32_t> order(N);
-    for (int e = 0; e < N; e++) order[e] = e;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
-        const int ka = env_to_inst[a], kb = env_to_inst[b];
-        const int ca = class_of(kj_of(h->insts[ka].J)), cb = class_of(kj_of(h->insts[kb].J));
-        if (ca != cb) return ca > cb;
-        return ka < kb;
-    });
+    int rc;
+    std::vector<int32_t> order;
     std::vector<JssTile> tiles;
-    for (int c = 0; c < 4; c++) h->class_tile_begin[c] = h->class_tile_end[c] = 0;
-    int pos = 0;
-    int cur_class = -1;
-    uint64_t off16 = 0;                                  // running state offset in 16-byte units
-    while (pos < N) {
-        const int k = env_to_inst[order[pos]];
-        const int c = class_of(kj_of(h->insts[k].J));
-        const uint32_t block16 = (uint32_t)h->insts[k].block_words / 4;
-        int end = pos;
-        while (end < N && env_to_inst[order[end]] == k) end++;
-        if (c != cur_class) {
-            if (cur_class >= 0) h->class_tile_end[cur_class] = (int)tiles.size();
-            h->class_tile_begin[c] = (int)tiles.size();
-            cur_class = c;
-        }
-        for (int f = pos; f < end; f += JSS_WARPS_PER_CTA) {
-            JssTile t;
-            const int cnt = std::min(JSS_WARPS_PER_CTA, end - f);
-            t.first = f;
-            t.inst_count = (k << 8) | cnt;
-            t.state_off16 = (uint32_t)off16;
-            t.block16 = block16;
-            off16 += (uint64_t)cnt * block16;
-            tiles.push_back(t);
-        }
-        pos = end;
-    }
-    if (cur_class >= 0) h->class_tile_end[cur_class] = (int)tiles.size();
-    h->n_tiles = (int)tiles.size();
-    if (off16 >= (1ull << 32)) return fail(h, JSS_ERR_UNSUPPORTED, "state exceeds 64 GiB");
-    const size_t state_words = (size_t)off16 * 4;
-
-    // mixed-batch step kernel: every persistent CTA gets an equal slice of EVERY lane class (tile counts differ by at
-    // most one per class; the extras are dithered with a different phase per class so that no CTA collects them all)
-    std::vector<JssCtaRange> ranges;
-    {
-        const int n_cta = std::max(1, std::min((int)tiles.size(), h->sm_count * JSS_MIN_CTAS));
-        ranges.resize((size_t)n_cta);
-        for (int c = 0; c < 4; c++) {                     // c = 3: KJ = 8, c = 2: KJ = 4, c = 1: KJ = 2, c = 0: KJ = 1
-            const int tb = h->class_tile_begin[c], n = h->class_tile_end[c] - tb;
-            const int shift = (c * n_cta) / 4;            // CTA that starts this class's Bresenham sequence
-            int given = 0;
-            for (int k = 0; k < n_cta; k++) {
-                const int b = (k + shift) % n_cta;
-                const int upto = (int)(((int64_t)(k + 1) * n) / n_cta);
-                int32_t *lo = c == 3 ? &ranges[b].a8 : (c == 2 ? &ranges[b].a4 : (c == 1 ? &ranges[b].a2 : &ranges[b].a1));
-                lo[0] = tb + given; lo[1] = tb + upto;
-                given = upto;
-            }
-        }
-    }
+    size_t state_words = 0;
+    if ((rc = plan_tiles(h, env_to_inst, order, tiles, state_words))) return rc;
+    const std::vector<JssCtaRange> ranges = plan_cta_ranges(h);
 
     JssParams &p = h->p;
     p.n_envs = N;
@@ -471,30 +541,8 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
         p.uniform_inst = uniform ? env_to_inst[0] : -1;   // then `order` is the identity (stable sort)
     }
     p.inst = h->d_inst; p.ops_pool = h->d_ops; p.len_pool = h->d_len; p.rem_pool = h->d_rem;
+    plan_smem_layouts(h, jmax, mmax, ops_max, rem_max);
 
-    {   // shared-memory layouts: [JssInst][ops u16][len i32][rem u16][per-warp regions], 16-byte aligned regions
-        const JssBlockGeom g = jss_block_geom(jmax, mmax);   // the geometry grows with J and M: batch maxima
-        JssSmemLayout sl{};
-        sl.off_len = (int32_t)sizeof(JssInst) + round_up(ops_max, 8) * 2;
-        sl.off_rem = sl.off_len + round_up(jmax, 4) * 4;
-        sl.off_warp0 = sl.off_rem + round_up(rem_max, 8) * 2;
-        // observation staging (7 floats per job slot); env_check_no_op (general instances) also keeps its 32-int
-        // per-warp machine-horizon table here, so never less than 32 words (tiny instances: 7 * Jcap < 32)
-        sl.scratch_words = std::max(7 * g.Jcap, 32);
-        h->sl_env = sl;
-        h->sl_env.warp_stride = sl.scratch_words * 4;
-        h->sl_env.off_scratch = 0;
-        h->sl_step_rem = sl;
-        h->sl_step_rem.off_scratch = 16 + g.words * 4;                                     // [mbarrier][state-in]
-        h->sl_step_rem.warp_stride = h->sl_step_rem.off_scratch + sl.scratch_words * 4 + g.words * 4;   // [scratch][state-out]
-        h->sl_step = h->sl_step_rem;                      // launches that stage no suffix sums leave their room to the L1
-        h->sl_step.off_warp0 = h->sl_step.off_rem;
-        h->sl_step_logits = h->sl_step;                   // + [logits row: jobs_max + 1 floats]
-        h->sl_step_logits.off_logits = h->sl_step.warp_stride;
-        h->sl_step_logits.warp_stride += round_up(4 * (jmax + 1), 16);
-    }
-
-    int rc;
     int32_t *d_order = nullptr;
     JssTile *d_tiles = nullptr;
     JssCtaRange *d_ranges = nullptr;
@@ -508,42 +556,9 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     p.tiles = d_tiles;
     p.cta_ranges = d_ranges;
     p.n_cta_ranges = (int32_t)ranges.size();
-    const size_t NJ = (size_t)N * jmax, NM = (size_t)N * mmax;
+    const size_t NJ = (size_t)N * jmax;
     if ((rc = dev_alloc(h, &p.state, state_words))) return rc;
-    if (h->create_flags & JSS_CREATE_HOST_MIRROR) {
-        // every per-transition output in one pinned, device-mapped host block (unified addressing: the device
-        // pointer equals the host pointer); meant for small batches -- the kernels write over PCIe
-        size_t off = 0;
-        auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-        const size_t o_mask = take(N * (size_t)p.mask_stride), o_obs = take(NJ * 7 * 4), o_sc = take((size_t)N * 16);
-        const size_t o_i[5] = {take(NJ * 4), take(NJ * 4), take(NJ * 4), take(NJ * 4), take(NJ * 4)};
-        const size_t o_tuam = take(NM * 4), o_legal = take(NJ), o_blocked = take(NJ), o_act = take((size_t)N * 4);
-        JSS_CUDA(h, cudaHostAlloc(&h->host_block, off, cudaHostAllocMapped | cudaHostAllocPortable));
-        memset(h->host_block, 0, off);
-        void *dev = nullptr;
-        JSS_CUDA(h, cudaHostGetDevicePointer(&dev, h->host_block, 0));
-        if (dev != h->host_block) return fail(h, JSS_ERR_CUDA, "host mirror needs unified addressing");
-        char *b = static_cast<char *>(h->host_block);
-        p.mask = reinterpret_cast<uint8_t *>(b + o_mask); p.obs = reinterpret_cast<float *>(b + o_obs);
-        p.scalars = reinterpret_cast<int32_t *>(b + o_sc);
-        p.x_todo = reinterpret_cast<int32_t *>(b + o_i[0]); p.x_tufco = reinterpret_cast<int32_t *>(b + o_i[1]);
-        p.x_idle_last = reinterpret_cast<int32_t *>(b + o_i[2]); p.x_total_idle = reinterpret_cast<int32_t *>(b + o_i[3]);
-        p.x_col4 = reinterpret_cast<int32_t *>(b + o_i[4]); p.x_tuam = reinterpret_cast<int32_t *>(b + o_tuam);
-        p.x_legal = reinterpret_cast<uint8_t *>(b + o_legal); p.x_blocked = reinterpret_cast<uint8_t *>(b + o_blocked);
-        h->mirror_actions = reinterpret_cast<int32_t *>(b + o_act);
-    } else {
-        if ((rc = dev_alloc(h, &p.mask, (size_t)N * p.mask_stride))) return rc;
-        if ((rc = dev_alloc(h, &p.obs, NJ * 7))) return rc;
-        if ((rc = dev_alloc(h, &p.scalars, (size_t)N * 4))) return rc;
-        if ((rc = dev_alloc(h, &p.x_todo, NJ))) return rc;
-        if ((rc = dev_alloc(h, &p.x_tufco, NJ))) return rc;
-        if ((rc = dev_alloc(h, &p.x_idle_last, NJ))) return rc;
-        if ((rc = dev_alloc(h, &p.x_total_idle, NJ))) return rc;
-        if ((rc = dev_alloc(h, &p.x_col4, NJ))) return rc;
-        if ((rc = dev_alloc(h, &p.x_tuam, NM))) return rc;
-        if ((rc = dev_alloc(h, &p.x_legal, NJ))) return rc;
-        if ((rc = dev_alloc(h, &p.x_blocked, NJ))) return rc;
-    }
+    if ((rc = alloc_outputs(h))) return rc;
     if (h->create_flags & JSS_CREATE_RECORD_SOLUTION) {
         if ((rc = dev_alloc(h, &p.solution, NJ * mmax, false))) return rc;
         JSS_CUDA(h, cudaMemset(p.solution, 0xff, NJ * mmax * 4));  // -1
@@ -616,8 +631,7 @@ int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mod
                     uint64_t step_index, int32_t *next_actions_dev, void *stream) {
     int rc = check_ready(h);
     if (rc) return rc;
-    if (!actions_dev || !next_actions_dev || rule < 0 || rule >= JSS_NUM_RULES ||
-        (coin_mode != JSS_COIN_DEVICE && coin_mode != JSS_COIN_NEVER))
+    if (!actions_dev || !next_actions_dev || !valid_rule_coin(rule, coin_mode))
         return fail(h, JSS_ERR_INVALID, "jss_step_sample: bad arguments (rule %d, coin %d)", rule, coin_mode);
     JssLaunch a{};
     a.mode = JSS_MODE_STEP;
@@ -649,7 +663,7 @@ int jss_policy(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_i
                void *stream) {
     int rc = check_ready(h);
     if (rc) return rc;
-    if (!actions_dev || rule < 0 || rule >= JSS_NUM_RULES || (coin_mode != JSS_COIN_DEVICE && coin_mode != JSS_COIN_NEVER))
+    if (!actions_dev || !valid_rule_coin(rule, coin_mode))
         return fail(h, JSS_ERR_INVALID, "jss_policy: bad arguments (rule %d, coin %d)", rule, coin_mode);
     JssLaunch a{};
     a.mode = JSS_MODE_POLICY;
@@ -661,7 +675,7 @@ int jss_policy(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_i
 int jss_rollout(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_steps, int write_obs, void *stream) {
     int rc = check_ready(h);
     if (rc) return rc;
-    if (rule < 0 || rule >= JSS_NUM_RULES || n_steps < 0)
+    if (!valid_rule_coin(rule, JSS_COIN_DEVICE) || n_steps < 0)
         return fail(h, JSS_ERR_INVALID, "jss_rollout: bad arguments (rule %d, n_steps %d)", rule, n_steps);
     JssLaunch a{};
     a.mode = JSS_MODE_ROLLOUT;
@@ -674,7 +688,7 @@ int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int
                      uint8_t *traj_mask, int32_t *traj_scalars, int32_t *traj_actions, void *stream) {
     int rc = check_ready(h);
     if (rc) return rc;
-    if (rule < 0 || rule >= JSS_NUM_RULES || n_steps < 0 || !traj_obs || !traj_mask || !traj_scalars)
+    if (!valid_rule_coin(rule, JSS_COIN_DEVICE) || n_steps < 0 || !traj_obs || !traj_mask || !traj_scalars)
         return fail(h, JSS_ERR_INVALID, "jss_rollout_traj: bad arguments (rule %d, n_steps %d)", rule, n_steps);
     if ((int64_t)n_steps * h->n_envs >= INT32_MAX)
         return fail(h, JSS_ERR_UNSUPPORTED, "jss_rollout_traj: n_steps * n_envs must stay below 2^31");

@@ -63,7 +63,7 @@ class JssEnv(_gym.Env if _gym is not None else object):
                 "real_obs": _Space("Box", low=0.0, high=1.0, shape=(J, 7), dtype=float)})
         self.solution = np.full((self.jobs, self.machines), -1, dtype=np.int64)       # jss_env.py:163
         self._arange = np.arange(J)
-        self._vec._L.jss_export_state(self._vec._h, self._vec._stream())
+        self._vec.export_state()
         self._pull()
 
     # ------------------------------------------------------------------ state mirror
@@ -139,7 +139,7 @@ class JssEnv(_gym.Env if _gym is not None else object):
         snap = self._vec.export_state()
         snap["flags"].bitwise_and_(~((N.FLAG_ERROR) << 8))
         self._vec.import_state(snap)
-        self._vec._L.jss_export_state(self._vec._h, self._vec._stream())
+        self._vec.export_state()
         self._pull()
         raise IndexError(message)
 
@@ -158,7 +158,7 @@ class JssEnv(_gym.Env if _gym is not None else object):
     def reset(self, *, seed=None, options=None):
         """Returns the observation only, like the reference (jss_env.py:145-181)."""
         self._vec.reset()
-        self._vec._L.jss_export_state(self._vec._h, self._vec._stream())
+        self._vec.export_state()
         self.solution = np.full((self.jobs, self.machines), -1, dtype=np.int64)
         self._pull()
         return self._get_current_state_representation()

@@ -29,6 +29,35 @@ def _instance_list(env_config: Optional[Dict[str, Any]]):
     return [load_instance(s) for s in specs], env_config.get("env_to_instance")
 
 
+def _rule_id(rule: Union[str, int]) -> int:
+    return N.RULES[rule.upper()] if isinstance(rule, str) else int(rule)
+
+
+def _coin_id(coin: str) -> int:
+    return N.COIN_DEVICE if coin == "device" else N.COIN_NEVER
+
+
+def _ptr(t):
+    """Pointer argument of a tensor (None: NULL).  A plain int: ctypes converts it for a c_void_p parameter, and the
+    hot methods pass ``t.data_ptr()`` directly for the same reason (no pointer object per call)."""
+    return None if t is None else t.data_ptr()
+
+
+def _host_buffer(shape, dtype):
+    """Host staging buffer, page-locked where the backend can pin (DMA target, device-mapped writes); a backend that
+    does not declare ``pin_memory`` gets ordinary pageable memory."""
+    import torch
+    return torch.empty(shape, dtype=dtype, pin_memory=getattr(N.backend, "pin_memory", False))
+
+
+def _state_views(b, n, J, M, view):
+    """The canonical-state arrays of jss_export_state, each made by ``view(ptr, shape, dtype)``."""
+    return {"todo": view(b.x_todo, (n, J), np.int32), "tufco": view(b.x_tufco, (n, J), np.int32),
+            "idle_last": view(b.x_idle_last, (n, J), np.int32), "total_idle": view(b.x_total_idle, (n, J), np.int32),
+            "col4": view(b.x_col4, (n, J), np.int32), "tuam": view(b.x_tuam, (n, M), np.int32),
+            "legal": view(b.x_legal, (n, J), np.uint8), "blocked": view(b.x_blocked, (n, J), np.uint8)}
+
+
 class JssVecEnv:
     def __init__(self, num_envs: int, env_config: Optional[Dict[str, Any]] = None, device: int = 0,
                  auto_reset: bool = False, record_solution: bool = False, env_id_base: int = 0, seed: int = 0,
@@ -92,32 +121,15 @@ class JssVecEnv:
         self.episode_count = w(b.episode_count, (n,), np.int32, d)
         self.last_makespan = w(b.last_makespan, (n,), np.int32, d)
         self.last_return = w(b.last_return, (n,), np.int32, d)
-        self._x = {
-            "todo": w(b.x_todo, (n, J), np.int32, d), "tufco": w(b.x_tufco, (n, J), np.int32, d),
-            "idle_last": w(b.x_idle_last, (n, J), np.int32, d), "total_idle": w(b.x_total_idle, (n, J), np.int32, d),
-            "col4": w(b.x_col4, (n, J), np.int32, d), "tuam": w(b.x_tuam, (n, M), np.int32, d),
-            "legal": w(b.x_legal, (n, J), np.uint8, d), "blocked": w(b.x_blocked, (n, J), np.uint8, d),
-        }
+        self._x = _state_views(b, n, J, M, lambda ptr, shape, dt: w(ptr, shape, dt, d))
         self.host = None
         if b.host_mirror:
             # JSS_CREATE_HOST_MIRROR: the same memory seen from the host (pinned, device-mapped): numpy views, no copies
-            def hv(ptr, shape, dt, strides=None):
-                dt = np.dtype(dt)
-                nbytes = (int(np.prod(shape)) * dt.itemsize if strides is None
-                          else sum((sh - 1) * st for sh, st in zip(shape, strides)) + dt.itemsize)
-                raw = np.frombuffer((ctypes.c_char * nbytes).from_address(int(ptr)), dtype=np.uint8)
-                if strides is None:
-                    return raw.view(dt).reshape(shape)
-                return np.lib.stride_tricks.as_strided(raw[: nbytes // dt.itemsize * dt.itemsize].view(dt) if dt.itemsize > 1 else raw,
-                                                       shape=shape, strides=strides)
-            sc = hv(b.reward, (n, 4), np.int32)
+            hv = N.host_view
             self.host = {
                 "action_mask": hv(b.action_mask, (n, J + 1), np.uint8, strides=(int(b.mask_stride), 1)),
-                "real_obs": hv(b.real_obs, (n, J, 7), np.float32), "scalars": sc,
-                "todo": hv(b.x_todo, (n, J), np.int32), "tufco": hv(b.x_tufco, (n, J), np.int32),
-                "idle_last": hv(b.x_idle_last, (n, J), np.int32), "total_idle": hv(b.x_total_idle, (n, J), np.int32),
-                "col4": hv(b.x_col4, (n, J), np.int32), "tuam": hv(b.x_tuam, (n, M), np.int32),
-                "legal": hv(b.x_legal, (n, J), np.uint8), "blocked": hv(b.x_blocked, (n, J), np.uint8),
+                "real_obs": hv(b.real_obs, (n, J, 7), np.float32), "scalars": hv(b.reward, (n, 4), np.int32),
+                **_state_views(b, n, J, M, hv),
                 "actions": hv(b.mirror_actions, (n,), np.int32),
             }
             self._mirror_actions = w(b.mirror_actions, (n,), np.int32, d)
@@ -147,46 +159,49 @@ class JssVecEnv:
     def _obs(self):
         return {"real_obs": self.real_obs, "action_mask": self.action_mask}
 
-    # ---------------------------------------------------------------- reference API, batched
-    def reset(self, mask=None):
-        """reset() of every env (or of the envs where `mask` is nonzero) -> obs (jss_env.py:145-181)."""
-        ptr = None
-        if mask is not None:
-            import torch
-            mask = torch.as_tensor(mask, device=self.device).to(torch.uint8).contiguous()
-            ptr = ctypes.c_void_p(mask.data_ptr())
-        N.check(self._h, self._L.jss_reset(self._h, ptr, self._stream()), "jss_reset")
-        return self._obs()
-
-    def step(self, actions):
-        """actions: int32[N] on the env's device (torch) or anything torch.as_tensor accepts."""
+    def _device_i32(self, actions):
+        """`actions` as a contiguous int32 tensor on the env's device (the tensor itself if it already is one)."""
         import torch
         a = torch.as_tensor(actions, device=self.device)
         if a.dtype != torch.int32 or not a.is_contiguous():
             a = a.to(torch.int32).contiguous()
-        N.check(self._h, self._L.jss_step(self._h, ctypes.c_void_p(a.data_ptr()), self._stream()), "jss_step")
+        return a
+
+    def _env_mask(self, mask):
+        """Env selection mask (nonzero = selected) as a contiguous uint8 device tensor; None selects every env."""
+        if mask is None:
+            return None
+        import torch
+        return torch.as_tensor(mask, device=self.device).to(torch.uint8).contiguous()
+
+    # ---------------------------------------------------------------- reference API, batched
+    def reset(self, mask=None):
+        """reset() of every env (or of the envs where `mask` is nonzero) -> obs (jss_env.py:145-181)."""
+        m = self._env_mask(mask)
+        N.check(self._h, self._L.jss_reset(self._h, _ptr(m), self._stream()), "jss_reset")
+        return self._obs()
+
+    def step(self, actions):
+        """actions: int32[N] on the env's device (torch) or anything torch.as_tensor accepts."""
+        a = self._device_i32(actions)
+        N.check(self._h, self._L.jss_step(self._h, a.data_ptr(), self._stream()), "jss_step")
         return self._obs(), self.reward, self.done, self._truncated, {}
 
     def step_export_host(self):
         """Host-mirror batches (the single-env facade): apply the actions written to ``self.host["actions"]`` and decode
         the new state into the x_* arrays in ONE launch (jss_step_export), then wait; afterwards every array of
         ``self.host`` is current.  No per-transition copies: the kernels write straight into the pinned block."""
-        rc = self._L.jss_step_export(self._h, ctypes.c_void_p(self._mirror_actions.data_ptr()), self._stream())
+        rc = self._L.jss_step_export(self._h, self._mirror_actions.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_step_export")
         N.backend.synchronize(self.device_index)
 
     def step_sample(self, actions, rule: Union[str, int] = "RANDOM", coin: str = "device", out=None):
         """step(actions) fused with policy(rule) for the next decision (one launch): returns the usual
         step tuple plus the int32[N] tensor of next actions (`out`, default: in place of `actions`)."""
-        import torch
-        a = torch.as_tensor(actions, device=self.device)
-        if a.dtype != torch.int32 or not a.is_contiguous():
-            a = a.to(torch.int32).contiguous()
+        a = self._device_i32(actions)
         out = a if out is None else out
-        r = N.RULES[rule.upper()] if isinstance(rule, str) else int(rule)
-        rc = self._L.jss_step_sample(self._h, ctypes.c_void_p(a.data_ptr()), r,
-                                     N.COIN_DEVICE if coin == "device" else N.COIN_NEVER, self.seed,
-                                     self._step_index, ctypes.c_void_p(out.data_ptr()), self._stream())
+        rc = self._L.jss_step_sample(self._h, a.data_ptr(), _rule_id(rule), _coin_id(coin), self.seed,
+                                     self._step_index, out.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_step_sample")
         self._step_index += 1
         return self._obs(), self.reward, self.done, self._truncated, {}, out
@@ -213,9 +228,8 @@ class JssVecEnv:
         for t, dt in ((actions_out, torch.int32), (log_prob_out, torch.float32)):
             if t.dtype != dt or t.shape != (n,) or not t.is_contiguous() or t.device != x.device:
                 raise ValueError(f"step_logits: outputs must be contiguous {dt} tensors of shape ({n},) on {x.device}")
-        rc = self._L.jss_step_logits(self._h, ctypes.c_void_p(x.data_ptr()), int(ld), self.seed, self._step_index,
-                                     ctypes.c_void_p(actions_out.data_ptr()), ctypes.c_void_p(log_prob_out.data_ptr()),
-                                     self._stream())
+        rc = self._L.jss_step_logits(self._h, x.data_ptr(), int(ld), self.seed, self._step_index,
+                                     actions_out.data_ptr(), log_prob_out.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_step_logits")
         self._step_index += 1
         return self._obs(), self.reward, self.done, self._truncated, {"actions": actions_out, "log_prob": log_prob_out}
@@ -226,13 +240,12 @@ class JssVecEnv:
     # ---------------------------------------------------------------- policies on device
     def policy(self, rule: Union[str, int] = "RANDOM", coin: str = "device", out=None, step_index=None):
         """Device-side action selection (masked-uniform sampler or a dispatching rule)."""
-        r = N.RULES[rule.upper()] if isinstance(rule, str) else int(rule)
+        r = _rule_id(rule)
         out = self._actions if out is None else out
         if step_index is None:
             step_index = self._step_index
             self._step_index += 1
-        rc = self._L.jss_policy(self._h, r, N.COIN_DEVICE if coin == "device" else N.COIN_NEVER, self.seed,
-                                int(step_index), ctypes.c_void_p(out.data_ptr()), self._stream())
+        rc = self._L.jss_policy(self._h, r, _coin_id(coin), self.seed, int(step_index), out.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_policy")
         return out
 
@@ -242,9 +255,8 @@ class JssVecEnv:
 
     def rollout(self, rule: Union[str, int], n_steps: int, write_obs: bool = True):
         """n_steps x (policy -> step) fused on device (DispatchingRule.run_episode, dispatching.py:55-75)."""
-        r = N.RULES[rule.upper()] if isinstance(rule, str) else int(rule)
-        rc = self._L.jss_rollout(self._h, r, self.seed, self._step_index, int(n_steps), int(bool(write_obs)),
-                                 self._stream())
+        rc = self._L.jss_rollout(self._h, _rule_id(rule), self.seed, self._step_index, int(n_steps),
+                                 int(bool(write_obs)), self._stream())
         N.check(self._h, rc, "jss_rollout")
         self._step_index += int(n_steps)
         return self._obs(), self.reward, self.done, self._truncated, {}
@@ -254,7 +266,7 @@ class JssVecEnv:
         {"real_obs": (K, N, J, 7) f32, "action_mask": (K, N, J+1) bool, "reward": (K, N) f32, "done": (K, N) bool,
         "actions": (K, N) i32, ...} as device tensors; pass the dict back as `out` to reuse the buffers."""
         import torch
-        r = N.RULES[rule.upper()] if isinstance(rule, str) else int(rule)
+        r = _rule_id(rule)
         K, n, J, ms = int(n_steps), self.num_envs, self.jobs, int(self._b.mask_stride)
         if out is None or out["_obs"].shape[0] != K:
             dev = self.device
@@ -268,11 +280,8 @@ class JssVecEnv:
             out["reward"] = out["_scalars"][:, :, 0].view(torch.float32)
             out["reward_raw"] = out["_scalars"][:, :, 1]
             out["time"] = out["_scalars"][:, :, 2]
-            out["done"] = (out["_scalars"][:, :, 3] & 1).bool() if N.backend.name != "cuda" else None
-        rc = self._L.jss_rollout_traj(self._h, r, self.seed, self._step_index, K,
-                                      ctypes.c_void_p(out["_obs"].data_ptr()), ctypes.c_void_p(out["_mask"].data_ptr()),
-                                      ctypes.c_void_p(out["_scalars"].data_ptr()), ctypes.c_void_p(out["actions"].data_ptr()),
-                                      self._stream())
+        rc = self._L.jss_rollout_traj(self._h, r, self.seed, self._step_index, K, _ptr(out["_obs"]), _ptr(out["_mask"]),
+                                      _ptr(out["_scalars"]), _ptr(out["actions"]), self._stream())
         N.check(self._h, rc, "jss_rollout_traj")
         self._step_index += K
         out["done"] = (out["_scalars"][:, :, 3] & 1).bool()       # lazily evaluated view of the done bit
@@ -285,19 +294,15 @@ class JssVecEnv:
         n, J = self.num_envs, self.jobs
         if not hasattr(self, "_host"):
             import torch
-            pin = N.backend.name == "cuda"
-            mk = lambda shape, dt: torch.empty(shape, dtype=dt, pin_memory=pin)   # noqa: E731
-            ms = int(self._b.mask_stride)
-            self._host = {"mask": mk((n, ms), torch.uint8), "obs": mk((n, J, 7), torch.float32),
-                          "scalars": mk((n, 4), torch.int32)}
+            self._host = {"mask": _host_buffer((n, int(self._b.mask_stride)), torch.uint8),
+                          "obs": _host_buffer((n, J, 7), torch.float32), "scalars": _host_buffer((n, 4), torch.int32)}
             sc = self._host["scalars"].numpy()
             self._host_views = {
                 "mask": self._host["mask"].numpy()[:, : J + 1].view(np.bool_), "obs": self._host["obs"].numpy(),
                 "reward": sc.view(np.float32)[:, 0], "done": sc.view(np.uint8)[:, 12].view(np.bool_)}
         hb, hv = self._host, self._host_views
-        rc = self._L.jss_step_host(self._h, ctypes.c_void_p(a.ctypes.data), ctypes.c_void_p(hb["mask"].data_ptr()),
-                                   ctypes.c_void_p(hb["obs"].data_ptr()) if want_obs else None,
-                                   ctypes.c_void_p(hb["scalars"].data_ptr()), self._stream())
+        rc = self._L.jss_step_host(self._h, ctypes.c_void_p(a.ctypes.data), _ptr(hb["mask"]),
+                                   _ptr(hb["obs"]) if want_obs else None, _ptr(hb["scalars"]), self._stream())
         N.check(self._h, rc, "jss_step_host")
         obs = {"real_obs": hv["obs"], "action_mask": hv["mask"]}
         return obs, hv["reward"], hv["done"], np.zeros(n, np.bool_), {}
@@ -314,15 +319,13 @@ class JssVecEnv:
         n, J = self.num_envs, self.jobs
         if not hasattr(self, "_pipe"):
             import torch
-            pin = N.backend.name == "cuda"
-            mk = lambda shape, dt: torch.empty(shape, dtype=dt, pin_memory=pin)   # noqa: E731
             ms = int(self._b.mask_stride)
             ws = int(self._L.jss_host_wire_stride(self._h))
-            self._pipe = [{"mask": mk((n, ms), torch.uint8), "obs": None, "wire": None, "wire_stride": ws, "n_dma": 0,
-                           "scalars": mk((n, 4), torch.int32), "actions": mk((n,), torch.int32), "packed": False,
-                           "expanded": True} for _ in range(2)]
+            self._pipe = [{"mask": _host_buffer((n, ms), torch.uint8), "obs": None, "wire": None, "wire_stride": ws,
+                           "n_dma": 0, "scalars": _host_buffer((n, 4), torch.int32),
+                           "actions": _host_buffer((n,), torch.int32), "packed": False, "expanded": True}
+                          for _ in range(2)]
             self._pipe_slot = 0
-            self._pipe_mk = mk
             self._pipe_inflight = 0
         if self._pipe_inflight >= 2:
             # the slot about to be reused belongs to the begin before the latest one: its transfers must have drained
@@ -332,10 +335,10 @@ class JssVecEnv:
         if b["obs"] is None:
             import torch
             # fp32 observation buffer: DMA target (pinned) in plain mode, expansion target in packed mode
-            b["obs"] = self._pipe_mk((n, J, 7), torch.float32)
+            b["obs"] = _host_buffer((n, J, 7), torch.float32)
         if packed and b["wire"] is None:
             import torch
-            b["wire"] = self._pipe_mk((n, b["wire_stride"]), torch.uint8)
+            b["wire"] = _host_buffer((n, b["wire_stride"]), torch.uint8)
         b["actions"].numpy()[:] = a                      # pinned copy: the H2D must not race with the caller's array
         b["packed"] = bool(packed)
         b["expanded"] = not packed
@@ -344,20 +347,14 @@ class JssVecEnv:
             g = 256 if n >= 4096 else 1
             b["n_dma"] = min(n, int(dma_fraction * n) // g * g)
         if packed and b["n_dma"] > 0:
-            rc = self._L.jss_host_step_begin_hybrid(self._h, ctypes.c_void_p(b["actions"].data_ptr()),
-                                                    ctypes.c_void_p(b["mask"].data_ptr()),
-                                                    ctypes.c_void_p(b["wire"].data_ptr()),
-                                                    ctypes.c_void_p(b["obs"].data_ptr()), b["n_dma"],
-                                                    ctypes.c_void_p(b["scalars"].data_ptr()), self._stream())
+            rc = self._L.jss_host_step_begin_hybrid(self._h, _ptr(b["actions"]), _ptr(b["mask"]), _ptr(b["wire"]),
+                                                    _ptr(b["obs"]), b["n_dma"], _ptr(b["scalars"]), self._stream())
         elif packed:
-            rc = self._L.jss_host_step_begin_packed(self._h, ctypes.c_void_p(b["actions"].data_ptr()),
-                                                    ctypes.c_void_p(b["mask"].data_ptr()),
-                                                    ctypes.c_void_p(b["wire"].data_ptr()),
-                                                    ctypes.c_void_p(b["scalars"].data_ptr()), self._stream())
+            rc = self._L.jss_host_step_begin_packed(self._h, _ptr(b["actions"]), _ptr(b["mask"]), _ptr(b["wire"]),
+                                                    _ptr(b["scalars"]), self._stream())
         else:
-            rc = self._L.jss_host_step_begin(self._h, ctypes.c_void_p(b["actions"].data_ptr()),
-                                             ctypes.c_void_p(b["mask"].data_ptr()), ctypes.c_void_p(b["obs"].data_ptr()),
-                                             ctypes.c_void_p(b["scalars"].data_ptr()), self._stream())
+            rc = self._L.jss_host_step_begin(self._h, _ptr(b["actions"]), _ptr(b["mask"]), _ptr(b["obs"]),
+                                             _ptr(b["scalars"]), self._stream())
         N.check(self._h, rc, "jss_host_step_begin")
         self._pipe_inflight = min(2, self._pipe_inflight + 1)
         return self._pipe_slot
@@ -377,9 +374,8 @@ class JssVecEnv:
         N.check(self._h, self._L.jss_host_wait(self._h, N.WAIT_OBS_PREV if previous else N.WAIT_OBS), "jss_host_wait")
         b = self._pipe[self._pipe_slot ^ (1 if previous else 0)]
         if b["packed"] and not b["expanded"]:
-            rc = self._L.jss_host_expand_obs_range(self._h, ctypes.c_void_p(b["wire"].data_ptr()),
-                                                   ctypes.c_void_p(b["scalars"].data_ptr()),
-                                                   ctypes.c_void_p(b["obs"].data_ptr()), int(b["n_dma"]), self.num_envs)
+            rc = self._L.jss_host_expand_obs_range(self._h, _ptr(b["wire"]), _ptr(b["scalars"]), _ptr(b["obs"]),
+                                                   int(b["n_dma"]), self.num_envs)
             N.check(self._h, rc, "jss_host_expand_obs")
             b["expanded"] = True
         return b["obs"].numpy()
@@ -388,6 +384,12 @@ class JssVecEnv:
     def host_configure(threads: int = 0, bind_numa_of_device: int = -1) -> int:
         """Size / bind the host worker pool (jss_host_configure); call before the first host helper runs."""
         return int(N.backend.library().jss_host_configure(int(threads), int(bind_numa_of_device)))
+
+    @staticmethod
+    def host_set_simd(level: int) -> int:
+        """Cap the SIMD level of the packed-observation expansion: 0 scalar, 1 AVX2, 2 AVX-512 (the default: best
+        available).  The three paths give identical results; this lets tests exercise each one."""
+        return int(N.backend.library().jss_host_set_simd(int(level)))
 
     def host_masked_random(self, mask: np.ndarray, step_index: int) -> np.ndarray:
         """Same draw as policy('RANDOM') but from a host mask (for host-side agents / tests)."""
@@ -413,26 +415,15 @@ class JssVecEnv:
     def export_state(self) -> Dict[str, Any]:
         """Canonical per-env integer state as device tensors (snapshot); see jss_b200.h."""
         N.check(self._h, self._L.jss_export_state(self._h, self._stream()), "jss_export_state")
-        d = dict(self._x)
-        d["t"] = self.current_time_step
-        d["flags"] = self._flags_done
-        return d
+        return {**self._x, "t": self.current_time_step, "flags": self._flags_done}
 
     def import_state(self, state: Dict[str, Any], mask=None):
         """Restore a snapshot taken with export_state() (tensors are copied into the library's buffers)."""
-        for k, dst in self._x.items():
+        for k, dst in {**self._x, "t": self.current_time_step, "flags": self._flags_done}.items():
             if state[k].data_ptr() != dst.data_ptr():
                 dst.copy_(state[k])
-        if state["t"].data_ptr() != self.current_time_step.data_ptr():
-            self.current_time_step.copy_(state["t"])
-        if state["flags"].data_ptr() != self._flags_done.data_ptr():
-            self._flags_done.copy_(state["flags"])
-        ptr = None
-        if mask is not None:
-            import torch
-            mask = torch.as_tensor(mask, device=self.device).to(torch.uint8).contiguous()
-            ptr = ctypes.c_void_p(mask.data_ptr())
-        N.check(self._h, self._L.jss_import_state(self._h, ptr, self._stream()), "jss_import_state")
+        m = self._env_mask(mask)
+        N.check(self._h, self._L.jss_import_state(self._h, _ptr(m), self._stream()), "jss_import_state")
 
     @property
     def launch_count(self) -> int:

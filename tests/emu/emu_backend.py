@@ -5,8 +5,6 @@ import ctypes
 import os
 import subprocess
 
-import numpy as np
-
 from jssenv_b200 import _native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -26,6 +24,7 @@ def build(force=False):
 
 class EmuBackend:
     name = "emu"
+    pin_memory = False
 
     def __init__(self):
         self._lib = None
@@ -45,20 +44,7 @@ class EmuBackend:
 
     def wrap(self, ptr, shape, dtype, device_index, strides=None):
         import torch
-        dt = np.dtype(dtype)
-        shape = tuple(int(s) for s in shape)
-        if strides is None:
-            nbytes = int(np.prod(shape)) * dt.itemsize
-        else:
-            nbytes = sum((s - 1) * st for s, st in zip(shape, strides)) + dt.itemsize
-        buf = (ctypes.c_char * max(nbytes, 1)).from_address(int(ptr))
-        flat = np.frombuffer(buf, dtype=np.uint8)
-        if strides is None:
-            arr = flat.view(dt).reshape(shape)
-        else:
-            arr = np.lib.stride_tricks.as_strided(flat.view(dt) if dt.itemsize == 1 else flat[: nbytes // dt.itemsize * dt.itemsize].view(dt),
-                                                  shape=shape, strides=strides)
-        return torch.from_numpy(arr)
+        return torch.from_numpy(_native.host_view(ptr, shape, dtype, strides))
 
     def synchronize(self, device_index):
         pass

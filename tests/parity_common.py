@@ -484,12 +484,12 @@ def check_host_pipeline_packed(make_env, names, seed, n_steps=80):
         # next step enqueued while the previous rows may still stream; every third step ships a share of the envs as
         # final fp32 rows by DMA (hybrid)
         env.host_step_begin(nxt, packed=True, dma_fraction=(0.0, 0.0, 0.4)[k % 3] if len(names) >= 4 else 0.0)
-        env._L.jss_host_set_simd(k % 3)                # scalar / AVX2 / AVX-512 expansion paths in turn
+        env.host_set_simd(k % 3)                       # scalar / AVX2 / AVX-512 expansion paths in turn
         got = env.host_wait_obs(previous=True)
         for i, J in enumerate(env.env_jobs):
             assert np.array_equal(got[i, :J].view(np.uint32), expected[i, :J].view(np.uint32)), (k, i)
         a = nxt
-    env._L.jss_host_set_simd(2)
+    env.host_set_simd(2)
     env.host_wait_obs()
     return env
 

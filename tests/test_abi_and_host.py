@@ -26,6 +26,33 @@ def test_header_symbols_exported_by_cuda_library():
     assert lib.jss_abi_version() == _native.JSS_ABI_VERSION
 
 
+def test_signature_table_matches_header_prototypes():
+    """Every prototype of include/jss_b200.h against _native.SIGNATURES: return type, parameter count, and a ctypes
+    type of the C type's width at every scalar position (a 32-bit entry would silently truncate a 64-bit seed)."""
+    from ctypes import c_char_p, c_double, c_int, c_int64, c_uint32, c_uint64, sizeof
+
+    from jssenv_b200 import _native
+    hdr = open(os.path.join(ROOT, "include", "jss_b200.h")).read()
+    code = re.sub(r"/\*.*?\*/", " ", hdr, flags=re.S)
+    protos = re.findall(r"([\w \t*]+?)\s*\b(jss_[a-z_]+)\s*\(([^)]*)\)\s*;", code)
+    assert {name for _, name, _ in protos} == set(_native.SIGNATURES)
+    scalar = {"int": c_int, "uint32_t": c_uint32, "int64_t": c_int64, "uint64_t": c_uint64, "double": c_double}
+    result = {"int": c_int, "int64_t": c_int64, "const char *": c_char_p, "void": None}
+    for ret, name, params in protos:
+        restype, argtypes = _native.SIGNATURES[name]
+        assert restype is result[" ".join(ret.replace("*", " * ").split())], name
+        params = [p.strip() for p in params.split(",")] if params.strip() not in ("", "void") else []
+        assert len(params) == len(argtypes), name
+        for k, (p, t) in enumerate(zip(params, argtypes)):
+            if "*" in p or "[" in p:                     # pointers, and arrays such as int64_t out[3]
+                assert sizeof(t) == sizeof(ctypes.c_void_p), (name, k, p)
+                continue
+            ctype = p.rsplit(None, 1)[0]                 # drop the parameter name
+            assert t is scalar[ctype], (name, k, p)
+            if ctype in ("int64_t", "uint64_t", "double"):
+                assert sizeof(t) == 8, (name, k, p)
+
+
 def test_no_cpu_fallback_without_gpu():
     """On a box without a CUDA device, constructing an env must fail loudly."""
     import torch
