@@ -3,7 +3,7 @@ tests/stubs on sys.path, so that the code paths that only exist when `gymnasium`
 the `jss-v1` registration (reference: JSSEnv/__init__.py:6-9), `gym.make('jss-v1', env_config=...)`
 (README.md:46-65), the gym.Env / gym.spaces publication of the facade (jss_env.py:97, 112-119), the
 `gymnasium.vector.VectorEnv` subclass path of JssGymVectorEnv and `create_env` (JSSEnv/utils.py:32-60).
-usage: python tests/gym_boundary_script.py emu|cuda"""
+usage: python tests/gym_boundary_script.py emu|gpu"""
 import os
 import sys
 
@@ -104,7 +104,7 @@ def main(backend):
 
 
 if __name__ == "__main__":
-    backend = sys.argv[1] if len(sys.argv) > 1 else "cuda"
+    backend = sys.argv[1] if len(sys.argv) > 1 else "gpu"
     if backend == "emu":
         from tests.emu.emu_backend import use_emulation
         with use_emulation():

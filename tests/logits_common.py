@@ -1,27 +1,13 @@
 """Backend-agnostic checks of jss_step_logits (the masked categorical draw from policy logits fused into the step):
-the native env (real CUDA library in tests/test_gpu_step_logits.py, host emulation of the same kernels in
-tests/test_emu_step_logits.py) against the float64 restatement of the draw in oracle/logits_oracle.py, and against a
-twin env stepped with jss_step(actions)."""
+the native env (tests/backends.py) against the float64 restatement of the draw in oracle/logits_oracle.py, and against
+a twin env stepped with jss_step(actions)."""
 import numpy as np
 
 from jssenv_b200 import _native as N
 from oracle import logits_oracle as LO
+from tests.parity_common import assert_twins_equal, np_, twin_envs
 
 BIG_ACTION = 1 << 20          # out of range: jss_step sets the error bit and leaves the env unchanged
-
-
-def _np(t):
-    return t.cpu().numpy() if hasattr(t, "cpu") else np.asarray(t)
-
-
-def _batch_cfg(names):
-    """names: instance names, or already-parsed (machine, duration) pairs, one entry per env."""
-    uniq = []
-    for n in names:
-        if not any(n is u or (isinstance(n, str) and n == u) for u in uniq):
-            uniq.append(n)
-    idx = [next(k for k, u in enumerate(uniq) if n is u or (isinstance(n, str) and n == u)) for n in names]
-    return {"instance_paths": uniq, "env_to_instance": idx}
 
 
 def _to_dev(env, arr):
@@ -40,21 +26,6 @@ def random_logits(rng, env, mask, ld, p_ninf=0.1, illegal=1e30):
         row[: Ji + 1][~mask[i, : Ji + 1]] = illegal
         row[Ji + 1:] = np.nan
     return x
-
-
-def assert_twins_equal(a_env, b_env, ctx, state=True):
-    """Outputs (bit for bit), exported state and statistics of two envs."""
-    for name in ("action_mask", "real_obs", "reward", "reward_raw", "done", "current_time_step", "flags",
-                 "episode_count", "last_makespan", "last_return"):
-        x, y = _np(getattr(a_env, name)), _np(getattr(b_env, name))
-        if x.dtype == np.float32:
-            x, y = x.view(np.uint32), y.view(np.uint32)
-        assert np.array_equal(x, y), (ctx, name)
-    if state:
-        xa, xb = a_env.export_state(), b_env.export_state()
-        for k in xa:
-            assert np.array_equal(_np(xa[k]), _np(xb[k])), (ctx, k)
-        assert a_env.stats() == b_env.stats(), ctx
 
 
 def check_draws(env, logits, mask, done, acts, logp, step_index, flags_after, ctx):
@@ -87,31 +58,23 @@ def check_step_logits(make_env, names, n_steps, seed, pad=3, state_every=25, aut
     """jss_step_logits on a batch, driven by seeded random logits (with -inf entries, huge values on illegal entries,
     ld > J+1): every draw against the oracle, and a twin env stepped with jss_step(actions) bit-identical after every
     step (the env of a bad-logits draw gets an out-of-range action there, which sets the same error bit)."""
-    cfg = _batch_cfg(names)
-    a_env = make_env(len(names), cfg, seed=seed, auto_reset=auto_reset)
-    b_env = make_env(len(names), cfg, seed=seed, auto_reset=auto_reset)
-    a_env.reset(); b_env.reset()
+    a_env, b_env = twin_envs(make_env, names, sort=False, seed=seed, auto_reset=auto_reset)
     rng = np.random.default_rng(seed)
     ld = a_env.jobs + 1 + pad
     decisions = agree = 0
     for k in range(n_steps):
-        mask, done = _np(a_env.action_mask).copy(), _np(a_env.done).copy()
+        mask, done = np_(a_env.action_mask).copy(), np_(a_env.done).copy()
         logits = random_logits(rng, a_env, mask, ld, illegal=np.nan if k % 2 else 1e30)
         _, _, _, _, info = a_env.step_logits(_to_dev(a_env, logits))
-        acts, logp = _np(info["actions"]).copy(), _np(info["log_prob"]).copy()
-        twin, d, g = check_draws(a_env, logits, mask, done, acts, logp, k, _np(a_env.flags), f"step {k}")
+        acts, logp = np_(info["actions"]).copy(), np_(info["log_prob"]).copy()
+        twin, d, g = check_draws(a_env, logits, mask, done, acts, logp, k, np_(a_env.flags), f"step {k}")
         decisions += d; agree += g
         b_env.step(twin)
-        assert_twins_equal(a_env, b_env, f"step {k}", state=(k % state_every == state_every - 1))
-    assert_twins_equal(a_env, b_env, "end")
+        full = k % state_every == state_every - 1
+        assert_twins_equal(a_env, b_env, f"step {k}", state=full, stats=full)
+    assert_twins_equal(a_env, b_env, "end", state=True, stats=True)
     assert decisions > 0 and agree >= 0.999 * decisions, (agree, decisions)
     return a_env
-
-
-def _step_both(a_env, b_env, logits, twin_actions):
-    _, _, _, _, info = a_env.step_logits(_to_dev(a_env, logits))
-    b_env.step(twin_actions)
-    return _np(info["actions"]).copy(), _np(info["log_prob"]).copy()
 
 
 def check_step_logits_edge_cases(make_env):
@@ -133,10 +96,10 @@ def check_step_logits_edge_cases(make_env):
             x["flags"][6] = int(x["flags"][6]) | (N.FLAG_NOOP_LEGAL << 8)
             x["flags"][7] = int(x["flags"][7]) | (N.FLAG_DONE << 8) | 1
             env.import_state(x)
-        mask = _np(a_env.action_mask).copy()
+        mask = np_(a_env.action_mask).copy()
         assert not mask[6, :J].any() and mask[6, J] and not mask[7].any() and not mask[0, 0]
-        before = {k: _np(v).copy() for k, v in a_env.export_state().items()}
-        obs0, mask0 = _np(a_env.real_obs).copy(), mask.copy()
+        before = {k: np_(v).copy() for k, v in a_env.export_state().items()}
+        obs0, mask0 = np_(a_env.real_obs).copy(), mask.copy()
         rng = np.random.default_rng(1)
         ld = J + 1 + 5
         logits = rng.standard_normal((n, ld)).astype(np.float32)
@@ -149,29 +112,29 @@ def check_step_logits_edge_cases(make_env):
         logits[6, J] = np.nan                             # the only legal action's logit is not read
         twin = np.array([3, BIG_ACTION, BIG_ACTION, BIG_ACTION, 0, 0, J, 0], np.int32)
         _, _, _, _, info = a_env.step_logits(_to_dev(a_env, logits))
-        acts, logp = _np(info["actions"]).copy(), _np(info["log_prob"]).copy()
+        acts, logp = np_(info["actions"]).copy(), np_(info["log_prob"]).copy()
         twin[4], twin[5] = acts[4], acts[5]
         b_env.step(twin)
         ctx = f"auto_reset={auto_reset}"
         assert acts[0] == 3 and logp[0] == 0.0, (ctx, acts[0], logp[0])
-        flags = _np(a_env.flags)
+        flags = np_(a_env.flags)
         for i in (1, 2, 3):
             assert acts[i] == N.ACTION_SKIP and np.isnan(logp[i]) and flags[i] & N.FLAG_ERROR, (ctx, i)
         for i in (4, 5):
             assert 1 <= acts[i] < J and mask[i, acts[i]], (ctx, i, acts[i])
         assert acts[6] == J and logp[6] == 0.0 and acts[7] == 0 and logp[7] == 0.0, (ctx, acts, logp)
-        twin_check, _, _ = check_draws(a_env, logits, mask, _np(before["flags"]) & 1, acts, logp, 0, flags, ctx)
+        twin_check, _, _ = check_draws(a_env, logits, mask, np_(before["flags"]) & 1, acts, logp, 0, flags, ctx)
         assert np.array_equal(twin_check[[0, 4, 5, 6, 7]], twin[[0, 4, 5, 6, 7]])
-        after = {k: _np(v).copy() for k, v in a_env.export_state().items()}
+        after = {k: np_(v).copy() for k, v in a_env.export_state().items()}
         for k in before:                                  # the erroring envs are unchanged
             if k != "flags":
                 assert np.array_equal(before[k][1:4], after[k][1:4]), (ctx, k)
-        assert np.array_equal(_np(a_env.real_obs)[1:4], obs0[1:4]) and np.array_equal(_np(a_env.action_mask)[1:4], mask0[1:4])
+        assert np.array_equal(np_(a_env.real_obs)[1:4], obs0[1:4]) and np.array_equal(np_(a_env.action_mask)[1:4], mask0[1:4])
         if auto_reset:                                    # the done env was reset by the call
-            assert int(a_env.current_time_step[7]) == 0 and _np(a_env.action_mask)[7, :J].all()
+            assert int(a_env.current_time_step[7]) == 0 and np_(a_env.action_mask)[7, :J].all()
         else:                                             # ... or stays frozen
-            assert np.array_equal(after["todo"][7], before["todo"][7]) and _np(a_env.done)[7]
-        assert_twins_equal(a_env, b_env, ctx)
+            assert np.array_equal(after["todo"][7], before["todo"][7]) and np_(a_env.done)[7]
+        assert_twins_equal(a_env, b_env, ctx, state=True, stats=True)
 
 
 def check_step_logits_shards(make_env, n_total=12, n_steps=120, seed=31):
@@ -189,18 +152,17 @@ def check_step_logits_shards(make_env, n_total=12, n_steps=120, seed=31):
     rng = np.random.default_rng(seed)
     ld = whole.jobs + 1
     for k in range(n_steps):
-        logits = random_logits(rng, whole, _np(whole.action_mask), ld)
+        logits = random_logits(rng, whole, np_(whole.action_mask), ld)
         dev = _to_dev(whole, logits)
         _, _, _, _, iw = whole.step_logits(dev)
-        aw, lw = _np(iw["actions"]).copy(), _np(iw["log_prob"]).copy()
+        aw, lw = np_(iw["actions"]).copy(), np_(iw["log_prob"]).copy()
         for s, lo, hi in zip(shards, cuts[:-1], cuts[1:]):
             _, _, _, _, i_s = s.step_logits(dev[lo:hi, : s.jobs + 1])   # row stride of the whole batch passed through as ld
-            assert np.array_equal(_np(i_s["actions"]), aw[lo:hi]), (k, lo)
-            assert np.array_equal(_np(i_s["log_prob"]).view(np.uint32), lw[lo:hi].view(np.uint32)), (k, lo)
-            for name in ("real_obs", "reward", "done", "current_time_step", "flags", "episode_count"):
-                assert np.array_equal(_np(getattr(s, name)), _np(getattr(whole, name))[lo:hi]), (k, name)
-            m_s = _np(s.action_mask)
-            assert np.array_equal(m_s, _np(whole.action_mask)[lo:hi, : s.jobs + 1]), k
+            assert np.array_equal(np_(i_s["actions"]), aw[lo:hi]), (k, lo)
+            assert np.array_equal(np_(i_s["log_prob"]).view(np.uint32), lw[lo:hi].view(np.uint32)), (k, lo)
+            assert_twins_equal(s, whole, k, rows=slice(lo, hi))
+            m_s = np_(s.action_mask)
+            assert np.array_equal(m_s, np_(whole.action_mask)[lo:hi, : s.jobs + 1]), k
 
 
 def check_step_logits_abi_errors(make_env):
@@ -222,7 +184,7 @@ def check_step_logits_abi_errors(make_env):
     assert b"jss_step_logits" in L.jss_last_error(h)
     assert L.jss_step_logits(h, p_l, J + 1, 0, 0, p_a, None, st) == 0   # log_prob_out may be NULL
     env.synchronize()
-    assert (_np(acts) >= 0).all()
+    assert (np_(acts) >= 0).all()
     with pytest.raises(ValueError):
         env.step_logits(logits[:, :J])
     with pytest.raises(ValueError):

@@ -1,6 +1,6 @@
-"""Backend-agnostic parity checks: the native env (real CUDA library in the `-m gpu`
-tests, host emulation of the same kernels in tests/test_emu_parity.py) against the CPU
-oracle and the golden fixtures recorded from the unmodified Python reference.
+"""Backend-agnostic parity checks: the native env (real CUDA library with `-m gpu`, host emulation of the same kernels
+in the CPU suite; tests/backends.py) against the CPU oracle and the golden fixtures recorded from the unmodified Python
+reference.
 
 Bars (BASELINE.md section 4): bit-exact action_mask / done / current_time_step / raw
 integer reward / integer state; |real_obs - ref| <= 1e-6 and scaled reward within
@@ -8,18 +8,73 @@ max(1e-6, 1.2e-7 * |r|) (fp32 device vs fp64 reference).
 """
 import numpy as np
 
-from jssenv_b200 import JssEnv, JssVecEnv
+from jssenv_b200 import JssEnv
 from jssenv_b200 import _native as N
 from jssenv_b200.dispatching import DISPATCHING_RULES, get_rule
 from jssenv_b200.instances import load_instance
 from oracle.jss_oracle import OracleEnv, OracleError
+from oracle.logits_oracle import hash3
 from tests.helpers import load_json, load_trace, replay_optimal
 
 OBS_TOL = 1e-6
+OUTPUTS = ("action_mask", "real_obs", "reward", "reward_raw", "done", "current_time_step", "flags", "episode_count",
+           "last_makespan", "last_return")
 
 
-def _np(t):
+def np_(t):
     return t.cpu().numpy() if hasattr(t, "cpu") else np.asarray(t)
+
+
+def batch_cfg(names, sort=True):
+    """Config of a batch whose env i runs names[i]: an instance name, or a parsed (machine, duration) pair, which is
+    told apart from the others by identity.  The instances are numbered in name order, or with sort=False in order of
+    first appearance; the numbering decides the tile layout the kernels run."""
+    def same(a, b):
+        return a is b or (isinstance(a, str) and a == b)
+    uniq = []
+    for n in names:
+        if not any(same(n, u) for u in uniq):
+            uniq.append(n)
+    if sort:
+        uniq.sort()
+    return {"instance_paths": uniq, "env_to_instance": [next(k for k, u in enumerate(uniq) if same(n, u)) for n in names]}
+
+
+def twin_envs(make_env, names, sort=True, **kw):
+    """Two envs of the same batch (batch_cfg(names, sort)) and arguments, both reset."""
+    cfg = batch_cfg(names, sort)
+    a_env, b_env = make_env(len(names), cfg, **kw), make_env(len(names), cfg, **kw)
+    a_env.reset(); b_env.reset()
+    return a_env, b_env
+
+
+def assert_twins_equal(a_env, b_env, ctx, rows=slice(None), state=False, stats=False):
+    """Every per-env output of a_env equals that of b_env's envs `rows`, bit for bit; with state / stats, the exported
+    state and the statistics too."""
+    for name in OUTPUTS:
+        x, y = np_(getattr(a_env, name)), np_(getattr(b_env, name))[rows]
+        if x.dtype == np.float32:
+            x, y = x.view(np.uint32), y.view(np.uint32)
+        assert np.array_equal(x, y), (ctx, name)
+    if state:
+        xa, xb = a_env.export_state(), b_env.export_state()
+        for k in xa:
+            assert np.array_equal(np_(xa[k]), np_(xb[k])[rows]), (ctx, k)
+    if stats:
+        assert a_env.stats() == b_env.stats(), ctx
+
+
+def oracle_episode(inst, choose):
+    """One oracle episode of `inst` (a name or a parsed pair) from reset to done, `choose(o, step)` picking each action.
+    Returns the makespan, the raw return and the number of steps."""
+    o = OracleEnv(*(load_instance(inst) if isinstance(inst, str) else inst))
+    o.reset()
+    done, step, total = False, 0, 0
+    while not done:
+        _, _, done, _, _ = o.step(choose(o, step))
+        total += o.last_raw_reward
+        step += 1
+    return o.current_time_step, total, step
 
 
 def rew_close(a, b):
@@ -28,10 +83,10 @@ def rew_close(a, b):
 
 def compare_env_to_oracle(env, i, o, obs, reward=None, done=None, raw=None, ctx=""):
     J = o.jobs
-    mask = _np(obs["action_mask"][i])
+    mask = np_(obs["action_mask"][i])
     assert np.array_equal(mask[: J + 1], o.legal_actions), f"{ctx}: mask env {i}"
     assert not mask[J + 1:].any(), f"{ctx}: padding mask bytes must stay 0"
-    ro = _np(obs["real_obs"][i])
+    ro = np_(obs["real_obs"][i])
     assert np.abs(ro[:J] - o.state).max() <= OBS_TOL, f"{ctx}: real_obs env {i}"
     assert ro.min() >= 0.0 and ro.max() <= 1.0
     assert int(env.current_time_step[i]) == o.current_time_step, f"{ctx}: time env {i}"
@@ -45,7 +100,7 @@ def compare_env_to_oracle(env, i, o, obs, reward=None, done=None, raw=None, ctx=
 
 def compare_exported_state(env, oracles, alive=None, ctx=""):
     """Every integer array of the reference, including the derived ones."""
-    x = {k: _np(v) for k, v in env.export_state().items()}
+    x = {k: np_(v) for k, v in env.export_state().items()}
     env.synchronize()
     for i, o in enumerate(oracles):
         if alive is not None and not alive[i]:
@@ -67,8 +122,7 @@ def compare_exported_state(env, oracles, alive=None, ctx=""):
 def check_random_batch(make_env, names, n_steps, seed, state_every=25, noop_force_every=0):
     """Mixed batch; the ORACLE side picks masked-random actions (optionally a forced no-op
     whenever an event is pending, like tests/test_solutions.py:762), both sides step."""
-    uniq = sorted(set(names))
-    env = make_env(len(names), {"instance_paths": uniq, "env_to_instance": [uniq.index(n) for n in names]})
+    env = make_env(len(names), batch_cfg(names))
     oracles = [OracleEnv(*load_instance(n)) for n in names]
     rng = np.random.default_rng(seed)
     obs = env.reset()
@@ -88,8 +142,8 @@ def check_random_batch(make_env, names, n_steps, seed, state_every=25, noop_forc
             else:
                 acts[i] = int(legal[rng.integers(len(legal))])
         obs, reward, done, trunc, info = env.step(acts)
-        reward, done, raw = _np(reward), _np(done), _np(env.reward_raw)
-        assert not _np(trunc).any() and info == {}
+        reward, done, raw = np_(reward), np_(done), np_(env.reward_raw)
+        assert not np_(trunc).any() and info == {}
         for i, o in enumerate(oracles):
             if not alive[i]:
                 continue
@@ -121,8 +175,8 @@ def check_golden_trace(make_env, path):
     J = tr["mask"].shape[1] - 1
 
     def check(k):
-        assert np.array_equal(_np(obs["action_mask"][0])[: J + 1], tr["mask"][k]), f"mask {k}"
-        assert np.abs(_np(obs["real_obs"][0])[:J] - tr["obs"][k]).max() <= OBS_TOL, f"obs {k}"
+        assert np.array_equal(np_(obs["action_mask"][0])[: J + 1], tr["mask"][k]), f"mask {k}"
+        assert np.abs(np_(obs["real_obs"][0])[:J] - tr["obs"][k]).max() <= OBS_TOL, f"obs {k}"
         assert int(env.current_time_step[0]) == tr["t"][k]
 
     check(0)
@@ -132,7 +186,7 @@ def check_golden_trace(make_env, path):
         assert bool(done[0]) == bool(tr["done"][k])
         check(k + 1)
         if k % 50 == 0:
-            x = {n: _np(v) for n, v in env.export_state().items()}
+            x = {n: np_(v) for n, v in env.export_state().items()}
             assert np.array_equal(x["todo"][0, :J], tr["todo"][k + 1])
             assert np.array_equal(x["blocked"][0, :J].astype(bool), tr["blocked"][k + 1])
             assert np.array_equal(x["tuam"][0, : tr["tuam"].shape[1]], tr["tuam"][k + 1])
@@ -212,8 +266,7 @@ def check_policy_kernels(make_env, names, n_steps, seed):
     """jss_policy for every rule vs the oracle's rule functions on identical states, with the
     coin uniform taken from the shared counter RNG; RANDOM vs the oracle's sampler and the
     host helper jss_host_masked_random."""
-    uniq = sorted(set(names))
-    env = make_env(len(names), {"instance_paths": uniq, "env_to_instance": [uniq.index(n) for n in names]}, seed=seed)
+    env = make_env(len(names), batch_cfg(names), seed=seed)
     oracles = [OracleEnv(*load_instance(n)) for n in names]
     obs = env.reset()
     for o in oracles:
@@ -223,8 +276,8 @@ def check_policy_kernels(make_env, names, n_steps, seed):
     for step in range(n_steps):
         # every rule on the CURRENT state (explicit step_index so all rules see the same coin)
         for rule in rules:
-            a_dev = _np(env.policy(rule, coin="device", step_index=step)).copy()
-            a_never = _np(env.policy(rule, coin="never", step_index=step)).copy()
+            a_dev = np_(env.policy(rule, coin="device", step_index=step)).copy()
+            a_never = np_(env.policy(rule, coin="never", step_index=step)).copy()
             for i, o in enumerate(oracles):
                 if not alive[i]:
                     continue
@@ -233,8 +286,8 @@ def check_policy_kernels(make_env, names, n_steps, seed):
                 assert a_dev[i] == exp, (step, rule, i, a_dev[i], exp)
                 exp_never, _ = o.rule_action(rule, 1.0)
                 assert a_never[i] == exp_never, (step, rule, i)
-        a = _np(env.policy("RANDOM", step_index=step)).copy()
-        host = env.host_masked_random(np.ascontiguousarray(_np(env.action_mask)), step)
+        a = np_(env.policy("RANDOM", step_index=step)).copy()
+        host = env.host_masked_random(np.ascontiguousarray(np_(env.action_mask)), step)
         for i, o in enumerate(oracles):
             if alive[i]:
                 assert a[i] == o.masked_random_action(env.seed, env.env_id_base + i, step), (step, i)
@@ -251,46 +304,19 @@ def check_policy_kernels(make_env, names, n_steps, seed):
             break
 
 
-def _hash3(seed, env, ctr):
-    """jssenv_b200/csrc/jss_rng.h restated for the tests."""
-    M32 = 0xFFFFFFFF
-
-    def fold(v):
-        return ((v & M32) ^ (((v >> 32) & M32) * 0x7FEB352D)) & M32
-
-    h = fold(seed) ^ ((fold(env) * 0x9E3779B1 + 0x85EBCA77) & M32) ^ ((fold(ctr) * 0xC2B2AE3D + 0x27D4EB2F) & M32)
-    h ^= h >> 16; h = (h * 0x85EBCA6B) & M32
-    h ^= h >> 13; h = (h * 0xC2B2AE35) & M32
-    h ^= h >> 16
-    return h
-
-
 def _coin_uniform(seed, env, ctr):
     """u = hash3(seed, env, ctr) / 2^32"""
-    return _hash3(seed, env, ctr) / 4294967296.0
+    return hash3(seed, env, ctr) / 4294967296.0
 
 
 def check_rollout_matches_steps(make_env, names, rule, n_steps, seed):
     """The fused rollout kernel == policy kernel + step kernel, transition for transition;
     and both == the oracle driven by the same counter RNG."""
-    if isinstance(names[0], str):
-        uniq = sorted(set(names))
-        cfg = {"instance_paths": uniq, "env_to_instance": [uniq.index(n) for n in names]}
-    else:                                          # already-parsed (machine, duration) pairs, one per env
-        cfg = {"instance_paths": list(names), "env_to_instance": list(range(len(names)))}
-    a_env = make_env(len(names), cfg, seed=seed, auto_reset=True)
-    b_env = make_env(len(names), cfg, seed=seed, auto_reset=True)
-    a_env.reset(); b_env.reset()
+    a_env, b_env = twin_envs(make_env, names, seed=seed, auto_reset=True)
     a_env.rollout(rule, n_steps, write_obs=True)
     for _ in range(n_steps):
         b_env.step(b_env.policy(rule))
-    for name in ("action_mask", "real_obs", "reward", "reward_raw", "done", "current_time_step", "flags",
-                 "episode_count", "last_makespan", "last_return"):
-        assert np.array_equal(_np(getattr(a_env, name)), _np(getattr(b_env, name))), name
-    xa, xb = a_env.export_state(), b_env.export_state()
-    for k in xa:
-        assert np.array_equal(_np(xa[k]), _np(xb[k])), k
-    assert a_env.stats() == b_env.stats()
+    assert_twins_equal(a_env, b_env, rule, state=True, stats=True)
     # oracle with the same RNG (auto-reset: a done env is reset by the next transition)
     for i, n in enumerate(names):
         o = OracleEnv(*load_instance(n))
@@ -313,8 +339,8 @@ def check_rollout_matches_steps(make_env, names, rule, n_steps, seed):
         assert int(a_env.current_time_step[i]) == o.current_time_step
         J = o.jobs
         if not done:
-            assert np.array_equal(_np(a_env.action_mask[i])[: J + 1], o.legal_actions)
-            assert np.abs(_np(a_env.real_obs[i])[:J] - o.state).max() <= OBS_TOL
+            assert np.array_equal(np_(a_env.action_mask[i])[: J + 1], o.legal_actions)
+            assert np.abs(np_(a_env.real_obs[i])[:J] - o.state).max() <= OBS_TOL
     return a_env
 
 
@@ -323,29 +349,29 @@ def check_errors_and_freeze(make_env):
     env = make_env(4, {"instance_path": "ta01"})
     o = OracleEnv(*load_instance("ta01"))
     obs = env.reset(); o.reset()
-    before = {k: _np(v).copy() for k, v in env.export_state().items()}
-    mask0, obs0 = _np(env.action_mask).copy(), _np(env.real_obs).copy()
+    before = {k: np_(v).copy() for k, v in env.export_state().items()}
+    mask0, obs0 = np_(env.action_mask).copy(), np_(env.real_obs).copy()
     # env0: no-op with empty queue (IndexError jss_env.py:517); env1: out of range; env2: skip; env3: legal
     env.step(np.array([env.jobs, 99, N.ACTION_SKIP, 3], np.int32))
-    flags = _np(env.flags)
+    flags = np_(env.flags)
     assert flags[0] & N.FLAG_ERROR and flags[1] & N.FLAG_ERROR and not flags[2] & N.FLAG_ERROR and not flags[3] & N.FLAG_ERROR
-    after = {k: _np(v).copy() for k, v in env.export_state().items()}
+    after = {k: np_(v).copy() for k, v in env.export_state().items()}
     for k in before:
         if k == "flags":
             continue
         assert np.array_equal(before[k][:3], after[k][:3]), k
-    assert np.array_equal(_np(env.action_mask)[:3], mask0[:3]) and np.array_equal(_np(env.real_obs)[:3], obs0[:3])
+    assert np.array_equal(np_(env.action_mask)[:3], mask0[:3]) and np.array_equal(np_(env.real_obs)[:3], obs0[:3])
     o.step(3)
     compare_env_to_oracle(env, 3, o, env._obs(), ctx="legal env next to erroring envs")
     # illegal job action: job 3 is now running -> not legal
     env.step(np.array([N.ACTION_SKIP] * 3 + [3], np.int32))
-    assert _np(env.flags)[3] & N.FLAG_ERROR
+    assert np_(env.flags)[3] & N.FLAG_ERROR
     compare_env_to_oracle(env, 3, o, env._obs(), ctx="illegal action leaves the env unchanged")
     # masked reset clears only env 0 and 3
     env.reset(np.array([1, 0, 0, 1], np.uint8))
-    flags = _np(env.flags)
+    flags = np_(env.flags)
     assert flags[0] == 0 and flags[3] == 0 and flags[1] & N.FLAG_ERROR
-    assert int(env.current_time_step[3]) == 0 and _np(env.action_mask)[3, : env.jobs].all()
+    assert int(env.current_time_step[3]) == 0 and np_(env.action_mask)[3, : env.jobs].all()
     return env
 
 
@@ -354,18 +380,17 @@ def check_auto_reset_and_stats(make_env, name, seed):
     o = OracleEnv(*load_instance(name))
     env.reset()
     n_steps = 2 * (2 * env.jobs * env.machines) + 10
-    ep_o, mk_o, ret_o, steps_o = [], [], [], 0
-    for i in range(1):
-        o.reset(); done = False; ret = 0
-        for step in range(n_steps):
-            if done:
-                o.reset(); done = False; ret = 0
-                continue
-            a = o.masked_random_action(seed, 0, step)
-            _, _, done, _, _ = o.step(a)
-            ret += o.last_raw_reward; steps_o += 1
-            if done:
-                mk_o.append(o.current_time_step); ret_o.append(ret)
+    mk_o, ret_o = [], []
+    o.reset(); done = False; ret = 0
+    for step in range(n_steps):
+        if done:
+            o.reset(); done = False; ret = 0
+            continue
+        a = o.masked_random_action(seed, 0, step)
+        _, _, done, _, _ = o.step(a)
+        ret += o.last_raw_reward
+        if done:
+            mk_o.append(o.current_time_step); ret_o.append(ret)
     for _ in range(n_steps):
         env.step(env.policy("RANDOM"))
     st = env.stats()
@@ -373,9 +398,9 @@ def check_auto_reset_and_stats(make_env, name, seed):
     assert int(env.last_return[0]) == ret_o[-1]
     # identity (SURVEY a9): raw episode return = 2*sum_op - M*makespan
     assert ret_o[-1] == 2 * o.sum_op - o.machines * mk_o[-1]
-    assert st["episodes"] == int(_np(env.episode_count).sum()) and st["episodes"] >= 6
+    assert st["episodes"] == int(np_(env.episode_count).sum()) and st["episodes"] >= 6
     assert st["min_makespan"] <= st["max_makespan"] and st["envs_error"] == 0
-    lm = _np(env.last_makespan)
+    lm = np_(env.last_makespan)
     assert st["min_makespan"] <= lm.min() and st["max_makespan"] >= lm.max()
     return env
 
@@ -386,19 +411,19 @@ def check_snapshot_restore(make_env, name, seed):
     for _ in range(40):
         env.step(env.policy("RANDOM"))
     snap = {k: v.clone() for k, v in env.export_state().items()}
-    mask, obs = _np(env.action_mask).copy(), _np(env.real_obs).copy()
+    mask, obs = np_(env.action_mask).copy(), np_(env.real_obs).copy()
     hist = []
     for k in range(30):
         a = env.policy("RANDOM", step_index=1000 + k).clone()
         env.step(a)
-        hist.append((_np(a).copy(), _np(env.action_mask).copy(), _np(env.reward_raw).copy()))
+        hist.append((np_(a).copy(), np_(env.action_mask).copy(), np_(env.reward_raw).copy()))
     env.import_state(snap)
-    assert np.array_equal(_np(env.action_mask), mask) and np.array_equal(_np(env.real_obs), obs)
+    assert np.array_equal(np_(env.action_mask), mask) and np.array_equal(np_(env.real_obs), obs)
     for k in range(30):
         a = env.policy("RANDOM", step_index=1000 + k)
-        assert np.array_equal(_np(a), hist[k][0])
+        assert np.array_equal(np_(a), hist[k][0])
         env.step(a)
-        assert np.array_equal(_np(env.action_mask), hist[k][1]) and np.array_equal(_np(env.reward_raw), hist[k][2])
+        assert np.array_equal(np_(env.action_mask), hist[k][1]) and np.array_equal(np_(env.reward_raw), hist[k][2])
     return env
 
 
@@ -406,35 +431,29 @@ def check_step_host(make_env, name, seed):
     env = make_env(5, {"instance_path": name}, seed=seed)
     ref = make_env(5, {"instance_path": name}, seed=seed)
     env.reset(); ref.reset()
-    mask = np.ascontiguousarray(_np(env.action_mask))
+    mask = np.ascontiguousarray(np_(env.action_mask))
     for k in range(60):
         a = env.host_masked_random(mask, k)
         obs, rew, done, trunc, _ = env.step_host(a)
         ref.step(a)
-        assert np.array_equal(obs["action_mask"], _np(ref.action_mask))
-        assert np.array_equal(obs["real_obs"], _np(ref.real_obs))
-        assert np.array_equal(rew, _np(ref.reward)) and np.array_equal(done, _np(ref.done))
+        assert np.array_equal(obs["action_mask"], np_(ref.action_mask))
+        assert np.array_equal(obs["real_obs"], np_(ref.real_obs))
+        assert np.array_equal(rew, np_(ref.reward)) and np.array_equal(done, np_(ref.done))
         mask = obs["action_mask"]
     return env
 
 
 def check_step_sample(make_env, names, rule, n_steps, seed):
     """jss_step_sample (step fused with the next decision) == policy kernel + step kernel."""
-    uniq = sorted(set(names))
-    cfg = {"instance_paths": uniq, "env_to_instance": [uniq.index(n) for n in names]}
-    a_env = make_env(len(names), cfg, seed=seed, auto_reset=True)
-    b_env = make_env(len(names), cfg, seed=seed, auto_reset=True)
-    a_env.reset(); b_env.reset()
+    a_env, b_env = twin_envs(make_env, names, seed=seed, auto_reset=True)
     act_a = a_env.policy(rule).clone()             # step_index 0
     b_env._step_index = 0
     for k in range(n_steps):
         act_b = b_env.policy(rule)                 # step_index k
-        assert np.array_equal(_np(act_a), _np(act_b)), f"actions differ at step {k}"
+        assert np.array_equal(np_(act_a), np_(act_b)), f"actions differ at step {k}"
         b_env.step(act_b)
         *_, act_a = a_env.step_sample(act_a, rule)  # applies step k, samples with step_index k+1
-        for name in ("action_mask", "real_obs", "reward", "reward_raw", "done", "current_time_step"):
-            assert np.array_equal(_np(getattr(a_env, name)), _np(getattr(b_env, name))), (k, name)
-    assert a_env.stats() == b_env.stats()
+        assert_twins_equal(a_env, b_env, k, stats=k == n_steps - 1)
     return a_env
 
 
@@ -443,16 +462,16 @@ def check_host_pipeline(make_env, name, seed):
     env = make_env(7, {"instance_path": name}, seed=seed)
     ref = make_env(7, {"instance_path": name}, seed=seed)
     env.reset(); ref.reset()
-    mask = np.ascontiguousarray(_np(env.action_mask))
+    mask = np.ascontiguousarray(np_(env.action_mask))
     a = env.host_masked_random(mask, 0)
     env.host_step_begin(a)
     for k in range(1, 80):
         mask, rew, done = env.host_wait_mask()
         ref.step(a)
-        assert np.array_equal(mask, _np(ref.action_mask)), k
-        assert np.array_equal(rew, _np(ref.reward)) and np.array_equal(done, _np(ref.done))
+        assert np.array_equal(mask, np_(ref.action_mask)), k
+        assert np.array_equal(rew, np_(ref.reward)) and np.array_equal(done, np_(ref.done))
         nxt = env.host_masked_random(mask, k)
-        obs_prev_expected = _np(ref.real_obs).copy()
+        obs_prev_expected = np_(ref.real_obs).copy()
         env.host_step_begin(nxt)                       # next step enqueued while the previous obs may still stream
         assert np.array_equal(env.host_wait_obs(previous=True), obs_prev_expected), k
         a = nxt
@@ -462,25 +481,21 @@ def check_host_pipeline(make_env, name, seed):
 def check_host_pipeline_packed(make_env, names, seed, n_steps=80):
     """Packed host-buffer path: 10-byte integer rows over the wire + host expansion == device real_obs BIT FOR BIT
     (and mask / reward / done as in the plain path), on a mixed batch, through done/auto-reset transitions."""
-    uniq = sorted(set(names))
-    cfg = {"instance_paths": uniq, "env_to_instance": [uniq.index(n) for n in names]}
-    env = make_env(len(names), cfg, seed=seed, auto_reset=True)
-    ref = make_env(len(names), cfg, seed=seed, auto_reset=True)
-    env.reset(); ref.reset()
+    env, ref = twin_envs(make_env, names, seed=seed, auto_reset=True)
     # get past the trivial all-zero start: a few hundred device steps on both
     for k in range(120):
         a0 = ref.policy("RANDOM", step_index=k)
-        ref.step(a0); env.step(_np(a0))
-    mask = np.ascontiguousarray(_np(env.action_mask))
+        ref.step(a0); env.step(np_(a0))
+    mask = np.ascontiguousarray(np_(env.action_mask))
     a = env.host_masked_random(mask, 1000)
     env.host_step_begin(a, packed=True)
     for k in range(1, n_steps):
         mask, rew, done = env.host_wait_mask()
         ref.step(a)
-        assert np.array_equal(mask, _np(ref.action_mask)), k
-        assert np.array_equal(rew, _np(ref.reward)) and np.array_equal(done, _np(ref.done))
+        assert np.array_equal(mask, np_(ref.action_mask)), k
+        assert np.array_equal(rew, np_(ref.reward)) and np.array_equal(done, np_(ref.done))
         nxt = env.host_masked_random(mask, 1000 + k)
-        expected = _np(ref.real_obs).copy()
+        expected = np_(ref.real_obs).copy()
         # next step enqueued while the previous rows may still stream; every third step ships a share of the envs as
         # final fp32 rows by DMA (hybrid)
         env.host_step_begin(nxt, packed=True, dma_fraction=(0.0, 0.0, 0.4)[k % 3] if len(names) >= 4 else 0.0)
@@ -526,7 +541,7 @@ def check_synthetic_shapes(make_env, shapes, n_steps, seed):
                 legal = np.flatnonzero(o.legal_actions)
                 acts[i] = int(legal[rng.integers(len(legal))])
         obs, reward, done, _, _ = env.step(acts)
-        reward, done, raw = _np(reward), _np(done), _np(env.reward_raw)
+        reward, done, raw = np_(reward), np_(done), np_(env.reward_raw)
         for i, o in enumerate(oracles):
             if not alive[i]:
                 continue
@@ -614,11 +629,8 @@ def check_tiny_uniform_batches(make_env, seed=50, shapes=((2, 2), (3, 4), (4, 3)
     for k, (J, M) in enumerate(shapes):
         inst = synthetic_instance(J, M, seed + k, max_dur=30)
         n = 16
-        cfg = {"instance_paths": [inst], "env_to_instance": [0] * n}
         for rule in ("RANDOM", "SPT"):
-            a_env = make_env(n, cfg, seed=seed + k, auto_reset=True)
-            b_env = make_env(n, cfg, seed=seed + k, auto_reset=True)
-            a_env.reset(); b_env.reset()
+            a_env, b_env = twin_envs(make_env, [inst] * n, seed=seed + k, auto_reset=True)
             n_steps = 6 * J * M + 7 if max_steps is None else min(max_steps, 6 * J * M + 7)
             a_env.rollout(rule, n_steps, write_obs=True)
             oracles = [OracleEnv(*inst) for _ in range(n)]
@@ -628,7 +640,7 @@ def check_tiny_uniform_batches(make_env, seed=50, shapes=((2, 2), (3, 4), (4, 3)
             for step in range(n_steps):
                 acts = b_env.policy(rule)
                 b_env.step(acts)
-                a_host = _np(acts)
+                a_host = np_(acts)
                 for i, o in enumerate(oracles):
                     if done[i]:
                         o.reset(); done[i] = False
@@ -638,10 +650,8 @@ def check_tiny_uniform_batches(make_env, seed=50, shapes=((2, 2), (3, 4), (4, 3)
                         assert a_host[i] == exp, (J, M, rule, step, i)
                         _, _, done[i], _, _ = o.step(int(a_host[i]))
                     compare_env_to_oracle(b_env, i, o, b_env._obs(), ctx=f"tiny {J}x{M} {rule} step {step}")
-            for name in ("action_mask", "real_obs", "reward", "reward_raw", "done", "current_time_step", "flags",
-                         "episode_count", "last_makespan", "last_return"):
-                assert np.array_equal(_np(getattr(a_env, name)), _np(getattr(b_env, name))), (J, M, rule, name)
-            assert a_env.stats() == b_env.stats() and a_env.stats()["envs_error"] == 0
+            assert_twins_equal(a_env, b_env, (J, M, rule), stats=True)
+            assert a_env.stats()["envs_error"] == 0
 
 
 def check_shard_invariance(make_env, n_total=24, n_steps=350, seed=77):
@@ -665,13 +675,11 @@ def check_shard_invariance(make_env, n_total=24, n_steps=350, seed=77):
                 aw = whole.policy(rule)
                 for s, lo, hi in zip(shards, cut[:-1], cut[1:]):
                     a_s = s.policy(rule)
-                    assert np.array_equal(_np(a_s), _np(aw)[lo:hi]), (rule, k, lo)
+                    assert np.array_equal(np_(a_s), np_(aw)[lo:hi]), (rule, k, lo)
                     s.step(a_s)
                 whole.step(aw)
                 for s, lo, hi in zip(shards, cut[:-1], cut[1:]):
-                    for name in ("action_mask", "real_obs", "reward", "reward_raw", "done", "current_time_step",
-                                 "episode_count", "last_makespan"):
-                        assert np.array_equal(_np(getattr(s, name)), _np(getattr(whole, name))[lo:hi]), (rule, k, name)
+                    assert_twins_equal(s, whole, (rule, k), rows=slice(lo, hi))
             # the gathered per-shard statistics equal the statistics of the unsharded batch
             from jssenv_b200.distributed import combine_stats, STATS_KEYS
             comb = combine_stats([[s.stats()[key] for key in STATS_KEYS] for s in shards])
@@ -683,23 +691,17 @@ def check_shard_invariance(make_env, n_total=24, n_steps=350, seed=77):
 
 def check_rollout_record(make_env, names, rule, n_steps, seed):
     """jss_rollout_traj: slot k of the recorded trajectory == the outputs after transition k of policy + step."""
-    uniq = sorted(set(names))
-    cfg = {"instance_paths": uniq, "env_to_instance": [uniq.index(n) for n in names]}
-    a_env = make_env(len(names), cfg, seed=seed, auto_reset=True)
-    b_env = make_env(len(names), cfg, seed=seed, auto_reset=True)
-    a_env.reset(); b_env.reset()
+    a_env, b_env = twin_envs(make_env, names, seed=seed, auto_reset=True)
     tr = a_env.rollout_record(rule, n_steps)
     for k in range(n_steps):
         acts = b_env.policy(rule)
-        assert np.array_equal(_np(tr["actions"][k]), _np(acts)), k
+        assert np.array_equal(np_(tr["actions"][k]), np_(acts)), k
         b_env.step(acts)
-        assert np.array_equal(_np(tr["action_mask"][k]), _np(b_env.action_mask)), k
-        assert np.array_equal(_np(tr["real_obs"][k]), _np(b_env.real_obs)), k
-        assert np.array_equal(_np(tr["reward"][k]), _np(b_env.reward)) and np.array_equal(_np(tr["done"][k]), _np(b_env.done)), k
-        assert np.array_equal(_np(tr["time"][k]), _np(b_env.current_time_step)), k
-    for name in ("action_mask", "real_obs", "reward", "done", "current_time_step", "episode_count", "last_makespan"):
-        assert np.array_equal(_np(getattr(a_env, name)), _np(getattr(b_env, name))), name
-    assert a_env.stats() == b_env.stats()
+        assert np.array_equal(np_(tr["action_mask"][k]), np_(b_env.action_mask)), k
+        assert np.array_equal(np_(tr["real_obs"][k]), np_(b_env.real_obs)), k
+        assert np.array_equal(np_(tr["reward"][k]), np_(b_env.reward)) and np.array_equal(np_(tr["done"][k]), np_(b_env.done)), k
+        assert np.array_equal(np_(tr["time"][k]), np_(b_env.current_time_step)), k
+    assert_twins_equal(a_env, b_env, "end", stats=True)
 
 
 def check_big_uniform_batches(make_env, seed=60, max_steps=150):
@@ -707,25 +709,21 @@ def check_big_uniform_batches(make_env, seed=60, max_steps=150):
     rollout == policy + step kernels == oracle; fused step + sampler; packed host path; single-env facade."""
     check_tiny_uniform_batches(make_env, seed=seed, shapes=((130, 4), (256, 6)), max_steps=max_steps)
     inst = synthetic_instance(200, 8, seed + 9, max_dur=50)
-    cfg = {"instance_paths": [inst], "env_to_instance": [0] * 9}
-    a_env = make_env(9, cfg, seed=seed, auto_reset=True)
-    b_env = make_env(9, cfg, seed=seed, auto_reset=True)
-    a_env.reset(); b_env.reset()
+    a_env, b_env = twin_envs(make_env, [inst] * 9, seed=seed, auto_reset=True)
     act_a = a_env.policy("MWR").clone()
     b_env._step_index = 0
     for k in range(max_steps):
         act_b = b_env.policy("MWR")
-        assert np.array_equal(_np(act_a), _np(act_b)), k
+        assert np.array_equal(np_(act_a), np_(act_b)), k
         b_env.step(act_b)
         *_, act_a = a_env.step_sample(act_a, "MWR")
-        for name in ("action_mask", "real_obs", "reward", "done", "current_time_step"):
-            assert np.array_equal(_np(getattr(a_env, name)), _np(getattr(b_env, name))), (k, name)
+        assert_twins_equal(a_env, b_env, k)
     # packed rows + host expansion == device real_obs, bit for bit
-    mask = np.ascontiguousarray(_np(a_env.action_mask))
+    mask = np.ascontiguousarray(np_(a_env.action_mask))
     a_env.host_step_begin(a_env.host_masked_random(mask, 7), packed=True)
     a_env.host_wait_mask()
     got = a_env.host_wait_obs()
-    assert np.array_equal(got.view(np.uint32), _np(a_env.real_obs).view(np.uint32))
+    assert np.array_equal(got.view(np.uint32), np_(a_env.real_obs).view(np.uint32))
     # facade on a 200-job instance
     env = JssEnv({"instance_path": inst})
     o = OracleEnv(*inst)

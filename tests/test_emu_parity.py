@@ -1,167 +1,7 @@
-"""Kernel logic + Python host layer under HOST EMULATION of the CUDA kernels (tests/emu):
-the same jss_device.cuh / jss_api.cu compiled with g++, 32 fibers per warp, strict
-collectives.  Pre-GPU safety net only -- the authoritative parity tests are the
-`-m gpu` ones in tests/test_gpu_parity.py, which run the real sm_90a library.
-Sizes are kept small so the CPU suite stays fast."""
-import os
+"""The parity tests of tests/parity_suite.py under HOST EMULATION of the CUDA kernels (tests/emu): the same
+jss_device.cuh / jss_api.cu compiled with g++, 32 fibers per warp, strict collectives.  Pre-GPU safety net only -- the
+authoritative parity tests are the `-m gpu` ones in tests/test_gpu_parity.py, which run the real sm_90a library."""
+from tests import parity_suite
+from tests.backends import collect
 
-import numpy as np
-import pytest
-
-from tests import parity_common as pc
-from tests.emu.emu_backend import use_emulation
-from tests.helpers import GOLDEN
-
-
-@pytest.fixture(autouse=True)
-def _emu():
-    with use_emulation():
-        yield
-
-
-def make_env(n, cfg, **kw):
-    from jssenv_b200 import JssVecEnv
-    return JssVecEnv(n, cfg, **kw)
-
-
-def test_emu_random_mixed_batch_all_lane_classes():
-    # KJ=1 (15, 20, 30 jobs), KJ=2 (50 jobs), KJ=4 (100 jobs), Demirkol (durations to 200)
-    names = ["ta01", "ta01", "ta11", "ta21", "ta31", "ta41", "dmu16", "ta51", "ta61", "ta71", "ta80"]
-    pc.check_random_batch(make_env, names, n_steps=400, seed=11)
-
-
-def test_emu_full_episode_ta80():
-    pc.check_random_batch(make_env, ["ta80"], n_steps=3000, seed=5, state_every=100)
-
-
-def test_emu_forced_noops():
-    pc.check_random_batch(make_env, ["ta01", "ta45", "ta62", "ta80"], n_steps=500, seed=3, noop_force_every=5)
-
-
-@pytest.mark.parametrize("name", ["trace_ta01_random0", "trace_ta01_forcednoop3", "trace_ta41_lowest0",
-                                  "trace_dmu16_random7", "trace_ta80_highest0"])
-def test_emu_golden_reference_trace(name):
-    pc.check_golden_trace(make_env, os.path.join(GOLDEN, name + ".npz"))
-
-
-@pytest.mark.parametrize("inst", ["ta01", "ta41", "ta51"])
-def test_emu_facade_optimal_makespan(inst):
-    pc.check_facade_optimal(inst)
-
-
-def test_emu_facade_attributes():
-    pc.check_facade_attributes("ta01", 400, seed=2)
-
-
-def test_emu_rules_seeded_ta01():
-    pc.check_rules_seeded("ta01")
-
-
-def test_emu_policy_kernels():
-    pc.check_policy_kernels(make_env, ["ta01", "ta31", "ta51", "ta80"], n_steps=150, seed=9)
-
-
-@pytest.mark.parametrize("rule", ["RANDOM", "FIFO", "MWR", "CR"])
-def test_emu_rollout_matches_steps(rule):
-    pc.check_rollout_matches_steps(make_env, ["ta01", "ta01", "ta51", "ta80"], rule, n_steps=330, seed=4)
-
-
-def test_emu_errors_freeze_reset():
-    pc.check_errors_and_freeze(make_env)
-
-
-def test_emu_auto_reset_and_stats():
-    pc.check_auto_reset_and_stats(make_env, "ta01", seed=6)
-
-
-def test_emu_snapshot_restore():
-    pc.check_snapshot_restore(make_env, "ta31", seed=8)
-
-
-def test_emu_step_host():
-    pc.check_step_host(make_env, "ta01", seed=1)
-
-
-@pytest.mark.parametrize("rule", ["RANDOM", "MWR", "LOR"])
-def test_emu_step_sample_fused(rule):
-    pc.check_step_sample(make_env, ["ta01", "ta51", "ta80"], rule, n_steps=300, seed=12)
-
-
-def test_emu_host_pipeline():
-    pc.check_host_pipeline(make_env, "ta01", seed=3)
-
-
-def test_emu_gym_vector_adapter_autoreset():
-    """next-step autoreset through the VectorEnv-style adapter: the step after `done` returns the reset obs."""
-    from jssenv_b200 import JssGymVectorEnv
-    env = JssGymVectorEnv(3, {"instance_path": "ta01"}, to_numpy=True, seed=5)
-    obs, info = env.reset()
-    assert obs["real_obs"].shape == (3, 15, 7) and obs["action_mask"][:, :15].all() and info == {}
-    seen_done = np.zeros(3, bool)
-    for k in range(600):
-        acts = np.array([np.flatnonzero(m)[0] if m.any() else 0 for m in obs["action_mask"]], np.int32)
-        prev_done = seen_done.copy()
-        obs, rew, done, trunc, info = env.step(acts)
-        for i in np.flatnonzero(prev_done & ~done):     # the transition right after a terminal one = reset
-            assert obs["action_mask"][i, :15].all() and rew[i] == 0.0 and obs["real_obs"][i, :, 1:].max() == 0.0
-        seen_done = done.copy()
-        if env.vec.episode_count.min() >= 2:
-            break
-    assert int(env.vec.episode_count.min()) >= 2
-    env.close()
-
-
-EDGE_SHAPES = [(1, 2, 9, True), (2, 2, 5, True), (33, 3, 30, True), (65, 5, 99, True), (127, 7, 50, True),
-               (128, 32, 2047, True), (32, 32, 200, True), (64, 20, 99, True), (17, 6, 40, False), (100, 20, 99, False),
-               (129, 3, 60, True), (200, 10, 99, True), (256, 32, 2047, True), (255, 5, 30, False)]   # 8 jobs per lane
-
-
-def test_emu_edge_shapes_and_limits():
-    pc.check_synthetic_shapes(make_env, EDGE_SHAPES, n_steps=260, seed=100)
-
-
-def test_emu_abi_error_codes():
-    pc.check_abi_error_codes(make_env)
-
-
-@pytest.mark.parametrize("rule", ["RANDOM", "CR", "FIFO"])
-def test_emu_step_sample_fused_uniform_batch(rule):
-    """Uniform batches take the kernel variant that reads the instance scalars from kernel parameters."""
-    pc.check_step_sample(make_env, ["ta80"] * 3, rule, n_steps=200, seed=13)
-    pc.check_step_sample(make_env, ["ta01"] * 9, rule, n_steps=200, seed=14)
-
-
-def test_emu_facade_errors():
-    pc.check_facade_errors()
-
-
-def test_emu_dispatching_api():
-    pc.check_dispatching_api(make_env)
-
-
-def test_emu_tiny_uniform_batches():
-    pc.check_tiny_uniform_batches(make_env)
-
-
-def test_emu_shard_invariance():
-    pc.check_shard_invariance(make_env, n_steps=150)
-
-
-def test_emu_host_pipeline_packed():
-    pc.check_host_pipeline_packed(make_env, ["ta01", "ta31", "ta51", "ta80", "dmu16"], seed=5)
-    pc.check_host_pipeline_packed(make_env, ["ta80"] * 3, seed=6)
-
-
-@pytest.mark.parametrize("rule", ["RANDOM", "FIFO"])
-def test_emu_rollout_record(rule):
-    pc.check_rollout_record(make_env, ["ta01", "ta01", "ta51", "ta80"], rule, n_steps=300, seed=3)
-
-
-def test_emu_uniform_many_tiles():
-    """Uniform batch with more tiles than (emulated) persistent CTAs, last tile partial."""
-    pc.check_step_sample(make_env, ["ta01"] * 70, "RANDOM", n_steps=40, seed=21)
-    pc.check_step_sample(make_env, ["ta01"] * 70, "LOR", n_steps=25, seed=22)
-
-
-def test_emu_big_uniform_batches():
-    pc.check_big_uniform_batches(make_env, max_steps=60)
+collect(globals(), parity_suite, "emu")

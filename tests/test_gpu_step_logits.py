@@ -1,87 +1,6 @@
 """jss_step_logits (masked categorical draw from policy logits fused into the step) on the real sm_90a library: the
-checks of tests/logits_common.py at GPU sizes, the distribution of the draw and its repeatability.  Run on an H100
-with `pytest -m gpu`."""
-import numpy as np
-import pytest
+tests of tests/step_logits_suite.py at GPU sizes.  Run on an H100 with `pytest -m gpu`."""
+from tests import step_logits_suite
+from tests.backends import collect
 
-from tests import logits_common as lc
-from tests.parity_common import synthetic_instance
-
-pytestmark = pytest.mark.gpu
-
-
-def make_env(n, cfg, **kw):
-    from jssenv_b200 import JssVecEnv
-    return JssVecEnv(n, cfg, **kw)
-
-
-def test_gpu_step_logits_mixed_batch():
-    names = ["ta01", "ta11", "ta21", "ta31", "ta41", "dmu16", "ta51", "ta61", "ta71", "ta80"] * 3
-    lc.check_step_logits(make_env, names, n_steps=1200, seed=3, state_every=100)
-
-
-def test_gpu_step_logits_uniform_ta01():
-    lc.check_step_logits(make_env, ["ta01"] * 300, n_steps=700, seed=4, state_every=100)
-
-
-def test_gpu_step_logits_uniform_ta80():
-    # through the end of the first episodes (about 2 236 transitions)
-    lc.check_step_logits(make_env, ["ta80"] * 40, n_steps=2600, seed=5, pad=0, state_every=200)
-
-
-def test_gpu_step_logits_big_instances():
-    big = synthetic_instance(200, 8, 9, max_dur=50)
-    lc.check_step_logits(make_env, [big] * 9, n_steps=400, seed=6, state_every=100)
-    lc.check_step_logits(make_env, [big, "ta01", "ta51", "ta80"] * 2, n_steps=400, seed=7, state_every=100)
-
-
-def test_gpu_step_logits_edge_cases():
-    lc.check_step_logits_edge_cases(make_env)
-
-
-def test_gpu_step_logits_shard_invariance():
-    lc.check_step_logits_shards(make_env, n_total=60, n_steps=600)
-
-
-def test_gpu_step_logits_abi_errors():
-    lc.check_step_logits_abi_errors(make_env)
-
-
-def test_gpu_step_logits_distribution():
-    """ta01 at N = 65 536 right after reset (every job legal, the no-op not), one shared logits row, one call: the
-    histogram of the drawn actions against the masked softmax, and every log_prob against log_softmax."""
-    import torch
-    from scipy.stats import chisquare
-    n = 65536
-    env = make_env(n, {"instance_path": "ta01"}, seed=11)
-    env.reset()
-    J = env.jobs
-    row = torch.randn(J + 1, generator=torch.Generator().manual_seed(0)).to(env.device)
-    _, _, _, _, info = env.step_logits(row.expand(n, J + 1))   # stride-0 rows: made contiguous by step_logits
-    acts = info["actions"].cpu().numpy()
-    assert acts.min() >= 0 and acts.max() < J
-    logp = torch.log_softmax(row[:J].double(), 0).cpu().numpy()
-    hist = np.bincount(acts, minlength=J)
-    res = chisquare(hist, np.exp(logp) * n)
-    assert res.pvalue > 1e-6, (res, hist)
-    assert np.abs(info["log_prob"].cpu().numpy() - logp[acts]).max() <= 1e-5 * (1 + np.abs(logp).max())
-
-
-def test_gpu_step_logits_repeatable():
-    """Same seed, same step index, same logits: identical actions and log_probs, whether from a second env or from
-    the same env after a reset."""
-    import torch
-    names = ["ta01", "ta41", "ta80"]
-    n = 3 * 1365
-    cfg = {"instance_paths": names, "env_to_instance": np.arange(n) % 3}
-    a_env, b_env = make_env(n, cfg, seed=21), make_env(n, cfg, seed=21)
-    a_env.reset(); b_env.reset()
-    logits = torch.randn((n, a_env.jobs + 1), generator=torch.Generator().manual_seed(1)).to(a_env.device)
-    runs = []
-    for env in (a_env, b_env, a_env):
-        env.reset()
-        env._step_index = 7
-        _, _, _, _, info = env.step_logits(logits)
-        runs.append((info["actions"].cpu().numpy(), info["log_prob"].cpu().numpy().view(np.uint32)))
-    for acts, lp in runs[1:]:
-        assert np.array_equal(acts, runs[0][0]) and np.array_equal(lp, runs[0][1])
+collect(globals(), step_logits_suite, "gpu")

@@ -1,23 +1,17 @@
 """The per-env state block keeps the five per-job integers in 10 bytes (jss_types.h): todo in 6 bits, tufco and col4
 in 11 bits each, idle_last and total_idle in 24 bits each.  These tests push every field to the edges of its range
 through jss_import_state / jss_export_state, and check that values outside the range are flagged instead of wrapped.
-Each check runs under the host emulation of the kernels and, with `-m gpu`, on the real sm_90a library."""
+Each check runs on both backends of tests/backends.py."""
 import numpy as np
-import pytest
 
 from tests import parity_common as pc
-from tests.emu.emu_backend import use_emulation
+from tests.backends import collect, native_test
 
 JSS_FLAG_ERROR = 2
 IDLE_MAX = (1 << 24) - 1
 DUR_MAX = 2047
 JOB_FIELDS = ("todo", "tufco", "col4", "idle_last", "total_idle")
 SHAPES = [(256, 32), (100, 20)]      # the largest supported shape (8 jobs per lane) and ta80's shape (4 per lane)
-
-
-def make_env(n, cfg, **kw):
-    from jssenv_b200 import JssVecEnv
-    return JssVecEnv(n, cfg, **kw)
 
 
 def _field_max(name, M):
@@ -33,7 +27,8 @@ def _set_row(x, name, i, J, values):
     x[name][i, :J] = torch.as_tensor(np.asarray(values, np.int32)).to(x[name].device)
 
 
-def check_roundtrip_at_limits(make_env):
+@native_test()
+def state_roundtrip_at_field_limits(make_env):
     """export -> import -> export returns every field unchanged, with every field at its maximum on some jobs, at 0
     on others, and random in-range values elsewhere (a field bleeding into its neighbour changes the result)."""
     insts = [pc.synthetic_instance(J, M, seed=70 + k, max_dur=DUR_MAX) for k, (J, M) in enumerate(SHAPES)]
@@ -56,18 +51,19 @@ def check_roundtrip_at_limits(make_env):
             _set_row(x, name, i, J, v)
             want[(i, name)] = v
     env.import_state(x)
-    y = {k: pc._np(v).copy() for k, v in env.export_state().items()}
+    y = {k: pc.np_(v).copy() for k, v in env.export_state().items()}
     env.synchronize()
     for (i, name), v in want.items():
         J = SHAPES[i % len(SHAPES)][0]
         assert np.array_equal(y[name][i, :J], v), (i, name)
     assert not ((y["flags"] >> 8) & JSS_FLAG_ERROR).any()
-    xt = {k: pc._np(v) for k, v in x.items()}
+    xt = {k: pc.np_(v) for k, v in x.items()}
     for name in ("tuam", "legal", "blocked", "t"):
         assert np.array_equal(y[name], xt[name]), name
 
 
-def check_out_of_range_import_flagged(make_env):
+@native_test()
+def out_of_range_import_flagged(make_env):
     """A value outside its field's range gives the env the sticky error bit and is clamped into the range; the
     other envs of the batch are imported as they are."""
     J, M = SHAPES[1]
@@ -90,7 +86,7 @@ def check_out_of_range_import_flagged(make_env):
         v[J - 1 - k % 4] = bad                     # a job slot of the last lanes, different ones across cases
         _set_row(x, name, k + 1, J, v)
     env.import_state(x)
-    y = {k: pc._np(v).copy() for k, v in env.export_state().items()}
+    y = {k: pc.np_(v).copy() for k, v in env.export_state().items()}
     env.synchronize()
     err = (y["flags"] >> 8) & JSS_FLAG_ERROR
     assert err[0] == 0
@@ -104,21 +100,4 @@ def check_out_of_range_import_flagged(make_env):
         assert np.array_equal(y[name][i, :J], v), (name, bad)
 
 
-def test_emu_state_roundtrip_at_field_limits():
-    with use_emulation():
-        check_roundtrip_at_limits(make_env)
-
-
-def test_emu_out_of_range_import_flagged():
-    with use_emulation():
-        check_out_of_range_import_flagged(make_env)
-
-
-@pytest.mark.gpu
-def test_gpu_state_roundtrip_at_field_limits():
-    check_roundtrip_at_limits(make_env)
-
-
-@pytest.mark.gpu
-def test_gpu_out_of_range_import_flagged():
-    check_out_of_range_import_flagged(make_env)
+collect(globals(), globals(), "emu", "gpu")
