@@ -74,7 +74,7 @@ struct jss_handle {
     JssParams p{};
     JssSmemLayout sl_env{}, sl_step{}, sl_step_rem{};   // shared-memory layouts of the generic / step kernels (step: without / with the suffix-sum table)
     JssSmemLayout sl_step_logits{};                // step kernels drawing the action from policy logits (a logits row per warp)
-    int class_tile_begin[4] = {0, 0, 0, 0}, class_tile_end[4] = {0, 0, 0, 0};  // KJ = 1, 2, 4, 8
+    int32_t class_tiles[JSS_LANE_CLASSES][2] = {};  // [class_tiles[c][0], class_tiles[c][1]): the tiles of lane class c
     int n_tiles = 0;
     std::map<std::pair<const void *, size_t>, int> ctas_per_sm;   // by kernel and dynamic shared memory (filled lazily)
     std::map<const void *, size_t> smem_optin;     // by kernel: the largest dynamic shared memory it was opted in to
@@ -123,8 +123,6 @@ int dev_alloc(jss_t *h, T **out, size_t count, bool zero = true) {
 }
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
-inline int kj_of(int J) { return J <= 32 ? 1 : (J <= 64 ? 2 : (J <= 128 ? 4 : 8)); }
-inline int class_of(int kj) { return kj == 1 ? 0 : (kj == 2 ? 1 : (kj == 4 ? 2 : 3)); }
 size_t smem_bytes(const JssSmemLayout &sl) { return (size_t)sl.off_warp0 + (size_t)JSS_WARPS_PER_CTA * sl.warp_stride; }
 
 // resident CTAs per SM of `kern` at `smem` bytes of dynamic shared memory; the first call per kernel and size also
@@ -149,31 +147,35 @@ int ctas_per_sm(jss_t *h, Kern kern, size_t smem, int &per_sm) {
 }
 
 typedef void (*JssKernel)(JssParams, JssLaunch, JssSmemLayout);
+template <int MODE>   // by lane class
+const JssKernel env_kernels[JSS_LANE_CLASSES] = {jss_env_kernel<1, MODE>, jss_env_kernel<2, MODE>,
+                                                 jss_env_kernel<4, MODE>, jss_env_kernel<8, MODE>};
+template <int SAMPLE>
+const JssKernel step_kernels[JSS_LANE_CLASSES] = {jss_step_kernel<1, SAMPLE>, jss_step_kernel<2, SAMPLE>,
+                                                  jss_step_kernel<4, SAMPLE>, jss_step_kernel<8, SAMPLE>};
+// the rules that read the suffix sums
+bool jss_rule_wants_rem(int rule) { return rule == JSS_RULE_MWR || rule == JSS_RULE_LWR || rule == JSS_RULE_CR; }
 
 // the fused step kernel: uniform batches by lane class, mixed batches by whether they hold instances with 129..256 jobs
 template <int SAMPLE>
 JssKernel step_kernel(const jss_t *h) {
     if (h->p.uniform_inst < 0)
-        return h->class_tile_end[3] > h->class_tile_begin[3] ? jss_step_mixed_kernel<SAMPLE, true>
-                                                               : jss_step_mixed_kernel<SAMPLE, false>;
-    switch (kj_of(h->insts[h->p.uniform_inst].J)) {
-    case 1: return jss_step_kernel<1, SAMPLE>;
-    case 2: return jss_step_kernel<2, SAMPLE>;
-    case 4: return jss_step_kernel<4, SAMPLE>;
-    default: return jss_step_kernel<8, SAMPLE>;
-    }
+        return h->class_tiles[3][1] > h->class_tiles[3][0] ? jss_step_mixed_kernel<SAMPLE, true>
+                                                           : jss_step_mixed_kernel<SAMPLE, false>;
+    return step_kernels<SAMPLE>[jss_lane_class(h->insts[h->p.uniform_inst].J)];
 }
 
 // one fused step launch (PDL).  A uniform batch runs min(tiles, resident CTAs) persistent CTAs over static strided
-// tiles; a mixed batch runs one CTA per JssCtaRange (all resident: SMs x 3).
+// tiles; a mixed batch runs one CTA per JssCtaRange, SMs x JSS_MIN_CTAS[2] of them.  Those are all resident unless the
+// batch holds instances with 129..256 jobs: that kernel fits one CTA per SM.
 int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
     // SAMPLE: 0 none, 1 masked-uniform sampler, 2 dispatching rule, 3 action drawn from policy logits before the step
     const int sample = a.logits ? 3 : a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
     const JssKernel kern = sample == 0 ? step_kernel<0>(h) : sample == 1 ? step_kernel<1>(h)
                          : sample == 2 ? step_kernel<2>(h) : step_kernel<3>(h);
     // only the rules that read the suffix sums stage them; the other launches leave their room to the L1
-    const JssSmemLayout &sl = sample == 3 ? h->sl_step_logits
-                            : sample == 2 && jss_rule_wants_rem(a.rule) ? h->sl_step_rem : h->sl_step;
+    a.stage = sample == 2 && jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
+    const JssSmemLayout &sl = sample == 3 ? h->sl_step_logits : a.stage & JSS_STAGE_REM ? h->sl_step_rem : h->sl_step;
     const size_t smem = smem_bytes(sl);
     int per_sm = 0, rc = ctas_per_sm(h, kern, smem, per_sm);
     if (rc) return rc;
@@ -189,32 +191,30 @@ int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
     return JSS_OK;
 }
 
-// the generic kernel of lane class KJ: MODE = JSS_MODE_RESET also serves export, import, pack and exporting steps
-template <int KJ>
-JssKernel env_kernel(int mode) {
-    if (mode == JSS_MODE_POLICY) return jss_env_kernel<KJ, JSS_MODE_POLICY>;
-    if (mode == JSS_MODE_ROLLOUT) return jss_env_kernel<KJ, JSS_MODE_ROLLOUT>;
-    return jss_env_kernel<KJ, JSS_MODE_RESET>;
-}
-
 int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
+    // the generic kernel: MODE = JSS_MODE_RESET also serves export, import, pack and exporting steps
+    const JssKernel *kerns = a.mode == JSS_MODE_POLICY ? env_kernels<JSS_MODE_POLICY>
+                           : a.mode == JSS_MODE_ROLLOUT ? env_kernels<JSS_MODE_ROLLOUT> : env_kernels<JSS_MODE_RESET>;
+    // what the launch reads: a rollout every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
+    // / CR), and the masked-uniform sampler no table at all (only J); the other modes ops / len
+    a.stage = a.mode == JSS_MODE_ROLLOUT ? JSS_STAGE_ALL
+            : a.mode != JSS_MODE_POLICY ? JSS_STAGE_OPS
+            : a.rule == JSS_RULE_RANDOM ? 0 : jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
     const JssSmemLayout &sl = h->sl_env;
     const size_t smem = smem_bytes(sl);
-    for (int c = 0; c < 4; c++) {               // one launch per lane class present
-        a.tile_begin = h->class_tile_begin[c];
-        a.tile_end = h->class_tile_end[c];
+    for (int c = 0; c < JSS_LANE_CLASSES; c++) {   // one launch per lane class present
+        a.tile_begin = h->class_tiles[c][0];
+        a.tile_end = h->class_tiles[c][1];
         const int n_tiles = a.tile_end - a.tile_begin;
         if (n_tiles <= 0) continue;
-        const JssKernel kern = c == 0 ? env_kernel<1>(a.mode) : c == 1 ? env_kernel<2>(a.mode)
-                             : c == 2 ? env_kernel<4>(a.mode) : env_kernel<8>(a.mode);
-        int per_sm = 0, rc = ctas_per_sm(h, kern, smem, per_sm);
+        int per_sm = 0, rc = ctas_per_sm(h, kerns[c], smem, per_sm);
         if (rc) return rc;
         // policy kernels touch ~50 B per env: latency-bound, so give every tile its own CTA
         // instead of a persistent loop with a dependent load per iteration
         const int grid = (a.mode == JSS_MODE_POLICY) ? n_tiles : std::min(n_tiles, h->sm_count * per_sm);
-        JSS_LAUNCH(kern, grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
+        JSS_LAUNCH(kerns[c], grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
         JSS_CUDA(h, cudaGetLastError());
         h->launches += 1;
     }
@@ -242,25 +242,22 @@ int plan_tiles(jss_t *h, const int32_t *env_to_inst, std::vector<int32_t> &order
     for (int e = 0; e < N; e++) order[e] = e;
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
         const int ka = env_to_inst[a], kb = env_to_inst[b];
-        const int ca = class_of(kj_of(h->insts[ka].J)), cb = class_of(kj_of(h->insts[kb].J));
+        const int ca = jss_lane_class(h->insts[ka].J), cb = jss_lane_class(h->insts[kb].J);
         if (ca != cb) return ca > cb;
         return ka < kb;
     });
-    for (int c = 0; c < 4; c++) h->class_tile_begin[c] = h->class_tile_end[c] = 0;
+    for (auto &r : h->class_tiles) r[0] = r[1] = 0;
     int pos = 0;
     int cur_class = -1;
     uint64_t off16 = 0;                                  // running state offset in 16-byte units
     while (pos < N) {
         const int k = env_to_inst[order[pos]];
-        const int c = class_of(kj_of(h->insts[k].J));
+        const int c = jss_lane_class(h->insts[k].J);
         const uint32_t block16 = (uint32_t)h->insts[k].block_words / 4;
         int end = pos;
         while (end < N && env_to_inst[order[end]] == k) end++;
-        if (c != cur_class) {
-            if (cur_class >= 0) h->class_tile_end[cur_class] = (int)tiles.size();
-            h->class_tile_begin[c] = (int)tiles.size();
-            cur_class = c;
-        }
+        if (c != cur_class) h->class_tiles[c][0] = (int)tiles.size();   // a class's tiles are contiguous
+        cur_class = c;
         for (int f = pos; f < end; f += JSS_WARPS_PER_CTA) {
             JssTile t;
             const int cnt = std::min(JSS_WARPS_PER_CTA, end - f);
@@ -271,9 +268,9 @@ int plan_tiles(jss_t *h, const int32_t *env_to_inst, std::vector<int32_t> &order
             off16 += (uint64_t)cnt * block16;
             tiles.push_back(t);
         }
+        h->class_tiles[c][1] = (int)tiles.size();
         pos = end;
     }
-    if (cur_class >= 0) h->class_tile_end[cur_class] = (int)tiles.size();
     h->n_tiles = (int)tiles.size();
     if (off16 >= (1ull << 32)) return fail(h, JSS_ERR_UNSUPPORTED, "state exceeds 64 GiB");
     state_words = (size_t)off16 * 4;
@@ -283,17 +280,16 @@ int plan_tiles(jss_t *h, const int32_t *env_to_inst, std::vector<int32_t> &order
 // mixed-batch step kernel: every persistent CTA gets an equal slice of EVERY lane class (tile counts differ by at
 // most one per class; the extras are dithered with a different phase per class so that no CTA collects them all)
 std::vector<JssCtaRange> plan_cta_ranges(const jss_t *h) {
-    const int n_cta = std::max(1, std::min(h->n_tiles, h->sm_count * JSS_MIN_CTAS));
+    const int n_cta = std::max(1, std::min(h->n_tiles, h->sm_count * JSS_MIN_CTAS[2]));
     std::vector<JssCtaRange> ranges((size_t)n_cta);
-    for (int c = 0; c < 4; c++) {                     // c = 3: KJ = 8, c = 2: KJ = 4, c = 1: KJ = 2, c = 0: KJ = 1
-        const int tb = h->class_tile_begin[c], n = h->class_tile_end[c] - tb;
-        const int shift = (c * n_cta) / 4;            // CTA that starts this class's Bresenham sequence
+    for (int c = 0; c < JSS_LANE_CLASSES; c++) {
+        const int tb = h->class_tiles[c][0], n = h->class_tiles[c][1] - tb;
+        const int shift = (c * n_cta) / JSS_LANE_CLASSES;   // CTA that starts this class's Bresenham sequence
         int given = 0;
         for (int k = 0; k < n_cta; k++) {
             const int b = (k + shift) % n_cta;
             const int upto = (int)(((int64_t)(k + 1) * n) / n_cta);
-            int32_t *lo = c == 3 ? &ranges[b].a8 : (c == 2 ? &ranges[b].a4 : (c == 1 ? &ranges[b].a2 : &ranges[b].a1));
-            lo[0] = tb + given; lo[1] = tb + upto;
+            ranges[b].tiles[c][0] = tb + given; ranges[b].tiles[c][1] = tb + upto;
             given = upto;
         }
     }
@@ -532,7 +528,7 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     p.n_envs = N;
     p.jobs_max = jmax;
     p.machines_max = mmax;
-    p.mask_stride = round_up(jmax + 1, jmax > 128 ? 8 : 4);   // the 8-jobs-per-lane class stores 8 mask bytes per lane
+    p.mask_stride = round_up(jmax + 1, jss_lane_slots(1 << jss_lane_class(jmax)));   // whole mask stores per lane
     p.create_flags = (int32_t)h->create_flags;
     p.env_id_base = h->env_id_base;
     {

@@ -102,12 +102,12 @@ JSS_DEV uint32_t jss_op_m(uint32_t op) { return op >> JSS_OP_SHIFT; }
 JSS_DEV int jss_op_d(uint32_t op) { return (int)(op & JSS_OP_DMASK); }
 template <int KJ>
 JSS_DEV constexpr uint32_t jss_legal_mask() { return (1u << KJ) - 1u; }
-// `lb` layout: bit i = job slot i legal, bit BS + i = blocked by a no-op (BS = 4 for KJ <= 4, 8 for KJ = 8); a lane's
-// bits are one byte of the state block (KJ <= 4) or one 16-bit word (KJ = 8: 129..256 jobs)
+// `lb` layout: bit i = job slot i legal, bit BS + i = blocked by a no-op, BS = jss_lane_slots(KJ); a lane's bits are
+// one byte of the state block (KJ <= 4) or one 16-bit word (KJ = 8: 129..256 jobs)
 template <int KJ>
-JSS_DEV constexpr int jss_bs() { return KJ == 8 ? 8 : 4; }
+JSS_DEV constexpr int jss_bs() { return jss_lane_slots(KJ); }
 template <int KJ>
-JSS_DEV constexpr int jss_bits_words() { return KJ == 8 ? 16 : 8; }   // int32 words of the per-lane bits region
+JSS_DEV constexpr int jss_bits_words() { return 2 * jss_lane_slots(KJ); }   // int32 words of the per-lane bits region
 
 // correctly rounded x / y for small non-negative integers given ry = RN(1/y): Markstein's
 // sequence q = RN(x*ry); r = x - q*y (exact, FMA); q' = RN(q + r*ry).  Checked exhaustively
@@ -319,7 +319,7 @@ JSS_DEV void env_load_bits_hdr(const int32_t *tail, int Mc, int lane, EnvRegs<KJ
 
 // `blk`: the env's state block (in global memory, or the step kernels' shared-memory copy)
 template <int KJ>
-JSS_DEV void env_load(const JssParams &p, const InstView &iv, const int32_t *blk, int lane, EnvRegs<KJ> &s) {
+JSS_DEV void env_load(const InstView &iv, const int32_t *blk, int lane, EnvRegs<KJ> &s) {
     const int Jc = iv.si->Jcap, Mc = iv.si->Mcap;   // geometry of the env's own instance
     if (KJ * lane < jss_J(iv)) env_load_jobs<KJ>(blk, Jc, lane, s);
     else env_clear_jobs<KJ>(iv, s);
@@ -332,8 +332,7 @@ JSS_DEV void env_load(const JssParams &p, const InstView &iv, const int32_t *blk
 // policy kernels read only what the rule looks at: bits + header always, todo for every
 // rule (current op / remaining work / remaining ops), idle_last for FIFO
 template <int KJ>
-JSS_DEV void env_load_for_policy(const JssParams &p, const InstView &iv, const int32_t *blk, int lane, EnvRegs<KJ> &s,
-                                 int rule) {
+JSS_DEV void env_load_for_policy(const InstView &iv, const int32_t *blk, int lane, EnvRegs<KJ> &s, int rule) {
     const int Jc = iv.si->Jcap, Mc = iv.si->Mcap;
     env_clear_jobs<KJ>(iv, s);
     if (rule != JSS_RULE_RANDOM && KJ * lane < jss_J(iv)) {
@@ -356,7 +355,7 @@ JSS_DEV void env_load_for_policy(const JssParams &p, const InstView &iv, const i
 }
 
 template <int KJ>
-JSS_DEV void env_store_to(const JssParams &p, const InstView &iv, int32_t *blk, int lane, const EnvRegs<KJ> &s) {
+JSS_DEV void env_store_to(const InstView &iv, int32_t *blk, int lane, const EnvRegs<KJ> &s) {
     const int Jc = iv.si->Jcap, Mc = iv.si->Mcap;
     // lanes past the last job hold the "finished job" padding values (todo == M, the rest 0): the whole block is
     // defined, including the padding of the u16 region w2 up to a multiple of 16 bytes
@@ -382,12 +381,12 @@ JSS_DEV void env_store_to(const JssParams &p, const InstView &iv, int32_t *blk, 
 }
 
 template <int KJ>
-JSS_DEV void env_store(const JssParams &p, const InstView &iv, int32_t *blk, int lane, const EnvRegs<KJ> &s) {
+JSS_DEV void env_store(const InstView &iv, int32_t *blk, int lane, const EnvRegs<KJ> &s) {
     // all lanes must have finished env_load (every lane reads the shared header words)
     // before any lane overwrites the block: paths such as the auto-reset have no
     // collective between load and store
     __syncwarp();
-    env_store_to<KJ>(p, iv, blk, lane, s);
+    env_store_to<KJ>(iv, blk, lane, s);
 }
 
 // jss_env.py:145-181
@@ -1041,6 +1040,9 @@ struct JssSmemLayout {
     int32_t off_scratch;    // step kernels: [mbarrier 16 B][state-in block][scratch][state-out block]; else 0
     int32_t off_logits;     // step kernels with SAMPLE = 3: [logits row, J + 1 floats] behind state-out; else 0
 };
+static_assert(sizeof(JssParams) == 248 && sizeof(JssLaunch) == 240 && sizeof(JssSmemLayout) == 32 &&
+              sizeof(JssTile) == 16 && sizeof(JssCtaRange) == 32,
+              "ptxas allocates the kernels' registers by the parameter offsets (JssParams::pad0_): measure a change");
 
 struct JssCtaSmem {         // the CTA-shared part
     JssInst *si;
@@ -1065,10 +1067,6 @@ JSS_DEV void jss_iv_shape(InstView &iv) {
 #define JSS_STAGE_OPS 1     // ops + jobs_length
 #define JSS_STAGE_REM 2     // suffix sums (rules MWR / LWR / CR)
 #define JSS_STAGE_ALL 3
-// the rules that read the suffix sums; the host sizes the shared-memory layout with the same predicate
-JSS_HD static inline bool jss_rule_wants_rem(int rule) {
-    return rule == JSS_RULE_MWR || rule == JSS_RULE_LWR || rule == JSS_RULE_CR;
-}
 
 JSS_DEV void jss_stage_instance(const JssParams &p, const JssInst &d, const JssCtaSmem &c, int what) {
     const int tid = threadIdx.x, nt = blockDim.x;
@@ -1161,7 +1159,7 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         if (a.env_mask && a.env_mask[env] == 0) return;
         env_reset_regs<KJ>(iv, s, lane);
         env_clear_solution(p, env, lane);
-        env_store<KJ>(p, iv, blk(), lane, s);
+        env_store<KJ>(iv, blk(), lane, s);
         env_emit_all<KJ>(p, iv, s, env, lane, scratch, 0);
         return;
     }
@@ -1169,15 +1167,15 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         if (a.env_mask && a.env_mask[env] == 0) return;
         env_import<KJ>(p, iv, s, env, lane);
         s.ep_steps = 0; s.ep_return = 0;
-        env_store<KJ>(p, iv, blk(), lane, s);
+        env_store<KJ>(iv, blk(), lane, s);
         env_emit_obs<KJ>(p, jss_out_default(p), iv, s, env, lane, scratch);
         env_emit_mask<KJ>(p, jss_out_default(p), iv, s, env, lane, (s.flags & JSS_FLAG_NOOP_LEGAL) != 0u);
         if (lane == 0) p.scalars[4 * (size_t)env + 3] = (int32_t)((s.flags << 8) | (s.flags & JSS_FLAG_DONE));
         return;
     }
     const uint64_t genv = p.env_id_base + (uint64_t)env;
-    if (mode == JSS_MODE_POLICY) env_load_for_policy<KJ>(p, iv, blk(), lane, s, a.rule);
-    else env_load<KJ>(p, iv, blk(), lane, s);
+    if (mode == JSS_MODE_POLICY) env_load_for_policy<KJ>(iv, blk(), lane, s, a.rule);
+    else env_load<KJ>(iv, blk(), lane, s);
     s.flags = jss_uniform(s.flags);                      // one word read by every lane (see jss_uniform)
     if (mode == JSS_MODE_EXPORT) { env_export<KJ>(p, iv, s, env, lane); return; }
     if (mode == JSS_MODE_PACK) { env_pack<KJ>(a, iv, s, env, lane, scratch); return; }
@@ -1194,7 +1192,7 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         const bool changed = env_step<KJ>(p, iv, s, env, lane, action, raw, hz);
         s.flags = jss_uniform(s.flags);
         if (changed) {
-            env_store<KJ>(p, iv, blk(), lane, s);
+            env_store<KJ>(iv, blk(), lane, s);
             env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
         } else if (s.flags != flags_in) {
             env_store_flags_only<KJ>(p, iv, blk(), s, env, lane);
@@ -1226,15 +1224,10 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
         }
     }
     if (dirty) {
-        env_store<KJ>(p, iv, blk(), lane, s);
+        env_store<KJ>(iv, blk(), lane, s);
         if (!a.write_obs || record) env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
     }
 }
-
-// 80 registers -> 3 CTAs = 24 warps per SM; 3 x ~45 KB of shared memory (ta80) fit the 228 KB of an sm_90 SM.  4 CTAs
-// would fit in shared memory, but at 64 registers the 4-jobs-per-lane step kernel spills (DESIGN.md section 4).
-#define JSS_MIN_CTAS 3
-#define JSS_MIN_CTAS_SMALL 4   // uniform batches with <= 32 jobs (KJ = 1) are latency-bound: 4 CTAs = 32 warps per SM at 64 registers
 
 template <int KJ, int MODE>
 __global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, 1)
@@ -1246,19 +1239,15 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     jss_cta_carve(sl, sm, c, iv);
     const int warp = jss_warp_index(), lane = threadIdx.x & 31;
     float *scratch = reinterpret_cast<float *>(sm + sl.off_warp0 + warp * sl.warp_stride);
-    // what the mode reads: the masked-uniform sampler looks at no instance table at all (only J); the other policies
-    // at ops / len (+ suffix sums for MWR / LWR / CR); everything that steps needs all tables
-    int what = JSS_STAGE_OPS;
-    if (MODE == JSS_MODE_ROLLOUT) what = JSS_STAGE_ALL;
-    if (MODE == JSS_MODE_POLICY)
-        what = a.rule == JSS_RULE_RANDOM ? 0 : jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
+    // a constant where MODE fixes the tables (the values launch_all sets): only a policy kernel branches on a.stage
+    const int stage = MODE == JSS_MODE_POLICY ? a.stage : MODE == JSS_MODE_ROLLOUT ? JSS_STAGE_ALL : JSS_STAGE_OPS;
     int staged = -1;
     for (int tile = a.tile_begin + (int)blockIdx.x; tile < a.tile_end; tile += (int)gridDim.x) {
         const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, tile, warp);
         const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
         if (inst != staged) {                            // CTA-uniform
             __syncthreads();
-            jss_stage_instance(p, p.inst[inst], c, what);
+            jss_stage_instance(p, p.inst[inst], c, stage);
             staged = inst;
             __syncthreads();
         }
@@ -1297,9 +1286,9 @@ struct JssWarpSmem {        // per-warp shared-memory regions of the step kernel
 
 // tiles tile, tile + tile_step, ... < tile_end of ONE lane class through the prefetch pipeline
 template <int KJ, int SAMPLE, bool UNI>
-JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSmemLayout &sl, InstView &iv,
-                            const JssCtaSmem &c, const JssWarpSmem &w, int warp, int lane, int tile, int tile_end,
-                            int tile_step, int &staged, uint32_t &phase) {
+JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv, const JssCtaSmem &c,
+                            const JssWarpSmem &w, int warp, int lane, int tile, int tile_end, int tile_step, int &staged,
+                            uint32_t &phase) {
     int env_next = -1, act_next = 0;
     // start the bulk load of the state block of this warp's env of tile `next` and fetch its action (SAMPLE = 3: start
     // the copy of its logits row, columns 0..J, one 4-byte cp.async per column)
@@ -1326,7 +1315,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
             const int inst = jss_tile(p, a, UNI, tile, warp).inst;
             if (inst != staged) {                        // CTA-uniform
                 __syncthreads();
-                jss_stage_instance(p, p.inst[inst], c, (SAMPLE == 2 && jss_rule_wants_rem(a.rule)) ? JSS_STAGE_ALL : JSS_STAGE_OPS);
+                jss_stage_instance(p, p.inst[inst], c, SAMPLE == 2 ? a.stage : JSS_STAGE_OPS);
                 staged = inst;
                 __syncthreads();
             }
@@ -1338,7 +1327,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
         if (env >= 0) {
             jss_mbar_wait(w.mbar, phase);                // this env's block has landed in shared memory
             phase ^= 1u;
-            env_load<KJ>(p, iv, w.state_in, lane, s);
+            env_load<KJ>(iv, w.state_in, lane, s);
             __syncwarp();                                // every lane has read the buffer
             if (SAMPLE == 3) {
                 jss_cp_async_wait();
@@ -1373,7 +1362,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, const JssSme
         }
         if (changed) {
             // new state -> shared staging -> one bulk store (every word of the block is rewritten)
-            env_store_to<KJ>(p, iv, w.state_out, lane, s);
+            env_store_to<KJ>(iv, w.state_out, lane, s);
             const JssTileWarp t = jss_tile(p, a, UNI, tile, warp);
             env_emit_all<KJ, true>(p, iv, s, env, lane, w.scratch, raw, w.scratch_sa,
                                    p.state + (size_t)t.off16 * 4, w.state_out_sa, t.blk16 * 16u);
@@ -1405,8 +1394,8 @@ JSS_DEV void jss_step_carve(const JssSmemLayout &sl, char *sm, int warp, JssWarp
 
 // Uniform batch (every env runs the same instance): static strided tiles, the per-instance scalars are
 // read from the kernel parameters (constant-bank operands), no CTA barrier after the first staging.
-template <int KJ, int SAMPLE>
-__global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, KJ == 1 ? JSS_MIN_CTAS_SMALL : (KJ == 8 ? 1 : JSS_MIN_CTAS))
+template <int KJ, int SAMPLE>   // 32 * KJ jobs: the largest instances of KJ's lane class
+__global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, JSS_MIN_CTAS[jss_lane_class(32 * KJ)])
 jss_step_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     JSS_SMEM_DECL(jss_smem);
     char *sm = reinterpret_cast<char *>(jss_smem);
@@ -1419,15 +1408,15 @@ jss_step_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     jss_step_carve(sl, sm, warp, w);
     if (lane == 0) jss_mbar_init(w.mbar);
     jss_pdl_launch_dependents();
-    // prologue on read-only data (overlaps the tail of the previous launch under PDL)
-    jss_stage_instance(p, p.inst[p.uniform_inst], c, (SAMPLE == 2 && jss_rule_wants_rem(a.rule)) ? JSS_STAGE_ALL : JSS_STAGE_OPS);
+    // prologue on read-only data (overlaps the tail of the previous launch under PDL); only a rule reads suffix sums
+    jss_stage_instance(p, p.inst[p.uniform_inst], c, SAMPLE == 2 ? a.stage : JSS_STAGE_OPS);
     __syncthreads();
     jss_pdl_wait();
     int staged = p.uniform_inst;
     uint32_t phase = 0;
     // Static strided tiles; the env after the current one is known one iteration ahead, which is what
     // the TMA prefetch needs.
-    jss_step_tiles<KJ, SAMPLE, true>(p, a, sl, iv, c, w, warp, lane, a.tile_begin + (int)blockIdx.x, a.tile_end,
+    jss_step_tiles<KJ, SAMPLE, true>(p, a, iv, c, w, warp, lane, a.tile_begin + (int)blockIdx.x, a.tile_end,
                                      (int)gridDim.x, staged, phase);
     if (lane == 0) jss_bulk_store_wait_all();            // shared memory must outlive the bulk reads
 }
@@ -1439,7 +1428,7 @@ jss_step_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
 // the CTAs that share an SM mostly execute the same 20-35 KB loop body (the three together are 67-86 KB, more than
 // the instruction cache holds).  Instance tables are re-staged only when the instance changes.
 template <int SAMPLE, bool BIG>   // BIG: the batch contains instances with 129..256 jobs (a fourth, 8-jobs-per-lane body)
-__global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, BIG ? 1 : JSS_MIN_CTAS)
+__global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, JSS_MIN_CTAS[BIG ? 3 : 2])
 jss_step_mixed_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     JSS_SMEM_DECL(jss_smem);
     char *sm = reinterpret_cast<char *>(jss_smem);
@@ -1451,15 +1440,16 @@ jss_step_mixed_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout 
     jss_step_carve(sl, sm, warp, w);
     if (lane == 0) jss_mbar_init(w.mbar);
     jss_pdl_launch_dependents();
-    const int4 r0 = reinterpret_cast<const int4 *>(p.cta_ranges + blockIdx.x)[0];   // [a4, b4) [a2, b2)
-    const int4 r1 = reinterpret_cast<const int4 *>(p.cta_ranges + blockIdx.x)[1];   // [a1, b1) [a8, b8)
+    // one 8-byte load per lane class: with two 16-byte loads <2, false> spills 36 / 44 bytes instead of 32 / 32
+    const int2 *range = reinterpret_cast<const int2 *>(p.cta_ranges[blockIdx.x].tiles);
+    const int2 r3 = range[3], r2 = range[2], r1 = range[1], r0 = range[0];
     jss_pdl_wait();
     int staged = -1;
     uint32_t phase = 0;
-    if (BIG) jss_step_tiles<8, SAMPLE, false>(p, a, sl, iv, c, w, warp, lane, r1.z, r1.w, 1, staged, phase);   // 129..256 jobs
-    jss_step_tiles<4, SAMPLE, false>(p, a, sl, iv, c, w, warp, lane, r0.x, r0.y, 1, staged, phase);
-    jss_step_tiles<2, SAMPLE, false>(p, a, sl, iv, c, w, warp, lane, r0.z, r0.w, 1, staged, phase);
-    jss_step_tiles<1, SAMPLE, false>(p, a, sl, iv, c, w, warp, lane, r1.x, r1.y, 1, staged, phase);
+    if (BIG) jss_step_tiles<8, SAMPLE, false>(p, a, iv, c, w, warp, lane, r3.x, r3.y, 1, staged, phase);
+    jss_step_tiles<4, SAMPLE, false>(p, a, iv, c, w, warp, lane, r2.x, r2.y, 1, staged, phase);
+    jss_step_tiles<2, SAMPLE, false>(p, a, iv, c, w, warp, lane, r1.x, r1.y, 1, staged, phase);
+    jss_step_tiles<1, SAMPLE, false>(p, a, iv, c, w, warp, lane, r0.x, r0.y, 1, staged, phase);
     if (lane == 0) jss_bulk_store_wait_all();            // shared memory must outlive the bulk reads
 }
 

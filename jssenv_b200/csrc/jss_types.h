@@ -18,6 +18,20 @@
 #endif
 #endif
 
+// ---- lane classes: lane l of an env's warp owns the KJ = 1 << jss_lane_class(J) jobs KJ*l .. KJ*l+KJ-1 ----------
+#define JSS_LANE_CLASSES 4   // KJ = 1, 2, 4, 8 for J <= 32, 64, 128, 256; each class has its own kernels
+JSS_HD static inline constexpr int jss_lane_class(int J) { return J <= 32 ? 0 : J <= 64 ? 1 : J <= 128 ? 2 : 3; }
+// Job slots a lane reserves, max(4, KJ): the state block pads J to a multiple of them and a mask row J + 1, and a
+// lane's legal / no-op-blocked bits are two fields of this width (one byte or one 16-bit word per lane).
+JSS_HD static inline constexpr int jss_lane_slots(int KJ) { return KJ > 4 ? KJ : 4; }
+// Resident CTAs per SM the step kernel of each lane class is built for: 80 registers -> 3 CTAs = 24 warps per SM, and
+// 3 x ~45 KB of shared memory (ta80) fit the 228 KB of an SM; at the 64 registers of 4 CTAs the 4-jobs-per-lane kernel
+// spills (DESIGN.md section 4).  <= 32 jobs are latency-bound: 4 CTAs at 64 registers.  8 jobs per lane: one CTA.
+// The entries do not grow with the class: a kernel that walks classes 0 .. c (the mixed step kernel) fits class c's.
+constexpr int JSS_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 3, 1};
+static_assert(JSS_MIN_CTAS[0] >= JSS_MIN_CTAS[1] && JSS_MIN_CTAS[1] >= JSS_MIN_CTAS[2] &&
+              JSS_MIN_CTAS[2] >= JSS_MIN_CTAS[3], "the mixed-batch step kernel takes its last class's entry");
+
 // ---- packed record of one job: the state block and the host wire rows both use it ------------------
 // The five per-job integers carry 76 bits, packed into three words (10 bytes):
 //   w0  u32  todo | tufco << 6 | col4 << 17          (bits 28..31: the legal bit in a wire record, 0 in the state block)
@@ -64,9 +78,8 @@ JSS_HD static inline int jss_job_total_idle(uint32_t w1, uint32_t w2) {
 // ---- per-env state block in HBM (every region 16-byte aligned) -------------------
 //   w0  u32[Jcap], w1  u32[Jcap], w2  u16[Jcap] (region padded to a multiple of 16 bytes): the job records
 //   tail:  [0, Mcap)  time_until_available_machine (int32)
-//   then 8 words  = 32 bytes, byte l = lane l's job bits: bit i legal(job KJ*l+i),
-//                   bit 4+i blocked by a no-op (action_illegal_no_op)
-//                   (instances with 129..256 jobs, KJ = 8: 16 words, one 16-bit word per lane, blocked = bit 8+i)
+//   then 2 * slots words (slots = jss_lane_slots(KJ)), byte / 16-bit word l = lane l's job bits: bit i legal(job
+//                   KJ*l+i), bit slots+i blocked by a no-op (action_illegal_no_op)
 //        4 words  header: current_time_step, flags, episode_steps, episode_return_raw
 // Jcap / Mcap are those of the ENV'S OWN instance (jss_block_geom), not batch maxima.
 // Not stored because derivable (SURVEY.md section 8 a13): event queue, illegal_actions
@@ -77,8 +90,7 @@ JSS_HD static inline int jss_job_total_idle(uint32_t w1, uint32_t w2) {
 #define JSS_HDR_EP_RETURN 3
 
 // State-block geometry of an instance in int32 words: the ONE definition the host (block offsets, shared-memory
-// sizing, JssInst) and the kernels use.  Per-lane slices are whole vectors: J rounded up to 4 (to 8 for the
-// 8-jobs-per-lane class, which also keeps 16 bits per lane in the bits region).
+// sizing, JssInst) and the kernels use.  Per-lane slices are whole vectors: J rounded up to the lane's job slots.
 struct JssBlockGeom {
     int32_t Jcap, Mcap;
     int32_t tail;    // first word of tuam (behind w0, w1 and the padded u16 region w2)
@@ -86,11 +98,12 @@ struct JssBlockGeom {
     int32_t words;   // whole block
 };
 JSS_HD static inline JssBlockGeom jss_block_geom(int J, int M) {
+    const int slots = jss_lane_slots(1 << jss_lane_class(J));
     JssBlockGeom g;
-    g.Jcap = J > 128 ? ((J + 7) & ~7) : ((J + 3) & ~3);
+    g.Jcap = (J + slots - 1) & ~(slots - 1);
     g.Mcap = (M + 3) & ~3;
     g.tail = 2 * g.Jcap + ((g.Jcap + 7) & ~7) / 2;
-    g.hdr = g.tail + g.Mcap + (J > 128 ? 16 : 8);
+    g.hdr = g.tail + g.Mcap + 2 * slots;
     g.words = g.hdr + 4;
     return g;
 }
@@ -120,8 +133,7 @@ struct JssTile {       // one CTA work item: up to `count` envs of ONE instance 
 };
 
 struct JssCtaRange {   // mixed batches: the tiles of one persistent CTA -- an equal slice of EVERY lane class
-    int32_t a4, b4, a2, b2;     // [a4, b4) KJ = 4 tiles, [a2, b2) KJ = 2 tiles,
-    int32_t a1, b1, a8, b8;     // [a1, b1) KJ = 1 tiles, [a8, b8) KJ = 8 tiles (instances with 129..256 jobs)
+    int32_t tiles[JSS_LANE_CLASSES][2];   // [tiles[c][0], tiles[c][1]): its tiles of class c (one 8-byte load each)
 };
 
 struct JssParams {
@@ -162,7 +174,7 @@ struct JssLaunch {           // per-launch arguments
     int32_t export_after;    // step through the generic kernel: also decode the new state into the x_* arrays (facade)
     uint64_t seed, step_index;
     uint32_t hash_key;       // jss_hash_key(seed, step_index), folded once per launch on the host (fused step + sampler)
-    uint32_t pad_key_;
+    int32_t stage;           // JSS_STAGE_*: the instance tables the launch stages in shared memory (launch_all)
     double cr_factor;        // CriticalRatio due_date_factor (dispatching.py:337-349); reference default 1.5
     const int32_t *actions;  // step
     int32_t *actions_out;    // policy
