@@ -13,7 +13,7 @@ import numpy as np
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG_DIR, "libjss_b200.so")
 
-JSS_ABI_VERSION = 2
+JSS_ABI_VERSION = 3
 ACTION_SKIP, ACTION_ADVANCE = -1, -2
 CREATE_AUTO_RESET, CREATE_RECORD_SOLUTION, CREATE_HOST_MIRROR = 1, 2, 4
 FLAG_DONE, FLAG_ERROR, FLAG_NOOP_LEGAL = 1, 2, 4
@@ -60,6 +60,8 @@ SIGNATURES = {
     "jss_set_cr_due_date_factor": (c_int, [_VP, c_double]),
     "jss_step_sample": (c_int, [_VP, _VP, c_int, c_int, c_uint64, c_uint64, _VP, _VP]),
     "jss_step_logits": (c_int, [_VP, _VP, c_int64, c_uint64, c_uint64, _VP, _VP, _VP]),
+    "jss_step_logits_record": (c_int, [_VP, _VP, c_int64, c_uint64, c_uint64, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "jss_refresh_obs": (c_int, [_VP, _VP]),
     "jss_rollout": (c_int, [_VP, c_int, c_uint64, c_uint64, c_int, c_int, _VP]),
     "jss_rollout_traj": (c_int, [_VP, c_int, c_uint64, c_uint64, c_int, _VP, _VP, _VP, _VP, _VP]),
     "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),

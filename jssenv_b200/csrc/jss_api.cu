@@ -56,6 +56,7 @@ struct jss_handle {
     int sm_count = 0;
     std::string err;
     int64_t launches = 0;
+    bool obs_stale = false;                        // a recording step left real_obs behind the state blocks
     double cr_factor = 1.5;                        // CriticalRatio(due_date_factor), dispatching.py:337
 
     std::vector<JssInst> insts;
@@ -169,13 +170,14 @@ JssKernel step_kernel(const jss_t *h) {
 // tiles; a mixed batch runs one CTA per JssCtaRange, SMs x JSS_MIN_CTAS[2] of them.  Those are all resident unless the
 // batch holds instances with 129..256 jobs: that kernel fits one CTA per SM.
 int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
-    // SAMPLE: 0 none, 1 masked-uniform sampler, 2 dispatching rule, 3 action drawn from policy logits before the step
-    const int sample = a.logits ? 3 : a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
+    // SAMPLE: 0 none, 1 masked-uniform sampler, 2 dispatching rule, 3 action drawn from policy logits before the step,
+    // 4 the same draw with the outputs recorded into the caller's slot
+    const int sample = a.logits ? (a.traj_obs ? 4 : 3) : a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
     const JssKernel kern = sample == 0 ? step_kernel<0>(h) : sample == 1 ? step_kernel<1>(h)
-                         : sample == 2 ? step_kernel<2>(h) : step_kernel<3>(h);
+                         : sample == 2 ? step_kernel<2>(h) : sample == 3 ? step_kernel<3>(h) : step_kernel<4>(h);
     // only the rules that read the suffix sums stage them; the other launches leave their room to the L1
     a.stage = sample == 2 && jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
-    const JssSmemLayout &sl = sample == 3 ? h->sl_step_logits : a.stage & JSS_STAGE_REM ? h->sl_step_rem : h->sl_step;
+    const JssSmemLayout &sl = sample >= 3 ? h->sl_step_logits : a.stage & JSS_STAGE_REM ? h->sl_step_rem : h->sl_step;
     const size_t smem = smem_bytes(sl);
     int per_sm = 0, rc = ctas_per_sm(h, kern, smem, per_sm);
     if (rc) return rc;
@@ -191,10 +193,27 @@ int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
     return JSS_OK;
 }
 
+int launch_all(jss_t *h, JssLaunch a, cudaStream_t st);
+
+// rewrite real_obs from the state blocks if a recording step left it stale (jss_refresh_obs)
+int refresh_obs(jss_t *h, cudaStream_t st) {
+    if (!h->obs_stale) return JSS_OK;
+    JssLaunch a{};
+    a.mode = JSS_MODE_REFRESH;
+    if (int rc = launch_all(h, a, st)) return rc;
+    h->obs_stale = false;
+    return JSS_OK;
+}
+
 int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
+    // every launch that may read or partly rewrite real_obs brings it up to date first, so each entry point keeps its
+    // meaning after a recording step (a plain step rewrites only the envs it changes)
+    const bool recording = a.mode == JSS_MODE_STEP && a.traj_obs;
+    if (!recording && a.mode != JSS_MODE_EXPORT && a.mode != JSS_MODE_POLICY && a.mode != JSS_MODE_REFRESH)
+        if (int rc = refresh_obs(h, st)) return rc;
     if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
-    // the generic kernel: MODE = JSS_MODE_RESET also serves export, import, pack and exporting steps
+    // the generic kernel: MODE = JSS_MODE_RESET also serves export, import, pack, refresh and exporting steps
     const JssKernel *kerns = a.mode == JSS_MODE_POLICY ? env_kernels<JSS_MODE_POLICY>
                            : a.mode == JSS_MODE_ROLLOUT ? env_kernels<JSS_MODE_ROLLOUT> : env_kernels<JSS_MODE_RESET>;
     // what the launch reads: a rollout every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
@@ -638,21 +657,58 @@ int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mod
     return launch_all(h, a, (cudaStream_t)stream);
 }
 
-int jss_step_logits(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
-                    int32_t *actions_out_dev, float *log_prob_out_dev, void *stream) {
-    int rc = check_ready(h);
-    if (rc) return rc;
+namespace {
+// the checks and the launch arguments jss_step_logits and jss_step_logits_record share
+int logits_launch(jss_t *h, const char *what, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
+                  int32_t *actions_out_dev, float *log_prob_out_dev, JssLaunch &a) {
     if (!logits_dev || !actions_out_dev || ld < (int64_t)h->p.jobs_max + 1)
-        return fail(h, JSS_ERR_INVALID, "jss_step_logits: bad arguments (logits %p, actions_out %p, ld %lld < jobs_max + 1 = %d)",
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (logits %p, actions_out %p, ld %lld < jobs_max + 1 = %d)", what,
                     (const void *)logits_dev, (void *)actions_out_dev, (long long)ld, h->p.jobs_max + 1);
-    JssLaunch a{};
+    a = JssLaunch{};
     a.mode = JSS_MODE_STEP;
     a.logits = logits_dev;
     a.logits_ld = ld;
     a.actions_out = actions_out_dev;
     a.log_prob_out = log_prob_out_dev;
     a.hash_key = jss_hash_key(seed, step_index);
+    return JSS_OK;
+}
+}  // namespace
+
+int jss_step_logits(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
+                    int32_t *actions_out_dev, float *log_prob_out_dev, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    JssLaunch a;
+    if ((rc = logits_launch(h, "jss_step_logits", logits_dev, ld, seed, step_index, actions_out_dev, log_prob_out_dev, a)))
+        return rc;
     return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_step_logits_record(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
+                           int32_t *actions_out_dev, float *log_prob_out_dev, float *obs_out_dev, uint8_t *mask_out_dev,
+                           int32_t *scalars_out_dev, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    JssLaunch a;
+    if ((rc = logits_launch(h, "jss_step_logits_record", logits_dev, ld, seed, step_index, actions_out_dev,
+                            log_prob_out_dev, a)))
+        return rc;
+    // the kernels store observation rows by bulk copy and scalar records as 16-byte vectors
+    const auto aligned = [](const void *ptr) { return ptr && ((uintptr_t)ptr & 15u) == 0; };
+    if (!aligned(obs_out_dev) || !aligned(mask_out_dev) || !aligned(scalars_out_dev))
+        return fail(h, JSS_ERR_INVALID, "jss_step_logits_record: obs_out %p, mask_out %p and scalars_out %p must be "
+                    "16-byte aligned device pointers", (void *)obs_out_dev, (void *)mask_out_dev, (void *)scalars_out_dev);
+    a.traj_obs = obs_out_dev; a.traj_mask = mask_out_dev; a.traj_scalars = scalars_out_dev;
+    if ((rc = launch_all(h, a, (cudaStream_t)stream))) return rc;
+    h->obs_stale = true;
+    return JSS_OK;
+}
+
+int jss_refresh_obs(jss_t *h, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    return refresh_obs(h, (cudaStream_t)stream);
 }
 
 int jss_policy(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_index, int32_t *actions_dev,

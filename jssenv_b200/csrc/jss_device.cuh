@@ -1038,7 +1038,7 @@ struct JssSmemLayout {
     int32_t warp_stride;    // bytes per warp region
     int32_t scratch_words;  // observation staging (7 floats per job slot), >= 32 words
     int32_t off_scratch;    // step kernels: [mbarrier 16 B][state-in block][scratch][state-out block]; else 0
-    int32_t off_logits;     // step kernels with SAMPLE = 3: [logits row, J + 1 floats] behind state-out; else 0
+    int32_t off_logits;     // step kernels with SAMPLE = 3, 4: [logits row, J + 1 floats] behind state-out; else 0
 };
 static_assert(sizeof(JssParams) == 248 && sizeof(JssLaunch) == 240 && sizeof(JssSmemLayout) == 32 &&
               sizeof(JssTile) == 16 && sizeof(JssCtaRange) == 32,
@@ -1179,6 +1179,7 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
     s.flags = jss_uniform(s.flags);                      // one word read by every lane (see jss_uniform)
     if (mode == JSS_MODE_EXPORT) { env_export<KJ>(p, iv, s, env, lane); return; }
     if (mode == JSS_MODE_PACK) { env_pack<KJ>(a, iv, s, env, lane, scratch); return; }
+    if (mode == JSS_MODE_REFRESH) { env_emit_obs<KJ>(p, jss_out_default(p), iv, s, env, lane, scratch); return; }
     if (mode == JSS_MODE_POLICY) {
         const uint32_t h = jss_hash3(a.seed, genv, a.step_index);
         const int act = env_select_action<KJ>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor);
@@ -1278,6 +1279,9 @@ JSS_DEV void jss_pdl_wait() {}
 // rule) from the freshly computed state, so a policy-driven loop is one launch per step.
 // SAMPLE = 3 takes the env's action from the caller's policy logits BEFORE the step (jss_step_logits): the next env's
 // logits row is prefetched like its state block, by 4-byte cp.async into the warp's logits slot.
+// SAMPLE = 4 is SAMPLE = 3 with the outputs redirected (jss_step_logits_record): the observation goes to the caller's
+// rollout slot (a.traj_obs) instead of real_obs, the mask and the scalar record to the slot and the env's buffers, and
+// an env the step left unchanged is emitted into the slot as well.
 struct JssWarpSmem {        // per-warp shared-memory regions of the step kernels
     int32_t *state_in, *state_out;
     float *scratch, *logits;
@@ -1290,8 +1294,8 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
                             const JssWarpSmem &w, int warp, int lane, int tile, int tile_end, int tile_step, int &staged,
                             uint32_t &phase) {
     int env_next = -1, act_next = 0;
-    // start the bulk load of the state block of this warp's env of tile `next` and fetch its action (SAMPLE = 3: start
-    // the copy of its logits row, columns 0..J, one 4-byte cp.async per column)
+    // start the bulk load of the state block of this warp's env of tile `next` and fetch its action (SAMPLE = 3, 4:
+    // start the copy of its logits row, columns 0..J, one 4-byte cp.async per column)
     const auto prefetch = [&](int next) {
         env_next = -1;
         if (next >= tile_end) return;
@@ -1299,7 +1303,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
         env_next = t.env;
         if (env_next >= 0) {
             if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)t.off16 * 4, t.blk16 * 16u, w.mbar);
-            if (SAMPLE == 3) {
+            if (SAMPLE >= 3) {
                 const int J = UNI ? a.uni.J : p.inst[t.inst].J;
                 const float *src = a.logits + (size_t)env_next * (size_t)a.logits_ld;
                 for (int k = lane; k <= J; k += 32) jss_cp_async4(w.logits_sa + 4u * (uint32_t)k, src + k);
@@ -1329,7 +1333,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
             phase ^= 1u;
             env_load<KJ>(iv, w.state_in, lane, s);
             __syncwarp();                                // every lane has read the buffer
-            if (SAMPLE == 3) {
+            if (SAMPLE >= 3) {
                 jss_cp_async_wait();
                 __syncwarp();                            // every lane's columns of the logits row have landed
                 int act;
@@ -1360,7 +1364,23 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
             const int nxt = env_select_action<KJ, SAMPLE == 1>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor);
             if (lane == 0) a.actions_out[env] = nxt;
         }
-        if (changed) {
+        if (SAMPLE == 4) {
+            // The slot is fresh memory: every env's rows go there, an unchanged env's with the zero-reward record of
+            // jss_rollout_traj (env_step leaves raw at 0 then).  One body serves both cases: an unchanged env's block is
+            // rewritten as it was loaded plus its new flags (what env_store_flags_only leaves) and its mask row as it was
+            // last emitted.  With a branch per case, jss_step_mixed_kernel<4, false> needs a 16-byte stack, not 8.
+            const JssOut slot{a.traj_obs, a.traj_mask, a.traj_scalars};
+            env_store_to<KJ>(iv, w.state_out, lane, s);
+            const JssTileWarp t = jss_tile(p, a, UNI, tile, warp);
+            // the new state block and the observation rows leave in one bulk group, as in env_emit_all
+            env_emit_obs<KJ, true>(p, slot, iv, s, env, lane, w.scratch, w.scratch_sa, p.state + (size_t)t.off16 * 4,
+                                   w.state_out_sa, t.blk16 * 16u);
+            const bool noop = (s.flags & JSS_FLAG_NOOP_LEGAL) != 0u;
+            env_emit_mask<KJ>(p, jss_out_default(p), iv, s, env, lane, noop);
+            if (changed || s.flags != flags_in) env_emit_scalars<KJ>(jss_out_default(p), iv, s, env, lane, raw);
+            env_emit_mask<KJ>(p, slot, iv, s, env, lane, noop);
+            env_emit_scalars<KJ>(slot, iv, s, env, lane, raw);
+        } else if (changed) {
             // new state -> shared staging -> one bulk store (every word of the block is rewritten)
             env_store_to<KJ>(iv, w.state_out, lane, s);
             const JssTileWarp t = jss_tile(p, a, UNI, tile, warp);
@@ -1388,7 +1408,7 @@ JSS_DEV void jss_step_carve(const JssSmemLayout &sl, char *sm, int warp, JssWarp
     // state-out staging sits right behind the observation staging (both leave by bulk store)
     w.state_out = reinterpret_cast<int32_t *>(w.scratch + sl.scratch_words);
     w.state_out_sa = w.scratch_sa + sl.scratch_words * 4;
-    w.logits = reinterpret_cast<float *>(wbase + sl.off_logits);   // behind state-out (SAMPLE = 3 layouts only)
+    w.logits = reinterpret_cast<float *>(wbase + sl.off_logits);   // behind state-out (SAMPLE = 3, 4 layouts only)
     w.logits_sa = w.mbar + sl.off_logits;
 }
 

@@ -179,7 +179,8 @@ struct JssLaunch {           // per-launch arguments
     const int32_t *actions;  // step
     int32_t *actions_out;    // policy
     const uint8_t *env_mask; // reset / import
-    // rollout with trajectory recording: outputs of step k of env e go to slot k * n_envs + e of these buffers
+    // rollout with trajectory recording: outputs of step k of env e go to slot k * n_envs + e of these buffers;
+    // jss_step_logits_record: env e's observation, mask and scalar record go to row e of traj_obs / mask / scalars
     float *traj_obs; uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
     uint8_t *wire;           // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
     int32_t wire_stride;
@@ -198,5 +199,6 @@ struct JssLaunch {           // per-launch arguments
 #define JSS_MODE_EXPORT 4
 #define JSS_MODE_IMPORT 5
 #define JSS_MODE_PACK 6     // packed observation wire rows for the host-buffer path (jss_host_step_begin_packed)
+#define JSS_MODE_REFRESH 7  // rewrite real_obs from the state blocks (jss_refresh_obs)
 
 #define JSS_WARPS_PER_CTA 8

@@ -7,6 +7,8 @@ truncated, info)`` (jss_env.py:403-481) with ``obs = {"real_obs": (N, J, 7) floa
 the observation entries are LIVE ALIASES of the environment's buffers (here: device
 memory owned by the native library), the no-op is action index ``J``, actions are
 not validated beyond setting a per-env error bit, and ``truncated`` is always False.
+One exception to the live alias: after ``step_logits_record()``, which writes the observation into the caller's
+rollout slot instead, ``real_obs`` is stale until the next non-recording call or ``refresh_obs()``.
 """
 import ctypes
 from typing import Any, Dict, Optional, Union
@@ -110,6 +112,7 @@ class JssVecEnv:
         import torch
         self._mask_u8 = w(b.action_mask, (n, J + 1), np.uint8, d, strides=(b.mask_stride, 1))
         self.action_mask = self._mask_u8.view(torch.bool)
+        # stale after step_logits_record() until the next non-recording call or refresh_obs()
         self.real_obs = w(b.real_obs, (n, J, 7), np.float32, d)
         ss = (int(b.scalar_stride),)      # the five scalar outputs are fields of one 16-byte record per env
         self.reward = w(b.reward, (n,), np.float32, d, strides=ss)
@@ -206,6 +209,18 @@ class JssVecEnv:
         self._step_index += 1
         return self._obs(), self.reward, self.done, self._truncated, {}, out
 
+    def _logits_arg(self, logits, what):
+        """`logits` as an (N, >= J+1) float32 device tensor with unit column stride (converted only if needed), and its
+        row stride `ld` in elements."""
+        import torch
+        n, J = self.num_envs, self.jobs
+        x = torch.as_tensor(logits, device=self.device)
+        if x.dim() != 2 or x.shape[0] != n or x.shape[1] < J + 1:
+            raise ValueError(f"{what}: logits must have shape ({n}, >= {J + 1}), got {tuple(x.shape)}")
+        if x.dtype != torch.float32 or x.stride(1) != 1 or (n > 1 and x.stride(0) < J + 1):
+            x = x.to(torch.float32).contiguous()
+        return x, (x.stride(0) if n > 1 else max(x.stride(0), J + 1))
+
     def step_logits(self, logits, actions_out=None, log_prob_out=None):
         """Step every env with an action drawn from policy logits (jss_step_logits, one launch): a masked categorical
         draw (Gumbel-max over the legal actions, RNG counter ``self._step_index``), then the step.  `logits`: (N, >= J+1)
@@ -214,13 +229,8 @@ class JssVecEnv:
         A done env gets action 0 and log_prob 0, an env whose only legal action is the no-op gets J_i and 0, and an env
         whose legal logits are bad (NaN / +inf, or all -inf) gets the error bit, action JSS_ACTION_SKIP and NaN."""
         import torch
-        n, J = self.num_envs, self.jobs
-        x = torch.as_tensor(logits, device=self.device)
-        if x.dim() != 2 or x.shape[0] != n or x.shape[1] < J + 1:
-            raise ValueError(f"step_logits: logits must have shape ({n}, >= {J + 1}), got {tuple(x.shape)}")
-        if x.dtype != torch.float32 or x.stride(1) != 1 or (n > 1 and x.stride(0) < J + 1):
-            x = x.to(torch.float32).contiguous()
-        ld = x.stride(0) if n > 1 else max(x.stride(0), J + 1)
+        n = self.num_envs
+        x, ld = self._logits_arg(logits, "step_logits")
         if actions_out is None:
             actions_out = torch.empty(n, dtype=torch.int32, device=self.device)
         if log_prob_out is None:
@@ -233,6 +243,77 @@ class JssVecEnv:
         N.check(self._h, rc, "jss_step_logits")
         self._step_index += 1
         return self._obs(), self.reward, self.done, self._truncated, {"actions": actions_out, "log_prob": log_prob_out}
+
+    def logits_trajectory(self, n_steps: int, out: Optional[Dict[str, Any]] = None):
+        """Rollout buffers for `n_steps` recorded logits steps (step_logits_record), as device tensors:
+        ``real_obs`` (K+1, N, J, 7) f32, ``action_mask`` (K+1, N, J+1) bool, and ``actions``, ``log_prob``, ``reward``,
+        ``reward_raw``, ``done``, ``time``, each (K, N).  Allocated zero-filled, or `out` reused when it has K steps;
+        either way the current observation and mask are copied into slot 0 (after refresh_obs()), so that
+        ``real_obs[k]`` is what the network sees at step k and ``real_obs[K]`` is the bootstrap observation."""
+        import torch
+        K, n, J, ms = int(n_steps), self.num_envs, self.jobs, int(self._b.mask_stride)
+        if out is None or out["actions"].shape[0] != K:
+            dev = self.device
+            # each observation / mask slot starts 16-byte aligned (jss_step_logits_record), whatever N and J are
+            obs_w, mask_w = -(-n * J * 7 // 4) * 4, -(-n * ms // 16) * 16
+            out = {"_obs": torch.zeros((K + 1, obs_w), dtype=torch.float32, device=dev),
+                   "_mask": torch.zeros((K + 1, mask_w), dtype=torch.uint8, device=dev),
+                   "_scalars": torch.zeros((K, n, 4), dtype=torch.int32, device=dev),
+                   "actions": torch.zeros((K, n), dtype=torch.int32, device=dev),
+                   "log_prob": torch.zeros((K, n), dtype=torch.float32, device=dev)}
+            out["real_obs"] = out["_obs"][:, : n * J * 7].view(K + 1, n, J, 7)
+            out["_mask_rows"] = out["_mask"][:, : n * ms].view(K + 1, n, ms)
+            out["action_mask"] = out["_mask_rows"][:, :, : J + 1].view(torch.bool)
+            out["reward"] = out["_scalars"][:, :, 0].view(torch.float32)
+            out["reward_raw"] = out["_scalars"][:, :, 1]
+            out["time"] = out["_scalars"][:, :, 2]
+            out["done"] = out["_scalars"].view(torch.uint8)[:, :, 12].view(torch.bool)   # low byte of flags << 8 | done
+        self._check_trajectory(out, "logits_trajectory")
+        self.refresh_obs()
+        out["real_obs"][0].copy_(self.real_obs)
+        out["_mask_rows"][0][:, : J + 1].copy_(self._mask_u8)
+        return out
+
+    def _check_trajectory(self, traj, what):
+        """The number of steps K of a logits_trajectory() dict, after checking that every buffer the kernel writes has
+        this env's layout (a dict made for another env would let it write past the tensors)."""
+        import torch
+        K, n, J, ms = traj["actions"].shape[0], self.num_envs, self.jobs, int(self._b.mask_stride)
+        want = {"real_obs": ((K + 1, n, J, 7), torch.float32), "_mask_rows": ((K + 1, n, ms), torch.uint8),
+                "_scalars": ((K, n, 4), torch.int32), "actions": ((K, n), torch.int32),
+                "log_prob": ((K, n), torch.float32)}
+        for name, (shape, dt) in want.items():
+            t = traj[name]
+            if tuple(t.shape) != shape or t.dtype != dt or t.device != self.device or not t[0].is_contiguous():
+                raise ValueError(f"{what}: trajectory buffer {name!r} is {tuple(t.shape)} {t.dtype} on {t.device}, "
+                                 f"this env needs {shape} {dt} on {self.device} (rows contiguous)")
+        return K
+
+    def step_logits_record(self, logits, traj: Dict[str, Any], k: int):
+        """step_logits() that records transition `k` straight into `traj` (a logits_trajectory() dict) in the same
+        launch (jss_step_logits_record): ``actions[k]``, ``log_prob[k]``, ``reward[k]``, ``reward_raw[k]``, ``done[k]``,
+        ``time[k]`` and the next observation ``real_obs[k+1]`` / ``action_mask[k+1]``.  An env the step left unchanged
+        (frozen done, error bit) records reward 0.  The env's own action_mask, rewards, state and statistics end up
+        exactly as after step_logits(); its real_obs is left stale (see refresh_obs()).  Returns the step tuple of the
+        slot's views."""
+        K = self._check_trajectory(traj, "step_logits_record")
+        if not 0 <= k < K:
+            raise ValueError(f"step_logits_record: step {k} outside the trajectory's {K} steps")
+        x, ld = self._logits_arg(logits, "step_logits_record")
+        acts, logp = traj["actions"][k], traj["log_prob"][k]
+        rc = self._L.jss_step_logits_record(self._h, x.data_ptr(), int(ld), self.seed, self._step_index, acts.data_ptr(),
+                                            logp.data_ptr(), traj["real_obs"][k + 1].data_ptr(),
+                                            traj["_mask_rows"][k + 1].data_ptr(), traj["_scalars"][k].data_ptr(),
+                                            self._stream())
+        N.check(self._h, rc, "jss_step_logits_record")
+        self._step_index += 1
+        obs = {"real_obs": traj["real_obs"][k + 1], "action_mask": traj["action_mask"][k + 1]}
+        return obs, traj["reward"][k], traj["done"][k], self._truncated, {"actions": acts, "log_prob": logp}
+
+    def refresh_obs(self):
+        """Bring ``real_obs`` up to date after recording steps (jss_refresh_obs; nothing to do otherwise).  Every other
+        native call does this by itself, so it is only needed to read ``real_obs`` right after step_logits_record()."""
+        N.check(self._h, self._L.jss_refresh_obs(self._h, self._stream()), "jss_refresh_obs")
 
     def get_legal_actions(self):
         return self.action_mask
