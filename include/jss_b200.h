@@ -238,6 +238,43 @@ int jss_step_logits_record(jss_t *h, const float *logits_dev, int64_t ld, uint64
                            int32_t *actions_out_dev, float *log_prob_out_dev, float *obs_out_dev, uint8_t *mask_out_dev,
                            int32_t *scalars_out_dev, void *stream);
 
+/* Step a batch greedily or epsilon-greedily from action scores (greedy evaluation of a trained policy, epsilon-greedy collection
+ * for a value-based agent): chooses every env's action from its row of scores, then applies it exactly as jss_step()
+ * would, in one launch, and writes the chosen actions and their log-probabilities under the epsilon-greedy policy.
+ *   scores_dev: logits or Q-values, with the layout, ld rule and columns of jss_step_logits(); only legal columns are
+ *     read, and scores of illegal actions are ignored whatever their value, NaN and +-inf included.
+ *   Bad scores: the rule of jss_step_logits() (a legal score NaN or +inf, or every legal score -inf), so a tensor is
+ *     accepted or refused the same way by both calls: sticky JSS_FLAG_ERROR, env unchanged, JSS_ACTION_SKIP, log_prob
+ *     NaN.  The test comes before the coin: whether an env errors never depends on the RNG, also at epsilon = 1.
+ *   Greedy action g: the legal action with the largest score, ties to the lowest index, the scores compared as IEEE
+ *     floats (-0.0 and +0.0 tie): np.argmax / torch.argmax over the legal entries.
+ *   Exploration: with H = jss_hash_env, h_env = jss_hash3 of (seed, env_id_base + i, step_index) (jss_rng.h) and
+ *     T = floor(epsilon * 2^32) (computed in double, exact, 0 <= T <= 2^32), the env explores iff H(h_env, 0) < T, and
+ *     then takes the action jss_pick maps (H(h_env, 1), n) to, over the set bits of its action_mask in ascending order,
+ *     n the number of legal actions (a legal no-op included): the mapping of JSS_RULE_RANDOM.  The coin and the pick use separate
+ *     hashes, so a small epsilon does not favour the lowest legal actions.  With epsilon = 0 the result does not depend
+ *     on seed or step_index.
+ *   log_prob_out_dev[i] = log((a == g ? 1 - e : 0) + e / n), e = T * 2^-32, in fp32: the log-probability of a under
+ *     the epsilon-greedy policy that chose it; exactly 0.0 whenever epsilon = 0.
+ *   Special cases: those of jss_step_logits() (done env: action 0, log_prob 0; only the no-op legal: action J_i,
+ *     log_prob 0, its score not read; no legal action at all: JSS_ACTION_SKIP, NaN).
+ *   actions_out_dev: device int32[N] (required); log_prob_out_dev: device fp32[N], NULL skips that store.
+ *   Returns JSS_ERR_INVALID for a NULL scores_dev / actions_out_dev, ld < jobs_max + 1, or epsilon NaN or outside
+ *   [0, 1].
+ * Bytes per ta80 env-step: 5 604, those of jss_step_logits().  Measured on an H100 SXM 80 GB HBM3 at a 700 W power
+ * limit (ta80, N = 65 536, median of three runs): 155.8 us per step at epsilon = 0 and 156.3 us at 0.05, against
+ * 260.5 us for masked_fill + argmax + jss_step() in torch and 159.9 us for jss_step_logits() (DESIGN.md section 4). */
+int jss_step_greedy(jss_t *h, const float *scores_dev, int64_t ld, double epsilon, uint64_t seed, uint64_t step_index,
+                    int32_t *actions_out_dev, float *log_prob_out_dev, void *stream);
+
+/* jss_step_greedy() that records the transition into the caller's rollout slot: it is to jss_step_greedy() what
+ * jss_step_logits_record() is to jss_step_logits().  The same slot layouts, 16-byte alignment rule (JSS_ERR_INVALID
+ * for a NULL or misaligned slot pointer) and zero-reward record of an unchanged env; real_obs is left stale
+ * (jss_refresh_obs()). */
+int jss_step_greedy_record(jss_t *h, const float *scores_dev, int64_t ld, double epsilon, uint64_t seed,
+                           uint64_t step_index, int32_t *actions_out_dev, float *log_prob_out_dev, float *obs_out_dev,
+                           uint8_t *mask_out_dev, int32_t *scalars_out_dev, void *stream);
+
 /* Rewrite real_obs from the state blocks after jss_step_logits_record(); returns at once when nothing is stale. */
 int jss_refresh_obs(jss_t *h, void *stream);
 

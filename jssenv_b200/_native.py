@@ -61,6 +61,8 @@ SIGNATURES = {
     "jss_step_sample": (c_int, [_VP, _VP, c_int, c_int, c_uint64, c_uint64, _VP, _VP]),
     "jss_step_logits": (c_int, [_VP, _VP, c_int64, c_uint64, c_uint64, _VP, _VP, _VP]),
     "jss_step_logits_record": (c_int, [_VP, _VP, c_int64, c_uint64, c_uint64, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "jss_step_greedy": (c_int, [_VP, _VP, c_int64, c_double, c_uint64, c_uint64, _VP, _VP, _VP]),
+    "jss_step_greedy_record": (c_int, [_VP, _VP, c_int64, c_double, c_uint64, c_uint64, _VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_refresh_obs": (c_int, [_VP, _VP]),
     "jss_rollout": (c_int, [_VP, c_int, c_uint64, c_uint64, c_int, c_int, _VP]),
     "jss_rollout_traj": (c_int, [_VP, c_int, c_uint64, c_uint64, c_int, _VP, _VP, _VP, _VP, _VP]),

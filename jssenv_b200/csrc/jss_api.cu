@@ -29,6 +29,7 @@ static cudaError_t jss_launch_pdl(void (*kern)(KArgs...), int grid, int block, s
 
 #include <algorithm>
 #include <climits>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -171,13 +172,17 @@ JssKernel step_kernel(const jss_t *h) {
 // batch holds instances with 129..256 jobs: that kernel fits one CTA per SM.
 int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
     // SAMPLE: 0 none, 1 masked-uniform sampler, 2 dispatching rule, 3 action drawn from policy logits before the step,
-    // 4 the same draw with the outputs recorded into the caller's slot
-    const int sample = a.logits ? (a.traj_obs ? 4 : 3) : a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
-    const JssKernel kern = sample == 0 ? step_kernel<0>(h) : sample == 1 ? step_kernel<1>(h)
-                         : sample == 2 ? step_kernel<2>(h) : sample == 3 ? step_kernel<3>(h) : step_kernel<4>(h);
+    // 4 the same draw with the outputs recorded into the caller's slot, 5 / 6 epsilon-greedy decode of the row (as 3 / 4)
+    const int sample = a.logits ? (a.greedy ? 5 : 3) + (a.traj_obs ? 1 : 0)
+                     : a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
+    static JssKernel (*const by_sample[])(const jss_t *) = {step_kernel<0>, step_kernel<1>, step_kernel<2>,
+                                                            step_kernel<3>, step_kernel<4>, step_kernel<5>,
+                                                            step_kernel<6>};
+    const JssKernel kern = by_sample[sample](h);
     // only the rules that read the suffix sums stage them; the other launches leave their room to the L1
     a.stage = sample == 2 && jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
-    const JssSmemLayout &sl = sample >= 3 ? h->sl_step_logits : a.stage & JSS_STAGE_REM ? h->sl_step_rem : h->sl_step;
+    const JssSmemLayout &sl = jss_step_takes_row(sample) ? h->sl_step_logits
+                            : a.stage & JSS_STAGE_REM ? h->sl_step_rem : h->sl_step;
     const size_t smem = smem_bytes(sl);
     int per_sm = 0, rc = ctas_per_sm(h, kern, smem, per_sm);
     if (rc) return rc;
@@ -673,6 +678,32 @@ int logits_launch(jss_t *h, const char *what, const float *logits_dev, int64_t l
     a.hash_key = jss_hash_key(seed, step_index);
     return JSS_OK;
 }
+
+// jss_step_greedy / _record: the checks and launch arguments of logits_launch, plus epsilon as the threshold
+// T = floor(epsilon 2^32) (exact in double, 0 .. 2^32) of the exploration coin
+int greedy_launch(jss_t *h, const char *what, const float *scores_dev, int64_t ld, double epsilon, uint64_t seed,
+                  uint64_t step_index, int32_t *actions_out_dev, float *log_prob_out_dev, JssLaunch &a) {
+    if (!(epsilon >= 0.0 && epsilon <= 1.0))
+        return fail(h, JSS_ERR_INVALID, "%s: epsilon %g is not in [0, 1]", what, epsilon);
+    if (int rc = logits_launch(h, what, scores_dev, ld, seed, step_index, actions_out_dev, log_prob_out_dev, a)) return rc;
+    a.greedy = 1;
+    a.explore_t = (uint64_t)std::floor(epsilon * 4294967296.0);
+    return JSS_OK;
+}
+
+// the recording step: the caller's slot pointers into `a`, then the launch, which leaves real_obs stale
+int launch_record(jss_t *h, const char *what, float *obs_out_dev, uint8_t *mask_out_dev, int32_t *scalars_out_dev,
+                  JssLaunch &a, cudaStream_t st) {
+    // the kernels store observation rows by bulk copy and scalar records as 16-byte vectors
+    const auto aligned = [](const void *ptr) { return ptr && ((uintptr_t)ptr & 15u) == 0; };
+    if (!aligned(obs_out_dev) || !aligned(mask_out_dev) || !aligned(scalars_out_dev))
+        return fail(h, JSS_ERR_INVALID, "%s: obs_out %p, mask_out %p and scalars_out %p must be 16-byte aligned device "
+                    "pointers", what, (void *)obs_out_dev, (void *)mask_out_dev, (void *)scalars_out_dev);
+    a.traj_obs = obs_out_dev; a.traj_mask = mask_out_dev; a.traj_scalars = scalars_out_dev;
+    if (int rc = launch_all(h, a, st)) return rc;
+    h->obs_stale = true;
+    return JSS_OK;
+}
 }  // namespace
 
 int jss_step_logits(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
@@ -688,21 +719,35 @@ int jss_step_logits(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed
 int jss_step_logits_record(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
                            int32_t *actions_out_dev, float *log_prob_out_dev, float *obs_out_dev, uint8_t *mask_out_dev,
                            int32_t *scalars_out_dev, void *stream) {
+    const char *what = "jss_step_logits_record";
     int rc = check_ready(h);
     if (rc) return rc;
     JssLaunch a;
-    if ((rc = logits_launch(h, "jss_step_logits_record", logits_dev, ld, seed, step_index, actions_out_dev,
+    if ((rc = logits_launch(h, what, logits_dev, ld, seed, step_index, actions_out_dev, log_prob_out_dev, a))) return rc;
+    return launch_record(h, what, obs_out_dev, mask_out_dev, scalars_out_dev, a, (cudaStream_t)stream);
+}
+
+int jss_step_greedy(jss_t *h, const float *scores_dev, int64_t ld, double epsilon, uint64_t seed, uint64_t step_index,
+                    int32_t *actions_out_dev, float *log_prob_out_dev, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    JssLaunch a;
+    if ((rc = greedy_launch(h, "jss_step_greedy", scores_dev, ld, epsilon, seed, step_index, actions_out_dev,
                             log_prob_out_dev, a)))
         return rc;
-    // the kernels store observation rows by bulk copy and scalar records as 16-byte vectors
-    const auto aligned = [](const void *ptr) { return ptr && ((uintptr_t)ptr & 15u) == 0; };
-    if (!aligned(obs_out_dev) || !aligned(mask_out_dev) || !aligned(scalars_out_dev))
-        return fail(h, JSS_ERR_INVALID, "jss_step_logits_record: obs_out %p, mask_out %p and scalars_out %p must be "
-                    "16-byte aligned device pointers", (void *)obs_out_dev, (void *)mask_out_dev, (void *)scalars_out_dev);
-    a.traj_obs = obs_out_dev; a.traj_mask = mask_out_dev; a.traj_scalars = scalars_out_dev;
-    if ((rc = launch_all(h, a, (cudaStream_t)stream))) return rc;
-    h->obs_stale = true;
-    return JSS_OK;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_step_greedy_record(jss_t *h, const float *scores_dev, int64_t ld, double epsilon, uint64_t seed,
+                           uint64_t step_index, int32_t *actions_out_dev, float *log_prob_out_dev, float *obs_out_dev,
+                           uint8_t *mask_out_dev, int32_t *scalars_out_dev, void *stream) {
+    const char *what = "jss_step_greedy_record";
+    int rc = check_ready(h);
+    if (rc) return rc;
+    JssLaunch a;
+    if ((rc = greedy_launch(h, what, scores_dev, ld, epsilon, seed, step_index, actions_out_dev, log_prob_out_dev, a)))
+        return rc;
+    return launch_record(h, what, obs_out_dev, mask_out_dev, scalars_out_dev, a, (cudaStream_t)stream);
 }
 
 int jss_refresh_obs(jss_t *h, void *stream) {

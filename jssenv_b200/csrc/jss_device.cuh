@@ -954,6 +954,67 @@ JSS_DEV int env_sample_logits(const InstView &iv, const EnvRegs<KJ> &s, int lane
     return act;
 }
 
+// Epsilon-greedy decode of a row of scores (logits or Q-values; jss_step_greedy).  The greedy action g is the legal
+// action with the largest score, ties to the lowest index, the scores compared as IEEE floats (-0 and +0 tie).  With
+// T = explore_t (0 .. 2^32, set on the host), the env explores iff jss_hash_env(h, 0) < T, and then takes the
+// masked-uniform pick of JSS_RULE_RANDOM drawn with jss_hash_env(h, 1): a separate hash, so that a small T does not
+// bias the pick to the lowest legal actions.  log_prob = log((a == g ? 1 - e : 0) + e / n), e = T * 2^-32, n = the
+// legal actions (the legal no-op included); exactly 0 for T = 0.  `row`, the special cases, the bad-row test (before
+// the coin, so it never depends on the RNG) and the return value are those of env_sample_logits.
+template <int KJ>
+JSS_DEV int env_greedy_scores(const InstView &iv, const EnvRegs<KJ> &s, int lane, const float *row, uint32_t h,
+                              uint64_t explore_t, int &act, float &logp) {
+    constexpr uint32_t LM = jss_legal_mask<KJ>();
+    const uint32_t flags = jss_uniform(s.flags);
+    const int J = jss_J(iv);
+    const bool noop = (flags & JSS_FLAG_NOOP_LEGAL) != 0u;
+    act = 0;
+    logp = 0.0f;
+    if (flags & JSS_FLAG_DONE) return 0;                 // reset or frozen by env_step, as with any action
+    if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u)) {      // only the no-op is legal (its score is not read)
+        act = noop ? J : JSS_ACTION_SKIP;
+        logp = noop ? 0.0f : JSS_F32_NAN;
+        return act;
+    }
+    // candidates: this lane's legal jobs in ascending order, then (lane 0) the legal no-op
+    bool bad = false;                                    // a legal score is NaN or +inf
+    uint32_t key = 0u;                                   // 0: below every candidate's key
+    int gidx = 1 << 20;
+#pragma unroll
+    for (int i = 0; i <= KJ; i++) {
+        const bool cand = i < KJ ? ((s.lb >> i) & 1u) != 0u : (lane == 0 && noop);
+        const int j = i < KJ ? KJ * lane + i : J;
+        if (cand) {
+            const float x = row[j];
+            bad = bad || !(x < JSS_F32_INF);
+            const uint32_t k = jss_f32_key(x + 0.0f);    // -0 + 0 = +0: jss_f32_key alone orders -0 below +0
+            if (k > key) { key = k; gidx = j; }
+        }
+    }
+    const uint32_t best = __reduce_max_sync(JSS_FULL, key);
+    if (__any_sync(JSS_FULL, bad) || jss_key_f32(best) == -JSS_F32_INF) {   // bad scores, or every legal one -inf
+        act = JSS_ACTION_SKIP;
+        logp = JSS_F32_NAN;
+        return JSS_INF;
+    }
+    const int g = (int)__reduce_min_sync(JSS_FULL, (unsigned)(key == best ? gidx : 1 << 20));
+    act = g;
+    if (explore_t != 0u) {                               // launch-uniform: a greedy launch neither counts nor draws
+        // the pick is env_select_action's JSS_RULE_RANDOM branch itself (its done / nothing-legal cases do not apply
+        // here).  n is its own REDUX.ADD: sharing the pick's prefix count means factoring it out of env_select_action,
+        // which changes the code of the masked-uniform step kernels (SAMPLE = 1).
+        if ((uint64_t)jss_hash_env(h, 0) < explore_t)
+            act = env_select_action<KJ, true>(iv, s, lane, JSS_RULE_RANDOM, JSS_COIN_NEVER, jss_hash_env(h, 1), 0.0);
+        const float n = (float)(__reduce_add_sync(JSS_FULL, (unsigned)__popc(s.lb & LM)) + (noop ? 1u : 0u));
+        const float e = (float)explore_t * 0x1p-32f;
+        // a == g: log(1 - y), y = e (n - 1) / n, through log1p while y is small (log would round 1 - y first); the
+        // 0 - y keeps y = 0 (n = 1) at log_prob +0
+        const float y = e * (n - 1.0f) / n;
+        logp = act != g ? logf(e / n) : y < 0.5f ? log1pf(0.0f - y) : logf((1.0f - e) + e / n);
+    }
+    return act;
+}
+
 // ---- canonical export / import (snapshot & restore; host attribute views) -------------
 template <int KJ>
 JSS_DEV void env_export(const JssParams &p, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane) {
@@ -1038,7 +1099,7 @@ struct JssSmemLayout {
     int32_t warp_stride;    // bytes per warp region
     int32_t scratch_words;  // observation staging (7 floats per job slot), >= 32 words
     int32_t off_scratch;    // step kernels: [mbarrier 16 B][state-in block][scratch][state-out block]; else 0
-    int32_t off_logits;     // step kernels with SAMPLE = 3, 4: [logits row, J + 1 floats] behind state-out; else 0
+    int32_t off_logits;     // step kernels that take a row: [logits row, J + 1 floats] behind state-out; else 0
 };
 static_assert(sizeof(JssParams) == 248 && sizeof(JssLaunch) == 240 && sizeof(JssSmemLayout) == 32 &&
               sizeof(JssTile) == 16 && sizeof(JssCtaRange) == 32,
@@ -1282,6 +1343,9 @@ JSS_DEV void jss_pdl_wait() {}
 // SAMPLE = 4 is SAMPLE = 3 with the outputs redirected (jss_step_logits_record): the observation goes to the caller's
 // rollout slot (a.traj_obs) instead of real_obs, the mask and the scalar record to the slot and the env's buffers, and
 // an env the step left unchanged is emitted into the slot as well.
+// SAMPLE = 5 / 6 are SAMPLE = 3 / 4 with the epsilon-greedy decode of the row (jss_step_greedy / _record).
+JSS_HD constexpr bool jss_step_takes_row(int sample) { return sample >= 3; }   // the action comes from a row (a.logits)
+JSS_HD constexpr bool jss_step_records(int sample) { return sample == 4 || sample == 6; }   // into the caller's slot
 struct JssWarpSmem {        // per-warp shared-memory regions of the step kernels
     int32_t *state_in, *state_out;
     float *scratch, *logits;
@@ -1293,9 +1357,10 @@ template <int KJ, int SAMPLE, bool UNI>
 JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv, const JssCtaSmem &c,
                             const JssWarpSmem &w, int warp, int lane, int tile, int tile_end, int tile_step, int &staged,
                             uint32_t &phase) {
+    constexpr bool ROW = jss_step_takes_row(SAMPLE), RECORD = jss_step_records(SAMPLE);
     int env_next = -1, act_next = 0;
-    // start the bulk load of the state block of this warp's env of tile `next` and fetch its action (SAMPLE = 3, 4:
-    // start the copy of its logits row, columns 0..J, one 4-byte cp.async per column)
+    // start the bulk load of the state block of this warp's env of tile `next` and fetch its action (a row: start the
+    // copy of its logits row, columns 0..J, one 4-byte cp.async per column)
     const auto prefetch = [&](int next) {
         env_next = -1;
         if (next >= tile_end) return;
@@ -1303,7 +1368,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
         env_next = t.env;
         if (env_next >= 0) {
             if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)t.off16 * 4, t.blk16 * 16u, w.mbar);
-            if (SAMPLE >= 3) {
+            if (ROW) {
                 const int J = UNI ? a.uni.J : p.inst[t.inst].J;
                 const float *src = a.logits + (size_t)env_next * (size_t)a.logits_ld;
                 for (int k = lane; k <= J; k += 32) jss_cp_async4(w.logits_sa + 4u * (uint32_t)k, src + k);
@@ -1333,13 +1398,14 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
             phase ^= 1u;
             env_load<KJ>(iv, w.state_in, lane, s);
             __syncwarp();                                // every lane has read the buffer
-            if (SAMPLE >= 3) {
+            if (ROW) {
                 jss_cp_async_wait();
                 __syncwarp();                            // every lane's columns of the logits row have landed
                 int act;
                 float logp;
-                action = env_sample_logits<KJ>(iv, s, lane, w.logits, jss_hash_env(a.hash_key, p.env_id_base + (uint64_t)env),
-                                               act, logp);
+                const uint32_t h = jss_hash_env(a.hash_key, p.env_id_base + (uint64_t)env);
+                action = SAMPLE >= 5 ? env_greedy_scores<KJ>(iv, s, lane, w.logits, h, a.explore_t, act, logp)
+                                     : env_sample_logits<KJ>(iv, s, lane, w.logits, h, act, logp);
                 if (lane == 0) {
                     a.actions_out[env] = act;
                     if (a.log_prob_out) a.log_prob_out[env] = logp;
@@ -1364,7 +1430,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
             const int nxt = env_select_action<KJ, SAMPLE == 1>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor);
             if (lane == 0) a.actions_out[env] = nxt;
         }
-        if (SAMPLE == 4) {
+        if (RECORD) {
             // The slot is fresh memory: every env's rows go there, an unchanged env's with the zero-reward record of
             // jss_rollout_traj (env_step leaves raw at 0 then).  One body serves both cases: an unchanged env's block is
             // rewritten as it was loaded plus its new flags (what env_store_flags_only leaves) and its mask row as it was
@@ -1408,7 +1474,7 @@ JSS_DEV void jss_step_carve(const JssSmemLayout &sl, char *sm, int warp, JssWarp
     // state-out staging sits right behind the observation staging (both leave by bulk store)
     w.state_out = reinterpret_cast<int32_t *>(w.scratch + sl.scratch_words);
     w.state_out_sa = w.scratch_sa + sl.scratch_words * 4;
-    w.logits = reinterpret_cast<float *>(wbase + sl.off_logits);   // behind state-out (SAMPLE = 3, 4 layouts only)
+    w.logits = reinterpret_cast<float *>(wbase + sl.off_logits);   // behind state-out (layouts of row steps only)
     w.logits_sa = w.mbar + sl.off_logits;
 }
 

@@ -170,9 +170,17 @@ struct JssParams {
 struct JssLaunch {           // per-launch arguments
     int32_t tile_begin, tile_end;
     int32_t mode;            // JSS_MODE_*
-    int32_t rule, coin_mode, n_steps, write_obs;
+    union {
+        int32_t rule;
+        int32_t greedy;      // steps from a row (a.logits): 0 categorical draw, 1 epsilon-greedy decode
+    };
+    int32_t coin_mode, n_steps, write_obs;
     int32_t export_after;    // step through the generic kernel: also decode the new state into the x_* arrays (facade)
-    uint64_t seed, step_index;
+    union {
+        uint64_t seed;
+        uint64_t explore_t;  // epsilon-greedy decode: an env explores iff jss_hash_env(h_env, 0) < explore_t, 0 .. 2^32
+    };
+    uint64_t step_index;
     uint32_t hash_key;       // jss_hash_key(seed, step_index), folded once per launch on the host (fused step + sampler)
     int32_t stage;           // JSS_STAGE_*: the instance tables the launch stages in shared memory (launch_all)
     double cr_factor;        // CriticalRatio due_date_factor (dispatching.py:337-349); reference default 1.5
@@ -180,13 +188,14 @@ struct JssLaunch {           // per-launch arguments
     int32_t *actions_out;    // policy
     const uint8_t *env_mask; // reset / import
     // rollout with trajectory recording: outputs of step k of env e go to slot k * n_envs + e of these buffers;
-    // jss_step_logits_record: env e's observation, mask and scalar record go to row e of traj_obs / mask / scalars
+    // jss_step_logits_record / jss_step_greedy_record: env e's observation, mask and scalar record go to row e of
+    // traj_obs / mask / scalars
     float *traj_obs; uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
     uint8_t *wire;           // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
     int32_t wire_stride;
     JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
-    // jss_step_logits: env i's logits at logits + i * logits_ld; the drawn actions go to actions_out, their
-    // log-probabilities to log_prob_out (may be NULL)
+    // jss_step_logits / jss_step_greedy: env i's logits (scores) at logits + i * logits_ld; the chosen actions go to
+    // actions_out, their log-probabilities to log_prob_out (may be NULL)
     const float *logits;
     float *log_prob_out;
     int64_t logits_ld;

@@ -7,8 +7,9 @@ truncated, info)`` (jss_env.py:403-481) with ``obs = {"real_obs": (N, J, 7) floa
 the observation entries are LIVE ALIASES of the environment's buffers (here: device
 memory owned by the native library), the no-op is action index ``J``, actions are
 not validated beyond setting a per-env error bit, and ``truncated`` is always False.
-One exception to the live alias: after ``step_logits_record()``, which writes the observation into the caller's
-rollout slot instead, ``real_obs`` is stale until the next non-recording call or ``refresh_obs()``.
+One exception to the live alias: after ``step_logits_record()`` or ``step_greedy_record()``, which write the
+observation into the caller's rollout slot instead, ``real_obs`` is stale until the next non-recording call or
+``refresh_obs()``.
 """
 import ctypes
 from typing import Any, Dict, Optional, Union
@@ -221,6 +222,50 @@ class JssVecEnv:
             x = x.to(torch.float32).contiguous()
         return x, (x.stride(0) if n > 1 else max(x.stride(0), J + 1))
 
+    @staticmethod
+    def _epsilon_arg(epsilon, what):
+        e = float(epsilon)
+        if not 0.0 <= e <= 1.0:                           # NaN included
+            raise ValueError(f"{what}: epsilon must be in [0, 1], got {epsilon!r}")
+        return e
+
+    def _row_call(self, what, x, ld, pre, acts, logp, slot=()):
+        """The native call of the steps that take their action from a row (`what` = step_logits, step_greedy or their
+        _record forms): jss_<what>(h, row, ld, *pre, seed, step_index, actions_out, log_prob_out, *slot, stream); then
+        the RNG counter advances."""
+        rc = getattr(self._L, "jss_" + what)(self._h, x.data_ptr(), int(ld), *pre, self.seed, self._step_index,
+                                             acts.data_ptr(), logp.data_ptr(), *slot, self._stream())
+        N.check(self._h, rc, "jss_" + what)
+        self._step_index += 1
+
+    def _row_step(self, what, rows, pre, actions_out, log_prob_out):
+        """step_logits / step_greedy: the row and output checks, the call, and the step tuple."""
+        import torch
+        n = self.num_envs
+        x, ld = self._logits_arg(rows, what)
+        if actions_out is None:
+            actions_out = torch.empty(n, dtype=torch.int32, device=self.device)
+        if log_prob_out is None:
+            log_prob_out = torch.empty(n, dtype=torch.float32, device=self.device)
+        for t, dt in ((actions_out, torch.int32), (log_prob_out, torch.float32)):
+            if t.dtype != dt or t.shape != (n,) or not t.is_contiguous() or t.device != x.device:
+                raise ValueError(f"{what}: outputs must be contiguous {dt} tensors of shape ({n},) on {x.device}")
+        self._row_call(what, x, ld, pre, actions_out, log_prob_out)
+        return self._obs(), self.reward, self.done, self._truncated, {"actions": actions_out, "log_prob": log_prob_out}
+
+    def _row_record(self, what, rows, pre, traj, k):
+        """step_logits_record / step_greedy_record: the trajectory and row checks, the call into slot `k`, and the step
+        tuple of the slot's views."""
+        K = self._check_trajectory(traj, what)
+        if not 0 <= k < K:
+            raise ValueError(f"{what}: step {k} outside the trajectory's {K} steps")
+        x, ld = self._logits_arg(rows, what)
+        acts, logp = traj["actions"][k], traj["log_prob"][k]
+        slot = (traj["real_obs"][k + 1].data_ptr(), traj["_mask_rows"][k + 1].data_ptr(), traj["_scalars"][k].data_ptr())
+        self._row_call(what, x, ld, pre, acts, logp, slot)
+        obs = {"real_obs": traj["real_obs"][k + 1], "action_mask": traj["action_mask"][k + 1]}
+        return obs, traj["reward"][k], traj["done"][k], self._truncated, {"actions": acts, "log_prob": logp}
+
     def step_logits(self, logits, actions_out=None, log_prob_out=None):
         """Step every env with an action drawn from policy logits (jss_step_logits, one launch): a masked categorical
         draw (Gumbel-max over the legal actions, RNG counter ``self._step_index``), then the step.  `logits`: (N, >= J+1)
@@ -228,21 +273,18 @@ class JssVecEnv:
         stride only if needed.  Returns the step tuple with ``{"actions": int32 (N,), "log_prob": float32 (N,)}`` as info.
         A done env gets action 0 and log_prob 0, an env whose only legal action is the no-op gets J_i and 0, and an env
         whose legal logits are bad (NaN / +inf, or all -inf) gets the error bit, action JSS_ACTION_SKIP and NaN."""
-        import torch
-        n = self.num_envs
-        x, ld = self._logits_arg(logits, "step_logits")
-        if actions_out is None:
-            actions_out = torch.empty(n, dtype=torch.int32, device=self.device)
-        if log_prob_out is None:
-            log_prob_out = torch.empty(n, dtype=torch.float32, device=self.device)
-        for t, dt in ((actions_out, torch.int32), (log_prob_out, torch.float32)):
-            if t.dtype != dt or t.shape != (n,) or not t.is_contiguous() or t.device != x.device:
-                raise ValueError(f"step_logits: outputs must be contiguous {dt} tensors of shape ({n},) on {x.device}")
-        rc = self._L.jss_step_logits(self._h, x.data_ptr(), int(ld), self.seed, self._step_index,
-                                     actions_out.data_ptr(), log_prob_out.data_ptr(), self._stream())
-        N.check(self._h, rc, "jss_step_logits")
-        self._step_index += 1
-        return self._obs(), self.reward, self.done, self._truncated, {"actions": actions_out, "log_prob": log_prob_out}
+        return self._row_step("step_logits", logits, (), actions_out, log_prob_out)
+
+    def step_greedy(self, scores, epsilon: float = 0.0, actions_out=None, log_prob_out=None):
+        """Step every env with the epsilon-greedy action of its scores (jss_step_greedy, one launch): the legal action
+        with the largest score (ties to the lowest index) with probability 1 - epsilon, else a uniformly random legal
+        action (RNG counter ``self._step_index``), then the step.  epsilon = 0 is greedy evaluation
+        (``deterministic=True``), epsilon > 0 the behaviour policy of a value-based agent.  `scores` (logits or
+        Q-values) are taken like step_logits' logits.  Returns the step tuple with ``{"actions", "log_prob"}`` as info;
+        log_prob is the action's log-probability under the epsilon-greedy policy (0 at epsilon = 0).  Done, no-op-only
+        and bad-score envs are handled as in step_logits()."""
+        e = self._epsilon_arg(epsilon, "step_greedy")
+        return self._row_step("step_greedy", scores, (e,), actions_out, log_prob_out)
 
     def logits_trajectory(self, n_steps: int, out: Optional[Dict[str, Any]] = None):
         """Rollout buffers for `n_steps` recorded logits steps (step_logits_record), as device tensors:
@@ -296,19 +338,13 @@ class JssVecEnv:
         (frozen done, error bit) records reward 0.  The env's own action_mask, rewards, state and statistics end up
         exactly as after step_logits(); its real_obs is left stale (see refresh_obs()).  Returns the step tuple of the
         slot's views."""
-        K = self._check_trajectory(traj, "step_logits_record")
-        if not 0 <= k < K:
-            raise ValueError(f"step_logits_record: step {k} outside the trajectory's {K} steps")
-        x, ld = self._logits_arg(logits, "step_logits_record")
-        acts, logp = traj["actions"][k], traj["log_prob"][k]
-        rc = self._L.jss_step_logits_record(self._h, x.data_ptr(), int(ld), self.seed, self._step_index, acts.data_ptr(),
-                                            logp.data_ptr(), traj["real_obs"][k + 1].data_ptr(),
-                                            traj["_mask_rows"][k + 1].data_ptr(), traj["_scalars"][k].data_ptr(),
-                                            self._stream())
-        N.check(self._h, rc, "jss_step_logits_record")
-        self._step_index += 1
-        obs = {"real_obs": traj["real_obs"][k + 1], "action_mask": traj["action_mask"][k + 1]}
-        return obs, traj["reward"][k], traj["done"][k], self._truncated, {"actions": acts, "log_prob": logp}
+        return self._row_record("step_logits_record", logits, (), traj, k)
+
+    def step_greedy_record(self, scores, traj: Dict[str, Any], k: int, epsilon: float = 0.0):
+        """step_greedy() that records transition `k` straight into `traj` (a logits_trajectory() dict) in the same
+        launch (jss_step_greedy_record), as step_logits_record() does for step_logits()."""
+        e = self._epsilon_arg(epsilon, "step_greedy_record")
+        return self._row_record("step_greedy_record", scores, (e,), traj, k)
 
     def refresh_obs(self):
         """Bring ``real_obs`` up to date after recording steps (jss_refresh_obs; nothing to do otherwise).  Every other
