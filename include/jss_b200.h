@@ -292,6 +292,37 @@ int jss_rollout(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_st
 int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_steps, float *traj_obs,
                      uint8_t *traj_mask, int32_t *traj_scalars, int32_t *traj_actions, void *stream);
 
+/* Runs a caller's static priority rule (DispatchingRule.run_episode, dispatching.py:21-75, with a table for the
+ * rule's key) to the end of every env's episode in one launch per lane class present: random-key / evolutionary
+ * metaheuristics scoring candidate priorities by makespan, one-shot priority policies, custom static rules.
+ *   Table: env i's priority of operation k of job j is prio_dev[i*ld_env + j*ld_job + k*ld_op] (device fp32), read
+ *     only for j < J_i and k < M_i.  Strides are in elements, may be 0 (broadcast) and are used in 64-bit index
+ *     arithmetic.  Only the entry of a legal job's current operation (k = todo_time_step_job[j]) is ever read.
+ *   Decision: among the legal jobs, the one with the largest priority; ties to the lowest job index; priorities are
+ *     compared as IEEE floats, so -0.0 and +0.0 tie (the argmax of jss_step_greedy()).  The no-op is taken only when no
+ *     job is legal and the no-op is (what the built-in rules do under JSS_COIN_NEVER).  There is no RNG: the result
+ *     does not depend on seed or step index.
+ *   Bad priorities (a NaN or +inf on a legal job's current operation, or every legal job at -inf: the bad-row rule of
+ *     jss_step_greedy()): the env gets the sticky JSS_FLAG_ERROR bit, is left in its state before that decision and
+ *     gets no further decisions in this call.
+ *   Loop: each env makes at most n_steps decisions and stops at the end of its episode.  An env never resets inside
+ *     the call, also under JSS_CREATE_AUTO_RESET, and an env that is done when the call starts is left untouched
+ *     (unlike jss_rollout(): the same table would only replay the same episode).  Episode statistics, solution
+ *     (JSS_CREATE_RECORD_SOLUTION) and jss_stats() are updated as by jss_step().  Afterwards every env's buffers
+ *     (real_obs, action_mask, the scalar record with the last transition's reward) hold its final state, as after
+ *     jss_rollout(write_obs = 0): an env equals a twin stepped with jss_step_greedy(rows, epsilon = 0) up to n_steps
+ *     times, rows[j] = the priority of job j's current operation and the no-op column -inf.
+ *   n_steps = 0 does nothing.  Returns JSS_ERR_INVALID for a NULL or not 4-byte-aligned prio_dev, a negative stride or
+ *     n_steps < 0, and JSS_ERR_STATE before jss_assign().
+ * Bytes per ta80 decision: the 4-byte priority of each legal job's current operation (L2 / HBM), nothing else; the
+ * state block is read and written once per call and the outputs written once.  Measured on an H100 SXM 80 GB HBM3 at
+ * a 700 W power limit (ta80, N = 65 536, reset to done, 2 000 decisions per episode, median of three rounds): 119.9 ms
+ * per batch with per-operation priorities (1.09 G decisions/s), against 1 259.8 ms for export_state + a torch gather
+ * + jss_step_greedy per decision; 118.1 ms with per-job priorities against 332.8 ms for the jss_step_greedy loop on
+ * the static row (DESIGN.md section 4). */
+int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op, int n_steps,
+                         void *stream);
+
 /* Host-buffer form of step(): copies actions H2D, steps, copies the results D2H with
  * contiguous DMA, synchronises.  Any output pointer may be NULL.  Host layouts equal the
  * device layouts: mask_host [N][mask_stride] bytes (row i: bytes 0..J_i), obs_host

@@ -220,7 +220,8 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
     // the generic kernel: MODE = JSS_MODE_RESET also serves export, import, pack, refresh and exporting steps
     const JssKernel *kerns = a.mode == JSS_MODE_POLICY ? env_kernels<JSS_MODE_POLICY>
-                           : a.mode == JSS_MODE_ROLLOUT ? env_kernels<JSS_MODE_ROLLOUT> : env_kernels<JSS_MODE_RESET>;
+                           : a.mode == JSS_MODE_ROLLOUT ? env_kernels<JSS_MODE_ROLLOUT>
+                           : a.mode == JSS_MODE_PRIORITY ? env_kernels<JSS_MODE_PRIORITY> : env_kernels<JSS_MODE_RESET>;
     // what the launch reads: a rollout every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
     // / CR), and the masked-uniform sampler no table at all (only J); the other modes ops / len
     a.stage = a.mode == JSS_MODE_ROLLOUT ? JSS_STAGE_ALL
@@ -794,6 +795,23 @@ int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int
     a.rule = rule; a.coin_mode = JSS_COIN_DEVICE; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
     a.n_steps = n_steps; a.write_obs = 1;
     a.traj_obs = traj_obs; a.traj_mask = traj_mask; a.traj_scalars = traj_scalars; a.traj_actions = traj_actions;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op, int n_steps,
+                         void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    if (!prio_dev || ((uintptr_t)prio_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || n_steps < 0)
+        return fail(h, JSS_ERR_INVALID, "jss_rollout_priority: bad arguments (prio %p must be 4-byte aligned, strides "
+                    "%lld / %lld / %lld >= 0, n_steps %d >= 0)", (const void *)prio_dev, (long long)ld_env,
+                    (long long)ld_job, (long long)ld_op, n_steps);
+    if (n_steps == 0) return JSS_OK;
+    JssLaunch a{};
+    a.mode = JSS_MODE_PRIORITY;
+    a.logits = prio_dev;
+    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
+    a.n_steps = n_steps;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 

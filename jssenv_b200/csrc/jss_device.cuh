@@ -954,6 +954,33 @@ JSS_DEV int env_sample_logits(const InstView &iv, const EnvRegs<KJ> &s, int lane
     return act;
 }
 
+// The legal action with the largest value, ties to the lowest index, the values compared as IEEE floats (-0 and +0
+// tie).  Candidates: this lane's legal jobs in ascending order, then (lane 0, if `noop`) the no-op J; `value(i, j)`
+// gives candidate j's value, i its slot in the lane (KJ for the no-op), and is called for candidates only.  Returns
+// false, leaving g alone, for a bad set: a candidate NaN or +inf, or every candidate -inf.  At least one job must be
+// legal.
+template <int KJ, typename Value>
+JSS_DEV bool env_legal_argmax(const EnvRegs<KJ> &s, int lane, int J, bool noop, const Value &value, int &g) {
+    bool bad = false;                                    // a candidate's value is NaN or +inf
+    uint32_t key = 0u;                                   // 0: below every candidate's key
+    int gidx = 1 << 20;
+#pragma unroll
+    for (int i = 0; i <= KJ; i++) {
+        const bool cand = i < KJ ? ((s.lb >> i) & 1u) != 0u : (lane == 0 && noop);
+        const int j = i < KJ ? KJ * lane + i : J;
+        if (cand) {
+            const float x = value(i, j);
+            bad = bad || !(x < JSS_F32_INF);
+            const uint32_t k = jss_f32_key(x + 0.0f);    // -0 + 0 = +0: jss_f32_key alone orders -0 below +0
+            if (k > key) { key = k; gidx = j; }
+        }
+    }
+    const uint32_t best = __reduce_max_sync(JSS_FULL, key);
+    if (__any_sync(JSS_FULL, bad) || jss_key_f32(best) == -JSS_F32_INF) return false;
+    g = (int)__reduce_min_sync(JSS_FULL, (unsigned)(key == best ? gidx : 1 << 20));
+    return true;
+}
+
 // Epsilon-greedy decode of a row of scores (logits or Q-values; jss_step_greedy).  The greedy action g is the legal
 // action with the largest score, ties to the lowest index, the scores compared as IEEE floats (-0 and +0 tie).  With
 // T = explore_t (0 .. 2^32, set on the host), the env explores iff jss_hash_env(h, 0) < T, and then takes the
@@ -976,28 +1003,12 @@ JSS_DEV int env_greedy_scores(const InstView &iv, const EnvRegs<KJ> &s, int lane
         logp = noop ? 0.0f : JSS_F32_NAN;
         return act;
     }
-    // candidates: this lane's legal jobs in ascending order, then (lane 0) the legal no-op
-    bool bad = false;                                    // a legal score is NaN or +inf
-    uint32_t key = 0u;                                   // 0: below every candidate's key
-    int gidx = 1 << 20;
-#pragma unroll
-    for (int i = 0; i <= KJ; i++) {
-        const bool cand = i < KJ ? ((s.lb >> i) & 1u) != 0u : (lane == 0 && noop);
-        const int j = i < KJ ? KJ * lane + i : J;
-        if (cand) {
-            const float x = row[j];
-            bad = bad || !(x < JSS_F32_INF);
-            const uint32_t k = jss_f32_key(x + 0.0f);    // -0 + 0 = +0: jss_f32_key alone orders -0 below +0
-            if (k > key) { key = k; gidx = j; }
-        }
-    }
-    const uint32_t best = __reduce_max_sync(JSS_FULL, key);
-    if (__any_sync(JSS_FULL, bad) || jss_key_f32(best) == -JSS_F32_INF) {   // bad scores, or every legal one -inf
+    int g;
+    if (!env_legal_argmax<KJ>(s, lane, J, noop, [&](int, int j) { return row[j]; }, g)) {   // bad, or all -inf
         act = JSS_ACTION_SKIP;
         logp = JSS_F32_NAN;
         return JSS_INF;
     }
-    const int g = (int)__reduce_min_sync(JSS_FULL, (unsigned)(key == best ? gidx : 1 << 20));
     act = g;
     if (explore_t != 0u) {                               // launch-uniform: a greedy launch neither counts nor draws
         // the pick is env_select_action's JSS_RULE_RANDOM branch itself (its done / nothing-legal cases do not apply
@@ -1013,6 +1024,24 @@ JSS_DEV int env_greedy_scores(const InstView &iv, const EnvRegs<KJ> &s, int lane
         logp = act != g ? logf(e / n) : y < 0.5f ? log1pf(0.0f - y) : logf((1.0f - e) + e / n);
     }
     return act;
+}
+
+// ---- caller's priority table (jss_rollout_priority) -------------------------------------------------------------
+// Env `env`'s next action under its priority table (a.logits, strides a.logits_ld / prio_ld_job / prio_ld_op): the
+// legal job whose current operation has the largest priority, by env_legal_argmax without the no-op; the no-op only
+// when no job is legal and it is.  Each lane loads the entries of its own legal jobs' current operations, nothing
+// else.  Returns JSS_INF for bad priorities and JSS_ACTION_SKIP when nothing is legal (an imported state).
+template <int KJ>
+JSS_DEV int env_priority_action(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane) {
+    constexpr uint32_t LM = jss_legal_mask<KJ>();
+    if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u))
+        return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
+    const float *row = a.logits + (int64_t)env * a.logits_ld;
+    int g = JSS_INF;
+    env_legal_argmax<KJ>(s, lane, jss_J(iv), false, [&](int i, int j) {
+        return row[(int64_t)j * a.prio_ld_job + (int64_t)jss_sel<KJ>(s.todo, i) * a.prio_ld_op];
+    }, g);
+    return g;
 }
 
 // ---- canonical export / import (snapshot & restore; host attribute views) -------------
@@ -1178,6 +1207,40 @@ JSS_DEV void env_store_flags_only(const JssParams &p, const InstView &iv, int32_
     }
 }
 
+// jss_rollout_priority: decisions (env_priority_action) until the episode ends, at most a.n_steps, without reset; a
+// done env is left as it is.  Bad priorities set the sticky error bit and end the env's call in its state before that
+// decision.  The outputs are written once at the end and equal what the jss_step_greedy calls the loop replaces leave:
+// the whole block and every output if a decision changed the env, else the flags and a zero-reward record if they
+// changed (the rollout's store covers only the first case, which its rules never leave).
+template <int KJ>
+JSS_DEV void env_priority_rollout(const JssParams &p, const JssLaunch &a, const InstView &iv, EnvRegs<KJ> &s, int32_t *blk,
+                                  int env, int lane, float *scratch) {
+    const uint32_t flags_in = s.flags;
+    bool dirty = false;
+    int raw = 0;                                         // the raw reward in the scalar record
+    for (int k = 0; k < a.n_steps && !(s.flags & JSS_FLAG_DONE); k++) {
+        const int act = jss_uniform(env_priority_action<KJ>(a, iv, s, env, lane));
+        if (act == JSS_ACTION_SKIP) break;               // nothing legal: no decision changes the env
+        const uint32_t flags_before = s.flags;
+        int r = 0;
+        bool changed = false;
+        if (act == JSS_INF) s.flags |= JSS_FLAG_ERROR;
+        else changed = env_step<KJ>(p, iv, s, env, lane, act, r, reinterpret_cast<int *>(scratch));
+        s.flags = jss_uniform(s.flags);
+        if (changed) { raw = r; dirty = true; continue; }
+        // unchanged, with the error bit (bad priorities, or a no-op without a pending event): every later decision
+        // would find the same state.  A new bit comes with a zero-reward record (env_store_flags_only).
+        if (s.flags != flags_before) raw = 0;
+        break;
+    }
+    if (dirty) {
+        env_store<KJ>(iv, blk, lane, s);
+        env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
+    } else if (s.flags != flags_in) {
+        env_store_flags_only<KJ>(p, iv, blk, s, env, lane);
+    }
+}
+
 // What warp `warp` of `tile` works on, and where that env's state block lives.  The kernels recompute it where they
 // store the block instead of carrying it in registers across a step or a rollout.
 struct JssTileWarp {
@@ -1241,6 +1304,7 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
     if (mode == JSS_MODE_EXPORT) { env_export<KJ>(p, iv, s, env, lane); return; }
     if (mode == JSS_MODE_PACK) { env_pack<KJ>(a, iv, s, env, lane, scratch); return; }
     if (mode == JSS_MODE_REFRESH) { env_emit_obs<KJ>(p, jss_out_default(p), iv, s, env, lane, scratch); return; }
+    if (MODE == JSS_MODE_PRIORITY) { env_priority_rollout<KJ>(p, a, iv, s, blk(), env, lane, scratch); return; }
     if (mode == JSS_MODE_POLICY) {
         const uint32_t h = jss_hash3(a.seed, genv, a.step_index);
         const int act = env_select_action<KJ>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor);
@@ -1291,8 +1355,15 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
     }
 }
 
+// Resident CTAs per SM the generic kernel is built for: one, except in the priority loop, which carries none of the
+// rules' code and keeps each env on chip for a whole episode, so that more warps per SM hide its latency.
+constexpr int JSS_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 3, 2};
+JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
+    return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)] : 1;
+}
+
 template <int KJ, int MODE>
-__global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, 1)
+__global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, jss_env_min_ctas(KJ, MODE))
 jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     JSS_SMEM_DECL(jss_smem);
     char *sm = reinterpret_cast<char *>(jss_smem);

@@ -179,8 +179,12 @@ struct JssLaunch {           // per-launch arguments
     union {
         uint64_t seed;
         uint64_t explore_t;  // epsilon-greedy decode: an env explores iff jss_hash_env(h_env, 0) < explore_t, 0 .. 2^32
+        int64_t prio_ld_job; // jss_rollout_priority: element stride between jobs of the priority table
     };
-    uint64_t step_index;
+    union {
+        uint64_t step_index;
+        int64_t prio_ld_op;  // jss_rollout_priority: element stride between operations of a job
+    };
     uint32_t hash_key;       // jss_hash_key(seed, step_index), folded once per launch on the host (fused step + sampler)
     int32_t stage;           // JSS_STAGE_*: the instance tables the launch stages in shared memory (launch_all)
     double cr_factor;        // CriticalRatio due_date_factor (dispatching.py:337-349); reference default 1.5
@@ -195,7 +199,8 @@ struct JssLaunch {           // per-launch arguments
     int32_t wire_stride;
     JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
     // jss_step_logits / jss_step_greedy: env i's logits (scores) at logits + i * logits_ld; the chosen actions go to
-    // actions_out, their log-probabilities to log_prob_out (may be NULL)
+    // actions_out, their log-probabilities to log_prob_out (may be NULL).  jss_rollout_priority: env i's priority of
+    // operation k of job j at logits + i * logits_ld + j * prio_ld_job + k * prio_ld_op
     const float *logits;
     float *log_prob_out;
     int64_t logits_ld;
@@ -209,5 +214,6 @@ struct JssLaunch {           // per-launch arguments
 #define JSS_MODE_IMPORT 5
 #define JSS_MODE_PACK 6     // packed observation wire rows for the host-buffer path (jss_host_step_begin_packed)
 #define JSS_MODE_REFRESH 7  // rewrite real_obs from the state blocks (jss_refresh_obs)
+#define JSS_MODE_PRIORITY 8 // run each env to the end of its episode on a caller's priority table (jss_rollout_priority)
 
 #define JSS_WARPS_PER_CTA 8

@@ -378,6 +378,31 @@ class JssVecEnv:
         self._step_index += int(n_steps)
         return self._obs(), self.reward, self.done, self._truncated, {}
 
+    def rollout_priority(self, priorities, n_steps: Optional[int] = None):
+        """Run a static priority rule to the end of every env's episode in one launch per lane class
+        (jss_rollout_priority): at each decision the legal job whose current operation has the largest priority
+        (ties to the lowest job index), the no-op only when no job is legal.  `priorities`: a 3-D tensor on the env's
+        device whose shape broadcasts to (N, J, M), J and M the batch maxima: (N, J, 1) gives one priority per job,
+        (1, J, M) one table for every env; converted to float32 only if needed.  Each env makes at most `n_steps`
+        decisions (default 2*J*M + 1, enough for any episode), never resets, and a done env is left untouched; bad
+        priorities (NaN / +inf on a legal current operation, or every legal job at -inf) set the error bit and stop
+        that env.  Returns the step tuple; the RNG counter does not advance."""
+        import torch
+        n, J, M = self.num_envs, self.jobs, self.machines
+        x = torch.as_tensor(priorities, device=self.device)
+        if x.dim() != 3 or any(s not in (1, t) for s, t in zip(x.shape, (n, J, M))):
+            raise ValueError(f"rollout_priority: priorities must be 3-D and broadcast to ({n}, {J}, {M}), "
+                             f"got {tuple(x.shape)}")
+        if x.dtype != torch.float32:
+            x = x.to(torch.float32)
+        v = x.expand(n, J, M)                            # broadcast dimensions get stride 0
+        if n_steps is None:
+            n_steps = 2 * J * M + 1
+        rc = self._L.jss_rollout_priority(self._h, v.data_ptr(), *(int(s) for s in v.stride()), int(n_steps),
+                                          self._stream())
+        N.check(self._h, rc, "jss_rollout_priority")
+        return self._obs(), self.reward, self.done, self._truncated, {}
+
     def rollout_record(self, rule: Union[str, int], n_steps: int, out: Optional[Dict[str, Any]] = None):
         """n_steps x (policy -> step) fused on device WITH the trajectory recorded (jss_rollout_traj): returns
         {"real_obs": (K, N, J, 7) f32, "action_mask": (K, N, J+1) bool, "reward": (K, N) f32, "done": (K, N) bool,
