@@ -323,6 +323,43 @@ int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int
 int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op, int n_steps,
                          void *stream);
 
+/* jss_rollout_priority() with every decision drawn from a softmax over a caller's logit table instead of its argmax,
+ * and each episode's log-probability and its gradient with respect to the table: sampling decoding of a one-shot
+ * scoring network (many schedules per instance from one broadcast table), ant-colony / cross-entropy search, and
+ * policy-gradient training of a network that emits per-operation logits once per instance.
+ *   Table, loop, done envs, outputs, n_steps = 0 and launches: those of jss_rollout_priority(), logits_dev in place of
+ *     prio_dev.  Only the entry of a legal job's current operation is ever read.
+ *   Decision d (0-based, counted per env within the call, no-op decisions included) of env i: with
+ *     h = jss_hash3(seed, env_id_base + i, step_index + d) and x_j the entry of job j's current operation, the
+ *     Gumbel-max draw of jss_step_logits() over the legal jobs, a = argmax(x_j + g_j) with g_j the Gumbel noise that
+ *     call draws for action j from h, ties to the lowest index, with log-probability x_a - mx - log sum exp(x - mx)
+ *     over the legal jobs (mx their maximum).
+ *     It equals, bit for bit, jss_step_logits(rows, seed, step_index + d) on the row rows[j] = x_j, no-op column -inf.
+ *     The no-op is taken only when no job is legal and it is; that decision draws nothing and has log-probability 0.
+ *   Bad entries (a NaN or +inf on a legal job's current operation, or every legal job at -inf: the bad-row rule of
+ *     jss_step_logits()): the env gets the sticky JSS_FLAG_ERROR bit, is left in its state before that decision and
+ *     gets no further decisions in this call.
+ *   log_prob_out_dev (device fp32 [N], required): env i's sum of its decisions' log-probabilities in this call, added
+ *     in fp32 in decision order; 0 for an env that is done at entry or makes no decision; NaN for an env a decision of
+ *     this call leaves with the error bit.
+ *   grad_out_dev (device fp32 [N][jobs_max][machines_max], contiguous: the layout of solution; NULL: no gradient):
+ *     G[i][j][k] = d log_prob_out[i] / d (env i's entry of operation k of job j)
+ *                = sum over env i's decisions t of (1[job j drawn at t] - p_t(j)) * 1[j legal at t and todo_j = k],
+ *     p_t the softmax over the legal jobs at t.  Every entry j < J_i, k < M_i is written, 0 for operations finished
+ *     before the call or never reached and for an env done at entry; an env that gets NaN gets all-zero rows, so that
+ *     masking it out leaves no NaN in a backward pass.  Entries past J_i / M_i are not written.  The kernel adds each
+ *     job's p_t in a register while its operation is current and stores the entry once, when the job is drawn: one
+ *     4-byte store per decision, the table of gradients is never read.
+ *   Returns JSS_ERR_INVALID for a NULL or not 4-byte-aligned logits_dev or log_prob_out_dev, a misaligned grad_out_dev,
+ *     a negative stride or n_steps < 0, and JSS_ERR_STATE before jss_assign().
+ * Measured on an H100 SXM 80 GB HBM3 at a 400 W power limit (ta80, N = 65 536, reset to done, 2 000 decisions per
+ * episode, median of three rounds): 156.6 ms per batch without the gradient, 162.2 ms with it and the torch backward,
+ * against 120.7 ms for jss_rollout_priority() on the same table and 1 330.1 ms for export_state + a torch gather +
+ * jss_step_logits per decision (DESIGN.md section 4). */
+int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                uint64_t seed, uint64_t step_index, int n_steps, float *log_prob_out_dev,
+                                float *grad_out_dev, void *stream);
+
 /* Host-buffer form of step(): copies actions H2D, steps, copies the results D2H with
  * contiguous DMA, synchronises.  Any output pointer may be NULL.  Host layouts equal the
  * device layouts: mask_host [N][mask_stride] bytes (row i: bytes 0..J_i), obs_host

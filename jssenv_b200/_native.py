@@ -67,6 +67,8 @@ SIGNATURES = {
     "jss_rollout": (c_int, [_VP, c_int, c_uint64, c_uint64, c_int, c_int, _VP]),
     "jss_rollout_traj": (c_int, [_VP, c_int, c_uint64, c_uint64, c_int, _VP, _VP, _VP, _VP, _VP]),
     "jss_rollout_priority": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_int, _VP]),
+    "jss_rollout_priority_sample": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int, _VP, _VP,
+                                            _VP]),
     "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_step_begin": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_wait": (c_int, [_VP, c_int]),

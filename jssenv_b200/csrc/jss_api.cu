@@ -221,7 +221,9 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     // the generic kernel: MODE = JSS_MODE_RESET also serves export, import, pack, refresh and exporting steps
     const JssKernel *kerns = a.mode == JSS_MODE_POLICY ? env_kernels<JSS_MODE_POLICY>
                            : a.mode == JSS_MODE_ROLLOUT ? env_kernels<JSS_MODE_ROLLOUT>
-                           : a.mode == JSS_MODE_PRIORITY ? env_kernels<JSS_MODE_PRIORITY> : env_kernels<JSS_MODE_RESET>;
+                           : a.mode == JSS_MODE_PRIORITY ? env_kernels<JSS_MODE_PRIORITY>
+                           : a.mode == JSS_MODE_PRIORITY_SAMPLE ? env_kernels<JSS_MODE_PRIORITY_SAMPLE>
+                           : env_kernels<JSS_MODE_RESET>;
     // what the launch reads: a rollout every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
     // / CR), and the masked-uniform sampler no table at all (only J); the other modes ops / len
     a.stage = a.mode == JSS_MODE_ROLLOUT ? JSS_STAGE_ALL
@@ -812,6 +814,30 @@ int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_
     a.logits = prio_dev;
     a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
     a.n_steps = n_steps;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                uint64_t seed, uint64_t step_index, int n_steps, float *log_prob_out_dev,
+                                float *grad_out_dev, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    if (!logits_dev || ((uintptr_t)logits_dev & 3u) || !log_prob_out_dev || ((uintptr_t)log_prob_out_dev & 3u) ||
+        ((uintptr_t)grad_out_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || n_steps < 0)
+        return fail(h, JSS_ERR_INVALID, "jss_rollout_priority_sample: bad arguments (logits %p and log_prob_out %p must "
+                    "be non-NULL, logits, log_prob_out and grad_out %p 4-byte aligned, strides %lld / %lld / %lld >= 0, "
+                    "n_steps %d >= 0)", (const void *)logits_dev, (void *)log_prob_out_dev, (void *)grad_out_dev,
+                    (long long)ld_env, (long long)ld_job, (long long)ld_op, n_steps);
+    if (n_steps == 0) return JSS_OK;
+    JssLaunch a{};
+    a.mode = JSS_MODE_PRIORITY_SAMPLE;
+    a.logits = logits_dev;
+    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
+    a.hash_key = jss_fold32(seed);                       // jss_hash3 reads the seed only through its fold
+    a.sample_step_index = step_index;
+    a.n_steps = n_steps;
+    a.log_prob_out = log_prob_out_dev;
+    a.grad_out = grad_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 

@@ -1044,6 +1044,62 @@ JSS_DEV int env_priority_action(const JssLaunch &a, const InstView &iv, const En
     return g;
 }
 
+// Env `env`'s next decision under its logit table (jss_rollout_priority_sample; the table as in env_priority_action):
+// the Gumbel-max draw of env_sample_logits over the legal jobs, x_j = the entry of job j's current operation.  It
+// equals env_sample_logits on the row x with the no-op column at -inf, bit for bit: the same keys and reductions, and
+// the sum of exponentials in the same order (the no-op's exp(-inf) adds +0).  Kept apart from env_sample_logits, which
+// reads a row in shared memory and puts the no-op among the candidates: a version shared with it would branch on both.
+// Writes logp = x_a - logsumexp(x) and each owned slot's p_i = softmax(x)_j (0 for a job that is not legal).  Returns
+// the drawn job; the no-op, logp and p left 0, when no job is legal and it is; JSS_INF for a bad table (the bad-row
+// rule of env_sample_logits); JSS_ACTION_SKIP when nothing is legal (an imported state).
+template <int KJ>
+JSS_DEV int env_priority_sample_action(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
+                                       uint32_t h, float &logp, float (&pr)[KJ]) {
+    constexpr uint32_t LM = jss_legal_mask<KJ>();
+    logp = 0.0f;
+#pragma unroll
+    for (int i = 0; i < KJ; i++) pr[i] = 0.0f;
+    if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u))
+        return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
+    const float *row = a.logits + (int64_t)env * a.logits_ld;
+    bool bad = false;                                    // a legal entry is NaN or +inf
+    uint32_t xkey = 0u, skey = 0u;                       // 0: below every candidate's key
+    int sidx = 1 << 20;
+    float x[KJ], sx = 0.0f;                              // sx: the entry of this lane's best candidate
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        x[i] = 0.0f;
+        if ((s.lb >> i) & 1u) {
+            const int j = KJ * lane + i;
+            x[i] = row[(int64_t)j * a.prio_ld_job + (int64_t)s.todo[i] * a.prio_ld_op];
+            bad = bad || !(x[i] < JSS_F32_INF);
+            xkey = max(xkey, jss_f32_key(x[i]));
+            const uint32_t k = jss_f32_key(x[i] + jss_gumbel(jss_hash_env(h, (uint64_t)j)));
+            if (k > skey) { skey = k; sidx = j; sx = x[i]; }
+        }
+    }
+    const float mx = jss_key_f32(__reduce_max_sync(JSS_FULL, xkey));
+    if (__any_sync(JSS_FULL, bad) || mx == -JSS_F32_INF) return JSS_INF;   // bad entries, or every legal one -inf
+    const uint32_t best = __reduce_max_sync(JSS_FULL, skey);
+    const int act = (int)__reduce_min_sync(JSS_FULL, (unsigned)(skey == best ? sidx : 1 << 20));
+    float sum = 0.0f;
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        if ((s.lb >> i) & 1u) {
+            pr[i] = jss_fast_exp(x[i] - mx);
+            sum += pr[i];
+        }
+    }
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) sum += __shfl_xor_sync(JSS_FULL, sum, off);   // the same sum in every lane
+    const float xa = __shfl_sync(JSS_FULL, sx, act / KJ);   // the drawn job's lane holds it as its best candidate
+    logp = (xa - mx) - jss_fast_log(sum);
+    const float inv = 1.0f / sum;
+#pragma unroll
+    for (int i = 0; i < KJ; i++) pr[i] *= inv;
+    return act;
+}
+
 // ---- canonical export / import (snapshot & restore; host attribute views) -------------
 template <int KJ>
 JSS_DEV void env_export(const JssParams &p, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane) {
@@ -1207,6 +1263,19 @@ JSS_DEV void env_store_flags_only(const JssParams &p, const InstView &iv, int32_
     }
 }
 
+// The end of a priority rollout: the whole block and every output if a decision changed the env, else the flags and a
+// zero-reward record if they changed.
+template <int KJ>
+JSS_DEV void env_store_rollout_end(const JssParams &p, const InstView &iv, int32_t *blk, const EnvRegs<KJ> &s, int env,
+                                   int lane, float *scratch, bool dirty, int raw, uint32_t flags_in) {
+    if (dirty) {
+        env_store<KJ>(iv, blk, lane, s);
+        env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
+    } else if (s.flags != flags_in) {
+        env_store_flags_only<KJ>(p, iv, blk, s, env, lane);
+    }
+}
+
 // jss_rollout_priority: decisions (env_priority_action) until the episode ends, at most a.n_steps, without reset; a
 // done env is left as it is.  Bad priorities set the sticky error bit and end the env's call in its state before that
 // decision.  The outputs are written once at the end and equal what the jss_step_greedy calls the loop replaces leave:
@@ -1233,12 +1302,88 @@ JSS_DEV void env_priority_rollout(const JssParams &p, const JssLaunch &a, const 
         if (s.flags != flags_before) raw = 0;
         break;
     }
-    if (dirty) {
-        env_store<KJ>(iv, blk, lane, s);
-        env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
-    } else if (s.flags != flags_in) {
-        env_store_flags_only<KJ>(p, iv, blk, s, env, lane);
+    env_store_rollout_end<KJ>(p, iv, blk, s, env, lane, scratch, dirty, raw, flags_in);
+}
+
+// jss_rollout_priority_sample: the loop of env_priority_rollout with the draws of env_priority_sample_action, decision
+// d with h = jss_hash3(seed, global env id, sample_step_index + d).  Besides its outputs: log_prob_out[env], the sum of
+// the decisions' log-probabilities in decision order (NaN if a decision of this call left the env unchanged with the
+// error bit), and, with grad_out, the gradient G of that sum with respect to the env's table entries,
+// G[j][k] = sum over the decisions t where job j is legal at operation k of (1[j drawn at t] - p_t(j)).  A job is legal
+// only at its current operation, which it leaves only after being drawn there, so each owned slot adds up its p_t in a
+// register and stores 1 - acc when drawn: one 4-byte store per decision, and the table of gradients is never read.  The
+// operations drawn before the call get 0, the first undrawn one at the end -acc and the later ones 0; an env that errs
+// gets 0
+// everywhere, so that a caller who masks it out gets no NaN in a backward pass.  Every store to a job's row comes from
+// the lane that owns the job, so program order orders them.
+template <int KJ>
+JSS_DEV void env_priority_sample_rollout(const JssParams &p, const JssLaunch &a, const InstView &iv, EnvRegs<KJ> &s,
+                                         int32_t *blk, int env, int lane, float *scratch) {
+    const int J = jss_J(iv), M = jss_M(iv);
+    float *grad = a.grad_out ? a.grad_out + (size_t)env * p.jobs_max * p.machines_max : nullptr;
+    const auto zero_ops = [&](int i, int k0, int k1) {   // operations k0 .. k1-1 of owned slot i
+        float *g = grad + (size_t)(KJ * lane + i) * p.machines_max;
+        for (int k = k0; k < k1; k++) g[k] = 0.0f;
+    };
+    // slot i's first operation not drawn yet: todo, or todo + 1 while the drawn operation todo runs (tufco > 0)
+    const auto undrawn = [&](int i) { return s.todo[i] + (s.tufco[i] > 0 ? 1 : 0); };
+    if (grad) {
+#pragma unroll
+        for (int i = 0; i < KJ; i++)
+            if (KJ * lane + i < J) zero_ops(i, 0, (s.flags & JSS_FLAG_DONE) ? M : undrawn(i));
     }
+    const uint64_t genv = p.env_id_base + (uint64_t)env;
+    const uint32_t flags_in = s.flags;
+    bool dirty = false, err = false;
+    int raw = 0;                                         // the raw reward in the scalar record
+    float lp = 0.0f, acc[KJ];
+#pragma unroll
+    for (int i = 0; i < KJ; i++) acc[i] = 0.0f;
+    for (int k = 0; k < a.n_steps && !(s.flags & JSS_FLAG_DONE); k++) {
+        const uint32_t h = jss_hash_env(jss_hash_key_folded(a.hash_key, a.sample_step_index + (uint64_t)k), genv);
+        float logp, pr[KJ];
+        const int act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
+        if (act == JSS_ACTION_SKIP) break;               // nothing legal: no decision changes the env
+        const uint32_t flags_before = s.flags;
+        int r = 0;
+        bool changed = false;
+        if (act == JSS_INF) {
+            s.flags |= JSS_FLAG_ERROR;
+        } else {
+            if (grad && act < J) {                       // a job drawn (act == J, the no-op, has no p_t)
+#pragma unroll
+                for (int i = 0; i < KJ; i++) {
+                    acc[i] += pr[i];
+                    if (KJ * lane + i == act) {
+                        grad[(size_t)act * p.machines_max + s.todo[i]] = 1.0f - acc[i];
+                        acc[i] = 0.0f;
+                    }
+                }
+            }
+            changed = env_step<KJ>(p, iv, s, env, lane, act, r, reinterpret_cast<int *>(scratch));
+        }
+        s.flags = jss_uniform(s.flags);
+        if (changed) { lp += logp; raw = r; dirty = true; continue; }
+        // unchanged, with the error bit: as in env_priority_rollout, and the call's log-probability is NaN
+        err = true;
+        if (s.flags != flags_before) raw = 0;
+        break;
+    }
+    if (grad) {
+#pragma unroll
+        for (int i = 0; i < KJ; i++) {
+            if (KJ * lane + i >= J) continue;
+            const int k0 = undrawn(i);
+            if (err) {
+                zero_ops(i, 0, M);
+            } else if (k0 < M) {
+                grad[(size_t)(KJ * lane + i) * p.machines_max + k0] = 0.0f - acc[i];   // +0 when never legal
+                zero_ops(i, k0 + 1, M);
+            }
+        }
+    }
+    if (lane == 0) a.log_prob_out[env] = err ? JSS_F32_NAN : lp;
+    env_store_rollout_end<KJ>(p, iv, blk, s, env, lane, scratch, dirty, raw, flags_in);
 }
 
 // What warp `warp` of `tile` works on, and where that env's state block lives.  The kernels recompute it where they
@@ -1305,6 +1450,10 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
     if (mode == JSS_MODE_PACK) { env_pack<KJ>(a, iv, s, env, lane, scratch); return; }
     if (mode == JSS_MODE_REFRESH) { env_emit_obs<KJ>(p, jss_out_default(p), iv, s, env, lane, scratch); return; }
     if (MODE == JSS_MODE_PRIORITY) { env_priority_rollout<KJ>(p, a, iv, s, blk(), env, lane, scratch); return; }
+    if (MODE == JSS_MODE_PRIORITY_SAMPLE) {
+        env_priority_sample_rollout<KJ>(p, a, iv, s, blk(), env, lane, scratch);
+        return;
+    }
     if (mode == JSS_MODE_POLICY) {
         const uint32_t h = jss_hash3(a.seed, genv, a.step_index);
         const int act = env_select_action<KJ>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor);
@@ -1357,9 +1506,13 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
 
 // Resident CTAs per SM the generic kernel is built for: one, except in the priority loop, which carries none of the
 // rules' code and keeps each env on chip for a whole episode, so that more warps per SM hide its latency.
+// The sampling loop likewise: the largest count per lane class that builds without a stack frame or spills (one CTA
+// more spills in every class).
 constexpr int JSS_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 3, 2};
+constexpr int JSS_PRIORITY_SAMPLE_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 2};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
-    return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)] : 1;
+    return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)] : 1;
 }
 
 template <int KJ, int MODE>

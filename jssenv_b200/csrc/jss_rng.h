@@ -36,6 +36,12 @@ JSS_HD static inline uint32_t jss_hash_env(uint32_t key, uint64_t env) {
     return h;
 }
 
+// jss_hash_key with the seed already folded: jss_hash_key(seed, ctr) == jss_hash_key_folded(jss_fold32(seed), ctr), so a
+// launch that varies the counter per env carries the seed in 32 bits
+JSS_HD static inline uint32_t jss_hash_key_folded(uint32_t seed_folded, uint64_t ctr) {
+    return seed_folded ^ (jss_fold32(ctr) * 0xC2B2AE3Du + 0x27D4EB2Fu);
+}
+
 // index in [0, count) -- multiply-high, no modulo bias worth speaking of
 JSS_HD static inline uint32_t jss_pick(uint32_t h, uint32_t count) {
     return (uint32_t)(((uint64_t)h * (uint64_t)count) >> 32);

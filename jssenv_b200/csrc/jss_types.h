@@ -185,22 +185,32 @@ struct JssLaunch {           // per-launch arguments
         uint64_t step_index;
         int64_t prio_ld_op;  // jss_rollout_priority: element stride between operations of a job
     };
-    uint32_t hash_key;       // jss_hash_key(seed, step_index), folded once per launch on the host (fused step + sampler)
+    uint32_t hash_key;       // jss_hash_key(seed, step_index), folded once per launch on the host (fused step + sampler);
+                             // jss_rollout_priority_sample: jss_fold32(seed), all of the seed that jss_hash3 reads
     int32_t stage;           // JSS_STAGE_*: the instance tables the launch stages in shared memory (launch_all)
-    double cr_factor;        // CriticalRatio due_date_factor (dispatching.py:337-349); reference default 1.5
+    union {
+        double cr_factor;    // CriticalRatio due_date_factor (dispatching.py:337-349); reference default 1.5
+        uint64_t sample_step_index;   // jss_rollout_priority_sample: the RNG counter of the env's first decision
+    };
     const int32_t *actions;  // step
     int32_t *actions_out;    // policy
     const uint8_t *env_mask; // reset / import
     // rollout with trajectory recording: outputs of step k of env e go to slot k * n_envs + e of these buffers;
     // jss_step_logits_record / jss_step_greedy_record: env e's observation, mask and scalar record go to row e of
-    // traj_obs / mask / scalars
-    float *traj_obs; uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
+    // traj_obs / mask / scalars.  jss_rollout_priority_sample: grad_out is the [N][jobs_max][machines_max] gradient of
+    // each env's log-probability with respect to its table entries (may be NULL)
+    union {
+        float *traj_obs;
+        float *grad_out;
+    };
+    uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
     uint8_t *wire;           // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
     int32_t wire_stride;
     JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
     // jss_step_logits / jss_step_greedy: env i's logits (scores) at logits + i * logits_ld; the chosen actions go to
-    // actions_out, their log-probabilities to log_prob_out (may be NULL).  jss_rollout_priority: env i's priority of
-    // operation k of job j at logits + i * logits_ld + j * prio_ld_job + k * prio_ld_op
+    // actions_out, their log-probabilities to log_prob_out (may be NULL).  jss_rollout_priority (_sample): env i's
+    // priority (logit) of operation k of job j at logits + i * logits_ld + j * prio_ld_job + k * prio_ld_op; _sample
+    // writes env i's episode log-probability to log_prob_out[i]
     const float *logits;
     float *log_prob_out;
     int64_t logits_ld;
@@ -215,5 +225,7 @@ struct JssLaunch {           // per-launch arguments
 #define JSS_MODE_PACK 6     // packed observation wire rows for the host-buffer path (jss_host_step_begin_packed)
 #define JSS_MODE_REFRESH 7  // rewrite real_obs from the state blocks (jss_refresh_obs)
 #define JSS_MODE_PRIORITY 8 // run each env to the end of its episode on a caller's priority table (jss_rollout_priority)
+#define JSS_MODE_PRIORITY_SAMPLE 9   // the same, each decision drawn from a softmax over the table's entries
+                                     // (jss_rollout_priority_sample)
 
 #define JSS_WARPS_PER_CTA 8

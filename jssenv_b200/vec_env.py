@@ -12,6 +12,7 @@ observation into the caller's rollout slot instead, ``real_obs`` is stale until 
 ``refresh_obs()``.
 """
 import ctypes
+import functools
 from typing import Any, Dict, Optional, Union
 
 import numpy as np
@@ -51,6 +52,31 @@ def _host_buffer(shape, dtype):
     does not declare ``pin_memory`` gets ordinary pageable memory."""
     import torch
     return torch.empty(shape, dtype=dtype, pin_memory=getattr(N.backend, "pin_memory", False))
+
+
+@functools.lru_cache(maxsize=None)
+def _sampled_log_prob():
+    """The autograd Function of JssVecEnv.rollout_priority_sample's log_prob (made on first use: torch is imported
+    lazily).  Forward runs the call with a gradient buffer; backward weights each env's gradient rows by the incoming
+    gradient and sums them over the table's broadcast dimensions."""
+    import torch
+
+    class SampledLogProb(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, logits, env, n_steps):
+            # zero-filled: the kernel leaves the entries past J_i / M_i alone, and a broadcast table sums over them
+            grad = torch.zeros((env.num_envs, env.jobs, env.machines), dtype=torch.float32, device=env.device)
+            log_prob = env._rollout_priority_sample(logits, n_steps, grad)
+            ctx.save_for_backward(grad)
+            ctx.shape, ctx.dtype = logits.shape, logits.dtype
+            return log_prob
+
+        @staticmethod
+        def backward(ctx, g):
+            (grad,) = ctx.saved_tensors
+            return (g[:, None, None] * grad).sum_to_size(ctx.shape).to(ctx.dtype), None, None
+
+    return SampledLogProb
 
 
 def _state_views(b, n, J, M, view):
@@ -402,6 +428,46 @@ class JssVecEnv:
                                           self._stream())
         N.check(self._h, rc, "jss_rollout_priority")
         return self._obs(), self.reward, self.done, self._truncated, {}
+
+    def rollout_priority_sample(self, logits, n_steps: Optional[int] = None):
+        """Run every env to the end of its episode in one launch per lane class, each decision drawn from the softmax
+        over the legal jobs of the entries of their current operations (jss_rollout_priority_sample; the no-op only
+        when no job is legal).  `logits` and `n_steps` are taken as rollout_priority's priorities and n_steps.  Decision
+        d of the call uses RNG counter ``self._step_index + d`` and equals a step_logits() draw on the gathered row;
+        the counter then advances by `n_steps`.  Returns the step tuple with ``{"log_prob": float32 (N,)}`` as info:
+        each env's sum of its decisions' log-probabilities in this call (NaN for an env that got the error bit).  When
+        `logits` requires grad (and grad mode is on), log_prob is differentiable with respect to it: the kernel also
+        writes d log_prob / d table, and broadcast tables such as (1, J, M) get the gradient summed over the envs."""
+        import torch
+        n, J, M = self.num_envs, self.jobs, self.machines
+        x = torch.as_tensor(logits, device=self.device)
+        if x.dim() != 3 or any(s not in (1, t) for s, t in zip(x.shape, (n, J, M))):
+            raise ValueError(f"rollout_priority_sample: logits must be 3-D and broadcast to ({n}, {J}, {M}), "
+                             f"got {tuple(x.shape)}")
+        n_steps = 2 * J * M + 1 if n_steps is None else int(n_steps)
+        if x.requires_grad and torch.is_grad_enabled():
+            log_prob = _sampled_log_prob().apply(x, self, n_steps)
+        else:
+            log_prob = self._rollout_priority_sample(x, n_steps, None)
+        return self._obs(), self.reward, self.done, self._truncated, {"log_prob": log_prob}
+
+    def _rollout_priority_sample(self, x, n_steps: int, grad_out):
+        """The native call of rollout_priority_sample on a checked table `x` (read through a detached float32 view,
+        strides passed through); writes the gradient to `grad_out` ((N, J, M) float32, or None); advances the RNG
+        counter.  Returns log_prob."""
+        import torch
+        n, J, M = self.num_envs, self.jobs, self.machines
+        v = x.detach()
+        if v.dtype != torch.float32:
+            v = v.to(torch.float32)
+        v = v.expand(n, J, M)                            # broadcast dimensions get stride 0
+        log_prob = torch.empty(n, dtype=torch.float32, device=self.device)
+        rc = self._L.jss_rollout_priority_sample(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
+                                                 self._step_index, n_steps, log_prob.data_ptr(), _ptr(grad_out),
+                                                 self._stream())
+        N.check(self._h, rc, "jss_rollout_priority_sample")
+        self._step_index += n_steps
+        return log_prob
 
     def rollout_record(self, rule: Union[str, int], n_steps: int, out: Optional[Dict[str, Any]] = None):
         """n_steps x (policy -> step) fused on device WITH the trajectory recorded (jss_rollout_traj): returns
