@@ -201,10 +201,15 @@ int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mod
  *     its jobs, column J_i its no-op (the columns of its action_mask row); columns past J_i are never read.
  *   Candidates: the actions legal in the env's current state (the action_mask the caller's network saw).  Logits of
  *     illegal actions are ignored whatever their value, NaN and +-inf included.
- *   Draw: Gumbel-max, a = argmax over legal a of logit[a] + g[a], g = -log(-log u[a]), ties to the lowest index, with
- *     u[a] = ((H(h_env, a) >> 8) + 0.5) * 2^-24, H = jss_hash_env and h_env = jss_hash3 of (seed, env_id_base + i,
- *     step_index) (jss_rng.h): replayable on the host and independent of sharding.  Computed in fp32.
- *   log_prob_out_dev[i] = logit[a] - logsumexp(legal logits), fp32, max-subtracted.
+ *   Draw: Gumbel-max, a = argmax over legal a of (logit[a] - mx) + g[a], mx the largest legal logit,
+ *     g = -log(-log u[a]), ties to the lowest index, with u[a] = ((H(h_env, a) >> 8) + 0.5) * 2^-24, H = jss_hash_env
+ *     and h_env = jss_hash3 of (seed, env_id_base + i, step_index) (jss_rng.h): replayable on the host and independent
+ *     of sharding.  Computed in fp32.  The key is max-subtracted so that the draw follows log_prob at any magnitude:
+ *     adding one constant to every legal logit changes neither the draw nor log_prob wherever it leaves their
+ *     differences exact, and tied logits at 1e30 are drawn uniformly.  Earlier builds keyed on logit[a] + g[a]: for
+ *     a given seed, the draw now differs from theirs only where the fp32 rounding of that sum decided it (large
+ *     logits, near ties).  The ABI is unchanged.
+ *   log_prob_out_dev[i] = (logit[a] - mx) - log sum exp(legal logits - mx), fp32.
  *   Special cases (as env_select_action / jss_step):
  *     done env: frozen, or reset under JSS_CREATE_AUTO_RESET, as by jss_step(); writes action 0, log_prob 0;
  *     only the no-op legal: action J_i, log_prob 0 (its logit is not read);
@@ -331,9 +336,10 @@ int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_
  *     prio_dev.  Only the entry of a legal job's current operation is ever read.
  *   Decision d (0-based, counted per env within the call, no-op decisions included) of env i: with
  *     h = jss_hash3(seed, env_id_base + i, step_index + d) and x_j the entry of job j's current operation, the
- *     Gumbel-max draw of jss_step_logits() over the legal jobs, a = argmax(x_j + g_j) with g_j the Gumbel noise that
- *     call draws for action j from h, ties to the lowest index, with log-probability x_a - mx - log sum exp(x - mx)
- *     over the legal jobs (mx their maximum).
+ *     Gumbel-max draw of jss_step_logits() over the legal jobs, a = argmax((x_j - mx) + g_j) in fp32 with mx the
+ *     largest legal x_j and g_j the Gumbel noise that call draws for action j from h, ties to the lowest index, with
+ *     log-probability (x_a - mx) - log sum exp(x - mx) over the legal jobs.  Like jss_step_logits(), it can draw
+ *     differently for a given seed than builds that keyed on x_j + g_j, where the fp32 rounding of that sum decided.
  *     It equals, bit for bit, jss_step_logits(rows, seed, step_index + d) on the row rows[j] = x_j, no-op column -inf.
  *     The no-op is taken only when no job is legal and it is; that decision draws nothing and has log-probability 0.
  *   Bad entries (a NaN or +inf on a legal job's current operation, or every legal job at -inf: the bad-row rule of

@@ -898,11 +898,14 @@ JSS_DEV float jss_gumbel(uint32_t bits) {
     return -jss_fast_log(e);
 }
 
-// Gumbel-max over the actions legal in the env's current state: a = argmax(logit[a] + g[a]) (lowest index on ties),
-// g[a] from jss_hash_env(h, a) with h = jss_hash3(seed, global env id, step_index), and
-// log_prob = logit[a] - logsumexp(legal logits).  `row` holds the env's logits, columns 0..J; only legal columns are
-// read.  Writes what the call reports to act / logp and returns the action to apply: the drawn one, 0 for a done env,
-// or, for bad logits, an out-of-range action, so that env_step sets the sticky error bit and changes nothing else.
+// Gumbel-max over the actions legal in the env's current state: a = argmax((logit[a] - mx) + g[a]) in fp32 (lowest
+// index on ties), mx the largest legal logit, g[a] from jss_hash_env(h, a) with h = jss_hash3(seed, global env id,
+// step_index), and log_prob = (logit[a] - mx) - log(sum exp(legal logit - mx)).  The key is formed on the max-
+// subtracted logit: on logit[a] itself, the noise would drown in the ulp of a large logit (every g lost at 1e30, ties
+// to the lowest index), and the draw would stop following the log_prob it reports.  `row` holds the env's logits,
+// columns 0..J; only legal columns are read.  Writes what the call reports to act / logp and returns the action to
+// apply: the drawn one, 0 for a done env, or, for bad logits, an out-of-range action, so that env_step sets the
+// sticky error bit and changes nothing else.
 template <int KJ>
 JSS_DEV int env_sample_logits(const InstView &iv, const EnvRegs<KJ> &s, int lane, const float *row, uint32_t h,
                               int &act, float &logp) {
@@ -920,18 +923,14 @@ JSS_DEV int env_sample_logits(const InstView &iv, const EnvRegs<KJ> &s, int lane
     }
     // candidates: this lane's legal jobs in ascending order, then (lane 0) the legal no-op
     bool bad = false;                                    // a legal logit is NaN or +inf
-    uint32_t xkey = 0u, skey = 0u;                       // 0: below every candidate's key
-    int sidx = 1 << 20;
+    uint32_t xkey = 0u;                                  // 0: below every candidate's key
 #pragma unroll
     for (int i = 0; i <= KJ; i++) {
         const bool cand = i < KJ ? ((s.lb >> i) & 1u) != 0u : (lane == 0 && noop);
-        const int j = i < KJ ? KJ * lane + i : J;
         if (cand) {
-            const float x = row[j];
+            const float x = row[i < KJ ? KJ * lane + i : J];
             bad = bad || !(x < JSS_F32_INF);
             xkey = max(xkey, jss_f32_key(x));
-            const uint32_t k = jss_f32_key(x + jss_gumbel(jss_hash_env(h, (uint64_t)j)));
-            if (k > skey) { skey = k; sidx = j; }
         }
     }
     const float mx = jss_key_f32(__reduce_max_sync(JSS_FULL, xkey));
@@ -940,14 +939,23 @@ JSS_DEV int env_sample_logits(const InstView &iv, const EnvRegs<KJ> &s, int lane
         logp = JSS_F32_NAN;
         return JSS_INF;
     }
-    const uint32_t best = __reduce_max_sync(JSS_FULL, skey);
-    act = (int)__reduce_min_sync(JSS_FULL, (unsigned)(skey == best ? sidx : 1 << 20));
+    // the keys and the exponentials in one pass over d = x - mx (-inf where x - mx overflows: never drawn)
+    uint32_t skey = 0u;                                  // 0: below every candidate's key
+    int sidx = 1 << 20;
     float sum = 0.0f;
 #pragma unroll
     for (int i = 0; i <= KJ; i++) {
         const bool cand = i < KJ ? ((s.lb >> i) & 1u) != 0u : (lane == 0 && noop);
-        if (cand) sum += jss_fast_exp(row[i < KJ ? KJ * lane + i : J] - mx);
+        const int j = i < KJ ? KJ * lane + i : J;
+        if (cand) {
+            const float d = row[j] - mx;
+            const uint32_t k = jss_f32_key(d + jss_gumbel(jss_hash_env(h, (uint64_t)j)));
+            if (k > skey) { skey = k; sidx = j; }
+            sum += jss_fast_exp(d);
+        }
     }
+    const uint32_t best = __reduce_max_sync(JSS_FULL, skey);
+    act = (int)__reduce_min_sync(JSS_FULL, (unsigned)(skey == best ? sidx : 1 << 20));
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) sum += __shfl_xor_sync(JSS_FULL, sum, off);   // the same sum in every lane
     logp = (row[act] - mx) - jss_fast_log(sum);
@@ -1063,37 +1071,39 @@ JSS_DEV int env_priority_sample_action(const JssLaunch &a, const InstView &iv, c
         return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
     const float *row = a.logits + (int64_t)env * a.logits_ld;
     bool bad = false;                                    // a legal entry is NaN or +inf
-    uint32_t xkey = 0u, skey = 0u;                       // 0: below every candidate's key
-    int sidx = 1 << 20;
-    float x[KJ], sx = 0.0f;                              // sx: the entry of this lane's best candidate
+    uint32_t xkey = 0u;                                  // 0: below every candidate's key
+    float x[KJ];
 #pragma unroll
     for (int i = 0; i < KJ; i++) {
         x[i] = 0.0f;
         if ((s.lb >> i) & 1u) {
-            const int j = KJ * lane + i;
-            x[i] = row[(int64_t)j * a.prio_ld_job + (int64_t)s.todo[i] * a.prio_ld_op];
+            x[i] = row[(int64_t)(KJ * lane + i) * a.prio_ld_job + (int64_t)s.todo[i] * a.prio_ld_op];
             bad = bad || !(x[i] < JSS_F32_INF);
             xkey = max(xkey, jss_f32_key(x[i]));
-            const uint32_t k = jss_f32_key(x[i] + jss_gumbel(jss_hash_env(h, (uint64_t)j)));
-            if (k > skey) { skey = k; sidx = j; sx = x[i]; }
         }
     }
     const float mx = jss_key_f32(__reduce_max_sync(JSS_FULL, xkey));
     if (__any_sync(JSS_FULL, bad) || mx == -JSS_F32_INF) return JSS_INF;   // bad entries, or every legal one -inf
-    const uint32_t best = __reduce_max_sync(JSS_FULL, skey);
-    const int act = (int)__reduce_min_sync(JSS_FULL, (unsigned)(skey == best ? sidx : 1 << 20));
-    float sum = 0.0f;
+    uint32_t skey = 0u;                                  // 0: below every candidate's key
+    int sidx = 1 << 20;
+    float sd = 0.0f, sum = 0.0f;                         // sd: x - mx of this lane's best candidate
 #pragma unroll
     for (int i = 0; i < KJ; i++) {
         if ((s.lb >> i) & 1u) {
-            pr[i] = jss_fast_exp(x[i] - mx);
+            const int j = KJ * lane + i;
+            const float d = x[i] - mx;
+            const uint32_t k = jss_f32_key(d + jss_gumbel(jss_hash_env(h, (uint64_t)j)));
+            if (k > skey) { skey = k; sidx = j; sd = d; }
+            pr[i] = jss_fast_exp(d);
             sum += pr[i];
         }
     }
+    const uint32_t best = __reduce_max_sync(JSS_FULL, skey);
+    const int act = (int)__reduce_min_sync(JSS_FULL, (unsigned)(skey == best ? sidx : 1 << 20));
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) sum += __shfl_xor_sync(JSS_FULL, sum, off);   // the same sum in every lane
-    const float xa = __shfl_sync(JSS_FULL, sx, act / KJ);   // the drawn job's lane holds it as its best candidate
-    logp = (xa - mx) - jss_fast_log(sum);
+    const float da = __shfl_sync(JSS_FULL, sd, act / KJ);   // the drawn job's lane holds it as its best candidate
+    logp = da - jss_fast_log(sum);
     const float inv = 1.0f / sum;
 #pragma unroll
     for (int i = 0; i < KJ; i++) pr[i] *= inv;

@@ -47,7 +47,9 @@ def gumbel(seed, env_id, step_index, n):
 def draw(logits, legal, done, seed, env_id, step_index):
     """One env's draw.  logits: its row (>= J+1 values), legal: bool[J+1] (the action_mask before the step),
     done: whether the env is done.  Returns (action, log_prob, error, scores): `error` tells whether the env gets the
-    sticky error bit, `scores` (float64[J+1], -inf off the candidates) are logit + g, or None if there was no draw."""
+    sticky error bit, `scores` (float64[J+1], -inf off the candidates) are (logit - mx) + g with mx the largest legal
+    logit, or None if there was no draw.  The scores are max-subtracted, as on the device: the same argmax as logit + g
+    in exact arithmetic, and in floating point they keep the noise when the logits are large (1e30 + g is 1e30)."""
     legal = np.asarray(legal, dtype=bool)
     J = legal.shape[0] - 1
     if done:
@@ -58,9 +60,9 @@ def draw(logits, legal, done, seed, env_id, step_index):
     x = np.asarray(logits, dtype=np.float64)[: J + 1][cand]
     if np.isnan(x).any() or np.isposinf(x).any() or np.isneginf(x).all():
         return ACTION_SKIP, float("nan"), True, None
-    scores = np.full(J + 1, -np.inf)
-    scores[cand] = x + gumbel(seed, env_id, step_index, J + 1)[cand]
-    a = int(np.argmax(scores))                            # first maximum: the lowest index on ties
     mx = x.max()
-    lse = mx + np.log(np.exp(x - mx).sum())
-    return a, float(logits[a]) - lse, False, scores
+    d = np.full(J + 1, -np.inf)
+    d[cand] = x - mx
+    scores = d + gumbel(seed, env_id, step_index, J + 1)
+    a = int(np.argmax(scores))                            # first maximum: the lowest index on ties
+    return a, float(d[a] - np.log(np.exp(d[cand]).sum())), False, scores

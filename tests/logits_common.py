@@ -54,17 +54,21 @@ def check_draws(env, logits, mask, done, acts, logp, step_index, flags_after, ct
     return twin, decisions, agree
 
 
-def check_step_logits(make_env, names, n_steps, seed, pad=3, state_every=25, auto_reset=True):
+def check_step_logits(make_env, names, n_steps, seed, pad=3, state_every=25, auto_reset=True, make_logits=None):
     """jss_step_logits on a batch, driven by seeded random logits (with -inf entries, huge values on illegal entries,
-    ld > J+1): every draw against the oracle, and a twin env stepped with jss_step(actions) bit-identical after every
-    step (the env of a bad-logits draw gets an out-of-range action there, which sets the same error bit)."""
+    ld > J+1; or `make_logits(rng, env, mask, ld, k)` at step k): every draw against the oracle, and a twin env
+    stepped with jss_step(actions) bit-identical after every step (the env of a bad-logits draw gets an out-of-range
+    action there, which sets the same error bit)."""
     a_env, b_env = twin_envs(make_env, names, sort=False, seed=seed, auto_reset=auto_reset)
     rng = np.random.default_rng(seed)
     ld = a_env.jobs + 1 + pad
     decisions = agree = 0
     for k in range(n_steps):
         mask, done = np_(a_env.action_mask).copy(), np_(a_env.done).copy()
-        logits = random_logits(rng, a_env, mask, ld, illegal=np.nan if k % 2 else 1e30)
+        if make_logits is None:
+            logits = random_logits(rng, a_env, mask, ld, illegal=np.nan if k % 2 else 1e30)
+        else:
+            logits = make_logits(rng, a_env, mask, ld, k)
         _, _, _, _, info = a_env.step_logits(_to_dev(a_env, logits))
         acts, logp = np_(info["actions"]).copy(), np_(info["log_prob"]).copy()
         twin, d, g = check_draws(a_env, logits, mask, done, acts, logp, k, np_(a_env.flags), f"step {k}")

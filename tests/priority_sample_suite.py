@@ -34,20 +34,24 @@ class Twin:
     def start(self):
         self.call = self._zero()
 
-    def steps(self, table, k, step_index):
-        """Up to k twin steps from RNG counter step_index (fewer once every env is done)."""
+    def steps(self, table, k, step_index, check=None):
+        """Up to k twin steps from RNG counter step_index (fewer once every env is done); `check(rows, mask, done,
+        actions, log_prob, counter)`, if given, sees each step's draw."""
         env = self.env
         J = env.jobs
         env._step_index = step_index
-        for _ in range(k):
+        for t in range(k):
             if np_(env.done).all():
                 return
             rows = greedy_rows(env, table)
             todo = np_(env.export_state()["todo"]).copy()
-            legal = np_(env.action_mask)[:, :J].copy()
+            mask = np_(env.action_mask).copy()
+            legal = mask[:, :J]
             done = np_(env.done).copy()
             _, _, _, _, info = env.step_logits(lc._to_dev(env, rows))
             acts, lp = np_(info["actions"]), np_(info["log_prob"])
+            if check is not None:
+                check(rows, mask, done, acts, lp, step_index + t)
             for d in (self.all, self.call):
                 d["log_prob"] = (d["log_prob"] + lp).astype(np.float32)
             for i in np.flatnonzero(~done):
