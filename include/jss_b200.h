@@ -366,6 +366,42 @@ int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_en
                                 uint64_t seed, uint64_t step_index, int n_steps, float *log_prob_out_dev,
                                 float *grad_out_dev, void *stream);
 
+/* Values every legal action of every env by a dispatching-rule rollout to the end of its episode, in one launch per
+ * lane class present, and changes nothing but the caller's table: the reference's copy.deepcopy(env) + step(a) +
+ * DispatchingRule.run_episode (dispatching.py:55-75) per legal action.  For the rollout (pilot) method -- take the
+ * action with the smallest value, repeat; with a deterministic rule never worse than the rule alone -- per-action
+ * teacher labels for imitation learning, and leaf values for tree search.
+ *   Candidates: the legal actions of env i's current state, the set bits of its action_mask row (jobs 0..J_i-1 and
+ *     the no-op J_i when it is legal).
+ *   Value: makespan_out_dev[i*ld + a] (device int32, 64-bit index arithmetic) is the current_time_step at which env
+ *     i's episode ends if it takes a now and then follows rule to the end.  The rule (any JSS_RULE_*, RANDOM
+ *     included) decides as jss_policy(rule, coin_mode, ...) would: its decision d (0-based, counted after the
+ *     candidate's step) hashes h = jss_hash3(seed, env_id_base + i, step_index + d), so every candidate of an env sees
+ *     the same random numbers, and CR uses the handle's due-date factor (jss_set_cr_due_date_factor()).  Equivalently,
+ *     a twin batch (same instances and env_id_base, auto-reset off, env i in the same state) stepped with a and then
+ *     with jss_policy(rule, coin_mode, seed, step_index + d) + jss_step() for d = 0, 1, ... until done ends at
+ *     current_time_step == makespan_out[i][a]; under JSS_COIN_DEVICE that tail is jss_rollout(rule, seed,
+ *     step_index, n).  Each candidate gets at most 2*J_i*M_i + 1 rule decisions (no episode is longer).
+ *   -1 is written for every column 0..J_i that is not a legal action, every column 0..J_i of an env that is done at
+ *     entry, and a candidate whose rollout stops before done: the rule finds nothing legal, a step leaves the env
+ *     unchanged with the error bit, or the bound trips (none of which a state reached from jss_reset() leads to).
+ *     Columns J_i+1 .. ld-1 are not written.
+ *   No side effects: state blocks, real_obs, action_mask, the scalar records, solution, episode statistics,
+ *     jss_stats(), flags and the stale-real_obs marker are as before, under JSS_CREATE_AUTO_RESET and
+ *     JSS_CREATE_RECORD_SOLUTION too.  An env with the sticky error bit is valued like any other.  The call reads only
+ *     the state blocks and neither needs nor triggers jss_refresh_obs().
+ *   Returns JSS_ERR_INVALID for a bad rule or coin mode, a NULL or not 4-byte-aligned makespan_out_dev or
+ *     ld < jobs_max + 1, and JSS_ERR_STATE before jss_assign().
+ * Bytes: per candidate the env's state block (L2) and one 4-byte store; per rule decision nothing beyond the staged
+ * instance tables.  One warp simulates one (env, candidate) at a time; a batch too small to fill the SMs spreads each
+ * env's candidates over several warps.  Measured on an H100 SXM 80 GB HBM3 at a 700 W power limit (MWR, device coin,
+ * median of three rounds): ta80 at N = 4 096 from reset 888.2 ms per call (409 600 candidates, 947 M decisions/s)
+ * against 1 969.5 ms for import_state + jss_step + jss_rollout per candidate column; after 500 random decisions 96.5
+ * against 1 631.3 ms; ta80 at N = 32 8.9 against 496.9 ms; ta01 at N = 65 536 101.3 against 185.0 ms (DESIGN.md
+ * section 4). */
+int jss_lookahead(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_index, int32_t *makespan_out_dev,
+                  int64_t ld, void *stream);
+
 /* Host-buffer form of step(): copies actions H2D, steps, copies the results D2H with
  * contiguous DMA, synchronises.  Any output pointer may be NULL.  Host layouts equal the
  * device layouts: mask_host [N][mask_stride] bytes (row i: bytes 0..J_i), obs_host

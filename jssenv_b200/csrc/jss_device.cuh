@@ -713,14 +713,15 @@ JSS_DEV void env_clear_solution(const JssParams &p, int env, int lane) {
 }
 
 // ---- step (jss_env.py:403-481) ---------------------------------------------------------
-// Returns true if the env changed (outputs must be re-emitted).
-template <int KJ>
+// Returns true if the env changed (outputs must be re-emitted).  BOOKKEEP = false (jss_lookahead's throw-away
+// simulations) changes nothing but the registers: no solution entry, no episode statistics, no auto-reset.
+template <int KJ, bool BOOKKEEP = true>
 JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, int env, int lane, int action,
                       int &raw_reward, int *hz) {
     raw_reward = 0;
     if (action == JSS_ACTION_SKIP) return false;
     if (s.flags & JSS_FLAG_DONE) {
-        if (p.create_flags & JSS_CREATE_AUTO_RESET) {
+        if (BOOKKEEP && (p.create_flags & JSS_CREATE_AUTO_RESET)) {
             env_reset_regs<KJ>(iv, s, lane);
             env_clear_solution(p, env, lane);
             return true;
@@ -745,7 +746,7 @@ JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, in
         s.tuam = ((uint32_t)lane == m_a) ? gain : s.tuam;            // :446
 #pragma unroll
         for (int i = 0; i < KJ; i++) s.tufco[i] = (lane == la && i == ia) ? gain : s.tufco[i];   // :447
-        if (p.solution && lane == la)                                 // :454
+        if (BOOKKEEP && p.solution && lane == la)                     // :454
             p.solution[((size_t)env * p.jobs_max + action) * p.machines_max + jss_sel<KJ>(s.todo, ia)] = s.t;
 #pragma unroll
         for (int i = 0; i < KJ; i++)
@@ -777,7 +778,7 @@ JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, in
     s.ep_return += raw_reward;
     if (nlegal == 0) {                                   // _is_done (:649)
         s.flags |= JSS_FLAG_DONE;
-        env_episode_end<KJ>(p, s, env, lane);
+        if (BOOKKEEP) env_episode_end<KJ>(p, s, env, lane);
     }
     return true;
 }
@@ -1423,6 +1424,46 @@ JSS_DEV JssTileWarp jss_tile(const JssParams &p, const JssLaunch &a, bool uni, i
     return t;
 }
 
+// ---- one-step lookahead over a dispatching rule (jss_lookahead) -------------------------------------------------
+// Work item (tile, sp) of a launch split S ways (a.n_steps): warp `warp` values its env of the tile at the candidates
+// c = sp, sp + S, ... <= J.  Each candidate is simulated in registers from the env's state block, which the call never
+// writes: load, step c, then the rule's decisions d = 0, 1, ... (RNG counter step_index + d, so every candidate of an
+// env sees the same numbers) until done, at most 2 J M + 1 of them, every step with env_step<KJ, false>.  Lane 0 stores
+// the end time, or -1 for an illegal candidate, an env done at entry, and a rollout that stops before done (the rule
+// finds nothing legal, a step leaves the env unchanged with the error bit, or the bound trips).  The block is reloaded
+// for each candidate (unchanged and L2-resident) instead of kept as a second register copy of the root state.
+template <int KJ>
+JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
+                           int lane, int sp, float *scratch) {
+    const int32_t *blk = p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4;
+    int32_t *out = a.actions_out + (int64_t)env * a.logits_ld;
+    const uint64_t genv = p.env_id_base + (uint64_t)env;
+    const int J = jss_J(iv), bound = 2 * J * jss_M(iv) + 1;
+    int *hz = reinterpret_cast<int *>(scratch);
+    for (int c = sp; c <= J; c += a.n_steps) {
+        EnvRegs<KJ> s;
+        env_load<KJ>(iv, blk, lane, s);
+        s.flags = jss_uniform(s.flags);
+        const uint32_t bits = __shfl_sync(JSS_FULL, s.lb, c < J ? c / KJ : 0);
+        const bool legal = !(s.flags & JSS_FLAG_DONE) &&
+                           (c < J ? ((bits >> (c % KJ)) & 1u) != 0u : (s.flags & JSS_FLAG_NOOP_LEGAL) != 0u);
+        int t = -1;
+        if (legal) {
+            int r;
+            bool ok = env_step<KJ, false>(p, iv, s, env, lane, c, r, hz);
+            s.flags = jss_uniform(s.flags);
+            for (int d = 0; ok && !(s.flags & JSS_FLAG_DONE) && d < bound; d++) {
+                const uint32_t h = jss_hash3(a.seed, genv, a.step_index + (uint64_t)d);
+                const int act = jss_uniform(env_select_action<KJ>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor));
+                ok = act != JSS_ACTION_SKIP && env_step<KJ, false>(p, iv, s, env, lane, act, r, hz);
+                s.flags = jss_uniform(s.flags);
+            }
+            if (s.flags & JSS_FLAG_DONE) t = s.t;
+        }
+        if (lane == 0) out[c] = t;
+    }
+}
+
 template <int KJ, int MODE>
 JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
                              int lane, float *scratch) {
@@ -1520,9 +1561,12 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
 // more spills in every class).
 constexpr int JSS_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 3, 2};
 constexpr int JSS_PRIORITY_SAMPLE_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 2};
+// The lookahead loop likewise (the rules' code, but no output emission).
+constexpr int JSS_LOOKAHEAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 4, 3, 2};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
     return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)] : 1;
+         : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_LOOKAHEAD ? JSS_LOOKAHEAD_MIN_CTAS[jss_lane_class(32 * KJ)] : 1;
 }
 
 template <int KJ, int MODE>
@@ -1535,6 +1579,25 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     jss_cta_carve(sl, sm, c, iv);
     const int warp = jss_warp_index(), lane = threadIdx.x & 31;
     float *scratch = reinterpret_cast<float *>(sm + sl.off_warp0 + warp * sl.warp_stride);
+    if (MODE == JSS_MODE_LOOKAHEAD) {
+        // work items (tile, sp), sp = 0 .. S-1, CTA-strided; a tile's S items are adjacent and share its instance
+        const int S = a.n_steps, n_items = (a.tile_end - a.tile_begin) * S;
+        int staged = -1;
+        for (int item = (int)blockIdx.x; item < n_items; item += (int)gridDim.x) {
+            const int tile = a.tile_begin + item / S;
+            const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, tile, warp);
+            const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
+            if (inst != staged) {                        // CTA-uniform
+                __syncthreads();
+                jss_stage_instance(p, p.inst[inst], c, JSS_STAGE_ALL);
+                staged = inst;
+                __syncthreads();
+            }
+            jss_iv_shape(iv);
+            if (env >= 0) env_lookahead<KJ>(p, a, iv, env, tile, warp, lane, item % S, scratch);
+        }
+        return;
+    }
     // a constant where MODE fixes the tables (the values launch_all sets): only a policy kernel branches on a.stage
     const int stage = MODE == JSS_MODE_POLICY ? a.stage : MODE == JSS_MODE_ROLLOUT ? JSS_STAGE_ALL : JSS_STAGE_OPS;
     int staged = -1;

@@ -469,6 +469,34 @@ class JssVecEnv:
         self._step_index += n_steps
         return log_prob
 
+    def lookahead(self, rule: Union[str, int] = "MWR", coin: str = "never", out=None):
+        """Value every legal action by a rollout of `rule` to the end of the episode, in one launch per lane class
+        (jss_lookahead), leaving the envs untouched: out[i, a] is the makespan env i reaches if it takes action a now
+        and then follows `rule` (as policy(rule, coin) with RNG counters ``self._step_index + d``, the same for every
+        action of an env), -1 for an action that is not legal, every action of a done env, and a rollout that stops
+        before done (only from an imported state).  Returns `out`, an (N, >= J+1) contiguous int32 device tensor;
+        by default a fresh (N, J+1) one filled with -1, so that the columns past an env's J_i read -1 too (the call
+        writes only columns 0..J_i).  coin="never" makes each value exact and the rollout method (take the argmin,
+        repeat) never worse than the rule alone; "device" gives the reference's 10 % wait draw.  The RNG counter
+        advances by 2*J*M + 1, the rule decisions a candidate may take."""
+        import torch
+        n, J = self.num_envs, self.jobs
+        if isinstance(rule, str) and rule.upper() not in N.RULES:
+            raise ValueError(f"lookahead: unknown rule {rule!r} (one of {sorted(N.RULES)})")
+        if coin not in ("never", "device"):
+            raise ValueError(f"lookahead: coin must be 'never' or 'device', got {coin!r}")
+        if out is None:
+            out = torch.full((n, J + 1), -1, dtype=torch.int32, device=self.device)
+        elif (not isinstance(out, torch.Tensor) or out.dtype != torch.int32 or out.dim() != 2 or out.shape[0] != n
+              or out.shape[1] < J + 1 or not out.is_contiguous() or out.device != self.device):
+            raise ValueError(f"lookahead: out must be a contiguous int32 tensor of shape ({n}, >= {J + 1}) on the "
+                             f"env's device")
+        rc = self._L.jss_lookahead(self._h, _rule_id(rule), _coin_id(coin), self.seed, self._step_index,
+                                   out.data_ptr(), int(out.shape[1]), self._stream())
+        N.check(self._h, rc, "jss_lookahead")
+        self._step_index += 2 * J * self.machines + 1
+        return out
+
     def rollout_record(self, rule: Union[str, int], n_steps: int, out: Optional[Dict[str, Any]] = None):
         """n_steps x (policy -> step) fused on device WITH the trajectory recorded (jss_rollout_traj): returns
         {"real_obs": (K, N, J, 7) f32, "action_mask": (K, N, J+1) bool, "reward": (K, N) f32, "done": (K, N) bool,
