@@ -102,7 +102,12 @@ typedef struct jss_buffers {
     int32_t machines_max;   /* M */
     int32_t mask_stride;    /* bytes per action_mask row (>= J+1, multiple of 4) */
     uint8_t *action_mask;   /* [N][mask_stride]; bytes 0..J_i = legal_actions of env i (jss_env.py:133) */
-    float *real_obs;        /* [N][J][7] fp32 (jss_env.py:102-111, 132)            */
+    float *real_obs;        /* [N][J][7] fp32 (jss_env.py:102-111, 132).  Invariant: at the entry of every
+                               step, real_obs[i] equals the observation of env i's state block, unless the handle
+                               has it marked stale (then the step re-emits it first).  The uniform-batch step
+                               kernels rely on it: they rewrite only the 32-byte sectors of a row the step changed.
+                               Every path that writes a state block emits the row or marks it stale; a caller must
+                               treat real_obs as read-only. */
     int32_t scalar_stride;  /* bytes between consecutive envs in the five per-env scalar arrays below
                                (they are fields of one 16-byte record per env, written with one store) */
     int32_t host_mirror;    /* 1: the output pointers below are host-readable (JSS_CREATE_HOST_MIRROR) */

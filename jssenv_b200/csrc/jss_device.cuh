@@ -60,6 +60,9 @@ struct EnvRegs {
     int t;             // current_time_step
     uint32_t flags;
     int ep_steps, ep_return;
+    // bit i: the step changed job slot i's row of real_obs (set conservatively; read only by the uniform step kernels'
+    // stores, which write back just the 32-byte sectors of the row that hold a marked job)
+    uint32_t dirty;
 };
 
 // ---- warp-uniformity hints -----------------------------------------------------------
@@ -405,7 +408,8 @@ JSS_DEV void env_reset_regs(const InstView &iv, EnvRegs<KJ> &s, int lane) {
 }
 
 // ---- increase_time_step (jss_env.py:495-637); returns hole_planning ---------------
-template <int KJ>
+// TRACK: mark in s.dirty the jobs whose rows the advance changes (the uniform step kernels' dirty-row stores)
+template <int KJ, bool TRACK = false>
 JSS_DEV int env_advance(const InstView &iv, EnvRegs<KJ> &s, int lane) {
     // next event = smallest positive machine countdown (the sorted event list of
     // the reference always equals {t + tuam[m] : tuam[m] > 0}, appendix A.1)
@@ -426,6 +430,7 @@ JSS_DEV int env_advance(const InstView &iv, EnvRegs<KJ> &s, int lane) {
         const bool running = was > 0;
         const bool finished = running && left <= 0;
         const bool waiting = !running && s.todo[i] < M;
+        if (TRACK) s.dirty |= (running || waiting) ? 1u << i : 0u;   // every unfinished job's row changes
         s.tufco[i] = left > 0 ? left : 0;                 // == max(0, was - diff); 0 stays 0
         const int slack = diff - was;                     // idle part of the step for a job finishing now
         s.total_idle[i] += finished ? slack : (waiting ? diff : 0);
@@ -582,7 +587,39 @@ struct JssOut {
 JSS_DEV JssOut jss_out_default(const JssParams &p) { return JssOut{p.obs, p.mask, p.scalars}; }
 
 // ---- observation / mask / reward (jss_env.py:102-134, 483-493) ---------------------
-template <int KJ, bool BULK = false>
+// The staged row (n16 16-byte chunks) leaves by the warp's own 16-byte stores, but only the chunks in a 32-byte sector
+// (absolute addresses: a row may start 16 bytes into one) that holds a job s.dirty marks: a sector is written whole or
+// not at all.  This relies on real_obs holding, at the step's entry, the observation of the state block it loaded
+// (jss_b200.h).  Bit k of word w of `sec`: sector 32 w + k counted from the one that holds dst[0].
+template <int KJ>
+JSS_DEV void env_store_dirty_row(const EnvRegs<KJ> &s, float *dst, const float *staged, int n16, int lane) {
+    constexpr int NW = (16 + 28 * 32 * KJ + 31) / 32 / 32 + 1;   // words for the largest row of the lane class
+    const int lead = (int)((uintptr_t)dst & 31u);
+    const int r0 = lead + 28 * KJ * lane;                    // this lane's first row byte, from dst's first sector
+    uint32_t loc = 0u;                                       // its jobs' sectors, from sector r0 >> 5 on
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        const int a = ((r0 & 31) + 28 * i) >> 5, b = ((r0 & 31) + 28 * i + 27) >> 5;
+        if (s.dirty & (1u << i)) loc |= (2u << b) - (1u << a);
+    }
+    const uint64_t v = (uint64_t)loc << ((r0 >> 5) & 31);
+    uint32_t sec[NW];
+#pragma unroll
+    for (int w = 0; w < NW; w++)
+        sec[w] = __reduce_or_sync(JSS_FULL, (r0 >> 10) == w ? (uint32_t)v : (r0 >> 10) + 1 == w ? (uint32_t)(v >> 32) : 0u);
+    // chunk k = lane + 32 it lies in sector 16 it + x: bit 16 (it & 1) + x of word it / 2 (or of the next word)
+    const int x = (lead + 16 * lane) >> 5;
+#pragma unroll
+    for (int it = 0; it < (56 * KJ + 31) / 32; it++) {   // 7 J / 4 <= 56 KJ chunks
+        const int k = lane + 32 * it, b = 16 * (it & 1) + x;
+        const uint32_t m = b < 32 ? sec[it / 2] : sec[it / 2 + 1 < NW ? it / 2 + 1 : NW - 1];
+        if (k < n16 && ((m >> (b & 31)) & 1u))
+            reinterpret_cast<float4 *>(dst)[k] = reinterpret_cast<const float4 *>(staged)[k];
+    }
+    __syncwarp();
+}
+
+template <int KJ, bool BULK = false, bool DIRTY = false>
 JSS_DEV void env_emit_obs(const JssParams &p, const JssOut &out, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
                           float *scratch, jss_saddr_t scratch_sa = jss_saddr_t(), void *st_dst = nullptr,
                           jss_saddr_t st_sa = jss_saddr_t(), uint32_t st_bytes = 0u) {
@@ -627,11 +664,13 @@ JSS_DEV void env_emit_obs(const JssParams &p, const JssOut &out, const InstView 
         __syncwarp();
         if (lane == 0) {
             if (st_bytes) jss_bulk_store(st_dst, st_sa, st_bytes);
-            if ((n & 3) == 0 && (p.jobs_max & 3) == 0) jss_bulk_store(dst, scratch_sa, (uint32_t)n * 4u);
+            if (!DIRTY && (n & 3) == 0 && (p.jobs_max & 3) == 0) jss_bulk_store(dst, scratch_sa, (uint32_t)n * 4u);
             jss_bulk_commit();           // ONE group for both copies (an empty group is legal)
         }
-        if ((n & 3) == 0 && (p.jobs_max & 3) == 0)
+        if ((n & 3) == 0 && (p.jobs_max & 3) == 0) {
+            if (DIRTY) env_store_dirty_row<KJ>(s, dst, scratch, n >> 2, lane);
             return;                      // the caller waits (wait_group.read) before reusing the staging buffers
+        }
     } else {
         __syncwarp();
     }
@@ -715,7 +754,7 @@ JSS_DEV void env_clear_solution(const JssParams &p, int env, int lane) {
 // ---- step (jss_env.py:403-481) ---------------------------------------------------------
 // Returns true if the env changed (outputs must be re-emitted).  BOOKKEEP = false (jss_lookahead's throw-away
 // simulations) changes nothing but the registers: no solution entry, no episode statistics, no auto-reset.
-template <int KJ, bool BOOKKEEP = true>
+template <int KJ, bool BOOKKEEP = true, bool TRACK = false>
 JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, int env, int lane, int action,
                       int &raw_reward, int *hz) {
     raw_reward = 0;
@@ -723,6 +762,7 @@ JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, in
     if (s.flags & JSS_FLAG_DONE) {
         if (BOOKKEEP && (p.create_flags & JSS_CREATE_AUTO_RESET)) {
             env_reset_regs<KJ>(iv, s, lane);
+            if (TRACK) s.dirty = ~0u;
             env_clear_solution(p, env, lane);
             return true;
         }
@@ -746,6 +786,7 @@ JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, in
         s.tuam = ((uint32_t)lane == m_a) ? gain : s.tuam;            // :446
 #pragma unroll
         for (int i = 0; i < KJ; i++) s.tufco[i] = (lane == la && i == ia) ? gain : s.tufco[i];   // :447
+        if (TRACK && lane == la) s.dirty |= 1u << ia;
         if (BOOKKEEP && p.solution && lane == la)                     // :454
             p.solution[((size_t)env * p.jobs_max + action) * p.machines_max + jss_sel<KJ>(s.todo, ia)] = s.t;
 #pragma unroll
@@ -761,7 +802,7 @@ JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, in
     for (;;) {
         st = __reduce_or_sync(JSS_FULL, ((s.lb & LM) != 0u ? 1u : 0u) | (s.tuam > 0 ? 2u : 0u));
         if (!(force || st == 2u)) break;                 // advance while nothing is legal and an event is pending
-        holes += env_advance<KJ>(iv, s, lane);
+        holes += env_advance<KJ, TRACK>(iv, s, lane);
         force = false;
         if (action == JSS_ACTION_ADVANCE) { raw_reward = -holes; return true; }   // heuristics / _is_done do NOT run
     }
@@ -1252,12 +1293,12 @@ JSS_DEV void jss_stage_instance(const JssParams &p, const JssInst &d, const JssC
     }
 }
 
-template <int KJ, bool BULK = false>
+template <int KJ, bool BULK = false, bool DIRTY = false>
 JSS_DEV void env_emit_all(const JssParams &p, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
                           float *scratch, int raw, jss_saddr_t scratch_sa = jss_saddr_t(), void *st_dst = nullptr,
                           jss_saddr_t st_sa = jss_saddr_t(), uint32_t st_bytes = 0u) {
     const JssOut out = jss_out_default(p);
-    env_emit_obs<KJ, BULK>(p, out, iv, s, env, lane, scratch, scratch_sa, st_dst, st_sa, st_bytes);
+    env_emit_obs<KJ, BULK, DIRTY>(p, out, iv, s, env, lane, scratch, scratch_sa, st_dst, st_sa, st_bytes);
     env_emit_mask<KJ>(p, out, iv, s, env, lane, (s.flags & JSS_FLAG_NOOP_LEGAL) != 0u);
     env_emit_scalars<KJ>(out, iv, s, env, lane, raw);
 }
@@ -1655,6 +1696,9 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
                             const JssWarpSmem &w, int warp, int lane, int tile, int tile_end, int tile_step, int &staged,
                             uint32_t &phase) {
     constexpr bool ROW = jss_step_takes_row(SAMPLE), RECORD = jss_step_records(SAMPLE);
+    // a uniform batch stepped by its actions or a rule stores only the changed sectors of a row (a row step, whose
+    // kernel also prefetches the row, has not been measured with it)
+    constexpr bool DIRTY = UNI && !ROW;
     int env_next = -1, act_next = 0;
     // start the bulk load of the state block of this warp's env of tile `next` and fetch its action (a row: start the
     // copy of its logits row, columns 0..J, one 4-byte cp.async per column)
@@ -1719,9 +1763,12 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
         // every lane holds the same flags word (one address, loaded by all lanes): say so -- ptxas already sees that
         // for the action and the time, a shuffle of those is folded away
         if (jss_hint_flags<KJ, UNI>()) s.flags = jss_uniform(s.flags);
-        const uint32_t flags_in = s.flags;
-        const bool changed = env_step<KJ>(p, iv, s, env, lane, action, raw, reinterpret_cast<int *>(w.scratch));
+        const uint32_t flags_in = s.flags, lb_in = s.lb;
+        if (DIRTY) s.dirty = 0u;
+        const bool changed =
+            env_step<KJ, true, DIRTY>(p, iv, s, env, lane, action, raw, reinterpret_cast<int *>(w.scratch));
         if (jss_hint_flags<KJ, UNI>()) s.flags = jss_uniform(s.flags);   // the no-op test returns from inside lane-dependent code
+        if (DIRTY) s.dirty |= (s.lb ^ lb_in) & jss_legal_mask<KJ>();   // a job's legal bit is column 0 of its row
         if (SAMPLE == 1 || SAMPLE == 2) {
             const uint32_t h = jss_hash_env(a.hash_key, p.env_id_base + (uint64_t)env);   // == jss_hash3(seed, genv, step_index)
             const int nxt = env_select_action<KJ, SAMPLE == 1>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor);
@@ -1747,7 +1794,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
             // new state -> shared staging -> one bulk store (every word of the block is rewritten)
             env_store_to<KJ>(iv, w.state_out, lane, s);
             const JssTileWarp t = jss_tile(p, a, UNI, tile, warp);
-            env_emit_all<KJ, true>(p, iv, s, env, lane, w.scratch, raw, w.scratch_sa,
+            env_emit_all<KJ, true, DIRTY>(p, iv, s, env, lane, w.scratch, raw, w.scratch_sa,
                                    p.state + (size_t)t.off16 * 4, w.state_out_sa, t.blk16 * 16u);
         } else if (s.flags != flags_in) {
             env_store_flags_only<KJ>(p, iv, p.state + (size_t)jss_tile(p, a, UNI, tile, warp).off16 * 4, s, env, lane);
