@@ -407,6 +407,41 @@ int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_en
 int jss_lookahead(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_index, int32_t *makespan_out_dev,
                   int64_t ld, void *stream);
 
+/* jss_lookahead() with the greedy decisions of a caller's priority table in place of a dispatching rule: every legal
+ * action of every env valued by a rollout of the table to the end of its episode, in one launch per lane class present,
+ * changing nothing but the caller's values.  The rollout method improves any deterministic base policy: the argmin of
+ * these values, taken at every decision, is never worse than the table's own greedy decode (jss_rollout_priority()),
+ * and it is the imitation label of expert iteration for the network that emitted the table.
+ *   Table: that of jss_rollout_priority(), entry prio_dev[i*ld_env + j*ld_job + k*ld_op] (strides in elements, 0 to
+ *     broadcast, 64-bit index arithmetic).  Only the entry of a legal job's current operation is ever read.
+ *   Candidates: those of jss_lookahead(), the set bits of env i's action_mask row.  The candidate is taken whatever its
+ *     priority, the no-op included (which the table's own decisions take only when no job is legal).
+ *   Value: makespan_out_dev[i*ld + a] is the current_time_step at which env i's episode ends if it takes a now and then
+ *     follows the table's decision of jss_rollout_priority(): the legal job whose current operation has the largest
+ *     priority, ties to the lowest index under IEEE comparison (-0.0 and +0.0 tie), the no-op only when no job is
+ *     legal.  Equivalently, a twin batch (same instances and env_id_base, auto-reset off, env i in the same state)
+ *     stepped with a and then with jss_rollout_priority(table, 2*J*M + 1) ends done at current_time_step ==
+ *     makespan_out[i][a].  Each candidate gets at most 2*J_i*M_i + 1 table decisions.  No RNG: the values depend on
+ *     neither seed nor step counter.
+ *   -1 is written as by jss_lookahead() (illegal columns 0..J_i, every column 0..J_i of an env done at entry), and for
+ *     a candidate whose rollout stops before done: a bad table at one of its decisions (a NaN or +inf on a legal job's
+ *     current operation, or every legal job at -inf: the bad-row rule of jss_rollout_priority()), nothing legal, a
+ *     step that leaves the env unchanged with the error bit, or the bound.  A bad table costs only the candidates whose
+ *     rollouts meet it and sets no error bit anywhere.  Columns J_i+1 .. ld-1 are not written.
+ *   No side effects: those of jss_lookahead().  The call reads only the state blocks and neither needs nor triggers
+ *     jss_refresh_obs().
+ *   Returns JSS_ERR_INVALID for a NULL or not 4-byte-aligned prio_dev or makespan_out_dev, a negative stride or
+ *     ld < jobs_max + 1, and JSS_ERR_STATE before jss_assign().
+ * Bytes: those of jss_lookahead(), plus per table decision the 4-byte priority of each legal job's current operation
+ * (L2 / HBM) in place of the suffix sums in shared memory.  Measured on an H100 SXM 80 GB HBM3 at a 700 W power limit
+ * (seeded per-env (N, J, M) table, median of three rounds): ta80 at N = 4 096 from reset 644.3 ms per call (409 600
+ * candidates, 1.27 G decisions/s) against 953.0 ms for import_state + jss_step + jss_rollout_priority per candidate
+ * column; after 500 random decisions 58.9 against 752.4 ms; ta80 at N = 32 6.64 against 347.4 ms; ta01 at N = 65 536
+ * 85.1 against 119.5 ms.  The MWR table runs 13-41 % faster than jss_lookahead(MWR, JSS_COIN_NEVER) on the same values
+ * (DESIGN.md section 4). */
+int jss_lookahead_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                           int32_t *makespan_out_dev, int64_t ld, void *stream);
+
 /* Host-buffer form of step(): copies actions H2D, steps, copies the results D2H with
  * contiguous DMA, synchronises.  Any output pointer may be NULL.  Host layouts equal the
  * device layouts: mask_host [N][mask_stride] bytes (row i: bytes 0..J_i), obs_host

@@ -70,6 +70,7 @@ SIGNATURES = {
     "jss_rollout_priority_sample": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int, _VP, _VP,
                                             _VP]),
     "jss_lookahead": (c_int, [_VP, c_int, c_int, c_uint64, c_uint64, _VP, c_int64, _VP]),
+    "jss_lookahead_priority": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP]),
     "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_step_begin": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_wait": (c_int, [_VP, c_int]),

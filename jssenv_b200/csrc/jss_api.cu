@@ -214,8 +214,9 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     // every launch that may read or partly rewrite real_obs brings it up to date first, so each entry point keeps its
     // meaning after a recording step (a plain step rewrites only the envs it changes)
     const bool recording = a.mode == JSS_MODE_STEP && a.traj_obs;
+    const bool lookahead = a.mode == JSS_MODE_LOOKAHEAD || a.mode == JSS_MODE_LOOKAHEAD_PRIORITY;
     if (!recording && a.mode != JSS_MODE_EXPORT && a.mode != JSS_MODE_POLICY && a.mode != JSS_MODE_REFRESH &&
-        a.mode != JSS_MODE_LOOKAHEAD)                    // the lookahead reads only state blocks and writes its table
+        !lookahead)                                      // the lookahead reads only state blocks and writes its table
         if (int rc = refresh_obs(h, st)) return rc;
     if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
@@ -225,9 +226,11 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
                            : a.mode == JSS_MODE_PRIORITY ? env_kernels<JSS_MODE_PRIORITY>
                            : a.mode == JSS_MODE_PRIORITY_SAMPLE ? env_kernels<JSS_MODE_PRIORITY_SAMPLE>
                            : a.mode == JSS_MODE_LOOKAHEAD ? env_kernels<JSS_MODE_LOOKAHEAD>
+                           : a.mode == JSS_MODE_LOOKAHEAD_PRIORITY ? env_kernels<JSS_MODE_LOOKAHEAD_PRIORITY>
                            : env_kernels<JSS_MODE_RESET>;
     // what the launch reads: a rollout or lookahead every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
-    // / CR), and the masked-uniform sampler no table at all (only J); the other modes ops / len
+    // / CR), and the masked-uniform sampler no table at all (only J); the other modes ops / len (the lookahead over a
+    // priority table too: the caller's table replaces the suffix sums)
     a.stage = a.mode == JSS_MODE_ROLLOUT || a.mode == JSS_MODE_LOOKAHEAD ? JSS_STAGE_ALL
             : a.mode != JSS_MODE_POLICY ? JSS_STAGE_OPS
             : a.rule == JSS_RULE_RANDOM ? 0 : jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
@@ -243,7 +246,7 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
         // policy kernels touch ~50 B per env: latency-bound, so give every tile its own CTA
         // instead of a persistent loop with a dependent load per iteration
         int grid = (a.mode == JSS_MODE_POLICY) ? n_tiles : std::min(n_tiles, h->sm_count * per_sm);
-        if (a.mode == JSS_MODE_LOOKAHEAD) {
+        if (lookahead) {
             // spread each tile's candidates over S work items when the tiles alone leave resident CTA slots empty:
             // S = 1 once they fill the SMs, up to the class's J + 1 (one candidate per item) for a small batch
             const int slots = h->sm_count * per_sm, jc = std::min(h->p.jobs_max, 32 << c);
@@ -864,6 +867,25 @@ int jss_lookahead(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t ste
     a.rule = rule; a.coin_mode = coin_mode; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
     a.actions_out = makespan_out_dev;
     a.logits_ld = ld;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_lookahead_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                           int32_t *makespan_out_dev, int64_t ld, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    if (!prio_dev || ((uintptr_t)prio_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || !makespan_out_dev ||
+        ((uintptr_t)makespan_out_dev & 3u) || ld < (int64_t)h->p.jobs_max + 1)
+        return fail(h, JSS_ERR_INVALID, "jss_lookahead_priority: bad arguments (prio %p and makespan_out %p must be "
+                    "4-byte aligned, strides %lld / %lld / %lld >= 0, ld %lld >= jobs_max + 1 = %d)",
+                    (const void *)prio_dev, (void *)makespan_out_dev, (long long)ld_env, (long long)ld_job,
+                    (long long)ld_op, (long long)ld, h->p.jobs_max + 1);
+    JssLaunch a{};
+    a.mode = JSS_MODE_LOOKAHEAD_PRIORITY;
+    a.logits = prio_dev;
+    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
+    a.actions_out = makespan_out_dev;
+    a.values_ld = ld;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 

@@ -1465,7 +1465,7 @@ JSS_DEV JssTileWarp jss_tile(const JssParams &p, const JssLaunch &a, bool uni, i
     return t;
 }
 
-// ---- one-step lookahead over a dispatching rule (jss_lookahead) -------------------------------------------------
+// ---- one-step lookahead over a dispatching rule or a priority table (jss_lookahead, jss_lookahead_priority) -----
 // Work item (tile, sp) of a launch split S ways (a.n_steps): warp `warp` values its env of the tile at the candidates
 // c = sp, sp + S, ... <= J.  Each candidate is simulated in registers from the env's state block, which the call never
 // writes: load, step c, then the rule's decisions d = 0, 1, ... (RNG counter step_index + d, so every candidate of an
@@ -1473,11 +1473,14 @@ JSS_DEV JssTileWarp jss_tile(const JssParams &p, const JssLaunch &a, bool uni, i
 // the end time, or -1 for an illegal candidate, an env done at entry, and a rollout that stops before done (the rule
 // finds nothing legal, a step leaves the env unchanged with the error bit, or the bound trips).  The block is reloaded
 // for each candidate (unchanged and L2-resident) instead of kept as a second register copy of the root state.
-template <int KJ>
+// PRIO (jss_lookahead_priority): the decisions after the candidate are env_priority_action's on the caller's table
+// (a.logits, its env stride a.logits_ld; the values' row stride is a.values_ld), no RNG; a bad table at a decision
+// (JSS_INF) stops that candidate's rollout, which then reads -1, and touches nothing else.
+template <int KJ, bool PRIO>
 JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
                            int lane, int sp, float *scratch) {
     const int32_t *blk = p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4;
-    int32_t *out = a.actions_out + (int64_t)env * a.logits_ld;
+    int32_t *out = a.actions_out + (int64_t)env * (PRIO ? a.values_ld : a.logits_ld);
     const uint64_t genv = p.env_id_base + (uint64_t)env;
     const int J = jss_J(iv), bound = 2 * J * jss_M(iv) + 1;
     int *hz = reinterpret_cast<int *>(scratch);
@@ -1494,9 +1497,15 @@ JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstVie
             bool ok = env_step<KJ, false>(p, iv, s, env, lane, c, r, hz);
             s.flags = jss_uniform(s.flags);
             for (int d = 0; ok && !(s.flags & JSS_FLAG_DONE) && d < bound; d++) {
-                const uint32_t h = jss_hash3(a.seed, genv, a.step_index + (uint64_t)d);
-                const int act = jss_uniform(env_select_action<KJ>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor));
-                ok = act != JSS_ACTION_SKIP && env_step<KJ, false>(p, iv, s, env, lane, act, r, hz);
+                int act;
+                if (PRIO) {
+                    act = jss_uniform(env_priority_action<KJ>(a, iv, s, env, lane));
+                } else {
+                    const uint32_t h = jss_hash3(a.seed, genv, a.step_index + (uint64_t)d);
+                    act = jss_uniform(env_select_action<KJ>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor));
+                }
+                ok = act != JSS_ACTION_SKIP && !(PRIO && act == JSS_INF) &&
+                     env_step<KJ, false>(p, iv, s, env, lane, act, r, hz);
                 s.flags = jss_uniform(s.flags);
             }
             if (s.flags & JSS_FLAG_DONE) t = s.t;
@@ -1604,10 +1613,14 @@ constexpr int JSS_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 3, 2};
 constexpr int JSS_PRIORITY_SAMPLE_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 2};
 // The lookahead loop likewise (the rules' code, but no output emission).
 constexpr int JSS_LOOKAHEAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 4, 3, 2};
+// The lookahead over a priority table likewise (the table's argmax in place of the rules): 31 / 48 / 56 / 80 registers
+// (CUDA 12.9, sm_90a); one CTA more spills in the classes with 2, 4 and 8 jobs per lane, and 8 is the SM's limit.
+constexpr int JSS_LOOKAHEAD_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {8, 5, 4, 3};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
     return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_LOOKAHEAD ? JSS_LOOKAHEAD_MIN_CTAS[jss_lane_class(32 * KJ)] : 1;
+         : mode == JSS_MODE_LOOKAHEAD ? JSS_LOOKAHEAD_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_LOOKAHEAD_PRIORITY ? JSS_LOOKAHEAD_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)] : 1;
 }
 
 template <int KJ, int MODE>
@@ -1620,8 +1633,10 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     jss_cta_carve(sl, sm, c, iv);
     const int warp = jss_warp_index(), lane = threadIdx.x & 31;
     float *scratch = reinterpret_cast<float *>(sm + sl.off_warp0 + warp * sl.warp_stride);
-    if (MODE == JSS_MODE_LOOKAHEAD) {
-        // work items (tile, sp), sp = 0 .. S-1, CTA-strided; a tile's S items are adjacent and share its instance
+    if (MODE == JSS_MODE_LOOKAHEAD || MODE == JSS_MODE_LOOKAHEAD_PRIORITY) {
+        // work items (tile, sp), sp = 0 .. S-1, CTA-strided; a tile's S items are adjacent and share its instance.  The
+        // rules read every table; the priority table replaces the suffix sums, so that lookahead stages ops / len only
+        constexpr bool PRIO = MODE == JSS_MODE_LOOKAHEAD_PRIORITY;
         const int S = a.n_steps, n_items = (a.tile_end - a.tile_begin) * S;
         int staged = -1;
         for (int item = (int)blockIdx.x; item < n_items; item += (int)gridDim.x) {
@@ -1630,12 +1645,12 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
             const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
             if (inst != staged) {                        // CTA-uniform
                 __syncthreads();
-                jss_stage_instance(p, p.inst[inst], c, JSS_STAGE_ALL);
+                jss_stage_instance(p, p.inst[inst], c, PRIO ? JSS_STAGE_OPS : JSS_STAGE_ALL);
                 staged = inst;
                 __syncthreads();
             }
             jss_iv_shape(iv);
-            if (env >= 0) env_lookahead<KJ>(p, a, iv, env, tile, warp, lane, item % S, scratch);
+            if (env >= 0) env_lookahead<KJ, PRIO>(p, a, iv, env, tile, warp, lane, item % S, scratch);
         }
         return;
     }

@@ -174,8 +174,8 @@ struct JssLaunch {           // per-launch arguments
         int32_t rule;
         int32_t greedy;      // steps from a row (a.logits): 0 categorical draw, 1 epsilon-greedy decode
     };
-    int32_t coin_mode, n_steps, write_obs;   // jss_lookahead: n_steps is S, the work items each tile's candidates
-                                             // are spread over (launch_all)
+    int32_t coin_mode, n_steps, write_obs;   // jss_lookahead (_priority): n_steps is S, the work items each tile's
+                                             // candidates are spread over (launch_all)
     int32_t export_after;    // step through the generic kernel: also decode the new state into the x_* arrays (facade)
     union {
         uint64_t seed;
@@ -192,9 +192,12 @@ struct JssLaunch {           // per-launch arguments
     union {
         double cr_factor;    // CriticalRatio due_date_factor (dispatching.py:337-349); reference default 1.5
         uint64_t sample_step_index;   // jss_rollout_priority_sample: the RNG counter of the env's first decision
+        int64_t values_ld;   // jss_lookahead_priority: env i's value of action a at actions_out + i * values_ld + a
+                             // (logits_ld is the table's env stride there)
     };
     const int32_t *actions;  // step
     int32_t *actions_out;    // policy; jss_lookahead: env i's value of action a at actions_out + i * logits_ld + a
+                             // (jss_lookahead_priority: + i * values_ld + a)
     const uint8_t *env_mask; // reset / import
     // rollout with trajectory recording: outputs of step k of env e go to slot k * n_envs + e of these buffers;
     // jss_step_logits_record / jss_step_greedy_record: env e's observation, mask and scalar record go to row e of
@@ -230,5 +233,7 @@ struct JssLaunch {           // per-launch arguments
                                      // (jss_rollout_priority_sample)
 #define JSS_MODE_LOOKAHEAD 10        // each legal action's makespan under a rule's rollout, the envs untouched
                                      // (jss_lookahead)
+#define JSS_MODE_LOOKAHEAD_PRIORITY 11   // the same under the greedy decisions of a caller's priority table
+                                         // (jss_lookahead_priority)
 
 #define JSS_WARPS_PER_CTA 8

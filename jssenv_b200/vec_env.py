@@ -413,15 +413,8 @@ class JssVecEnv:
         decisions (default 2*J*M + 1, enough for any episode), never resets, and a done env is left untouched; bad
         priorities (NaN / +inf on a legal current operation, or every legal job at -inf) set the error bit and stop
         that env.  Returns the step tuple; the RNG counter does not advance."""
-        import torch
-        n, J, M = self.num_envs, self.jobs, self.machines
-        x = torch.as_tensor(priorities, device=self.device)
-        if x.dim() != 3 or any(s not in (1, t) for s, t in zip(x.shape, (n, J, M))):
-            raise ValueError(f"rollout_priority: priorities must be 3-D and broadcast to ({n}, {J}, {M}), "
-                             f"got {tuple(x.shape)}")
-        if x.dtype != torch.float32:
-            x = x.to(torch.float32)
-        v = x.expand(n, J, M)                            # broadcast dimensions get stride 0
+        J, M = self.jobs, self.machines
+        v = self._table_view(self._table_arg(priorities, "rollout_priority", "priorities"))
         if n_steps is None:
             n_steps = 2 * J * M + 1
         rc = self._L.jss_rollout_priority(self._h, v.data_ptr(), *(int(s) for s in v.stride()), int(n_steps),
@@ -439,11 +432,8 @@ class JssVecEnv:
         `logits` requires grad (and grad mode is on), log_prob is differentiable with respect to it: the kernel also
         writes d log_prob / d table, and broadcast tables such as (1, J, M) get the gradient summed over the envs."""
         import torch
-        n, J, M = self.num_envs, self.jobs, self.machines
-        x = torch.as_tensor(logits, device=self.device)
-        if x.dim() != 3 or any(s not in (1, t) for s, t in zip(x.shape, (n, J, M))):
-            raise ValueError(f"rollout_priority_sample: logits must be 3-D and broadcast to ({n}, {J}, {M}), "
-                             f"got {tuple(x.shape)}")
+        J, M = self.jobs, self.machines
+        x = self._table_arg(logits, "rollout_priority_sample", "logits")
         n_steps = 2 * J * M + 1 if n_steps is None else int(n_steps)
         if x.requires_grad and torch.is_grad_enabled():
             log_prob = _sampled_log_prob().apply(x, self, n_steps)
@@ -456,12 +446,8 @@ class JssVecEnv:
         strides passed through); writes the gradient to `grad_out` ((N, J, M) float32, or None); advances the RNG
         counter.  Returns log_prob."""
         import torch
-        n, J, M = self.num_envs, self.jobs, self.machines
-        v = x.detach()
-        if v.dtype != torch.float32:
-            v = v.to(torch.float32)
-        v = v.expand(n, J, M)                            # broadcast dimensions get stride 0
-        log_prob = torch.empty(n, dtype=torch.float32, device=self.device)
+        v = self._table_view(x)
+        log_prob = torch.empty(self.num_envs, dtype=torch.float32, device=self.device)
         rc = self._L.jss_rollout_priority_sample(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
                                                  self._step_index, n_steps, log_prob.data_ptr(), _ptr(grad_out),
                                                  self._stream())
@@ -479,22 +465,66 @@ class JssVecEnv:
         writes only columns 0..J_i).  coin="never" makes each value exact and the rollout method (take the argmin,
         repeat) never worse than the rule alone; "device" gives the reference's 10 % wait draw.  The RNG counter
         advances by 2*J*M + 1, the rule decisions a candidate may take."""
-        import torch
-        n, J = self.num_envs, self.jobs
+        J = self.jobs
         if isinstance(rule, str) and rule.upper() not in N.RULES:
             raise ValueError(f"lookahead: unknown rule {rule!r} (one of {sorted(N.RULES)})")
         if coin not in ("never", "device"):
             raise ValueError(f"lookahead: coin must be 'never' or 'device', got {coin!r}")
-        if out is None:
-            out = torch.full((n, J + 1), -1, dtype=torch.int32, device=self.device)
-        elif (not isinstance(out, torch.Tensor) or out.dtype != torch.int32 or out.dim() != 2 or out.shape[0] != n
-              or out.shape[1] < J + 1 or not out.is_contiguous() or out.device != self.device):
-            raise ValueError(f"lookahead: out must be a contiguous int32 tensor of shape ({n}, >= {J + 1}) on the "
-                             f"env's device")
+        out = self._values_out(out, "lookahead")
         rc = self._L.jss_lookahead(self._h, _rule_id(rule), _coin_id(coin), self.seed, self._step_index,
                                    out.data_ptr(), int(out.shape[1]), self._stream())
         N.check(self._h, rc, "jss_lookahead")
         self._step_index += 2 * J * self.machines + 1
+        return out
+
+    def lookahead_priority(self, priorities, out=None):
+        """Value every legal action by a greedy rollout of the priority table `priorities` to the end of the episode, in
+        one launch per lane class (jss_lookahead_priority), leaving the envs untouched: out[i, a] is the makespan env i
+        reaches if it takes action a now and then follows the table as rollout_priority() does (the legal job whose
+        current operation has the largest priority, ties to the lowest index, the no-op only when no job is legal); -1
+        for an action that is not legal, every action of a done env, and a rollout that stops before done, such as one
+        that meets a bad entry (NaN / +inf on a legal current operation, or every legal job at -inf; no error bit is
+        set).  `priorities` is taken as by rollout_priority(); a table that requires grad is read detached (the values
+        have no gradient).  `out` is taken and returned as by lookahead().  The argmin of the values, taken at every
+        decision, is never worse than rollout_priority(priorities) from the same state.  No RNG: the counter does not
+        advance."""
+        v = self._table_view(self._table_arg(priorities, "lookahead_priority", "priorities"))
+        out = self._values_out(out, "lookahead_priority")
+        rc = self._L.jss_lookahead_priority(self._h, v.data_ptr(), *(int(s) for s in v.stride()), out.data_ptr(),
+                                            int(out.shape[1]), self._stream())
+        N.check(self._h, rc, "jss_lookahead_priority")
+        return out
+
+    def _table_arg(self, x, who: str, what: str):
+        """A caller's priority / logit table as a tensor on the env's device, refused unless it is 3-D and broadcasts
+        to (N, J, M), J and M the batch maxima."""
+        import torch
+        n, J, M = self.num_envs, self.jobs, self.machines
+        x = torch.as_tensor(x, device=self.device)
+        if x.dim() != 3 or any(s not in (1, t) for s, t in zip(x.shape, (n, J, M))):
+            raise ValueError(f"{who}: {what} must be 3-D and broadcast to ({n}, {J}, {M}), got {tuple(x.shape)}")
+        return x
+
+    def _table_view(self, x):
+        """The (N, J, M) float32 view the kernels read of a checked table: detached, converted only if needed, and
+        expanded so that broadcast dimensions get stride 0 (the strides are passed through)."""
+        import torch
+        v = x.detach()
+        if v.dtype != torch.float32:
+            v = v.to(torch.float32)
+        return v.expand(self.num_envs, self.jobs, self.machines)
+
+    def _values_out(self, out, who: str):
+        """The (N, >= J+1) contiguous int32 device table a lookahead writes: `out` once checked, else a fresh (N, J+1)
+        one filled with -1."""
+        import torch
+        n, J = self.num_envs, self.jobs
+        if out is None:
+            return torch.full((n, J + 1), -1, dtype=torch.int32, device=self.device)
+        if (not isinstance(out, torch.Tensor) or out.dtype != torch.int32 or out.dim() != 2 or out.shape[0] != n
+                or out.shape[1] < J + 1 or not out.is_contiguous() or out.device != self.device):
+            raise ValueError(f"{who}: out must be a contiguous int32 tensor of shape ({n}, >= {J + 1}) on the "
+                             f"env's device")
         return out
 
     def rollout_record(self, rule: Union[str, int], n_steps: int, out: Optional[Dict[str, Any]] = None):
