@@ -71,6 +71,11 @@ SIGNATURES = {
                                             _VP]),
     "jss_lookahead": (c_int, [_VP, c_int, c_int, c_uint64, c_uint64, _VP, c_int64, _VP]),
     "jss_lookahead_priority": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP]),
+    "jss_sample_episodes": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, _VP, c_int64,
+                                    _VP]),
+    "jss_sample_episodes_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, c_int64,
+                                         c_int, _VP, _VP]),
+    "jss_sample_episodes_solution": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, _VP, _VP, _VP]),
     "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_step_begin": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_wait": (c_int, [_VP, c_int]),
@@ -145,6 +150,12 @@ class CudaBackend:
     def synchronize(self, device_index):
         import torch
         torch.cuda.synchronize(device_index)
+
+    def warp_slots(self, device_index):
+        """Warps the device keeps resident at once: SMs x resident threads per SM / 32."""
+        import torch
+        prop = torch.cuda.get_device_properties(device_index)
+        return prop.multi_processor_count * prop.max_threads_per_multi_processor // 32
 
 
 backend = CudaBackend()   # tests/emu swaps this object; product code never does

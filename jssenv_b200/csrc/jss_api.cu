@@ -215,8 +215,9 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     // meaning after a recording step (a plain step rewrites only the envs it changes)
     const bool recording = a.mode == JSS_MODE_STEP && a.traj_obs;
     const bool lookahead = a.mode == JSS_MODE_LOOKAHEAD || a.mode == JSS_MODE_LOOKAHEAD_PRIORITY;
+    const bool samples = jss_mode_samples(a.mode);
     if (!recording && a.mode != JSS_MODE_EXPORT && a.mode != JSS_MODE_POLICY && a.mode != JSS_MODE_REFRESH &&
-        !lookahead)                                      // the lookahead reads only state blocks and writes its table
+        !lookahead && !samples)                          // these read only state blocks and write the caller's buffers
         if (int rc = refresh_obs(h, st)) return rc;
     if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
@@ -227,6 +228,9 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
                            : a.mode == JSS_MODE_PRIORITY_SAMPLE ? env_kernels<JSS_MODE_PRIORITY_SAMPLE>
                            : a.mode == JSS_MODE_LOOKAHEAD ? env_kernels<JSS_MODE_LOOKAHEAD>
                            : a.mode == JSS_MODE_LOOKAHEAD_PRIORITY ? env_kernels<JSS_MODE_LOOKAHEAD_PRIORITY>
+                           : a.mode == JSS_MODE_SAMPLE_EPISODES ? env_kernels<JSS_MODE_SAMPLE_EPISODES>
+                           : a.mode == JSS_MODE_SAMPLE_EPISODES_GRAD ? env_kernels<JSS_MODE_SAMPLE_EPISODES_GRAD>
+                           : a.mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION ? env_kernels<JSS_MODE_SAMPLE_EPISODES_SOLUTION>
                            : env_kernels<JSS_MODE_RESET>;
     // what the launch reads: a rollout or lookahead every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
     // / CR), and the masked-uniform sampler no table at all (only J); the other modes ops / len (the lookahead over a
@@ -245,13 +249,20 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
         if (rc) return rc;
         // policy kernels touch ~50 B per env: latency-bound, so give every tile its own CTA
         // instead of a persistent loop with a dependent load per iteration
-        int grid = (a.mode == JSS_MODE_POLICY) ? n_tiles : std::min(n_tiles, h->sm_count * per_sm);
+        const int slots = h->sm_count * per_sm;
+        int grid = (a.mode == JSS_MODE_POLICY) ? n_tiles : std::min(n_tiles, slots);
         if (lookahead) {
             // spread each tile's candidates over S work items when the tiles alone leave resident CTA slots empty:
             // S = 1 once they fill the SMs, up to the class's J + 1 (one candidate per item) for a small batch
-            const int slots = h->sm_count * per_sm, jc = std::min(h->p.jobs_max, 32 << c);
+            const int jc = std::min(h->p.jobs_max, 32 << c);
             a.n_steps = n_tiles >= slots ? 1 : std::min(jc + 1, (slots + n_tiles - 1) / n_tiles);
             grid = std::min(n_tiles * a.n_steps, slots);
+        } else if (samples) {
+            // the draws: each tile's K samples spread over S work items in the same way, up to S = K; the gradient
+            // keeps the caller's split (one work item per chunk), the solution replay one work item per tile
+            if (a.mode == JSS_MODE_SAMPLE_EPISODES)
+                a.n_steps = n_tiles >= slots ? 1 : std::min(a.n_samples, (slots + n_tiles - 1) / n_tiles);
+            grid = (int)std::min<int64_t>((int64_t)n_tiles * a.n_steps, slots);
         }
         JSS_LAUNCH(kerns[c], grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
         JSS_CUDA(h, cudaGetLastError());
@@ -886,6 +897,95 @@ int jss_lookahead_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int6
     a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
     a.actions_out = makespan_out_dev;
     a.values_ld = ld;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+namespace {
+
+bool bad_ptr(const void *ptr) { return !ptr || ((uintptr_t)ptr & 3u); }
+
+// the arguments jss_sample_episodes and its replays share: the table as jss_rollout_priority_sample takes it, the seed
+// and counter; k and ld where the call has them (has_k)
+int sample_episodes_args(jss_t *h, const char *who, const float *logits, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                         uint64_t seed, uint64_t step_index, bool has_k, int64_t k, int64_t ld, JssLaunch &a) {
+    if (bad_ptr(logits) || ld_env < 0 || ld_job < 0 || ld_op < 0)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (logits %p must be 4-byte aligned, strides %lld / %lld / "
+                    "%lld >= 0)", who, (const void *)logits, (long long)ld_env, (long long)ld_job, (long long)ld_op);
+    if (has_k) {
+        const uint64_t bound = 2ull * (uint64_t)h->p.jobs_max * (uint64_t)h->p.machines_max + 1;
+        if (k < 1 || ld < k || (uint64_t)k > UINT64_MAX / bound)
+            return fail(h, JSS_ERR_INVALID, "%s: bad arguments (k %lld >= 1 with k * (2 * J * M + 1) below 2^64, "
+                        "ld %lld >= k)", who, (long long)k, (long long)ld);
+        if (k > INT32_MAX)
+            return fail(h, JSS_ERR_UNSUPPORTED, "%s: k must stay below 2^31", who);
+    }
+    a.logits = logits;
+    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
+    a.hash_key = jss_fold32(seed);                       // jss_hash3 reads the seed only through its fold
+    a.sample_step_index = step_index;
+    a.n_samples = (int)k;
+    a.samples_ld = ld;
+    return JSS_OK;
+}
+
+}  // namespace
+
+int jss_sample_episodes(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                        uint64_t seed, uint64_t step_index, int64_t k, int32_t *makespan_out_dev,
+                        float *log_prob_out_dev, int64_t ld, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    const char *who = "jss_sample_episodes";
+    if (bad_ptr(makespan_out_dev) || bad_ptr(log_prob_out_dev))
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p and log_prob_out %p must be 4-byte "
+                    "aligned)", who, (void *)makespan_out_dev, (void *)log_prob_out_dev);
+    JssLaunch a{};
+    a.mode = JSS_MODE_SAMPLE_EPISODES;
+    if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
+        return rc;
+    a.actions_out = makespan_out_dev;
+    a.log_prob_out = log_prob_out_dev;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_sample_episodes_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                             uint64_t seed, uint64_t step_index, int64_t k, const float *weights_dev, int64_t ld,
+                             int split, float *grad_out_dev, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    const char *who = "jss_sample_episodes_grad";
+    if (bad_ptr(weights_dev) || bad_ptr(grad_out_dev) || split < 1 || split > k)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (weights %p and grad_out %p must be 4-byte aligned, "
+                    "1 <= split %d <= k %lld)", who, (const void *)weights_dev, (void *)grad_out_dev, split,
+                    (long long)k);
+    if ((int64_t)h->n_tiles * split > INT32_MAX)
+        return fail(h, JSS_ERR_UNSUPPORTED, "%s: split * tiles must stay below 2^31", who);
+    JssLaunch a{};
+    a.mode = JSS_MODE_SAMPLE_EPISODES_GRAD;
+    if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
+        return rc;
+    a.weights = weights_dev;
+    a.n_steps = split;
+    a.grad_out = grad_out_dev;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                 uint64_t seed, uint64_t step_index, const int32_t *sample_dev,
+                                 int32_t *solution_out_dev, void *stream) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    const char *who = "jss_sample_episodes_solution";
+    if (bad_ptr(sample_dev) || bad_ptr(solution_out_dev))
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (sample %p and solution_out %p must be 4-byte aligned)",
+                    who, (const void *)sample_dev, (void *)solution_out_dev);
+    JssLaunch a{};
+    a.mode = JSS_MODE_SAMPLE_EPISODES_SOLUTION;
+    if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, false, 0, 0, a)))
+        return rc;
+    a.actions = sample_dev;
+    a.solution_out = solution_out_dev;
+    a.n_steps = 1;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 

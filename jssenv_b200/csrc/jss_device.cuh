@@ -754,9 +754,11 @@ JSS_DEV void env_clear_solution(const JssParams &p, int env, int lane) {
 // ---- step (jss_env.py:403-481) ---------------------------------------------------------
 // Returns true if the env changed (outputs must be re-emitted).  BOOKKEEP = false (jss_lookahead's throw-away
 // simulations) changes nothing but the registers: no solution entry, no episode statistics, no auto-reset.
-template <int KJ, bool BOOKKEEP = true, bool TRACK = false>
+// SOL_OUT (with BOOKKEEP = false: jss_sample_episodes_solution's replay) writes the allocated operation's start time
+// into the caller's `sol_out`, which has the layout of p.solution, and nothing else.
+template <int KJ, bool BOOKKEEP = true, bool TRACK = false, bool SOL_OUT = false>
 JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, int env, int lane, int action,
-                      int &raw_reward, int *hz) {
+                      int &raw_reward, int *hz, int32_t *sol_out = nullptr) {
     raw_reward = 0;
     if (action == JSS_ACTION_SKIP) return false;
     if (s.flags & JSS_FLAG_DONE) {
@@ -789,6 +791,8 @@ JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, in
         if (TRACK && lane == la) s.dirty |= 1u << ia;
         if (BOOKKEEP && p.solution && lane == la)                     // :454
             p.solution[((size_t)env * p.jobs_max + action) * p.machines_max + jss_sel<KJ>(s.todo, ia)] = s.t;
+        if (SOL_OUT && lane == la)
+            sol_out[((size_t)env * p.jobs_max + action) * p.machines_max + jss_sel<KJ>(s.todo, ia)] = s.t;
 #pragma unroll
         for (int i = 0; i < KJ; i++)
             // every job waiting for machine m_a: no longer legal (:455-461), no longer
@@ -1514,6 +1518,126 @@ JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstVie
     }
 }
 
+// ---- K episodes per env drawn from a logit table, the envs untouched (jss_sample_episodes, _grad, _solution) -----
+// Sample s of env `env` is jss_rollout_priority_sample's loop run in registers from the env's state block, which the
+// call never writes: at most B = 2 jobs_max machines_max + 1 decisions of env_priority_sample_action, decision d at RNG
+// counter a.sample_step_index + s B + d, each step with env_step<KJ, false>.  It ends done, errs (a bad table, or a
+// step that leaves the env unchanged: log-probability NaN) or stops (nothing legal, or the bound).  The block is
+// reloaded for each sample, as the lookahead reloads it for each candidate.
+// JSS_MODE_SAMPLE_EPISODES: work item (tile, sp) of a launch split S ways (a.n_steps) takes the samples s = sp, sp + S,
+//   ... < K and stores each one's makespan (-1 unless done) and log-probability at column s of the env's rows (row
+//   stride a.samples_ld); an env done at entry gets -1 and 0 in each of those columns.
+// JSS_MODE_SAMPLE_EPISODES_GRAD: work item (tile, c), c < split (a.n_steps), takes the samples s = c, c + split, ... in
+//   increasing s and adds w_s G_s into chunk c of a.grad_out with env_priority_sample_rollout's accumulator: w_s (1 -
+//   acc) at a drawn operation, w_s (0 - acc) at each job's first undrawn one at the end.  Each entry is read and written
+//   only by the lane that owns its job, in program order, so a chunk's sums do not depend on the schedule.  A sample
+//   that errs adds nothing.  Only a non-finite table entry or an imported legal job without an operation can make a
+//   sample err after its first draw (a no-op is drawn only from an imported state, at decision 0, before any add), so
+//   an env with either has each sample first run without adds to find out.  Samples with w_s == 0 and envs done at
+//   entry are skipped.
+// JSS_MODE_SAMPLE_EPISODES_SOLUTION: one work item per tile; env i replays sample a.actions[i] (none if < 0) and writes
+//   the start time of each operation it starts into a.solution_out.
+JSS_HD constexpr bool jss_mode_samples(int mode) {
+    return mode == JSS_MODE_SAMPLE_EPISODES || mode == JSS_MODE_SAMPLE_EPISODES_GRAD ||
+           mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION;
+}
+template <int KJ, int MODE>
+JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile,
+                                 int warp, int lane, int sp, float *scratch) {
+    constexpr bool GRAD = MODE == JSS_MODE_SAMPLE_EPISODES_GRAD, SOL = MODE == JSS_MODE_SAMPLE_EPISODES_SOLUTION;
+    const int32_t *blk = p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4;
+    const uint64_t genv = p.env_id_base + (uint64_t)env;
+    const int J = jss_J(iv), M = jss_M(iv), bound = 2 * p.jobs_max * p.machines_max + 1;
+    const int64_t row = (int64_t)env * a.samples_ld;
+    int *hz = reinterpret_cast<int *>(scratch);
+    EnvRegs<KJ> s;
+    env_load<KJ>(iv, blk, lane, s);
+    s.flags = jss_uniform(s.flags);
+    int first = sp, end = a.n_samples, stride = a.n_steps;
+    if (SOL) {
+        first = jss_uniform(a.actions[env]);
+        end = first + 1; stride = 1;
+        if (first < 0) return;
+    }
+    if (s.flags & JSS_FLAG_DONE) {
+        if (!GRAD && !SOL && lane == 0)
+            for (int k = first; k < end; k += stride) { a.actions_out[row + k] = -1; a.log_prob_out[row + k] = 0.0f; }
+        return;
+    }
+    float *grad = nullptr;
+    bool check = false;                                  // GRAD: a sample may err after an add
+    if (GRAD) {
+        grad = a.grad_out + ((size_t)sp * p.n_envs + env) * p.jobs_max * p.machines_max;
+        const float *tab = a.logits + (int64_t)env * a.logits_ld;
+        bool clean = true;
+#pragma unroll 1
+        for (int i = 0; i < KJ; i++) {
+            const int j = KJ * lane + i;
+            if (j >= J) break;
+            clean = clean && !(((s.lb >> i) & 1u) && jss_sel<KJ>(s.op, i) == JSS_OP_NONE);
+            for (int k = 0; k < M; k++) {
+                const float x = tab[(int64_t)j * a.prio_ld_job + (int64_t)k * a.prio_ld_op];
+                clean = clean && x > -JSS_F32_INF && x < JSS_F32_INF;
+            }
+        }
+        check = __any_sync(JSS_FULL, !clean);
+    }
+    for (int smp = first; smp < end; smp += stride) {
+        float w = 0.0f;
+        if (GRAD) {
+            w = __int_as_float(jss_uniform(__float_as_int(a.weights[row + smp])));
+            if (w == 0.0f) continue;
+        }
+        const uint64_t c0 = a.sample_step_index + (uint64_t)smp * (uint64_t)bound;
+        // GRAD: pass 0 (only where `check`) finds out whether the sample errs, pass 1 adds
+        for (int pass = (GRAD && !check) ? 1 : 0; pass < (GRAD ? 2 : 1); pass++) {
+            const bool add = GRAD && pass == 1;
+            env_load<KJ>(iv, blk, lane, s);
+            s.flags = jss_uniform(s.flags);
+            bool err = false;
+            float lp = 0.0f, acc[KJ];
+#pragma unroll
+            for (int i = 0; i < KJ; i++) acc[i] = 0.0f;
+            for (int d = 0; d < bound && !(s.flags & JSS_FLAG_DONE); d++) {
+                const uint32_t h = jss_hash_env(jss_hash_key_folded(a.hash_key, c0 + (uint64_t)d), genv);
+                float logp, pr[KJ];
+                const int act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
+                if (act == JSS_ACTION_SKIP) break;       // nothing legal: no decision changes the env
+                int r;
+                bool changed = false;
+                if (act != JSS_INF) {
+                    if (add && act < J) {                // a job drawn (the no-op has no p_t)
+#pragma unroll
+                        for (int i = 0; i < KJ; i++) {
+                            acc[i] += pr[i];
+                            if (KJ * lane + i == act) {
+                                grad[(size_t)act * p.machines_max + s.todo[i]] += w * (1.0f - acc[i]);
+                                acc[i] = 0.0f;
+                            }
+                        }
+                    }
+                    changed = env_step<KJ, false, false, SOL>(p, iv, s, env, lane, act, r, hz, a.solution_out);
+                }
+                s.flags = jss_uniform(s.flags);
+                if (!changed) { err = true; break; }
+                lp += logp;
+            }
+            if (!GRAD && !SOL && lane == 0) {
+                a.actions_out[row + smp] = (s.flags & JSS_FLAG_DONE) ? s.t : -1;
+                a.log_prob_out[row + smp] = err ? JSS_F32_NAN : lp;
+            }
+            if (err) break;                              // GRAD: no adds, or none yet (decision 0 of pass 1)
+            if (add) {
+#pragma unroll
+                for (int i = 0; i < KJ; i++) {
+                    const int j = KJ * lane + i, k0 = s.todo[i] + (s.tufco[i] > 0 ? 1 : 0);
+                    if (j < J && k0 < M) grad[(size_t)j * p.machines_max + k0] += w * (0.0f - acc[i]);
+                }
+            }
+        }
+    }
+}
+
 template <int KJ, int MODE>
 JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
                              int lane, float *scratch) {
@@ -1616,11 +1740,21 @@ constexpr int JSS_LOOKAHEAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 4, 3, 2};
 // The lookahead over a priority table likewise (the table's argmax in place of the rules): 31 / 48 / 56 / 80 registers
 // (CUDA 12.9, sm_90a); one CTA more spills in the classes with 2, 4 and 8 jobs per lane, and 8 is the SM's limit.
 constexpr int JSS_LOOKAHEAD_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {8, 5, 4, 3};
+// The sampled episodes likewise, per mode (CUDA 12.9, sm_90a): the draws at 32 / 32 / 39 / 72 registers, their replay
+// with the gradient adds at 56 / 64 / 64 / 122, the solution replay at 40 / 48 / 40 / 72.  ptxas is not monotonic
+// here: the draws with 4 jobs per lane spill at 5 CTAs but not at 6, and spill again at 7.
+constexpr int JSS_SAMPLE_EPISODES_MIN_CTAS[JSS_LANE_CLASSES] = {8, 8, 6, 3};
+constexpr int JSS_SAMPLE_EPISODES_GRAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 4, 4, 2};
+constexpr int JSS_SAMPLE_EPISODES_SOLUTION_MIN_CTAS[JSS_LANE_CLASSES] = {6, 5, 6, 3};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
     return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_LOOKAHEAD ? JSS_LOOKAHEAD_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_LOOKAHEAD_PRIORITY ? JSS_LOOKAHEAD_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)] : 1;
+         : mode == JSS_MODE_LOOKAHEAD_PRIORITY ? JSS_LOOKAHEAD_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_SAMPLE_EPISODES ? JSS_SAMPLE_EPISODES_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_SAMPLE_EPISODES_GRAD ? JSS_SAMPLE_EPISODES_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION ? JSS_SAMPLE_EPISODES_SOLUTION_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : 1;
 }
 
 template <int KJ, int MODE>
@@ -1633,10 +1767,11 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     jss_cta_carve(sl, sm, c, iv);
     const int warp = jss_warp_index(), lane = threadIdx.x & 31;
     float *scratch = reinterpret_cast<float *>(sm + sl.off_warp0 + warp * sl.warp_stride);
-    if (MODE == JSS_MODE_LOOKAHEAD || MODE == JSS_MODE_LOOKAHEAD_PRIORITY) {
+    if (MODE == JSS_MODE_LOOKAHEAD || MODE == JSS_MODE_LOOKAHEAD_PRIORITY || jss_mode_samples(MODE)) {
         // work items (tile, sp), sp = 0 .. S-1, CTA-strided; a tile's S items are adjacent and share its instance.  The
         // rules read every table; the priority table replaces the suffix sums, so that lookahead stages ops / len only
-        constexpr bool PRIO = MODE == JSS_MODE_LOOKAHEAD_PRIORITY;
+        // (and so do the sampled episodes)
+        constexpr bool PRIO = MODE != JSS_MODE_LOOKAHEAD;
         const int S = a.n_steps, n_items = (a.tile_end - a.tile_begin) * S;
         int staged = -1;
         for (int item = (int)blockIdx.x; item < n_items; item += (int)gridDim.x) {
@@ -1650,7 +1785,9 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
                 __syncthreads();
             }
             jss_iv_shape(iv);
-            if (env >= 0) env_lookahead<KJ, PRIO>(p, a, iv, env, tile, warp, lane, item % S, scratch);
+            if (env < 0) continue;
+            if (jss_mode_samples(MODE)) env_sample_episodes<KJ, MODE>(p, a, iv, env, tile, warp, lane, item % S, scratch);
+            else env_lookahead<KJ, PRIO>(p, a, iv, env, tile, warp, lane, item % S, scratch);
         }
         return;
     }

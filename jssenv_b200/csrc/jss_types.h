@@ -173,9 +173,11 @@ struct JssLaunch {           // per-launch arguments
     union {
         int32_t rule;
         int32_t greedy;      // steps from a row (a.logits): 0 categorical draw, 1 epsilon-greedy decode
+        int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env
     };
     int32_t coin_mode, n_steps, write_obs;   // jss_lookahead (_priority): n_steps is S, the work items each tile's
-                                             // candidates are spread over (launch_all)
+                                             // candidates are spread over (launch_all); jss_sample_episodes: the
+                                             // work items each tile's samples are spread over (_grad: the chunks)
     int32_t export_after;    // step through the generic kernel: also decode the new state into the x_* arrays (facade)
     union {
         uint64_t seed;
@@ -195,10 +197,20 @@ struct JssLaunch {           // per-launch arguments
         int64_t values_ld;   // jss_lookahead_priority: env i's value of action a at actions_out + i * values_ld + a
                              // (logits_ld is the table's env stride there)
     };
-    const int32_t *actions;  // step
-    int32_t *actions_out;    // policy; jss_lookahead: env i's value of action a at actions_out + i * logits_ld + a
-                             // (jss_lookahead_priority: + i * values_ld + a)
-    const uint8_t *env_mask; // reset / import
+    union {
+        const int32_t *actions;  // step; jss_sample_episodes_solution: the sample each env replays (< 0: none)
+        const float *weights;    // jss_sample_episodes_grad: sample s of env i weighs weights[i * samples_ld + s]
+    };
+    union {
+        int32_t *actions_out;    // policy; jss_lookahead: env i's value of action a at actions_out + i * logits_ld + a
+                                 // (jss_lookahead_priority: + i * values_ld + a); jss_sample_episodes: sample s's
+                                 // makespan at actions_out + i * samples_ld + s
+        int32_t *solution_out;   // jss_sample_episodes_solution: [N][jobs_max][machines_max] start times
+    };
+    union {
+        const uint8_t *env_mask; // reset / import
+        int64_t samples_ld;      // jss_sample_episodes (_grad): row stride of the per-sample outputs / weights
+    };
     // rollout with trajectory recording: outputs of step k of env e go to slot k * n_envs + e of these buffers;
     // jss_step_logits_record / jss_step_greedy_record: env e's observation, mask and scalar record go to row e of
     // traj_obs / mask / scalars.  jss_rollout_priority_sample: grad_out is the [N][jobs_max][machines_max] gradient of
@@ -235,5 +247,11 @@ struct JssLaunch {           // per-launch arguments
                                      // (jss_lookahead)
 #define JSS_MODE_LOOKAHEAD_PRIORITY 11   // the same under the greedy decisions of a caller's priority table
                                          // (jss_lookahead_priority)
+#define JSS_MODE_SAMPLE_EPISODES 12      // K episodes per env drawn from a logit table, the envs untouched
+                                         // (jss_sample_episodes)
+#define JSS_MODE_SAMPLE_EPISODES_GRAD 13       // their replay, adding the weighted gradients into the caller's
+                                               // chunks (jss_sample_episodes_grad)
+#define JSS_MODE_SAMPLE_EPISODES_SOLUTION 14   // the replay of one sample per env, writing the start times
+                                               // (jss_sample_episodes_solution)
 
 #define JSS_WARPS_PER_CTA 8

@@ -79,6 +79,34 @@ def _sampled_log_prob():
     return SampledLogProb
 
 
+@functools.lru_cache(maxsize=None)
+def _episodes_log_prob():
+    """The autograd Function of JssVecEnv.sample_episodes' log_prob (made on first use).  Forward draws the episodes and
+    saves the table and the RNG counter; backward replays the draws (jss_sample_episodes_grad) with the incoming (N, k)
+    gradient as weights, sums the chunks and then over the table's broadcast dimensions.  The replay starts from the
+    envs' state at backward time, which must still be their state at forward time."""
+    import torch
+
+    class EpisodesLogProb(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, logits, env, k, step_index):
+            makespan, log_prob = env._sample_episodes(logits, k, step_index)
+            ctx.save_for_backward(logits)              # torch's version counter refuses a table changed in place
+            ctx.env, ctx.k, ctx.step_index = env, k, step_index
+            ctx.mark_non_differentiable(makespan)
+            return makespan, log_prob
+
+        @staticmethod
+        def backward(ctx, _, g):
+            (logits,) = ctx.saved_tensors
+            env = ctx.env
+            split = min(ctx.k, -(-env._warp_slots() // env.num_envs))
+            grad = env._sample_episodes_grad(logits, ctx.k, ctx.step_index, g, split)
+            return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None, None
+
+    return EpisodesLogProb
+
+
 def _state_views(b, n, J, M, view):
     """The canonical-state arrays of jss_export_state, each made by ``view(ptr, shape, dtype)``."""
     return {"todo": view(b.x_todo, (n, J), np.int32), "tufco": view(b.x_tufco, (n, J), np.int32),
@@ -494,6 +522,74 @@ class JssVecEnv:
                                             int(out.shape[1]), self._stream())
         N.check(self._h, rc, "jss_lookahead_priority")
         return out
+
+    def sample_episodes(self, logits, k: int, solution: bool = False):
+        """Draw `k` whole episodes per env from the logit table `logits`, each from the env's current state, in one
+        launch per lane class (jss_sample_episodes), leaving the envs untouched.  With B = 2*J*M + 1, sample s of env i
+        is the episode rollout_priority_sample(logits) would draw from this state with the RNG counter at
+        ``self._step_index + s*B``; the counter then advances by k*B.  `logits` is taken as by rollout_priority_sample().
+        Returns a dict of device tensors: ``"makespan"`` (N, k) int32, the end time of each sample (-1 if it does not
+        end done: a bad table entry on its path, or an env done now); ``"log_prob"`` (N, k) float32, each sample's
+        log-probability (NaN where it meets a bad entry, 0 for an env done now); ``"best"`` (N,) int64, the lowest-index
+        sample of smallest makespan, -1 if none ended; with `solution`, ``"solution"`` (N, J, M) int32, the start times
+        of the best sample's operations over this env's solution so far (-1 without record_solution).  When `logits`
+        requires grad (and grad mode is on), log_prob is differentiable with respect to it: the backward replays the
+        draws, so the envs must not be stepped or reset between this call and the backward."""
+        import torch
+        J, M = self.jobs, self.machines
+        x = self._table_arg(logits, "sample_episodes", "logits")
+        if int(k) < 1:
+            raise ValueError(f"sample_episodes: k must be at least 1, got {k!r}")
+        k, step_index = int(k), self._step_index
+        if x.requires_grad and torch.is_grad_enabled():
+            makespan, log_prob = _episodes_log_prob().apply(x, self, k, step_index)
+        else:
+            makespan, log_prob = self._sample_episodes(x, k, step_index)
+        self._step_index += k * (2 * J * M + 1)
+        ended = makespan >= 0
+        best = torch.where(ended, makespan, torch.iinfo(torch.int32).max).argmin(1)
+        best = torch.where(ended.any(1), best, -1)
+        out = {"makespan": makespan, "log_prob": log_prob, "best": best}
+        if solution:
+            sol = (self.solution.clone() if self.solution is not None
+                   else torch.full((self.num_envs, J, M), -1, dtype=torch.int32, device=self.device))
+            v = self._table_view(x)
+            b32 = best.to(torch.int32)
+            rc = self._L.jss_sample_episodes_solution(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
+                                                      step_index, b32.data_ptr(), sol.data_ptr(), self._stream())
+            N.check(self._h, rc, "jss_sample_episodes_solution")
+            out["solution"] = sol
+        return out
+
+    def _sample_episodes(self, x, k: int, step_index: int):
+        """The native call of sample_episodes on a checked table `x` at RNG counter `step_index`: (makespan, log_prob),
+        each (N, k)."""
+        import torch
+        v = self._table_view(x)
+        makespan = torch.empty((self.num_envs, k), dtype=torch.int32, device=self.device)
+        log_prob = torch.empty((self.num_envs, k), dtype=torch.float32, device=self.device)
+        rc = self._L.jss_sample_episodes(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed, step_index,
+                                         k, makespan.data_ptr(), log_prob.data_ptr(), k, self._stream())
+        N.check(self._h, rc, "jss_sample_episodes")
+        return makespan, log_prob
+
+    def _sample_episodes_grad(self, x, k: int, step_index: int, weights, split: int):
+        """The native backward of sample_episodes: the (split, N, J, M) float32 chunks of sum_s weights[:, s] *
+        d log_prob[:, s] / d table, replayed from the current state at RNG counter `step_index`."""
+        import torch
+        v = self._table_view(x)
+        w = weights.detach().to(torch.float32).contiguous()
+        grad = torch.zeros((split, self.num_envs, self.jobs, self.machines), dtype=torch.float32, device=self.device)
+        rc = self._L.jss_sample_episodes_grad(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
+                                              step_index, k, w.data_ptr(), k, int(split), grad.data_ptr(),
+                                              self._stream())
+        N.check(self._h, rc, "jss_sample_episodes_grad")
+        return grad
+
+    def _warp_slots(self):
+        """Resident warps of the env's device (1 for a backend that does not say: one gradient chunk)."""
+        slots = getattr(N.backend, "warp_slots", None)
+        return slots(self.device_index) if slots is not None else 1
 
     def _table_arg(self, x, who: str, what: str):
         """A caller's priority / logit table as a tensor on the env's device, refused unless it is 3-D and broadcasts
