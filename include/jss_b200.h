@@ -157,7 +157,9 @@ int jss_load_instances(jss_t *h, int n_inst, const int32_t *jobs, const int32_t 
                        const int64_t *offsets, const int32_t *machine, const int32_t *duration);
 
 /* env i runs instance env_to_inst[i] (host pointer, n_envs entries); allocates
- * all device buffers.  Must follow jss_load_instances. */
+ * all device buffers and resets every env.  Must follow jss_load_instances.
+ * Synchronous: returns once its device work has completed, so the batch may be
+ * stepped at once on any stream. */
 int jss_assign(jss_t *h, const int32_t *env_to_inst);
 
 int jss_get_buffers(jss_t *h, jss_buffers *out);
@@ -505,8 +507,10 @@ int jss_step_host(jss_t *h, const int32_t *actions_host, uint8_t *mask_host, flo
  * for a host policy to choose the next actions); JSS_WAIT_OBS until its observation has landed.
  * A new begin may follow WAIT_MASK while the previous observation is still streaming into ITS host
  * buffer (callers alternate two pinned observation buffers and call WAIT_OBS before reading one).
- * The pipeline is ordered after the work already enqueued on `after_stream` (the caller's stream);
- * call jss_host_wait(JSS_WAIT_OBS) before going back to the stream-ordered entry points. */
+ * The pipeline is ordered after the work already enqueued on `after_stream` (the caller's stream),
+ * and every stream-ordered entry point (those taking a `stream`) orders its stream after the latest
+ * begin, observation transfer included, without blocking the host: a device step, export or
+ * statistics call made right after a begin acts on the state that begin left. */
 #define JSS_WAIT_MASK 1
 #define JSS_WAIT_OBS 2       /* observation of the latest begin */
 #define JSS_WAIT_OBS_PREV 3  /* observation of the begin before the latest one */

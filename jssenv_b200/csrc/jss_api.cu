@@ -37,6 +37,7 @@ static cudaError_t jss_launch_pdl(void (*kern)(KArgs...), int grid, int block, s
 #include <sched.h>
 #include <cctype>
 #include <map>
+#include <mutex>
 #include <utility>
 #include <vector>
 
@@ -46,6 +47,11 @@ static cudaError_t jss_launch_pdl(void (*kern)(KArgs...), int grid, int block, s
 namespace {
 
 std::string g_create_error;
+
+// the dynamic shared memory each kernel is opted in to, by (device, kernel): the attribute belongs to the kernel on its
+// device, so every handle of the process shares it (smem_optin)
+std::mutex g_optin_mutex;
+std::map<std::pair<int, const void *>, size_t> g_smem_optin;
 
 }  // namespace
 
@@ -79,7 +85,6 @@ struct jss_handle {
     int32_t class_tiles[JSS_LANE_CLASSES][2] = {};  // [class_tiles[c][0], class_tiles[c][1]): the tiles of lane class c
     int n_tiles = 0;
     std::map<std::pair<const void *, size_t>, int> ctas_per_sm;   // by kernel and dynamic shared memory (filled lazily)
-    std::map<const void *, size_t> smem_optin;     // by kernel: the largest dynamic shared memory it was opted in to
     std::vector<int32_t> env_inst;
 
     // host-buffer stepping
@@ -127,20 +132,30 @@ int dev_alloc(jss_t *h, T **out, size_t count, bool zero = true) {
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 size_t smem_bytes(const JssSmemLayout &sl) { return (size_t)sl.off_warp0 + (size_t)JSS_WARPS_PER_CTA * sl.warp_stride; }
 
+// opts `kern` in to `smem` bytes of dynamic shared memory if that is more than 48 KB and more than it has now.  The
+// opt-in is one limit per kernel and device, shared by every handle of the process, so it only ever grows: lowering it
+// for a smaller layout would make the next launch with a larger one -- of this handle or of another -- fail.
+template <typename Kern>
+int smem_optin(jss_t *h, Kern kern, size_t smem) {
+    if (smem <= 48 * 1024) return JSS_OK;
+    std::lock_guard<std::mutex> lock(g_optin_mutex);
+    size_t &optin = g_smem_optin[{h->device, reinterpret_cast<const void *>(kern)}];
+    if (smem > optin) {
+        JSS_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        optin = smem;
+    }
+    return JSS_OK;
+}
+
 // resident CTAs per SM of `kern` at `smem` bytes of dynamic shared memory; the first call per kernel and size also
-// opts the kernel in to more than 48 KB.  Keyed by size too: the rule-sampling step kernels run with and without the
-// suffix-sum table.  The opt-in is one limit per kernel, so it only ever grows: lowering it for the smaller layout
-// would make the next launch with the larger one fail.
+// opts the kernel in to them (smem_optin).  Keyed by size too: the rule-sampling step kernels run with and without the
+// suffix-sum table.
 template <typename Kern>
 int ctas_per_sm(jss_t *h, Kern kern, size_t smem, int &per_sm) {
     const void *key = reinterpret_cast<const void *>(kern);
     int &n = h->ctas_per_sm[{key, smem}];
     if (n == 0) {
-        size_t &optin = h->smem_optin[key];
-        if (smem > 48 * 1024 && smem > optin) {
-            JSS_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            optin = smem;
-        }
+        if (int rc = smem_optin(h, kern, smem)) return rc;
         JSS_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, JSS_WARPS_PER_CTA * 32, smem));
         if (n < 1) { n = 0; return fail(h, JSS_ERR_CUDA, "kernel does not fit on an SM (smem %zu B)", smem); }
     }
@@ -280,6 +295,17 @@ int check_ready(jss_t *h) {
     if (!h) return JSS_ERR_INVALID;
     if (!h->assigned) return fail(h, JSS_ERR_STATE, "jss_load_instances + jss_assign must be called first");
     JSS_CUDA(h, cudaSetDevice(h->device));
+    return JSS_OK;
+}
+
+// check_ready for an entry point that works on `stream`: it also orders the stream after the latest
+// jss_host_step_begin (its step, result copies and observation transfer), which runs on the handle's own streams and
+// reads and writes the same state, outputs and action buffer.  The pipeline's own launches on s_compute are ordered
+// already.  Nothing to do before the first begin.
+int check_ready(jss_t *h, void *stream) {
+    if (int rc = check_ready(h)) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (h->pipe_ready && st != h->s_compute) JSS_CUDA(h, cudaStreamWaitEvent(st, h->ev_obs[h->pipe_cur], 0));
     return JSS_OK;
 }
 
@@ -619,7 +645,11 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     if ((rc = dev_alloc(h, &h->dev_actions, (size_t)N))) return rc;
     h->assigned = true;
     // a fresh batch starts reset, like a freshly constructed + reset reference env
-    return jss_reset(h, nullptr, nullptr);
+    if ((rc = jss_reset(h, nullptr, nullptr))) return rc;
+    // the memsets above and this reset run on the legacy default stream, which a caller's non-blocking stream does not
+    // wait for: return only once they have completed, so the batch may be stepped at once on any stream
+    JSS_CUDA(h, cudaStreamSynchronize(nullptr));
+    return JSS_OK;
 }
 
 int jss_get_buffers(jss_t *h, jss_buffers *out) {
@@ -644,7 +674,7 @@ int jss_get_buffers(jss_t *h, jss_buffers *out) {
 }
 
 int jss_reset(jss_t *h, const uint8_t *env_mask_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     JssLaunch a{};
     a.mode = JSS_MODE_RESET;
@@ -653,7 +683,7 @@ int jss_reset(jss_t *h, const uint8_t *env_mask_dev, void *stream) {
 }
 
 int jss_step(jss_t *h, const int32_t *actions_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!actions_dev) return fail(h, JSS_ERR_INVALID, "jss_step: actions_dev is NULL");
     JssLaunch a{};
@@ -663,7 +693,7 @@ int jss_step(jss_t *h, const int32_t *actions_dev, void *stream) {
 }
 
 int jss_step_export(jss_t *h, const int32_t *actions_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!actions_dev) return fail(h, JSS_ERR_INVALID, "jss_step_export: actions_dev is NULL");
     JssLaunch a{};
@@ -675,7 +705,7 @@ int jss_step_export(jss_t *h, const int32_t *actions_dev, void *stream) {
 
 int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mode, uint64_t seed,
                     uint64_t step_index, int32_t *next_actions_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!actions_dev || !next_actions_dev || !valid_rule_coin(rule, coin_mode))
         return fail(h, JSS_ERR_INVALID, "jss_step_sample: bad arguments (rule %d, coin %d)", rule, coin_mode);
@@ -734,7 +764,7 @@ int launch_record(jss_t *h, const char *what, float *obs_out_dev, uint8_t *mask_
 
 int jss_step_logits(jss_t *h, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
                     int32_t *actions_out_dev, float *log_prob_out_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     JssLaunch a;
     if ((rc = logits_launch(h, "jss_step_logits", logits_dev, ld, seed, step_index, actions_out_dev, log_prob_out_dev, a)))
@@ -746,7 +776,7 @@ int jss_step_logits_record(jss_t *h, const float *logits_dev, int64_t ld, uint64
                            int32_t *actions_out_dev, float *log_prob_out_dev, float *obs_out_dev, uint8_t *mask_out_dev,
                            int32_t *scalars_out_dev, void *stream) {
     const char *what = "jss_step_logits_record";
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     JssLaunch a;
     if ((rc = logits_launch(h, what, logits_dev, ld, seed, step_index, actions_out_dev, log_prob_out_dev, a))) return rc;
@@ -755,7 +785,7 @@ int jss_step_logits_record(jss_t *h, const float *logits_dev, int64_t ld, uint64
 
 int jss_step_greedy(jss_t *h, const float *scores_dev, int64_t ld, double epsilon, uint64_t seed, uint64_t step_index,
                     int32_t *actions_out_dev, float *log_prob_out_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     JssLaunch a;
     if ((rc = greedy_launch(h, "jss_step_greedy", scores_dev, ld, epsilon, seed, step_index, actions_out_dev,
@@ -768,7 +798,7 @@ int jss_step_greedy_record(jss_t *h, const float *scores_dev, int64_t ld, double
                            uint64_t step_index, int32_t *actions_out_dev, float *log_prob_out_dev, float *obs_out_dev,
                            uint8_t *mask_out_dev, int32_t *scalars_out_dev, void *stream) {
     const char *what = "jss_step_greedy_record";
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     JssLaunch a;
     if ((rc = greedy_launch(h, what, scores_dev, ld, epsilon, seed, step_index, actions_out_dev, log_prob_out_dev, a)))
@@ -777,14 +807,14 @@ int jss_step_greedy_record(jss_t *h, const float *scores_dev, int64_t ld, double
 }
 
 int jss_refresh_obs(jss_t *h, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     return refresh_obs(h, (cudaStream_t)stream);
 }
 
 int jss_policy(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_index, int32_t *actions_dev,
                void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!actions_dev || !valid_rule_coin(rule, coin_mode))
         return fail(h, JSS_ERR_INVALID, "jss_policy: bad arguments (rule %d, coin %d)", rule, coin_mode);
@@ -796,7 +826,7 @@ int jss_policy(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_i
 }
 
 int jss_rollout(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_steps, int write_obs, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!valid_rule_coin(rule, JSS_COIN_DEVICE) || n_steps < 0)
         return fail(h, JSS_ERR_INVALID, "jss_rollout: bad arguments (rule %d, n_steps %d)", rule, n_steps);
@@ -809,7 +839,7 @@ int jss_rollout(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_st
 
 int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int n_steps, float *traj_obs,
                      uint8_t *traj_mask, int32_t *traj_scalars, int32_t *traj_actions, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!valid_rule_coin(rule, JSS_COIN_DEVICE) || n_steps < 0 || !traj_obs || !traj_mask || !traj_scalars)
         return fail(h, JSS_ERR_INVALID, "jss_rollout_traj: bad arguments (rule %d, n_steps %d)", rule, n_steps);
@@ -825,7 +855,7 @@ int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int
 
 int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op, int n_steps,
                          void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!prio_dev || ((uintptr_t)prio_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || n_steps < 0)
         return fail(h, JSS_ERR_INVALID, "jss_rollout_priority: bad arguments (prio %p must be 4-byte aligned, strides "
@@ -843,7 +873,7 @@ int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_
 int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                                 uint64_t seed, uint64_t step_index, int n_steps, float *log_prob_out_dev,
                                 float *grad_out_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!logits_dev || ((uintptr_t)logits_dev & 3u) || !log_prob_out_dev || ((uintptr_t)log_prob_out_dev & 3u) ||
         ((uintptr_t)grad_out_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || n_steps < 0)
@@ -866,7 +896,7 @@ int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_en
 
 int jss_lookahead(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_index, int32_t *makespan_out_dev,
                   int64_t ld, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!valid_rule_coin(rule, coin_mode) || !makespan_out_dev || ((uintptr_t)makespan_out_dev & 3u) ||
         ld < (int64_t)h->p.jobs_max + 1)
@@ -883,7 +913,7 @@ int jss_lookahead(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t ste
 
 int jss_lookahead_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                            int32_t *makespan_out_dev, int64_t ld, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!prio_dev || ((uintptr_t)prio_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || !makespan_out_dev ||
         ((uintptr_t)makespan_out_dev & 3u) || ld < (int64_t)h->p.jobs_max + 1)
@@ -933,7 +963,7 @@ int sample_episodes_args(jss_t *h, const char *who, const float *logits, int64_t
 int jss_sample_episodes(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                         uint64_t seed, uint64_t step_index, int64_t k, int32_t *makespan_out_dev,
                         float *log_prob_out_dev, int64_t ld, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     const char *who = "jss_sample_episodes";
     if (bad_ptr(makespan_out_dev) || bad_ptr(log_prob_out_dev))
@@ -951,7 +981,7 @@ int jss_sample_episodes(jss_t *h, const float *logits_dev, int64_t ld_env, int64
 int jss_sample_episodes_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                              uint64_t seed, uint64_t step_index, int64_t k, const float *weights_dev, int64_t ld,
                              int split, float *grad_out_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     const char *who = "jss_sample_episodes_grad";
     if (bad_ptr(weights_dev) || bad_ptr(grad_out_dev) || split < 1 || split > k)
@@ -973,7 +1003,7 @@ int jss_sample_episodes_grad(jss_t *h, const float *logits_dev, int64_t ld_env, 
 int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                                  uint64_t seed, uint64_t step_index, const int32_t *sample_dev,
                                  int32_t *solution_out_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     const char *who = "jss_sample_episodes_solution";
     if (bad_ptr(sample_dev) || bad_ptr(solution_out_dev))
@@ -991,7 +1021,7 @@ int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_e
 
 int jss_step_host(jss_t *h, const int32_t *actions_host, uint8_t *mask_host, float *obs_host,
                   int32_t *scalars_host, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!actions_host) return fail(h, JSS_ERR_INVALID, "jss_step_host: actions_host is NULL");
     cudaStream_t st = (cudaStream_t)stream;
@@ -1016,7 +1046,7 @@ namespace {
 // wire_host != NULL: envs [max(n_dma, 0), N) ship packed integer rows.
 int host_step_begin_impl(jss_t *h, const int32_t *actions_host, uint8_t *mask_host, float *obs_host, uint8_t *wire_host,
                          int32_t *scalars_host, void *after_stream, int n_dma = -1) {
-    int rc = check_ready(h);
+    int rc = check_ready(h);           // the pipeline orders itself: s_compute follows after_stream and itself
     if (rc) return rc;
     if (!actions_host) return fail(h, JSS_ERR_INVALID, "jss_host_step_begin: actions_host is NULL");
     const JssParams &p = h->p;
@@ -1085,8 +1115,8 @@ int host_step_begin_impl(jss_t *h, const int32_t *actions_host, uint8_t *mask_ho
         a.wire_stride = (int32_t)h->wire_stride;
         if ((rc = launch_all(h, a, sc))) return rc;
     }
-    // the copy stream never runs ahead of the step (also when nothing large is copied: JSS_WAIT_OBS is the barrier
-    // callers take before going back to the stream-ordered entry points)
+    // the copy stream never runs ahead of the step (also when nothing large is copied: ev_obs is what JSS_WAIT_OBS and
+    // the stream-ordered entry points wait for)
     JSS_CUDA(h, cudaEventRecord(h->ev_staged, sc));
     JSS_CUDA(h, cudaStreamWaitEvent(h->s_copy, h->ev_staged, 0));
     if (wire_host && n_fp32 < N) {       // the packed rows first: the host has to expand them, the fp32 rows are final
@@ -1198,7 +1228,7 @@ int jss_host_wait(jss_t *h, int what) {
 }
 
 int jss_stats(jss_t *h, int64_t *out_host, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     if (!out_host) return fail(h, JSS_ERR_INVALID, "jss_stats: out_host is NULL");
     cudaStream_t st = (cudaStream_t)stream;
@@ -1221,7 +1251,7 @@ int jss_stats(jss_t *h, int64_t *out_host, void *stream) {
 }
 
 int jss_export_state(jss_t *h, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     JssLaunch a{};
     a.mode = JSS_MODE_EXPORT;
@@ -1229,7 +1259,7 @@ int jss_export_state(jss_t *h, void *stream) {
 }
 
 int jss_import_state(jss_t *h, const uint8_t *env_mask_dev, void *stream) {
-    int rc = check_ready(h);
+    int rc = check_ready(h, stream);
     if (rc) return rc;
     JssLaunch a{};
     a.mode = JSS_MODE_IMPORT;

@@ -676,7 +676,8 @@ class JssVecEnv:
         packed=True ships the observation as 10-byte integer records per job instead of 28 bytes of fp32
         (jss_host_step_begin_packed); host_wait_obs() then expands them to the exact float observation.
         dma_fraction > 0 (with packed): that share of the envs ships final fp32 rows by DMA instead, so PCIe and the
-        host cores each work on their part in parallel (jss_host_step_begin_hybrid)."""
+        host cores each work on their part in parallel (jss_host_step_begin_hybrid).  The step is ordered after the work
+        on the current stream, and every later call of this env, on any stream, after the step and its transfers."""
         a = np.ascontiguousarray(actions, dtype=np.int32)
         n, J = self.num_envs, self.jobs
         if not hasattr(self, "_pipe"):
@@ -781,6 +782,10 @@ class JssVecEnv:
 
     def import_state(self, state: Dict[str, Any], mask=None):
         """Restore a snapshot taken with export_state() (tensors are copied into the library's buffers)."""
+        if getattr(self, "_pipe_inflight", 0):
+            # the copies below are torch ops, which the library cannot order after a host_step_begin still writing
+            # the time and flags; its own entry points can
+            N.check(self._h, self._L.jss_host_wait(self._h, N.WAIT_OBS), "jss_host_wait")
         for k, dst in {**self._x, "t": self.current_time_step, "flags": self._flags_done}.items():
             if state[k].data_ptr() != dst.data_ptr():
                 dst.copy_(state[k])
