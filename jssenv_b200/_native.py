@@ -18,6 +18,7 @@ ACTION_SKIP, ACTION_ADVANCE = -1, -2
 CREATE_AUTO_RESET, CREATE_RECORD_SOLUTION, CREATE_HOST_MIRROR = 1, 2, 4
 FLAG_DONE, FLAG_ERROR, FLAG_NOOP_LEGAL = 1, 2, 4
 COIN_DEVICE, COIN_NEVER = 0, 1
+MAX_BEAM_WIDTH = 32   # JSS_MAX_BEAM_WIDTH
 WAIT_MASK, WAIT_OBS, WAIT_OBS_PREV = 1, 2, 3
 RULES = {"RANDOM": 0, "SPT": 1, "FIFO": 2, "MWR": 3, "LWR": 4, "MOR": 5, "LOR": 6, "CR": 7}
 STATS_KEYS = ("episodes", "steps", "sum_makespan", "min_makespan", "max_makespan", "sum_return",
@@ -76,6 +77,7 @@ SIGNATURES = {
     "jss_sample_episodes_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, c_int64,
                                          c_int, _VP, _VP]),
     "jss_sample_episodes_solution": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, _VP, _VP, _VP]),
+    "jss_beam_search": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_int, _VP, _VP, c_int64, _VP, _VP]),
     "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_step_begin": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_wait": (c_int, [_VP, c_int]),

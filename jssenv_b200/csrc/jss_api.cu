@@ -78,6 +78,8 @@ struct jss_handle {
     uint16_t *d_ops = nullptr, *d_rem = nullptr;
     int32_t *d_len = nullptr;
     unsigned long long *d_stats = nullptr;
+    uint16_t *beam_trace = nullptr;                // jss_beam_search's backpointers (first call with an order)
+    size_t beam_trace_bytes = 0;
 
     JssParams p{};
     JssSmemLayout sl_env{}, sl_step{}, sl_step_rem{};   // shared-memory layouts of the generic / step kernels (step: without / with the suffix-sum table)
@@ -215,6 +217,27 @@ int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
 
 int launch_all(jss_t *h, JssLaunch a, cudaStream_t st);
 
+// jss_beam_search's shared-memory layout: the instance tables without the suffix sums, env_check_no_op's 32-word
+// table per warp, then the beam region of width W (jss_beam_smem) with blocks of the batch maxima
+JssSmemLayout beam_layout(const jss_t *h) {
+    JssSmemLayout sl = h->sl_env;
+    sl.off_warp0 = sl.off_rem;
+    sl.warp_stride = 32 * 4;
+    return sl;
+}
+size_t beam_smem(const jss_t *h, int W) {
+    return smem_bytes(beam_layout(h)) +
+           jss_beam_smem(nullptr, W, jss_block_geom(h->p.jobs_max, h->p.machines_max).words, nullptr);
+}
+// the persistent grid of lane class c's beam search launch: one work item per env, at most the resident CTAs
+int beam_grid(jss_t *h, int c, int W, int &grid) {
+    const int n_items = (h->class_tiles[c][1] - h->class_tiles[c][0]) * JSS_WARPS_PER_CTA;
+    int per_sm = 0;
+    if (int rc = ctas_per_sm(h, env_kernels<JSS_MODE_BEAM_SEARCH>[c], beam_smem(h, W), per_sm)) return rc;
+    grid = std::min(n_items, h->sm_count * per_sm);
+    return JSS_OK;
+}
+
 // rewrite real_obs from the state blocks if a recording step left it stale (jss_refresh_obs)
 int refresh_obs(jss_t *h, cudaStream_t st) {
     if (!h->obs_stale) return JSS_OK;
@@ -230,9 +253,9 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     // meaning after a recording step (a plain step rewrites only the envs it changes)
     const bool recording = a.mode == JSS_MODE_STEP && a.traj_obs;
     const bool lookahead = a.mode == JSS_MODE_LOOKAHEAD || a.mode == JSS_MODE_LOOKAHEAD_PRIORITY;
-    const bool samples = jss_mode_samples(a.mode);
+    const bool samples = jss_mode_samples(a.mode), beam = a.mode == JSS_MODE_BEAM_SEARCH;
     if (!recording && a.mode != JSS_MODE_EXPORT && a.mode != JSS_MODE_POLICY && a.mode != JSS_MODE_REFRESH &&
-        !lookahead && !samples)                          // these read only state blocks and write the caller's buffers
+        !lookahead && !samples && !beam)                 // these read only state blocks and write the caller's buffers
         if (int rc = refresh_obs(h, st)) return rc;
     if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
@@ -246,6 +269,7 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
                            : a.mode == JSS_MODE_SAMPLE_EPISODES ? env_kernels<JSS_MODE_SAMPLE_EPISODES>
                            : a.mode == JSS_MODE_SAMPLE_EPISODES_GRAD ? env_kernels<JSS_MODE_SAMPLE_EPISODES_GRAD>
                            : a.mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION ? env_kernels<JSS_MODE_SAMPLE_EPISODES_SOLUTION>
+                           : beam ? env_kernels<JSS_MODE_BEAM_SEARCH>
                            : env_kernels<JSS_MODE_RESET>;
     // what the launch reads: a rollout or lookahead every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
     // / CR), and the masked-uniform sampler no table at all (only J); the other modes ops / len (the lookahead over a
@@ -253,8 +277,8 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     a.stage = a.mode == JSS_MODE_ROLLOUT || a.mode == JSS_MODE_LOOKAHEAD ? JSS_STAGE_ALL
             : a.mode != JSS_MODE_POLICY ? JSS_STAGE_OPS
             : a.rule == JSS_RULE_RANDOM ? 0 : jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
-    const JssSmemLayout &sl = h->sl_env;
-    const size_t smem = smem_bytes(sl);
+    const JssSmemLayout sl = beam ? beam_layout(h) : h->sl_env;
+    const size_t smem = beam ? beam_smem(h, a.beam_width) : smem_bytes(sl);
     for (int c = 0; c < JSS_LANE_CLASSES; c++) {   // one launch per lane class present
         a.tile_begin = h->class_tiles[c][0];
         a.tile_end = h->class_tiles[c][1];
@@ -278,6 +302,8 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
             if (a.mode == JSS_MODE_SAMPLE_EPISODES)
                 a.n_steps = n_tiles >= slots ? 1 : std::min(a.n_samples, (slots + n_tiles - 1) / n_tiles);
             grid = (int)std::min<int64_t>((int64_t)n_tiles * a.n_steps, slots);
+        } else if (beam) {
+            if (int rc = beam_grid(h, c, a.beam_width, grid)) return rc;   // the grid the trace is sized for
         }
         JSS_LAUNCH(kerns[c], grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
         JSS_CUDA(h, cudaGetLastError());
@@ -481,6 +507,7 @@ void jss_destroy(jss_t *h) {
         cudaStreamDestroy(h->s_compute); cudaStreamDestroy(h->s_copy);
     }
     for (void *ptr : h->allocs) cudaFree(ptr);
+    if (h->beam_trace) cudaFree(h->beam_trace);
     if (h->host_block) cudaFreeHost(h->host_block);
     delete h;
 }
@@ -1016,6 +1043,53 @@ int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_e
     a.actions = sample_dev;
     a.solution_out = solution_out_dev;
     a.n_steps = 1;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_beam_search(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op, int width,
+                    int32_t *makespan_out_dev, float *score_out_dev, int64_t ld, int32_t *order_out_dev, void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    if (bad_ptr(logits_dev) || ld_env < 0 || ld_job < 0 || ld_op < 0 || bad_ptr(makespan_out_dev) ||
+        bad_ptr(score_out_dev) || ((uintptr_t)order_out_dev & 3u) || width < 1 || width > JSS_MAX_BEAM_WIDTH ||
+        ld < width)
+        return fail(h, JSS_ERR_INVALID, "jss_beam_search: bad arguments (logits %p, makespan_out %p and score_out %p "
+                    "must be non-NULL, they and order_out %p 4-byte aligned, strides %lld / %lld / %lld >= 0, "
+                    "1 <= width %d <= %d, ld %lld >= width)", (const void *)logits_dev, (void *)makespan_out_dev,
+                    (void *)score_out_dev, (void *)order_out_dev, (long long)ld_env, (long long)ld_job,
+                    (long long)ld_op, width, JSS_MAX_BEAM_WIDTH, (long long)ld);
+    JssLaunch a{};
+    a.mode = JSS_MODE_BEAM_SEARCH;
+    a.logits = logits_dev;
+    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
+    a.beam_width = width;
+    a.actions_out = makespan_out_dev;
+    a.log_prob_out = score_out_dev;
+    a.samples_ld = ld;
+    a.order_out = order_out_dev;
+    if (order_out_dev) {
+        // the trace: W backpointers per round (at most jobs_max * machines_max rounds) for each CTA of the largest grid
+        int grid_max = 0;
+        for (int c = 0; c < JSS_LANE_CLASSES; c++) {
+            if (h->class_tiles[c][1] <= h->class_tiles[c][0]) continue;
+            int grid = 0;
+            if ((rc = beam_grid(h, c, width, grid))) return rc;
+            grid_max = std::max(grid_max, grid);
+        }
+        const size_t need = (size_t)grid_max * width * h->p.jobs_max * h->p.machines_max * sizeof(uint16_t);
+        if (need > h->beam_trace_bytes) {
+            if (h->beam_trace) {                         // cudaFree waits for the launches that may still use it
+                JSS_CUDA(h, cudaFree(h->beam_trace));
+                h->beam_trace = nullptr;
+                h->beam_trace_bytes = 0;
+            }
+            void *ptr = nullptr;
+            JSS_CUDA(h, cudaMalloc(&ptr, need));
+            h->beam_trace = static_cast<uint16_t *>(ptr);
+            h->beam_trace_bytes = need;
+        }
+        a.beam_trace = h->beam_trace;
+    }
     return launch_all(h, a, (cudaStream_t)stream);
 }
 

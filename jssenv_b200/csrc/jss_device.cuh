@@ -1638,6 +1638,227 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
     }
 }
 
+// ---- beam search over a logit table, the envs untouched (jss_beam_search) -----------------------------------------
+// Each owned legal job's log-probability under the table, lp[i] = (x - mx) - log(sum exp(x - mx)) over the legal jobs,
+// with the loads, reductions and fast exp / log of env_priority_sample_action in the same order, so that lp of the job
+// it draws equals its logp bit for bit.  Kept apart from it so that its code (and the sampling kernels') stays as it
+// is.  At least one job must be legal; returns false for a bad row (the bad-table rule of env_priority_sample_action).
+template <int KJ>
+JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ]) {
+    const float *row = a.logits + (int64_t)env * a.logits_ld;
+    bool bad = false;                                    // a legal entry is NaN or +inf
+    uint32_t xkey = 0u;                                  // 0: below every candidate's key
+    float x[KJ];
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        x[i] = 0.0f;
+        if ((s.lb >> i) & 1u) {
+            x[i] = row[(int64_t)(KJ * lane + i) * a.prio_ld_job + (int64_t)s.todo[i] * a.prio_ld_op];
+            bad = bad || !(x[i] < JSS_F32_INF);
+            xkey = max(xkey, jss_f32_key(x[i]));
+        }
+    }
+    const float mx = jss_key_f32(__reduce_max_sync(JSS_FULL, xkey));
+    if (__any_sync(JSS_FULL, bad) || mx == -JSS_F32_INF) return false;
+    float sum = 0.0f;
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        x[i] -= mx;
+        if ((s.lb >> i) & 1u) sum += jss_fast_exp(x[i]);
+    }
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) sum += __shfl_xor_sync(JSS_FULL, sum, off);   // the same sum in every lane
+    const float ls = jss_fast_log(sum);
+#pragma unroll
+    for (int i = 0; i < KJ; i++) lp[i] = x[i] - ls;
+    return true;
+}
+
+// Candidate key of the selection order: score descending (jss_f32_key of score + 0, so -0 and +0 tie), then parent slot
+// ascending, then job ascending -- the larger key is the better candidate, and no two candidates of a round share one.
+// The low word holds ~(parent << 8 | job), 13 bits, which the u16 backpointer of a round keeps.
+JSS_DEV uint64_t jss_beam_key(uint32_t score_key, int parent, int job) {
+    return ((uint64_t)score_key << 32) | (uint32_t)~(uint32_t)(parent << 8 | job);
+}
+
+// The beam region of the CTA's shared memory for width W and state blocks of `bw` words (jss_block_geom of the batch
+// maxima): [blocks: 2][W][bw] int32 | [cand: W][W] u64 | [sel: W] u64 | [score: 2][W] f32 | [cnt: W] i32 | [bad] i32.
+// jss_beam_search sizes it with the same function.
+struct JssBeamSmem {
+    int32_t *blocks;
+    uint64_t *cand, *sel;
+    float *score;
+    int32_t *cnt, *bad;
+};
+JSS_HD inline size_t jss_beam_smem(char *base, int W, int bw, JssBeamSmem *b) {
+    const size_t o_cand = (size_t)2 * W * bw * 4, o_sel = o_cand + (size_t)8 * W * W, o_score = o_sel + (size_t)8 * W;
+    const size_t o_cnt = o_score + (size_t)8 * W, o_bad = o_cnt + (size_t)4 * W, end = (o_bad + 4 + 15) & ~(size_t)15;
+    if (b) {
+        b->blocks = reinterpret_cast<int32_t *>(base);
+        b->cand = reinterpret_cast<uint64_t *>(base + o_cand);
+        b->sel = reinterpret_cast<uint64_t *>(base + o_sel);
+        b->score = reinterpret_cast<float *>(base + o_score);
+        b->cnt = reinterpret_cast<int32_t *>(base + o_cnt);
+        b->bad = reinterpret_cast<int32_t *>(base + o_bad);
+    }
+    return end;
+}
+
+// One env searched by the whole CTA (`root`: its state block, never written).  The beams are state blocks in shared
+// memory, double-buffered: round r reads buffer r & 1 and writes the other.  Per round (R rounds, the operations not
+// started at entry; jss_b200.h):
+//   1. warp w expands the beams b = w, w + 8, ...: forced no-ops (stored back in place), the log-probabilities of the
+//      legal jobs (env_table_logp), and the beam's best min(W, candidates) children in key order, by W argmax passes;
+//   2. the CTA ranks every candidate against the others' sorted lists; rank < W becomes slot rank;
+//   3. warp w loads the parent block of each of its new slots, steps the job with env_step<KJ, false> and stores the
+//      result in the other buffer; lane 0 records the backpointer parent << 8 | job in the trace (a.beam_trace).
+// At the end warp 0 writes the slot outputs and, with a.order_out, walks the trace back from the best slot: each job's
+// allocations in reverse are its operations M-1, M-2, ... (a complete beam has allocated every operation).
+template <int KJ>
+JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, const int32_t *root,
+                             int warp, int lane, int *hz, char *bsm) {
+    constexpr uint32_t LM = jss_legal_mask<KJ>();
+    const int W = a.beam_width, bw = jss_block_geom(p.jobs_max, p.machines_max).words;
+    const int J = jss_J(iv), M = jss_M(iv), nw = iv.si->block_words;
+    JssBeamSmem bs;
+    jss_beam_smem(bsm, W, bw, &bs);
+    const auto slot = [&](int buf, int b) { return bs.blocks + (size_t)(buf * W + b) * bw; };
+    uint16_t *trace = a.beam_trace ? a.beam_trace + (size_t)blockIdx.x * W * p.jobs_max * p.machines_max : nullptr;
+    __syncthreads();                                     // the previous env's last reads of the region are done
+    for (int k = (int)threadIdx.x; k < nw / 4; k += (int)blockDim.x)
+        reinterpret_cast<int4 *>(bs.blocks)[k] = reinterpret_cast<const int4 *>(root)[k];
+    if (threadIdx.x == 0) { bs.score[0] = 0.0f; bs.bad[0] = 0; }
+    __syncthreads();
+    EnvRegs<KJ> s;
+    env_load<KJ>(iv, bs.blocks, lane, s);
+    s.flags = jss_uniform(s.flags);
+    const bool done0 = (s.flags & JSS_FLAG_DONE) != 0u;
+    int left = 0;                                        // operations not started: R, summed over the warp
+#pragma unroll
+    for (int i = 0; i < KJ; i++) left += max(0, M - s.todo[i] - (s.tufco[i] > 0 ? 1 : 0));
+    const int R = done0 ? 0 : (int)__reduce_add_sync(JSS_FULL, (unsigned)left);
+    int n = 1, cur = 0;                                  // live slots, and the buffer that holds them
+    for (int r = 0; r < R && n > 0; r++) {
+        for (int b = warp; b < n; b += JSS_WARPS_PER_CTA) {   // 1. expand
+            int32_t *blk = slot(cur, b);
+            env_load<KJ>(iv, blk, lane, s);
+            s.flags = jss_uniform(s.flags);
+            const float sc = bs.score[cur * W + b];
+            bool ok = sc == sc, moved = false;           // NaN: the step into this slot failed (an imported state)
+            while (ok && !__any_sync(JSS_FULL, (s.lb & LM) != 0u)) {   // forced no-ops
+                int raw;
+                ok = (s.flags & JSS_FLAG_NOOP_LEGAL) && env_step<KJ, false>(p, iv, s, env, lane, J, raw, hz);
+                s.flags = jss_uniform(s.flags);
+                moved = true;
+            }
+            if (ok && moved) env_store<KJ>(iv, blk, lane, s);
+            int taken = 0;
+            float lp[KJ];
+            if (ok && !env_table_logp<KJ>(a, s, env, lane, lp)) {
+                ok = false;
+                if (lane == 0) bs.bad[0] = 1;
+            }
+            if (ok) {
+                uint32_t key[KJ];                        // 0: not a candidate, or already taken
+                int nc = 0;
+#pragma unroll
+                for (int i = 0; i < KJ; i++) {
+                    const float cs = sc + lp[i];
+                    key[i] = ((s.lb >> i) & 1u) && cs > -JSS_F32_INF ? jss_f32_key(cs + 0.0f) : 0u;
+                    nc += key[i] != 0u;
+                }
+                taken = min(W, (int)__reduce_add_sync(JSS_FULL, (unsigned)nc));
+                for (int q = 0; q < taken; q++) {
+                    uint32_t lk = 0u;
+                    int lj = 1 << 20;
+#pragma unroll
+                    for (int i = 0; i < KJ; i++)
+                        if (key[i] > lk) { lk = key[i]; lj = KJ * lane + i; }
+                    const uint32_t best = __reduce_max_sync(JSS_FULL, lk);
+                    const int j = (int)__reduce_min_sync(JSS_FULL, (unsigned)(lk == best ? lj : 1 << 20));
+#pragma unroll
+                    for (int i = 0; i < KJ; i++)
+                        if (KJ * lane + i == j) key[i] = 0u;
+                    if (lane == 0) bs.cand[b * W + q] = jss_beam_key(best, b, j);
+                }
+            }
+            if (lane == 0) bs.cnt[b] = taken;
+        }
+        __syncthreads();
+        int total = 0;                                   // 2. select
+        for (int b = 0; b < n; b++) total += bs.cnt[b];
+        for (int e = (int)threadIdx.x; e < n * W; e += (int)blockDim.x) {
+            const int b = e / W;
+            if (e - b * W >= bs.cnt[b]) continue;
+            const uint64_t k = bs.cand[e];
+            int rank = 0;
+            for (int b2 = 0; b2 < n; b2++) {             // each list is sorted, best first
+                const uint64_t *c2 = bs.cand + b2 * W;
+                const int n2 = bs.cnt[b2];
+                for (int q = 0; q < n2 && c2[q] > k; q++) rank++;
+            }
+            if (rank < W) bs.sel[rank] = k;
+        }
+        __syncthreads();
+        const int nn = min(W, total), nxt = cur ^ 1;
+        for (int b = warp; b < nn; b += JSS_WARPS_PER_CTA) {   // 3. step the kept children
+            const uint64_t k = bs.sel[b];
+            const uint32_t pj = ~(uint32_t)k;
+            const int parent = (int)(pj >> 8), j = (int)(pj & 255u);
+            env_load<KJ>(iv, slot(cur, parent), lane, s);
+            s.flags = jss_uniform(s.flags);
+            int raw;
+            const bool ok = env_step<KJ, false>(p, iv, s, env, lane, j, raw, hz);
+            env_store<KJ>(iv, slot(nxt, b), lane, s);
+            if (lane == 0) {
+                bs.score[nxt * W + b] = ok ? jss_key_f32((uint32_t)(k >> 32)) : JSS_F32_NAN;
+                if (trace) trace[(size_t)r * W + b] = (uint16_t)pj;
+            }
+        }
+        __syncthreads();
+        n = nn;
+        cur = nxt;
+    }
+    if (warp != 0) return;
+    // outputs: lane b reports slot b
+    const int b = lane;
+    int t = -1;
+    float sc = -JSS_F32_INF;
+    if (!done0 && b < n) {
+        const int32_t *hdr = slot(cur, b) + nw - 4;
+        const float x = bs.score[cur * W + b];
+        if ((hdr[JSS_HDR_FLAGS] & JSS_FLAG_DONE) && x == x) { t = hdr[JSS_HDR_T]; sc = x; }
+    }
+    const bool any = __any_sync(JSS_FULL, t >= 0);
+    if (done0) sc = 0.0f;
+    else if (!any && bs.bad[0]) sc = JSS_F32_NAN;
+    if (b < W) {
+        a.actions_out[(int64_t)env * a.samples_ld + b] = t;
+        a.log_prob_out[(int64_t)env * a.samples_ld + b] = sc;
+    }
+    if (!a.order_out) return;
+    // the best slot: smallest makespan, ties to the lowest slot (t < 2^24)
+    const int best = any ? (int)(__reduce_min_sync(JSS_FULL, t >= 0 ? ((uint32_t)t << 5) | (uint32_t)b : ~0u) & 31u) : -1;
+    int32_t *ord = a.order_out + (size_t)env * p.jobs_max * p.machines_max;
+    int seen[KJ];                                        // allocations of each owned job met so far, walking back
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        seen[i] = 0;
+        if (KJ * lane + i < J)
+            for (int k = 0; k < M; k++) ord[(size_t)(KJ * lane + i) * p.machines_max + k] = -1;
+    }
+    if (best < 0) return;
+    int at = best;
+    for (int r = R - 1; r >= 0; r--) {
+        const uint32_t pj = jss_uniform((uint32_t)trace[(size_t)r * W + at]);   // every lane reads the same entry
+        const int j = (int)(pj & 255u);
+        at = (int)(pj >> 8);
+#pragma unroll
+        for (int i = 0; i < KJ; i++)
+            if (KJ * lane + i == j) { ord[(size_t)j * p.machines_max + (M - 1 - seen[i])] = r; seen[i]++; }
+    }
+}
+
 template <int KJ, int MODE>
 JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
                              int lane, float *scratch) {
@@ -1746,6 +1967,9 @@ constexpr int JSS_LOOKAHEAD_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {8, 5, 4, 3};
 constexpr int JSS_SAMPLE_EPISODES_MIN_CTAS[JSS_LANE_CLASSES] = {8, 8, 6, 3};
 constexpr int JSS_SAMPLE_EPISODES_GRAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 4, 4, 2};
 constexpr int JSS_SAMPLE_EPISODES_SOLUTION_MIN_CTAS[JSS_LANE_CLASSES] = {6, 5, 6, 3};
+// The beam search likewise: 60 / 75 / 113 / 175 registers (CUDA 12.9, sm_90a); one CTA more spills in the classes with
+// 2, 4 and 8 jobs per lane.  Its shared memory (2 W state blocks) bounds the resident CTAs at large W anyway.
+constexpr int JSS_BEAM_SEARCH_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
     return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
@@ -1754,6 +1978,7 @@ JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
          : mode == JSS_MODE_SAMPLE_EPISODES ? JSS_SAMPLE_EPISODES_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_SAMPLE_EPISODES_GRAD ? JSS_SAMPLE_EPISODES_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION ? JSS_SAMPLE_EPISODES_SOLUTION_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_BEAM_SEARCH ? JSS_BEAM_SEARCH_MIN_CTAS[jss_lane_class(32 * KJ)]
          : 1;
 }
 
@@ -1767,6 +1992,29 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     jss_cta_carve(sl, sm, c, iv);
     const int warp = jss_warp_index(), lane = threadIdx.x & 31;
     float *scratch = reinterpret_cast<float *>(sm + sl.off_warp0 + warp * sl.warp_stride);
+    if (MODE == JSS_MODE_BEAM_SEARCH) {
+        // work item = one env (tile, warp slot), CTA-strided; the per-warp regions hold only env_check_no_op's table,
+        // and the beam region follows them
+        char *bsm = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;
+        const int n_items = (a.tile_end - a.tile_begin) * JSS_WARPS_PER_CTA;
+        int staged = -1;
+        for (int item = (int)blockIdx.x; item < n_items; item += (int)gridDim.x) {
+            const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, a.tile_begin + item / JSS_WARPS_PER_CTA,
+                                           item % JSS_WARPS_PER_CTA);
+            const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
+            if (env < 0) continue;                       // CTA-uniform
+            if (inst != staged) {
+                __syncthreads();
+                jss_stage_instance(p, p.inst[inst], c, JSS_STAGE_OPS);
+                staged = inst;
+                __syncthreads();
+            }
+            jss_iv_shape(iv);
+            env_beam_search<KJ>(p, a, iv, env, p.state + (size_t)t.off16 * 4, warp, lane,
+                                reinterpret_cast<int *>(scratch), bsm);
+        }
+        return;
+    }
     if (MODE == JSS_MODE_LOOKAHEAD || MODE == JSS_MODE_LOOKAHEAD_PRIORITY || jss_mode_samples(MODE)) {
         // work items (tile, sp), sp = 0 .. S-1, CTA-strided; a tile's S items are adjacent and share its instance.  The
         // rules read every table; the priority table replaces the suffix sums, so that lookahead stages ops / len only

@@ -174,6 +174,7 @@ struct JssLaunch {           // per-launch arguments
         int32_t rule;
         int32_t greedy;      // steps from a row (a.logits): 0 categorical draw, 1 epsilon-greedy decode
         int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env
+        int32_t beam_width;  // jss_beam_search: W, the beams kept per env
     };
     int32_t coin_mode, n_steps, write_obs;   // jss_lookahead (_priority): n_steps is S, the work items each tile's
                                              // candidates are spread over (launch_all); jss_sample_episodes: the
@@ -200,24 +201,30 @@ struct JssLaunch {           // per-launch arguments
     union {
         const int32_t *actions;  // step; jss_sample_episodes_solution: the sample each env replays (< 0: none)
         const float *weights;    // jss_sample_episodes_grad: sample s of env i weighs weights[i * samples_ld + s]
+        uint16_t *beam_trace;    // jss_beam_search with an order: per CTA, W backpointers per round (NULL: no order)
     };
     union {
         int32_t *actions_out;    // policy; jss_lookahead: env i's value of action a at actions_out + i * logits_ld + a
                                  // (jss_lookahead_priority: + i * values_ld + a); jss_sample_episodes: sample s's
                                  // makespan at actions_out + i * samples_ld + s
         int32_t *solution_out;   // jss_sample_episodes_solution: [N][jobs_max][machines_max] start times
+                                 // (jss_beam_search: slot b's makespan at actions_out + i * samples_ld + b)
     };
     union {
         const uint8_t *env_mask; // reset / import
-        int64_t samples_ld;      // jss_sample_episodes (_grad): row stride of the per-sample outputs / weights
+        int64_t samples_ld;      // jss_sample_episodes (_grad): row stride of the per-sample outputs / weights;
+                                 // jss_beam_search: of the per-slot outputs
     };
     // rollout with trajectory recording: outputs of step k of env e go to slot k * n_envs + e of these buffers;
     // jss_step_logits_record / jss_step_greedy_record: env e's observation, mask and scalar record go to row e of
     // traj_obs / mask / scalars.  jss_rollout_priority_sample: grad_out is the [N][jobs_max][machines_max] gradient of
     // each env's log-probability with respect to its table entries (may be NULL)
+    // jss_beam_search: order_out is the [N][jobs_max][machines_max] order of each env's best slot (may be NULL), and
+    // slot b's score goes to log_prob_out + i * samples_ld + b
     union {
         float *traj_obs;
         float *grad_out;
+        int32_t *order_out;
     };
     uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
     uint8_t *wire;           // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
@@ -253,5 +260,7 @@ struct JssLaunch {           // per-launch arguments
                                                // chunks (jss_sample_episodes_grad)
 #define JSS_MODE_SAMPLE_EPISODES_SOLUTION 14   // the replay of one sample per env, writing the start times
                                                // (jss_sample_episodes_solution)
+#define JSS_MODE_BEAM_SEARCH 15          // beam search over a logit table, one env per CTA, the envs untouched
+                                         // (jss_beam_search)
 
 #define JSS_WARPS_PER_CTA 8

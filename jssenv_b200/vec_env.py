@@ -561,6 +561,45 @@ class JssVecEnv:
             out["solution"] = sol
         return out
 
+    def beam_search(self, logits, width: int, order: bool = False):
+        """Decode the logit table `logits` by beam search from each env's current state, in one launch per lane class
+        (jss_beam_search), leaving the envs untouched.  Each round allocates one job per beam: every legal job of every
+        beam is a candidate scored by the beam's score plus the job's log-probability under the softmax over the legal
+        jobs' current-operation entries (exactly rollout_priority_sample()'s), and the `width` best candidates -- score
+        descending, then parent slot, then job index -- are kept.  A beam takes the no-op only when no job is legal and
+        it is.  After the last operation every kept beam is complete, and its score is, bit for bit, the log_prob
+        rollout_priority_sample() reports for the same episode.  `logits` is taken as by rollout_priority_sample(); a
+        table that requires grad is read detached (the search has no gradient).  Deterministic: the RNG counter does
+        not advance.  Returns a dict of device tensors: ``"makespan"`` (N, width) int32 and ``"score"`` (N, width)
+        float32 of the final slots, best score first (-1 and -inf for a slot without a complete beam, -1 and NaN in
+        every slot of an env whose every beam met a bad entry, -1 and 0 for an env done now); ``"best"`` (N,) int64,
+        the lowest slot of smallest makespan, -1 if none; with `order`, ``"order"`` (N, J, M) int32, the round at which
+        the best slot allocates each operation (-1 for operations started before the call, and everywhere for an env
+        without a complete beam).  The best schedule is replayed greedily from the same state by::
+
+            env.rollout_priority(-out["order"])    # ends done at out["makespan"][i, out["best"][i]]
+        """
+        import torch
+        x = self._table_arg(logits, "beam_search", "logits")
+        if not 1 <= int(width) <= N.MAX_BEAM_WIDTH:
+            raise ValueError(f"beam_search: width must be in 1..{N.MAX_BEAM_WIDTH}, got {width!r}")
+        width = int(width)
+        v = self._table_view(x)
+        makespan = torch.empty((self.num_envs, width), dtype=torch.int32, device=self.device)
+        score = torch.empty((self.num_envs, width), dtype=torch.float32, device=self.device)
+        ord_ = (torch.full((self.num_envs, self.jobs, self.machines), -1, dtype=torch.int32, device=self.device)
+                if order else None)
+        rc = self._L.jss_beam_search(self._h, v.data_ptr(), *(int(s) for s in v.stride()), width,
+                                     makespan.data_ptr(), score.data_ptr(), width, _ptr(ord_), self._stream())
+        N.check(self._h, rc, "jss_beam_search")
+        ended = makespan >= 0
+        best = torch.where(ended, makespan, torch.iinfo(torch.int32).max).argmin(1)
+        best = torch.where(ended.any(1), best, -1)
+        out = {"makespan": makespan, "score": score, "best": best}
+        if order:
+            out["order"] = ord_
+        return out
+
     def _sample_episodes(self, x, k: int, step_index: int):
         """The native call of sample_episodes on a checked table `x` at RNG counter `step_index`: (makespan, log_prob),
         each (N, k)."""
