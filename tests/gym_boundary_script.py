@@ -21,6 +21,7 @@ def main(backend):
     from jssenv_b200 import JssEnv, JssGymVectorEnv, create_env
     from jssenv_b200.instances import load_instance
     from oracle.jss_oracle import OracleEnv
+    from tests.parity_common import assert_facade_obs_exact, assert_obs_exact, assert_reward_exact
     assert "jss-v1" in gym.envs.registration.registry, "import must register the reference's id"
     assert jssenv_b200.register_gymnasium() is True
 
@@ -43,7 +44,8 @@ def main(backend):
         oo, r2, d2, _, _ = o.step(a)
         assert reward == r2 and isinstance(reward, float), (reward, r2)      # float64 quotient, bit-equal
         assert done == d2 and truncated is False and info == {}
-        assert np.array_equal(obs["action_mask"], oo["action_mask"]) and np.abs(obs["real_obs"] - oo["real_obs"]).max() <= 1e-6
+        assert np.array_equal(obs["action_mask"], oo["action_mask"])
+        assert_facade_obs_exact(obs["real_obs"], oo["real_obs"], steps)
         total += reward; steps += 1
     assert env.current_time_step == o.current_time_step and env.last_time_step == o.current_time_step
     env.close()
@@ -79,10 +81,11 @@ def main(backend):
                 was_done[i] = False
             else:
                 _, r, d, _, _ = o.step(int(acts[i]))
-                assert abs(rew[i] - r) <= max(1e-6, 1.2e-7 * abs(r)) and bool(term[i]) == d
+                assert_reward_exact(rew[i], r, (k, i))
+                assert bool(term[i]) == d
                 was_done[i] = d
             assert np.array_equal(obs["action_mask"][i].astype(bool), o.legal_actions)
-            assert np.abs(obs["real_obs"][i] - o.state).max() <= 1e-6
+            assert_obs_exact(obs["real_obs"][i], o.state, (k, i))
         assert not trunc.any()
     assert int(venv.vec.episode_count.min()) >= 2
     venv.close()

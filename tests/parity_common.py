@@ -2,9 +2,12 @@
 in the CPU suite; tests/backends.py) against the CPU oracle and the golden fixtures recorded from the unmodified Python
 reference.
 
-Bars (BASELINE.md section 4): bit-exact action_mask / done / current_time_step / raw
-integer reward / integer state; |real_obs - ref| <= 1e-6 and scaled reward within
-max(1e-6, 1.2e-7 * |r|) (fp32 device vs fp64 reference).
+Bars: bit-exact action_mask / done / current_time_step / raw integer reward / integer state; real_obs and the scaled
+reward bit for bit the reference's float64 quotients rounded once to fp32 (assert_obs_exact, assert_reward_exact).  Each
+reference entry is one float64 division of two integers below 2^24, so it is correctly rounded, and rounding it to fp32
+gives the correctly rounded fp32 quotient (53 >= 2 * 24 + 2: no double-rounding error) -- the value the kernels' jss_div
+claims to emit.  The facade's float64 observation is the device's fp32 one widened, its float64 reward the reference's
+own quotient.
 """
 import numpy as np
 
@@ -16,7 +19,6 @@ from oracle.jss_oracle import OracleEnv, OracleError
 from oracle.logits_oracle import hash3
 from tests.helpers import load_json, load_trace, replay_optimal
 
-OBS_TOL = 1e-6
 OUTPUTS = ("action_mask", "real_obs", "reward", "reward_raw", "done", "current_time_step", "flags", "episode_count",
            "last_makespan", "last_return")
 
@@ -77,8 +79,33 @@ def oracle_episode(inst, choose):
     return o.current_time_step, total, step
 
 
-def rew_close(a, b):
-    return abs(float(a) - float(b)) <= max(1e-6, 1.2e-7 * abs(float(b)))
+def _assert_f32_exact(got, ref, what, ctx):
+    got = np.asarray(got)
+    assert got.dtype == np.float32, (ctx, what, got.dtype)
+    want = np.asarray(ref, np.float64).astype(np.float32)
+    bad = got.view(np.uint32) != want.view(np.uint32)
+    if bad.any():
+        k = tuple(int(i) for i in np.argwhere(bad)[0]) if bad.ndim else ()
+        raise AssertionError(f"{ctx}: {what} differs from the correctly rounded reference at {int(bad.sum())} entries; "
+                             f"first at {k}: got {got[k]!r}, want {want[k]!r} (float64 {np.asarray(ref)[k]!r})")
+
+
+def assert_obs_exact(got_f32, ref_f64, ctx=""):
+    """The device's fp32 observation entries equal the reference's float64 ones rounded once to fp32, bit for bit."""
+    _assert_f32_exact(got_f32, ref_f64, "real_obs", ctx)
+
+
+def assert_reward_exact(got_f32, ref_f64, ctx=""):
+    """The device's fp32 scaled reward(s) equal the reference's float64 ones rounded once to fp32, bit for bit."""
+    _assert_f32_exact(got_f32, ref_f64, "reward", ctx)
+
+
+def assert_facade_obs_exact(got_f64, ref_f64, ctx=""):
+    """The facade's float64 observation is the device's fp32 one widened: float64(float32(reference)), bit for bit."""
+    got = np.asarray(got_f64)
+    assert got.dtype == np.float64, (ctx, got.dtype)
+    want = np.asarray(ref_f64, np.float64).astype(np.float32).astype(np.float64)
+    assert np.array_equal(got.view(np.uint64), want.view(np.uint64)), f"{ctx}: facade real_obs"
 
 
 def compare_env_to_oracle(env, i, o, obs, reward=None, done=None, raw=None, ctx=""):
@@ -87,11 +114,11 @@ def compare_env_to_oracle(env, i, o, obs, reward=None, done=None, raw=None, ctx=
     assert np.array_equal(mask[: J + 1], o.legal_actions), f"{ctx}: mask env {i}"
     assert not mask[J + 1:].any(), f"{ctx}: padding mask bytes must stay 0"
     ro = np_(obs["real_obs"][i])
-    assert np.abs(ro[:J] - o.state).max() <= OBS_TOL, f"{ctx}: real_obs env {i}"
+    assert_obs_exact(ro[:J], o.state, f"{ctx}: env {i}")
     assert ro.min() >= 0.0 and ro.max() <= 1.0
     assert int(env.current_time_step[i]) == o.current_time_step, f"{ctx}: time env {i}"
     if reward is not None:
-        assert rew_close(reward[0], reward[1]), f"{ctx}: reward {reward}"
+        assert_reward_exact(np.float32(reward[0]), reward[1], f"{ctx}: env {i}")
     if raw is not None:
         assert int(raw[0]) == int(raw[1]), f"{ctx}: raw reward {raw}"
     if done is not None:
@@ -176,13 +203,13 @@ def check_golden_trace(make_env, path):
 
     def check(k):
         assert np.array_equal(np_(obs["action_mask"][0])[: J + 1], tr["mask"][k]), f"mask {k}"
-        assert np.abs(np_(obs["real_obs"][0])[:J] - tr["obs"][k]).max() <= OBS_TOL, f"obs {k}"
+        assert_obs_exact(np_(obs["real_obs"][0])[:J], tr["obs"][k], f"obs {k}")
         assert int(env.current_time_step[0]) == tr["t"][k]
 
     check(0)
     for k, a in enumerate(tr["actions"]):
         obs, reward, done, _, _ = env.step(np.array([a], np.int32))
-        assert rew_close(reward[0], tr["reward"][k]), f"reward {k}"
+        assert_reward_exact(np_(reward)[0], tr["reward"][k], f"reward {k}")
         assert bool(done[0]) == bool(tr["done"][k])
         check(k + 1)
         if k % 50 == 0:
@@ -226,14 +253,14 @@ def check_facade_attributes(inst, n_steps, seed):
         assert env.next_time_step == o.next_time_step
         assert env.current_time_step == o.current_time_step
         assert obs["real_obs"].dtype == np.float64 and obs["real_obs"].shape == (o.jobs, 7)
-        assert np.abs(env.state - o.state).max() <= OBS_TOL
+        assert_facade_obs_exact(env.state, o.state)
         if done:
             break
         legal = np.flatnonzero(o.legal_actions)
         a = int(legal[rng.integers(len(legal))])
         obs, r, done, trunc, info = env.step(a)
         _, r2, d2, _, _ = o.step(a)
-        assert rew_close(r, r2) and done == d2 and trunc is False and info == {}
+        assert r == r2 and done == d2 and trunc is False and info == {}     # float64 quotient, bit-equal
     env.close()
 
 
@@ -340,7 +367,7 @@ def check_rollout_matches_steps(make_env, names, rule, n_steps, seed):
         J = o.jobs
         if not done:
             assert np.array_equal(np_(a_env.action_mask[i])[: J + 1], o.legal_actions)
-            assert np.abs(np_(a_env.real_obs[i])[:J] - o.state).max() <= OBS_TOL
+            assert_obs_exact(np_(a_env.real_obs[i])[:J], o.state, (n, i))
     return a_env
 
 
@@ -598,7 +625,7 @@ def check_facade_errors():
         env.step(env.jobs + 5)
     obs, r, done, _, _ = env.step(4)           # still usable, still in lock-step with the oracle
     oo, r2, d2, _, _ = o.step(4)
-    assert np.array_equal(obs["action_mask"], oo["action_mask"]) and rew_close(r, r2) and done == d2
+    assert np.array_equal(obs["action_mask"], oo["action_mask"]) and r == r2 and done == d2
     assert env.render() is not None and len(env.render()) == 2
     env.close()
 
@@ -734,8 +761,9 @@ def check_big_uniform_batches(make_env, seed=60, max_steps=150):
         a = int(legal[rng.integers(len(legal))])
         obs, r, done, _, _ = env.step(a)
         oo, r2, d2, _, _ = o.step(a)
-        assert np.array_equal(obs["action_mask"], oo["action_mask"]) and np.abs(obs["real_obs"] - oo["real_obs"]).max() <= OBS_TOL
-        assert rew_close(r, r2) and done == d2
+        assert np.array_equal(obs["action_mask"], oo["action_mask"])
+        assert_facade_obs_exact(obs["real_obs"], oo["real_obs"])
+        assert r == r2 and done == d2
         assert np.array_equal(env.todo_time_step_job, o.todo_time_step_job) and np.array_equal(env.machine_legal, o.machine_legal)
         if done:
             break
