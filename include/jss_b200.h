@@ -537,6 +537,64 @@ int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_e
 int jss_beam_search(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op, int width,
                     int32_t *makespan_out_dev, float *score_out_dev, int64_t ld, int32_t *order_out_dev, void *stream);
 
+/* Stochastic beam search (Kool, van Hoof, Welling, ICML 2019) over a caller's logit table, in one launch per lane class
+ * present, leaving the envs untouched: W *distinct* episodes per env drawn without replacement from the distribution
+ * jss_rollout_priority_sample() samples from, each with its perturbed log-probability (its key).
+ *   Shared with jss_beam_search(): the table, the rounds, forced no-ops, the candidates (legal jobs with logp_j > -inf),
+ *     the dropping of beams on bad rows, done-at-entry envs and 1 <= W <= JSS_MAX_BEAM_WIDTH.  A slot's log_prob is its
+ *     beam score, accumulated as jss_beam_search() accumulates it, so it equals, bit for bit, the log_prob
+ *     jss_rollout_priority_sample() reports for the same episode.
+ *   Perturbation (top-down Gumbel): the root beam has key T = 0.  In round r a beam in slot b with score phi_b and key
+ *     T_b gives each candidate j the value G_j = (phi_b + lp_j) + g_j, g_j = -log(-log u), u = ((H(h, b * 256 + j) >> 8)
+ *     + 0.5) * 2^-24, H = jss_hash_env and h = jss_hash3(seed, env_id_base + i, step_index + r) (jss_rng.h): the
+ *     uniforms can be restated on the host.  With Z = max_j G_j, the candidate
+ *     attaining Z (lowest job on ties) gets key exactly T_b, every other one min(T_b, T_b - max(v, 0) - log1p(e^-|v|)),
+ *     v = T_b - G_j + log(1 - e^(G_j - Z)).
+ *   Selection: that of jss_beam_search() with the key in place of the score (key descending, then parent slot, then
+ *     job); the W best become slots 0 .. W-1.
+ *   Outputs (device, row stride ld >= width): makespan_out_dev[i*ld + b] (int32), log_prob_out_dev and key_out_dev
+ *     (fp32) of final slot b; -1 / -inf / -inf for a slot without a complete beam; -1 / NaN / NaN in every slot of an env
+ *     whose beams all met a bad row; -1 / 0 / 0 in every slot of an env done at entry.  Columns width .. ld-1 are not
+ *     written.
+ *   order_out_dev (NULL, or device int32 [N][width][jobs_max][machines_max]): every slot's allocation round of each
+ *     operation, in jss_beam_search()'s order format; -1 for operations started before the call and in every entry of a
+ *     slot without a complete beam.  Entries past J_i / M_i are not written.  It uses jss_beam_search()'s handle-owned
+ *     trace under the same rule: calls with an order on one handle must not overlap on different streams.
+ *   No side effects, as jss_beam_search(); the call reads the RNG counters step_index .. step_index + R_i - 1.
+ *   Returns JSS_ERR_INVALID for a NULL (order_out_dev aside) or not 4-byte-aligned pointer, a negative stride, width < 1
+ *     or > JSS_MAX_BEAM_WIDTH, or ld < width; JSS_ERR_CUDA if the trace cannot be allocated; JSS_ERR_STATE before
+ *     jss_assign(). */
+int jss_sample_without_replacement(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                   uint64_t seed, uint64_t step_index, int width, int32_t *makespan_out_dev,
+                                   float *log_prob_out_dev, float *key_out_dev, int64_t ld, int32_t *order_out_dev,
+                                   void *stream);
+
+/* The teacher-forced log-likelihood of k given operation orders per env under a caller's logit table, each from the
+ * env's current state, in one launch per lane class present, leaving the envs untouched.
+ *   order_dev: device int32 [N][k][jobs_max][machines_max].  Order s of env i stands for the episode that
+ *     jss_rollout_priority() on the table -order[i][s] runs from env i's current state: the legal job with the smallest
+ *     entry at its current operation, ties to the lowest index, the no-op only when no job is legal.  The orders of
+ *     jss_beam_search() and jss_sample_without_replacement() are such tables.
+ *   Table: that of jss_rollout_priority_sample().  log_prob_out_dev[i*ld + s] (fp32) is the sum of the episode's
+ *     decisions' log-probabilities under it, each computed as jss_rollout_priority_sample() computes the log-probability
+ *     of the job it draws; forced no-ops add 0.  NaN where a decision meets a bad row (the episode stops there).
+ *     makespan_out_dev[i*ld + s] (int32) is the end time if the episode ends done, else -1.  An env done at entry reads
+ *     -1 / 0.  No RNG, no side effects (those of jss_lookahead()).
+ *   Returns JSS_ERR_INVALID for a NULL or not 4-byte-aligned pointer, a negative stride, k < 1 or ld < k; JSS_ERR_STATE
+ *     before jss_assign(). */
+int jss_order_log_prob(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                       const int32_t *order_dev, int64_t k, int32_t *makespan_out_dev, float *log_prob_out_dev,
+                       int64_t ld, void *stream);
+
+/* The gradient of jss_order_log_prob(): adds sum_s weights_dev[i*ld + s] * d log_prob[i][s] / d table into grad_out_dev,
+ * device fp32 [split][N][jobs_max][machines_max], with jss_sample_episodes_grad()'s accumulator and chunking: chunk c
+ * takes the orders s = c (mod split), deterministic for a given split, no atomics.  Orders of weight 0, orders whose
+ * episode meets a bad row and envs done at entry add nothing.  Returns JSS_ERR_INVALID as jss_order_log_prob() does and
+ * for a split outside 1..k. */
+int jss_order_log_prob_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                            const int32_t *order_dev, int64_t k, const float *weights_dev, int64_t ld, int split,
+                            float *grad_out_dev, void *stream);
+
 /* Host-buffer form of step(): copies actions H2D, steps, copies the results D2H with
  * contiguous DMA, synchronises.  Any output pointer may be NULL.  Host layouts equal the
  * device layouts: mask_host [N][mask_stride] bytes (row i: bytes 0..J_i), obs_host

@@ -78,6 +78,11 @@ SIGNATURES = {
                                          c_int, _VP, _VP]),
     "jss_sample_episodes_solution": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, _VP, _VP, _VP]),
     "jss_beam_search": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_int, _VP, _VP, c_int64, _VP, _VP]),
+    "jss_sample_without_replacement": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int, _VP, _VP,
+                                               _VP, c_int64, _VP, _VP]),
+    "jss_order_log_prob": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, _VP, c_int64, _VP]),
+    "jss_order_log_prob_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, c_int64, c_int, _VP,
+                                        _VP]),
     "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_step_begin": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_wait": (c_int, [_VP, c_int]),

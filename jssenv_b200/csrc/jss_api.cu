@@ -225,15 +225,17 @@ JssSmemLayout beam_layout(const jss_t *h) {
     sl.warp_stride = 32 * 4;
     return sl;
 }
-size_t beam_smem(const jss_t *h, int W) {
+size_t beam_smem(const jss_t *h, int W, bool swor) {
     return smem_bytes(beam_layout(h)) +
-           jss_beam_smem(nullptr, W, jss_block_geom(h->p.jobs_max, h->p.machines_max).words, nullptr);
+           jss_beam_smem(nullptr, W, jss_block_geom(h->p.jobs_max, h->p.machines_max).words, nullptr, swor);
 }
-// the persistent grid of lane class c's beam search launch: one work item per env, at most the resident CTAs
-int beam_grid(jss_t *h, int c, int W, int &grid) {
+// the persistent grid of lane class c's beam search launch (swor: the stochastic one): one work item per env, at most
+// the resident CTAs
+int beam_grid(jss_t *h, int c, int W, bool swor, int &grid) {
     const int n_items = (h->class_tiles[c][1] - h->class_tiles[c][0]) * JSS_WARPS_PER_CTA;
     int per_sm = 0;
-    if (int rc = ctas_per_sm(h, env_kernels<JSS_MODE_BEAM_SEARCH>[c], beam_smem(h, W), per_sm)) return rc;
+    const JssKernel k = swor ? env_kernels<JSS_MODE_SWOR>[c] : env_kernels<JSS_MODE_BEAM_SEARCH>[c];
+    if (int rc = ctas_per_sm(h, k, beam_smem(h, W, swor), per_sm)) return rc;
     grid = std::min(n_items, h->sm_count * per_sm);
     return JSS_OK;
 }
@@ -253,7 +255,8 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
     // meaning after a recording step (a plain step rewrites only the envs it changes)
     const bool recording = a.mode == JSS_MODE_STEP && a.traj_obs;
     const bool lookahead = a.mode == JSS_MODE_LOOKAHEAD || a.mode == JSS_MODE_LOOKAHEAD_PRIORITY;
-    const bool samples = jss_mode_samples(a.mode), beam = a.mode == JSS_MODE_BEAM_SEARCH;
+    const bool samples = jss_mode_samples(a.mode), swor = a.mode == JSS_MODE_SWOR;
+    const bool beam = a.mode == JSS_MODE_BEAM_SEARCH || swor;
     if (!recording && a.mode != JSS_MODE_EXPORT && a.mode != JSS_MODE_POLICY && a.mode != JSS_MODE_REFRESH &&
         !lookahead && !samples && !beam)                 // these read only state blocks and write the caller's buffers
         if (int rc = refresh_obs(h, st)) return rc;
@@ -269,6 +272,9 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
                            : a.mode == JSS_MODE_SAMPLE_EPISODES ? env_kernels<JSS_MODE_SAMPLE_EPISODES>
                            : a.mode == JSS_MODE_SAMPLE_EPISODES_GRAD ? env_kernels<JSS_MODE_SAMPLE_EPISODES_GRAD>
                            : a.mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION ? env_kernels<JSS_MODE_SAMPLE_EPISODES_SOLUTION>
+                           : a.mode == JSS_MODE_ORDER_LOG_PROB ? env_kernels<JSS_MODE_ORDER_LOG_PROB>
+                           : a.mode == JSS_MODE_ORDER_LOG_PROB_GRAD ? env_kernels<JSS_MODE_ORDER_LOG_PROB_GRAD>
+                           : swor ? env_kernels<JSS_MODE_SWOR>
                            : beam ? env_kernels<JSS_MODE_BEAM_SEARCH>
                            : env_kernels<JSS_MODE_RESET>;
     // what the launch reads: a rollout or lookahead every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
@@ -278,7 +284,7 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
             : a.mode != JSS_MODE_POLICY ? JSS_STAGE_OPS
             : a.rule == JSS_RULE_RANDOM ? 0 : jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
     const JssSmemLayout sl = beam ? beam_layout(h) : h->sl_env;
-    const size_t smem = beam ? beam_smem(h, a.beam_width) : smem_bytes(sl);
+    const size_t smem = beam ? beam_smem(h, a.beam_width, swor) : smem_bytes(sl);
     for (int c = 0; c < JSS_LANE_CLASSES; c++) {   // one launch per lane class present
         a.tile_begin = h->class_tiles[c][0];
         a.tile_end = h->class_tiles[c][1];
@@ -297,13 +303,14 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
             a.n_steps = n_tiles >= slots ? 1 : std::min(jc + 1, (slots + n_tiles - 1) / n_tiles);
             grid = std::min(n_tiles * a.n_steps, slots);
         } else if (samples) {
-            // the draws: each tile's K samples spread over S work items in the same way, up to S = K; the gradient
-            // keeps the caller's split (one work item per chunk), the solution replay one work item per tile
-            if (a.mode == JSS_MODE_SAMPLE_EPISODES)
+            // the draws (and the order likelihoods): each tile's K samples spread over S work items in the same way, up
+            // to S = K; the gradients keep the caller's split (one work item per chunk), the solution replay one work
+            // item per tile
+            if (a.mode == JSS_MODE_SAMPLE_EPISODES || a.mode == JSS_MODE_ORDER_LOG_PROB)
                 a.n_steps = n_tiles >= slots ? 1 : std::min(a.n_samples, (slots + n_tiles - 1) / n_tiles);
             grid = (int)std::min<int64_t>((int64_t)n_tiles * a.n_steps, slots);
         } else if (beam) {
-            if (int rc = beam_grid(h, c, a.beam_width, grid)) return rc;   // the grid the trace is sized for
+            if (int rc = beam_grid(h, c, a.beam_width, swor, grid)) return rc;   // the grid the trace is sized for
         }
         JSS_LAUNCH(kerns[c], grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
         JSS_CUDA(h, cudaGetLastError());
@@ -961,6 +968,32 @@ namespace {
 
 bool bad_ptr(const void *ptr) { return !ptr || ((uintptr_t)ptr & 3u); }
 
+// a.beam_trace for a (stochastic) beam search of width W that writes orders: W backpointers per round (at most
+// jobs_max * machines_max rounds) for each CTA of the largest grid, owned by the handle and grown as needed
+int beam_trace(jss_t *h, int width, bool swor, JssLaunch &a) {
+    int grid_max = 0;
+    for (int c = 0; c < JSS_LANE_CLASSES; c++) {
+        if (h->class_tiles[c][1] <= h->class_tiles[c][0]) continue;
+        int grid = 0;
+        if (int rc = beam_grid(h, c, width, swor, grid)) return rc;
+        grid_max = std::max(grid_max, grid);
+    }
+    const size_t need = (size_t)grid_max * width * h->p.jobs_max * h->p.machines_max * sizeof(uint16_t);
+    if (need > h->beam_trace_bytes) {
+        if (h->beam_trace) {                             // cudaFree waits for the launches that may still use it
+            JSS_CUDA(h, cudaFree(h->beam_trace));
+            h->beam_trace = nullptr;
+            h->beam_trace_bytes = 0;
+        }
+        void *ptr = nullptr;
+        JSS_CUDA(h, cudaMalloc(&ptr, need));
+        h->beam_trace = static_cast<uint16_t *>(ptr);
+        h->beam_trace_bytes = need;
+    }
+    a.beam_trace = h->beam_trace;
+    return JSS_OK;
+}
+
 // the arguments jss_sample_episodes and its replays share: the table as jss_rollout_priority_sample takes it, the seed
 // and counter; k and ld where the call has them (has_k)
 int sample_episodes_args(jss_t *h, const char *who, const float *logits, int64_t ld_env, int64_t ld_job, int64_t ld_op,
@@ -1067,29 +1100,98 @@ int jss_beam_search(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t l
     a.log_prob_out = score_out_dev;
     a.samples_ld = ld;
     a.order_out = order_out_dev;
-    if (order_out_dev) {
-        // the trace: W backpointers per round (at most jobs_max * machines_max rounds) for each CTA of the largest grid
-        int grid_max = 0;
-        for (int c = 0; c < JSS_LANE_CLASSES; c++) {
-            if (h->class_tiles[c][1] <= h->class_tiles[c][0]) continue;
-            int grid = 0;
-            if ((rc = beam_grid(h, c, width, grid))) return rc;
-            grid_max = std::max(grid_max, grid);
-        }
-        const size_t need = (size_t)grid_max * width * h->p.jobs_max * h->p.machines_max * sizeof(uint16_t);
-        if (need > h->beam_trace_bytes) {
-            if (h->beam_trace) {                         // cudaFree waits for the launches that may still use it
-                JSS_CUDA(h, cudaFree(h->beam_trace));
-                h->beam_trace = nullptr;
-                h->beam_trace_bytes = 0;
-            }
-            void *ptr = nullptr;
-            JSS_CUDA(h, cudaMalloc(&ptr, need));
-            h->beam_trace = static_cast<uint16_t *>(ptr);
-            h->beam_trace_bytes = need;
-        }
-        a.beam_trace = h->beam_trace;
-    }
+    if (order_out_dev && (rc = beam_trace(h, width, false, a))) return rc;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_sample_without_replacement(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                   uint64_t seed, uint64_t step_index, int width, int32_t *makespan_out_dev,
+                                   float *log_prob_out_dev, float *key_out_dev, int64_t ld, int32_t *order_out_dev,
+                                   void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    if (bad_ptr(logits_dev) || ld_env < 0 || ld_job < 0 || ld_op < 0 || bad_ptr(makespan_out_dev) ||
+        bad_ptr(log_prob_out_dev) || bad_ptr(key_out_dev) || ((uintptr_t)order_out_dev & 3u) || width < 1 ||
+        width > JSS_MAX_BEAM_WIDTH || ld < width)
+        return fail(h, JSS_ERR_INVALID, "jss_sample_without_replacement: bad arguments (logits %p, makespan_out %p, "
+                    "log_prob_out %p and key_out %p must be non-NULL, they and order_out %p 4-byte aligned, strides "
+                    "%lld / %lld / %lld >= 0, 1 <= width %d <= %d, ld %lld >= width)", (const void *)logits_dev,
+                    (void *)makespan_out_dev, (void *)log_prob_out_dev, (void *)key_out_dev, (void *)order_out_dev,
+                    (long long)ld_env, (long long)ld_job, (long long)ld_op, width, JSS_MAX_BEAM_WIDTH, (long long)ld);
+    JssLaunch a{};
+    a.mode = JSS_MODE_SWOR;
+    a.logits = logits_dev;
+    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
+    a.hash_key = jss_fold32(seed);                       // jss_hash3 reads the seed only through its fold
+    a.sample_step_index = step_index;
+    a.beam_width = width;
+    a.actions_out = makespan_out_dev;
+    a.log_prob_out = log_prob_out_dev;
+    a.key_out = key_out_dev;
+    a.samples_ld = ld;
+    a.order_out = order_out_dev;
+    if (order_out_dev && (rc = beam_trace(h, width, true, a))) return rc;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+namespace {
+
+// the arguments jss_order_log_prob and its gradient share: the table as jss_rollout_priority_sample takes it, k orders
+// per env, and ld
+int order_log_prob_args(jss_t *h, const char *who, const float *logits, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                        const int32_t *order, int64_t k, int64_t ld, JssLaunch &a) {
+    if (bad_ptr(logits) || ld_env < 0 || ld_job < 0 || ld_op < 0 || bad_ptr(order) || k < 1 || ld < k)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (logits %p and order %p must be non-NULL and 4-byte "
+                    "aligned, strides %lld / %lld / %lld >= 0, k %lld >= 1, ld %lld >= k)", who, (const void *)logits,
+                    (const void *)order, (long long)ld_env, (long long)ld_job, (long long)ld_op, (long long)k,
+                    (long long)ld);
+    if (k > INT32_MAX)
+        return fail(h, JSS_ERR_UNSUPPORTED, "%s: k must stay below 2^31", who);
+    a.logits = logits;
+    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
+    a.order_in = order;
+    a.n_samples = (int)k;
+    a.samples_ld = ld;
+    return JSS_OK;
+}
+
+}  // namespace
+
+int jss_order_log_prob(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                       const int32_t *order_dev, int64_t k, int32_t *makespan_out_dev, float *log_prob_out_dev,
+                       int64_t ld, void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    const char *who = "jss_order_log_prob";
+    if (bad_ptr(makespan_out_dev) || bad_ptr(log_prob_out_dev))
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p and log_prob_out %p must be non-NULL and "
+                    "4-byte aligned)", who, (void *)makespan_out_dev, (void *)log_prob_out_dev);
+    JssLaunch a{};
+    a.mode = JSS_MODE_ORDER_LOG_PROB;
+    if ((rc = order_log_prob_args(h, who, logits_dev, ld_env, ld_job, ld_op, order_dev, k, ld, a))) return rc;
+    a.actions_out = makespan_out_dev;
+    a.log_prob_out = log_prob_out_dev;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_order_log_prob_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                            const int32_t *order_dev, int64_t k, const float *weights_dev, int64_t ld, int split,
+                            float *grad_out_dev, void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    const char *who = "jss_order_log_prob_grad";
+    if (bad_ptr(weights_dev) || bad_ptr(grad_out_dev) || split < 1 || split > k)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (weights %p and grad_out %p must be non-NULL and 4-byte "
+                    "aligned, 1 <= split %d <= k %lld)", who, (const void *)weights_dev, (void *)grad_out_dev, split,
+                    (long long)k);
+    if ((int64_t)h->n_tiles * split > INT32_MAX)
+        return fail(h, JSS_ERR_UNSUPPORTED, "%s: split * tiles must stay below 2^31", who);
+    JssLaunch a{};
+    a.mode = JSS_MODE_ORDER_LOG_PROB_GRAD;
+    if ((rc = order_log_prob_args(h, who, logits_dev, ld_env, ld_job, ld_op, order_dev, k, ld, a))) return rc;
+    a.weights = weights_dev;
+    a.n_steps = split;
+    a.grad_out = grad_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 

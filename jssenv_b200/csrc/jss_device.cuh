@@ -1537,14 +1537,51 @@ JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstVie
 //   entry are skipped.
 // JSS_MODE_SAMPLE_EPISODES_SOLUTION: one work item per tile; env i replays sample a.actions[i] (none if < 0) and writes
 //   the start time of each operation it starts into a.solution_out.
+// JSS_MODE_ORDER_LOG_PROB / _GRAD: the loop of JSS_MODE_SAMPLE_EPISODES / _GRAD with the decisions of env_order_action
+//   on order s of the env (a.order_in) in place of the draws; no RNG.
 JSS_HD constexpr bool jss_mode_samples(int mode) {
     return mode == JSS_MODE_SAMPLE_EPISODES || mode == JSS_MODE_SAMPLE_EPISODES_GRAD ||
-           mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION;
+           mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION || mode == JSS_MODE_ORDER_LOG_PROB ||
+           mode == JSS_MODE_ORDER_LOG_PROB_GRAD;
+}
+template <int KJ>
+JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ]);
+// Env `env`'s next decision under an operation order `ord` (row stride machines_max; jss_order_log_prob): that of
+// env_priority_action on the table -ord, the legal job whose current operation has the smallest entry, ties to the
+// lowest job.  Writes logp, its log-probability under the logit table a.logits by env_table_logp (so that a beam's score
+// and the order's log-probability agree bit for bit), and each owned slot's p_i = exp(lp_i) (0 for a job that is not
+// legal).  Returns as env_priority_sample_action does: the no-op, logp and p left 0, when no job is legal and it is;
+// JSS_INF for a bad table row; JSS_ACTION_SKIP when nothing is legal.
+template <int KJ>
+JSS_DEV int env_order_action(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
+                             const int32_t *ord, int mstride, float &logp, float (&pr)[KJ]) {
+    constexpr uint32_t LM = jss_legal_mask<KJ>();
+    logp = 0.0f;
+#pragma unroll
+    for (int i = 0; i < KJ; i++) pr[i] = 0.0f;
+    if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u))
+        return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
+    int act = JSS_INF;
+    env_legal_argmax<KJ>(s, lane, jss_J(iv), false, [&](int i, int j) {
+        return -(float)ord[(size_t)j * mstride + jss_sel<KJ>(s.todo, i)];
+    }, act);
+    float lp[KJ];
+    if (!env_table_logp<KJ>(a, s, env, lane, lp)) return JSS_INF;
+    float la = 0.0f;
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        if ((s.lb >> i) & 1u) pr[i] = jss_fast_exp(lp[i]);
+        if (KJ * lane + i == act) la = lp[i];
+    }
+    logp = __shfl_sync(JSS_FULL, la, act / KJ);
+    return act;
 }
 template <int KJ, int MODE>
 JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile,
                                  int warp, int lane, int sp, float *scratch) {
-    constexpr bool GRAD = MODE == JSS_MODE_SAMPLE_EPISODES_GRAD, SOL = MODE == JSS_MODE_SAMPLE_EPISODES_SOLUTION;
+    constexpr bool ORD = MODE == JSS_MODE_ORDER_LOG_PROB || MODE == JSS_MODE_ORDER_LOG_PROB_GRAD;
+    constexpr bool GRAD = MODE == JSS_MODE_SAMPLE_EPISODES_GRAD || MODE == JSS_MODE_ORDER_LOG_PROB_GRAD;
+    constexpr bool SOL = MODE == JSS_MODE_SAMPLE_EPISODES_SOLUTION;
     const int32_t *blk = p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4;
     const uint64_t genv = p.env_id_base + (uint64_t)env;
     const int J = jss_J(iv), M = jss_M(iv), bound = 2 * p.jobs_max * p.machines_max + 1;
@@ -1589,6 +1626,7 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
             if (w == 0.0f) continue;
         }
         const uint64_t c0 = a.sample_step_index + (uint64_t)smp * (uint64_t)bound;
+        const int32_t *ord = ORD ? a.order_in + ((size_t)env * a.n_samples + smp) * p.jobs_max * p.machines_max : nullptr;
         // GRAD: pass 0 (only where `check`) finds out whether the sample errs, pass 1 adds
         for (int pass = (GRAD && !check) ? 1 : 0; pass < (GRAD ? 2 : 1); pass++) {
             const bool add = GRAD && pass == 1;
@@ -1599,9 +1637,14 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
 #pragma unroll
             for (int i = 0; i < KJ; i++) acc[i] = 0.0f;
             for (int d = 0; d < bound && !(s.flags & JSS_FLAG_DONE); d++) {
-                const uint32_t h = jss_hash_env(jss_hash_key_folded(a.hash_key, c0 + (uint64_t)d), genv);
                 float logp, pr[KJ];
-                const int act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
+                int act;
+                if (ORD) {
+                    act = jss_uniform(env_order_action<KJ>(a, iv, s, env, lane, ord, p.machines_max, logp, pr));
+                } else {
+                    const uint32_t h = jss_hash_env(jss_hash_key_folded(a.hash_key, c0 + (uint64_t)d), genv);
+                    act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
+                }
                 if (act == JSS_ACTION_SKIP) break;       // nothing legal: no decision changes the env
                 int r;
                 bool changed = false;
@@ -1682,17 +1725,20 @@ JSS_DEV uint64_t jss_beam_key(uint32_t score_key, int parent, int job) {
 }
 
 // The beam region of the CTA's shared memory for width W and state blocks of `bw` words (jss_block_geom of the batch
-// maxima): [blocks: 2][W][bw] int32 | [cand: W][W] u64 | [sel: W] u64 | [score: 2][W] f32 | [cnt: W] i32 | [bad] i32.
-// jss_beam_search sizes it with the same function.
+// maxima): [blocks: 2][W][bw] int32 | [cand: W][W] u64 | [sel: W] u64 | [score: 2][W] f32 | [cnt: W] i32 | [bad] i32,
+// and for the stochastic beam search (swor) then [cscore: W][W] f32 | [key: 2][W] f32, the candidates' scores and the
+// slots' keys.  jss_beam_search and jss_sample_without_replacement size it with the same function.
 struct JssBeamSmem {
     int32_t *blocks;
     uint64_t *cand, *sel;
     float *score;
     int32_t *cnt, *bad;
+    float *cscore, *key;
 };
-JSS_HD inline size_t jss_beam_smem(char *base, int W, int bw, JssBeamSmem *b) {
+JSS_HD inline size_t jss_beam_smem(char *base, int W, int bw, JssBeamSmem *b, bool swor = false) {
     const size_t o_cand = (size_t)2 * W * bw * 4, o_sel = o_cand + (size_t)8 * W * W, o_score = o_sel + (size_t)8 * W;
     const size_t o_cnt = o_score + (size_t)8 * W, o_bad = o_cnt + (size_t)4 * W, end = (o_bad + 4 + 15) & ~(size_t)15;
+    const size_t o_key = end + (size_t)4 * W * W, end_swor = (o_key + (size_t)8 * W + 15) & ~(size_t)15;
     if (b) {
         b->blocks = reinterpret_cast<int32_t *>(base);
         b->cand = reinterpret_cast<uint64_t *>(base + o_cand);
@@ -1700,8 +1746,40 @@ JSS_HD inline size_t jss_beam_smem(char *base, int W, int bw, JssBeamSmem *b) {
         b->score = reinterpret_cast<float *>(base + o_score);
         b->cnt = reinterpret_cast<int32_t *>(base + o_cnt);
         b->bad = reinterpret_cast<int32_t *>(base + o_bad);
+        b->cscore = reinterpret_cast<float *>(base + end);
+        b->key = reinterpret_cast<float *>(base + o_key);
     }
-    return end;
+    return swor ? end_swor : end;
+}
+
+// log(1 - e^x) for x <= 0 (-inf at 0), through expm1 near 0 and log1p below -log 2 (Maechler's split)
+JSS_DEV float jss_log1mexp(float x) {
+    return x > -0.693147181f ? logf(-expm1f(x)) : log1pf(-expf(x));
+}
+
+// Walks the trace of a search with R rounds back from slot `at` of the last round (-1: none) and writes the round at
+// which that beam allocates each operation into `ord` (row stride machines_max), -1 for every operation it does not
+// allocate; each job's allocations in reverse are its operations M-1, M-2, ... (a complete beam has allocated every
+// operation).  Every lane reads the same trace entries.
+template <int KJ>
+JSS_DEV void jss_beam_order(const JssParams &p, const uint16_t *trace, int W, int R, int J, int M, int lane, int at,
+                            int32_t *ord) {
+    int seen[KJ];                                        // allocations of each owned job met so far, walking back
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        seen[i] = 0;
+        if (KJ * lane + i < J)
+            for (int k = 0; k < M; k++) ord[(size_t)(KJ * lane + i) * p.machines_max + k] = -1;
+    }
+    if (at < 0) return;
+    for (int r = R - 1; r >= 0; r--) {
+        const uint32_t pj = jss_uniform((uint32_t)trace[(size_t)r * W + at]);   // every lane reads the same entry
+        const int j = (int)(pj & 255u);
+        at = (int)(pj >> 8);
+#pragma unroll
+        for (int i = 0; i < KJ; i++)
+            if (KJ * lane + i == j) { ord[(size_t)j * p.machines_max + (M - 1 - seen[i])] = r; seen[i]++; }
+    }
 }
 
 // One env searched by the whole CTA (`root`: its state block, never written).  The beams are state blocks in shared
@@ -1712,22 +1790,31 @@ JSS_HD inline size_t jss_beam_smem(char *base, int W, int bw, JssBeamSmem *b) {
 //   2. the CTA ranks every candidate against the others' sorted lists; rank < W becomes slot rank;
 //   3. warp w loads the parent block of each of its new slots, steps the job with env_step<KJ, false> and stores the
 //      result in the other buffer; lane 0 records the backpointer parent << 8 | job in the trace (a.beam_trace).
-// At the end warp 0 writes the slot outputs and, with a.order_out, walks the trace back from the best slot: each job's
-// allocations in reverse are its operations M-1, M-2, ... (a complete beam has allocated every operation).
-template <int KJ>
+// At the end warp 0 writes the slot outputs and, with a.order_out, walks the trace back from the best slot
+// (jss_beam_order).
+// SWOR (jss_sample_without_replacement): the stochastic beam search.  Each slot also carries a key T (the root's is 0).
+// In step 1 each candidate j of beam b gets G_j = (score_b + lp_j) + g_j, g_j the Gumbel noise of
+// jss_hash_env(jss_hash3(seed, global env, step_index + r), b * 256 + j), and Z = max G; the candidate attaining Z
+// (lowest job on ties) gets key T_b, every other one min(T_b, T_b - max(v, 0) - log1p(e^-|v|)), v = T_b - G_j +
+// log(1 - e^(G_j - Z)).  The selection ranks the keys in place of the scores; step 2 carries the kept candidates'
+// scores over, step 3 their keys.  At the end every warp walks the trace back from its slots b = warp, warp + 8, ...
+template <int KJ, bool SWOR>
 JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, const int32_t *root,
                              int warp, int lane, int *hz, char *bsm) {
     constexpr uint32_t LM = jss_legal_mask<KJ>();
     const int W = a.beam_width, bw = jss_block_geom(p.jobs_max, p.machines_max).words;
     const int J = jss_J(iv), M = jss_M(iv), nw = iv.si->block_words;
     JssBeamSmem bs;
-    jss_beam_smem(bsm, W, bw, &bs);
+    jss_beam_smem(bsm, W, bw, &bs, SWOR);
     const auto slot = [&](int buf, int b) { return bs.blocks + (size_t)(buf * W + b) * bw; };
     uint16_t *trace = a.beam_trace ? a.beam_trace + (size_t)blockIdx.x * W * p.jobs_max * p.machines_max : nullptr;
     __syncthreads();                                     // the previous env's last reads of the region are done
     for (int k = (int)threadIdx.x; k < nw / 4; k += (int)blockDim.x)
         reinterpret_cast<int4 *>(bs.blocks)[k] = reinterpret_cast<const int4 *>(root)[k];
-    if (threadIdx.x == 0) { bs.score[0] = 0.0f; bs.bad[0] = 0; }
+    if (threadIdx.x == 0) {
+        bs.score[0] = 0.0f; bs.bad[0] = 0;
+        if (SWOR) bs.key[0] = 0.0f;
+    }
     __syncthreads();
     EnvRegs<KJ> s;
     env_load<KJ>(iv, bs.blocks, lane, s);
@@ -1739,6 +1826,8 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
     const int R = done0 ? 0 : (int)__reduce_add_sync(JSS_FULL, (unsigned)left);
     int n = 1, cur = 0;                                  // live slots, and the buffer that holds them
     for (int r = 0; r < R && n > 0; r++) {
+        const uint32_t hr = SWOR ? jss_hash_env(jss_hash_key_folded(a.hash_key, a.sample_step_index + (uint64_t)r),
+                                                p.env_id_base + (uint64_t)env) : 0u;
         for (int b = warp; b < n; b += JSS_WARPS_PER_CTA) {   // 1. expand
             int32_t *blk = slot(cur, b);
             env_load<KJ>(iv, blk, lane, s);
@@ -1767,6 +1856,31 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
                     key[i] = ((s.lb >> i) & 1u) && cs > -JSS_F32_INF ? jss_f32_key(cs + 0.0f) : 0u;
                     nc += key[i] != 0u;
                 }
+                if (SWOR) {                              // the perturbed values G, Z and the keys in their place
+                    const float T = bs.key[cur * W + b];
+                    float g[KJ];
+                    uint32_t zk = 0u;
+                    int zj = 1 << 20;
+#pragma unroll
+                    for (int i = 0; i < KJ; i++) {
+                        g[i] = (sc + lp[i]) + jss_gumbel(jss_hash_env(hr, (uint64_t)(b * 256 + KJ * lane + i)));
+                        const uint32_t k = jss_f32_key(g[i] + 0.0f);
+                        if (key[i] != 0u && k > zk) { zk = k; zj = KJ * lane + i; }
+                    }
+                    const uint32_t zbest = __reduce_max_sync(JSS_FULL, zk);
+                    zj = (int)__reduce_min_sync(JSS_FULL, (unsigned)(zk == zbest ? zj : 1 << 20));
+                    const float Z = jss_key_f32(zbest);
+#pragma unroll
+                    for (int i = 0; i < KJ; i++) {
+                        if (key[i] == 0u) continue;
+                        float kv = T;
+                        if (KJ * lane + i != zj) {
+                            const float v = T - g[i] + jss_log1mexp(g[i] - Z);
+                            kv = fminf(T, T - fmaxf(v, 0.0f) - log1pf(expf(-fabsf(v))));
+                        }
+                        key[i] = jss_f32_key(kv + 0.0f);
+                    }
+                }
                 taken = min(W, (int)__reduce_add_sync(JSS_FULL, (unsigned)nc));
                 for (int q = 0; q < taken; q++) {
                     uint32_t lk = 0u;
@@ -1780,6 +1894,14 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
                     for (int i = 0; i < KJ; i++)
                         if (KJ * lane + i == j) key[i] = 0u;
                     if (lane == 0) bs.cand[b * W + q] = jss_beam_key(best, b, j);
+                    if (SWOR) {
+                        float cj = 0.0f;
+#pragma unroll
+                        for (int i = 0; i < KJ; i++)
+                            if (KJ * lane + i == j) cj = sc + lp[i];
+                        cj = __shfl_sync(JSS_FULL, cj, j / KJ);
+                        if (lane == 0) bs.cscore[b * W + q] = cj;
+                    }
                 }
             }
             if (lane == 0) bs.cnt[b] = taken;
@@ -1797,7 +1919,10 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
                 const int n2 = bs.cnt[b2];
                 for (int q = 0; q < n2 && c2[q] > k; q++) rank++;
             }
-            if (rank < W) bs.sel[rank] = k;
+            if (rank < W) {
+                bs.sel[rank] = k;
+                if (SWOR) bs.score[(cur ^ 1) * W + rank] = bs.cscore[e];
+            }
         }
         __syncthreads();
         const int nn = min(W, total), nxt = cur ^ 1;
@@ -1811,7 +1936,12 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
             const bool ok = env_step<KJ, false>(p, iv, s, env, lane, j, raw, hz);
             env_store<KJ>(iv, slot(nxt, b), lane, s);
             if (lane == 0) {
-                bs.score[nxt * W + b] = ok ? jss_key_f32((uint32_t)(k >> 32)) : JSS_F32_NAN;
+                if (SWOR) {                              // the score came with the selection
+                    bs.key[nxt * W + b] = jss_key_f32((uint32_t)(k >> 32));
+                    if (!ok) bs.score[nxt * W + b] = JSS_F32_NAN;
+                } else {
+                    bs.score[nxt * W + b] = ok ? jss_key_f32((uint32_t)(k >> 32)) : JSS_F32_NAN;
+                }
                 if (trace) trace[(size_t)r * W + b] = (uint16_t)pj;
             }
         }
@@ -1819,44 +1949,41 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
         n = nn;
         cur = nxt;
     }
+    // slot b holds a complete beam
+    const auto complete = [&](int b) {
+        return !done0 && b < n && (slot(cur, b)[nw - 4 + JSS_HDR_FLAGS] & JSS_FLAG_DONE) &&
+               bs.score[cur * W + b] == bs.score[cur * W + b];
+    };
+    if (SWOR && a.order_out) {
+        for (int b = warp; b < W; b += JSS_WARPS_PER_CTA)
+            jss_beam_order<KJ>(p, trace, W, R, J, M, lane, complete(b) ? b : -1,
+                               a.order_out + ((size_t)env * W + b) * p.jobs_max * p.machines_max);
+    }
     if (warp != 0) return;
     // outputs: lane b reports slot b
     const int b = lane;
     int t = -1;
-    float sc = -JSS_F32_INF;
+    float sc = -JSS_F32_INF, ky = -JSS_F32_INF;
     if (!done0 && b < n) {
         const int32_t *hdr = slot(cur, b) + nw - 4;
         const float x = bs.score[cur * W + b];
-        if ((hdr[JSS_HDR_FLAGS] & JSS_FLAG_DONE) && x == x) { t = hdr[JSS_HDR_T]; sc = x; }
+        if ((hdr[JSS_HDR_FLAGS] & JSS_FLAG_DONE) && x == x) {
+            t = hdr[JSS_HDR_T]; sc = x;
+            if (SWOR) ky = bs.key[cur * W + b];
+        }
     }
     const bool any = __any_sync(JSS_FULL, t >= 0);
-    if (done0) sc = 0.0f;
-    else if (!any && bs.bad[0]) sc = JSS_F32_NAN;
+    if (done0) sc = ky = 0.0f;
+    else if (!any && bs.bad[0]) sc = ky = JSS_F32_NAN;
     if (b < W) {
         a.actions_out[(int64_t)env * a.samples_ld + b] = t;
         a.log_prob_out[(int64_t)env * a.samples_ld + b] = sc;
+        if (SWOR) a.key_out[(int64_t)env * a.samples_ld + b] = ky;
     }
-    if (!a.order_out) return;
+    if (SWOR || !a.order_out) return;
     // the best slot: smallest makespan, ties to the lowest slot (t < 2^24)
     const int best = any ? (int)(__reduce_min_sync(JSS_FULL, t >= 0 ? ((uint32_t)t << 5) | (uint32_t)b : ~0u) & 31u) : -1;
-    int32_t *ord = a.order_out + (size_t)env * p.jobs_max * p.machines_max;
-    int seen[KJ];                                        // allocations of each owned job met so far, walking back
-#pragma unroll
-    for (int i = 0; i < KJ; i++) {
-        seen[i] = 0;
-        if (KJ * lane + i < J)
-            for (int k = 0; k < M; k++) ord[(size_t)(KJ * lane + i) * p.machines_max + k] = -1;
-    }
-    if (best < 0) return;
-    int at = best;
-    for (int r = R - 1; r >= 0; r--) {
-        const uint32_t pj = jss_uniform((uint32_t)trace[(size_t)r * W + at]);   // every lane reads the same entry
-        const int j = (int)(pj & 255u);
-        at = (int)(pj >> 8);
-#pragma unroll
-        for (int i = 0; i < KJ; i++)
-            if (KJ * lane + i == j) { ord[(size_t)j * p.machines_max + (M - 1 - seen[i])] = r; seen[i]++; }
-    }
+    jss_beam_order<KJ>(p, trace, W, R, J, M, lane, best, a.order_out + (size_t)env * p.jobs_max * p.machines_max);
 }
 
 template <int KJ, int MODE>
@@ -1970,6 +2097,13 @@ constexpr int JSS_SAMPLE_EPISODES_SOLUTION_MIN_CTAS[JSS_LANE_CLASSES] = {6, 5, 6
 // The beam search likewise: 60 / 75 / 113 / 175 registers (CUDA 12.9, sm_90a); one CTA more spills in the classes with
 // 2, 4 and 8 jobs per lane.  Its shared memory (2 W state blocks) bounds the resident CTAs at large W anyway.
 constexpr int JSS_BEAM_SEARCH_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
+// The stochastic beam search likewise: 64 / 75 / 113 / 176 registers (CUDA 12.9, sm_90a).  The order likelihood at
+// 40 / 62 / 64 / 92 registers, its gradient at 64 / 72 / 64 / 143; one CTA more spills in every class of the
+// likelihood but the one with 1 job per lane (untried at 7), and in the classes with 2 and 8 jobs per lane of the
+// gradient.
+constexpr int JSS_SWOR_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
+constexpr int JSS_ORDER_LOG_PROB_MIN_CTAS[JSS_LANE_CLASSES] = {6, 4, 4, 2};
+constexpr int JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 1};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
     return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
@@ -1979,6 +2113,9 @@ JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
          : mode == JSS_MODE_SAMPLE_EPISODES_GRAD ? JSS_SAMPLE_EPISODES_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION ? JSS_SAMPLE_EPISODES_SOLUTION_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_BEAM_SEARCH ? JSS_BEAM_SEARCH_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_SWOR ? JSS_SWOR_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_ORDER_LOG_PROB ? JSS_ORDER_LOG_PROB_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_ORDER_LOG_PROB_GRAD ? JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
          : 1;
 }
 
@@ -1992,7 +2129,7 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     jss_cta_carve(sl, sm, c, iv);
     const int warp = jss_warp_index(), lane = threadIdx.x & 31;
     float *scratch = reinterpret_cast<float *>(sm + sl.off_warp0 + warp * sl.warp_stride);
-    if (MODE == JSS_MODE_BEAM_SEARCH) {
+    if (MODE == JSS_MODE_BEAM_SEARCH || MODE == JSS_MODE_SWOR) {
         // work item = one env (tile, warp slot), CTA-strided; the per-warp regions hold only env_check_no_op's table,
         // and the beam region follows them
         char *bsm = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;
@@ -2010,8 +2147,8 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
                 __syncthreads();
             }
             jss_iv_shape(iv);
-            env_beam_search<KJ>(p, a, iv, env, p.state + (size_t)t.off16 * 4, warp, lane,
-                                reinterpret_cast<int *>(scratch), bsm);
+            env_beam_search<KJ, MODE == JSS_MODE_SWOR>(p, a, iv, env, p.state + (size_t)t.off16 * 4, warp, lane,
+                                                       reinterpret_cast<int *>(scratch), bsm);
         }
         return;
     }

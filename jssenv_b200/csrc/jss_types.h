@@ -173,8 +173,9 @@ struct JssLaunch {           // per-launch arguments
     union {
         int32_t rule;
         int32_t greedy;      // steps from a row (a.logits): 0 categorical draw, 1 epsilon-greedy decode
-        int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env
-        int32_t beam_width;  // jss_beam_search: W, the beams kept per env
+        int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env; jss_order_log_prob (_grad):
+                             // K, the orders per env
+        int32_t beam_width;  // jss_beam_search, jss_sample_without_replacement: W, the beams kept per env
     };
     int32_t coin_mode, n_steps, write_obs;   // jss_lookahead (_priority): n_steps is S, the work items each tile's
                                              // candidates are spread over (launch_all); jss_sample_episodes: the
@@ -197,6 +198,8 @@ struct JssLaunch {           // per-launch arguments
         uint64_t sample_step_index;   // jss_rollout_priority_sample: the RNG counter of the env's first decision
         int64_t values_ld;   // jss_lookahead_priority: env i's value of action a at actions_out + i * values_ld + a
                              // (logits_ld is the table's env stride there)
+        const int32_t *order_in;   // jss_order_log_prob (_grad): order s of env i at order_in + (i * n_samples + s) *
+                                   // jobs_max * machines_max
     };
     union {
         const int32_t *actions;  // step; jss_sample_episodes_solution: the sample each env replays (< 0: none)
@@ -227,7 +230,12 @@ struct JssLaunch {           // per-launch arguments
         int32_t *order_out;
     };
     uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
-    uint8_t *wire;           // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
+    // jss_sample_without_replacement: slot b's score goes to log_prob_out and its key to key_out + i * samples_ld + b,
+    // and order_out is the [N][W][jobs_max][machines_max] order of every slot (may be NULL)
+    union {
+        uint8_t *wire;       // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
+        float *key_out;
+    };
     int32_t wire_stride;
     JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
     // jss_step_logits / jss_step_greedy: env i's logits (scores) at logits + i * logits_ld; the chosen actions go to
@@ -262,5 +270,11 @@ struct JssLaunch {           // per-launch arguments
                                                // (jss_sample_episodes_solution)
 #define JSS_MODE_BEAM_SEARCH 15          // beam search over a logit table, one env per CTA, the envs untouched
                                          // (jss_beam_search)
+#define JSS_MODE_SWOR 16                 // the same perturbed by top-down Gumbel noise: W distinct episodes drawn
+                                         // without replacement (jss_sample_without_replacement)
+#define JSS_MODE_ORDER_LOG_PROB 17       // the log-likelihood of K given operation orders per env under a logit
+                                         // table, the envs untouched (jss_order_log_prob)
+#define JSS_MODE_ORDER_LOG_PROB_GRAD 18  // its weighted gradient, added into the caller's chunks
+                                         // (jss_order_log_prob_grad)
 
 #define JSS_WARPS_PER_CTA 8

@@ -107,6 +107,37 @@ def _episodes_log_prob():
     return EpisodesLogProb
 
 
+@functools.lru_cache(maxsize=None)
+def _order_log_prob_fn():
+    """The autograd Function of the log_prob of JssVecEnv.order_log_prob and JssVecEnv.sample_without_replacement
+    (made on first use).  Forward runs `run(logits)`, which returns the (N, k) log_prob first, the (N, k, J, M) int32
+    orders last and any other outputs between, and saves the table and the orders; backward calls
+    jss_order_log_prob_grad with the incoming (N, k) gradient as weights, sums the chunks and then over the table's
+    broadcast dimensions.  The orders are replayed from the envs' state at backward time, which must still be their
+    state at forward time."""
+    import torch
+
+    class OrderLogProb(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, logits, env, run):
+            outs = run(logits)
+            ctx.save_for_backward(logits, outs[-1])    # torch's version counter refuses a table changed in place
+            ctx.env = env
+            ctx.mark_non_differentiable(*outs[1:])
+            return outs
+
+        @staticmethod
+        def backward(ctx, g, *_):
+            logits, order = ctx.saved_tensors
+            env = ctx.env
+            k = order.shape[1]
+            split = min(k, -(-env._warp_slots() // env.num_envs))
+            grad = env._order_log_prob_grad(logits, order, g, split)
+            return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None
+
+    return OrderLogProb
+
+
 def _state_views(b, n, J, M, view):
     """The canonical-state arrays of jss_export_state, each made by ``view(ptr, shape, dtype)``."""
     return {"todo": view(b.x_todo, (n, J), np.int32), "tufco": view(b.x_tufco, (n, J), np.int32),
@@ -599,6 +630,113 @@ class JssVecEnv:
         if order:
             out["order"] = ord_
         return out
+
+    def sample_without_replacement(self, logits, k: int, order: bool = False):
+        """Draw `k` distinct episodes per env without replacement from the logit table `logits` by stochastic beam
+        search (Kool et al., 2019), each from the env's current state, in one launch per lane class
+        (jss_sample_without_replacement), leaving the envs untouched.  The distribution is the one
+        rollout_priority_sample() draws from; the search is beam_search()'s with each candidate's score perturbed by
+        top-down Gumbel noise and the beams ranked by that perturbed log-probability (the key).  `logits` is taken as by
+        rollout_priority_sample(); 1 <= k <= MAX_BEAM_WIDTH.  The RNG counter advances by J*M (the batch maxima).
+        Returns a dict of device tensors: ``"makespan"`` (N, k) int32, ``"log_prob"`` (N, k) float32 (bit for bit the
+        log_prob rollout_priority_sample() reports for the same episode) and ``"key"`` (N, k) float32, key descending
+        (-1 / -inf / -inf for a slot without a complete beam, -1 / NaN / NaN in every slot of an env whose every beam
+        met a bad entry, -1 / 0 / 0 for an env done now); ``"best"`` (N,) int64, the lowest slot of smallest makespan,
+        -1 if none; with `order`, ``"order"`` (N, k, J, M) int32, every slot's allocation round of each operation in
+        beam_search()'s format (-1 for operations started before the call, and everywhere in a slot without a complete
+        beam).  When `logits` requires grad (and grad mode is on), log_prob is differentiable with respect to it: the
+        backward replays the slots' orders (order_log_prob()), so the envs must not be stepped or reset between this
+        call and the backward.  With k + 1 draws, ``key[:, k]`` is the threshold of the priority-sampling estimator
+        (INTEGRATION.md)."""
+        import torch
+        x = self._table_arg(logits, "sample_without_replacement", "logits")
+        if not 1 <= int(k) <= N.MAX_BEAM_WIDTH:
+            raise ValueError(f"sample_without_replacement: k must be in 1..{N.MAX_BEAM_WIDTH}, got {k!r}")
+        k, step_index = int(k), self._step_index
+        grad = x.requires_grad and torch.is_grad_enabled()
+        run = functools.partial(self._sample_without_replacement, k=k, step_index=step_index, order=order or grad)
+        if grad:
+            log_prob, makespan, key, ord_ = _order_log_prob_fn().apply(x, self, run)
+        else:
+            log_prob, makespan, key, ord_ = run(x)
+        self._step_index += self.jobs * self.machines
+        ended = makespan >= 0
+        best = torch.where(ended, makespan, torch.iinfo(torch.int32).max).argmin(1)
+        best = torch.where(ended.any(1), best, -1)
+        out = {"makespan": makespan, "log_prob": log_prob, "key": key, "best": best}
+        if order:
+            out["order"] = ord_
+        return out
+
+    def _sample_without_replacement(self, x, k: int, step_index: int, order: bool):
+        """The native call of sample_without_replacement on a checked table `x` at RNG counter `step_index`:
+        (log_prob, makespan, key, order), order None unless asked for."""
+        import torch
+        v = self._table_view(x)
+        n = self.num_envs
+        makespan = torch.empty((n, k), dtype=torch.int32, device=self.device)
+        log_prob = torch.empty((n, k), dtype=torch.float32, device=self.device)
+        key = torch.empty((n, k), dtype=torch.float32, device=self.device)
+        ord_ = (torch.full((n, k, self.jobs, self.machines), -1, dtype=torch.int32, device=self.device)
+                if order else None)
+        rc = self._L.jss_sample_without_replacement(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
+                                                    step_index, k, makespan.data_ptr(), log_prob.data_ptr(),
+                                                    key.data_ptr(), k, _ptr(ord_), self._stream())
+        N.check(self._h, rc, "jss_sample_without_replacement")
+        return log_prob, makespan, key, ord_
+
+    def order_log_prob(self, logits, order):
+        """The log-likelihood under the logit table `logits` of given operation orders, each from the env's current
+        state, in one launch per lane class (jss_order_log_prob), leaving the envs untouched.  `order` is (N, J, M) or
+        (N, k, J, M) integer: order s of env i stands for the episode rollout_priority(-order[i, s]) runs from this
+        state (the orders of beam_search() and sample_without_replacement() replay their beams).  `logits` is taken as
+        by rollout_priority_sample().  Returns ``(log_prob, makespan)``, each (N,) or (N, k): log_prob float32, the sum
+        of the decisions' log-probabilities computed as rollout_priority_sample() computes them (forced no-ops add 0;
+        NaN where a decision meets a bad entry; 0 for an env done now), makespan int32, the end time (-1 unless the
+        episode ends done).  When `logits` requires grad (and grad mode is on), log_prob is differentiable with respect
+        to it (jss_order_log_prob_grad); the envs must not be stepped or reset between this call and the backward."""
+        import torch
+        x = self._table_arg(logits, "order_log_prob", "logits")
+        n, J, M = self.num_envs, self.jobs, self.machines
+        o = torch.as_tensor(order, device=self.device)
+        single = o.dim() == 3
+        if (o.dim() not in (3, 4) or o.shape[0] != n or tuple(o.shape[-2:]) != (J, M) or o.is_floating_point()
+                or o.is_complex() or o.dtype == torch.bool or (o.dim() == 4 and o.shape[1] < 1)):
+            raise ValueError(f"order_log_prob: order must be an integer tensor of shape ({n}, {J}, {M}) or "
+                             f"({n}, k, {J}, {M}), got {tuple(o.shape)} {o.dtype}")
+        o = o.reshape(n, -1, J, M).to(torch.int32).contiguous()
+        run = functools.partial(self._order_log_prob, order=o)
+        if x.requires_grad and torch.is_grad_enabled():
+            log_prob, makespan, _ = _order_log_prob_fn().apply(x, self, run)
+        else:
+            log_prob, makespan, _ = run(x)
+        return (log_prob[:, 0], makespan[:, 0]) if single else (log_prob, makespan)
+
+    def _order_log_prob(self, x, order):
+        """The native call of order_log_prob on a checked table `x` and (N, k, J, M) contiguous int32 orders:
+        (log_prob, makespan, order)."""
+        import torch
+        v = self._table_view(x)
+        k = order.shape[1]
+        makespan = torch.empty((self.num_envs, k), dtype=torch.int32, device=self.device)
+        log_prob = torch.empty((self.num_envs, k), dtype=torch.float32, device=self.device)
+        rc = self._L.jss_order_log_prob(self._h, v.data_ptr(), *(int(s) for s in v.stride()), order.data_ptr(), k,
+                                        makespan.data_ptr(), log_prob.data_ptr(), k, self._stream())
+        N.check(self._h, rc, "jss_order_log_prob")
+        return log_prob, makespan, order
+
+    def _order_log_prob_grad(self, x, order, weights, split: int):
+        """The native backward of order_log_prob: the (split, N, J, M) float32 chunks of sum_s weights[:, s] *
+        d log_prob[:, s] / d table for the (N, k, J, M) int32 orders, replayed from the current state."""
+        import torch
+        v = self._table_view(x)
+        k = order.shape[1]
+        w = weights.detach().to(torch.float32).contiguous()
+        grad = torch.zeros((split, self.num_envs, self.jobs, self.machines), dtype=torch.float32, device=self.device)
+        rc = self._L.jss_order_log_prob_grad(self._h, v.data_ptr(), *(int(s) for s in v.stride()), order.data_ptr(),
+                                             k, w.data_ptr(), k, int(split), grad.data_ptr(), self._stream())
+        N.check(self._h, rc, "jss_order_log_prob_grad")
+        return grad
 
     def _sample_episodes(self, x, k: int, step_index: int):
         """The native call of sample_episodes on a checked table `x` at RNG counter `step_index`: (makespan, log_prob),
