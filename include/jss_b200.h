@@ -569,6 +569,43 @@ int jss_sample_without_replacement(jss_t *h, const float *logits_dev, int64_t ld
                                    float *log_prob_out_dev, float *key_out_dev, int64_t ld, int32_t *order_out_dev,
                                    void *stream);
 
+/* One round of beam search for a policy that reads the observation at every decision: the per-round form of
+ * jss_beam_search(), with a logit row per beam in place of the table, on a handle whose envs are the beams.  One launch
+ * per lane class present (one group per CTA).
+ *   Groups: the N envs form G = N / width groups; group g is envs g*W .. g*W + W-1 and its slot b is env g*W + b.  Every
+ *     env of a group must run the same instance: a group is one search.
+ *   Scores: score_dev, caller-owned fp32 [N], is read and written.  A slot is live iff its score is finite.  A search
+ *     starts with score = [0, -inf, ..., -inf] per group and its start state in slot 0; the other slots' states are
+ *     never read.
+ *   Rows: logits_dev[env*ld + j] (ld >= jobs_max + 1), read only at the legal jobs j of a live, not-done beam; the no-op
+ *     column is never read.
+ *   One call is one round of jss_beam_search() per group, so that rows gathered from a table at each slot's todo give
+ *     jss_beam_search()'s result bit for bit:
+ *     1. Expand: a live, not-done beam with a legal job has as candidates its legal jobs j with score + logp_j > -inf,
+ *        logp_j computed as jss_beam_search() computes it with x_j = row[j].  A bad row (NaN or +inf at a legal job, or
+ *        every legal job at -inf) gives no candidate and sets the group's bad_out; a live beam with no legal job, or
+ *        done, gives none.
+ *     2. Select: the W best candidates in jss_beam_search()'s order (score descending, -0 = +0, then parent slot, then
+ *        job) become slots 0 .. nn-1.
+ *     3. Step: new slot b gets its parent's state as at call entry, stepped with its job, then the no-op as long as no
+ *        job is legal and the no-op is.  Its score is the candidate's, or NaN if a step fails (an imported state).
+ *        Slots nn .. W-1 get score -inf; their state is left as it is (stale).
+ *     A group without a live, not-done beam is untouched: its states and scores are left as they are.
+ *   Outputs (device int32): parent_out_dev[env] and action_out_dev[env], the new slot's parent slot and job, -1 / -1 for
+ *     an empty slot, b / -1 for slot b of an untouched group (so a walk back through the rounds is uniform);
+ *     bad_out_dev[g] is 1 if a beam of group g met a bad row in this call, else 0.
+ *   A written slot's state block, real_obs row, action_mask row and scalar record equal, bit for bit, those of a twin
+ *     that ran jss_step(job) and then jss_step(J) for each forced no-op; the rows are written whole.  Statistics,
+ *     solution, the error bit and auto-reset are not touched, and no RNG is used.  A stale real_obs is refreshed first.
+ *   Returns JSS_ERR_INVALID for a NULL or not 4-byte-aligned pointer, width < 1 or > JSS_MAX_BEAM_WIDTH, N not divisible
+ *     by width, ld < jobs_max + 1 or a group that mixes instances; JSS_ERR_STATE before jss_assign().
+ * Measured on an H100 SXM 80 GB HBM3 at a 700 W power limit with a linear policy on real_obs in torch (median of three
+ * rounds): ta80 at G = 256, W = 16 from reset 288 ms per search (144 us per round, policy included) against 2 789 ms for
+ * the torch loop of export_state / top-W / import_state / jss_step on the same N*W envs and 205 ms for one
+ * jss_step_greedy per round; ta01 at G = 4 096, W = 8 34.9 against 286 ms (DESIGN.md section 4). */
+int jss_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, float *score_dev, int32_t *parent_out_dev,
+                  int32_t *action_out_dev, int32_t *bad_out_dev, void *stream);
+
 /* The teacher-forced log-likelihood of k given operation orders per env under a caller's logit table, each from the
  * env's current state, in one launch per lane class present, leaving the envs untouched.
  *   order_dev: device int32 [N][k][jobs_max][machines_max].  Order s of env i stands for the episode that

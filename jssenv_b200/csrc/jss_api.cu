@@ -80,6 +80,12 @@ struct jss_handle {
     unsigned long long *d_stats = nullptr;
     uint16_t *beam_trace = nullptr;                // jss_beam_search's backpointers (first call with an order)
     size_t beam_trace_bytes = 0;
+    struct BeamGroups {                            // jss_beam_step's group records of one width (beam_groups)
+        int32_t *dev = nullptr;
+        int32_t ranges[JSS_LANE_CLASSES][2] = {};  // [ranges[c][0], ranges[c][1]): the records of lane class c
+        std::string err;                           // why the width cannot be used ("": it can)
+    };
+    std::map<int, BeamGroups> beam_groups;         // by width, built by the first call with it
 
     JssParams p{};
     JssSmemLayout sl_env{}, sl_step{}, sl_step_rem{};   // shared-memory layouts of the generic / step kernels (step: without / with the suffix-sum table)
@@ -88,6 +94,7 @@ struct jss_handle {
     int n_tiles = 0;
     std::map<std::pair<const void *, size_t>, int> ctas_per_sm;   // by kernel and dynamic shared memory (filled lazily)
     std::vector<int32_t> env_inst;
+    std::vector<uint32_t> env_off16;               // each env's state block, in 16-byte units (tile order)
 
     // host-buffer stepping
     int32_t *dev_actions = nullptr;
@@ -633,6 +640,9 @@ int jss_assign(jss_t *h, const int32_t *env_to_inst) {
     size_t state_words = 0;
     if ((rc = plan_tiles(h, env_to_inst, order, tiles, state_words))) return rc;
     const std::vector<JssCtaRange> ranges = plan_cta_ranges(h);
+    h->env_off16.assign(N, 0);
+    for (const JssTile &t : tiles)
+        for (int w = 0; w < (t.inst_count & 255); w++) h->env_off16[order[t.first + w]] = t.state_off16 + w * t.block16;
 
     JssParams &p = h->p;
     p.n_envs = N;
@@ -1132,6 +1142,113 @@ int jss_sample_without_replacement(jss_t *h, const float *logits_dev, int64_t ld
     a.order_out = order_out_dev;
     if (order_out_dev && (rc = beam_trace(h, width, true, a))) return rc;
     return launch_all(h, a, (cudaStream_t)stream);
+}
+
+namespace {
+
+// jss_beam_step's group records for width W, built once per handle and width: per group [g, instance, the W slots'
+// block offsets in 16-byte units] (blocks are in tile order, and a group need not align with tiles), grouped by lane
+// class and, within one, by instance, so that a CTA restages the instance tables rarely.  Leaves `out` null with the
+// reason in the handle's error if the width does not divide N or a group mixes instances.
+int beam_groups(jss_t *h, int W, const jss_handle::BeamGroups *&out) {
+    out = nullptr;
+    auto it = h->beam_groups.find(W);
+    if (it == h->beam_groups.end()) {
+        jss_handle::BeamGroups bg;
+        const int N = h->n_envs, G = N / W;
+        if (N % W) {
+            bg.err = "jss_beam_step: width " + std::to_string(W) + " does not divide the " + std::to_string(N) + " envs";
+        } else {
+            for (int g = 0; g < G && bg.err.empty(); g++)
+                for (int b = 1; b < W; b++)
+                    if (h->env_inst[g * W + b] != h->env_inst[g * W]) {
+                        bg.err = "jss_beam_step: group " + std::to_string(g) + " (envs " + std::to_string(g * W) + " .. " +
+                                 std::to_string(g * W + W - 1) + ") mixes instances";
+                        break;
+                    }
+        }
+        if (bg.err.empty()) {
+            std::vector<int32_t> grp(G);
+            for (int g = 0; g < G; g++) grp[g] = g;
+            const auto cls = [&](int g) { return jss_lane_class(h->insts[h->env_inst[g * W]].J); };
+            std::stable_sort(grp.begin(), grp.end(), [&](int x, int y) {
+                if (cls(x) != cls(y)) return cls(x) < cls(y);
+                return h->env_inst[x * W] < h->env_inst[y * W];
+            });
+            std::vector<int32_t> rec((size_t)G * (W + 2));
+            for (int r = 0; r < G; r++) {
+                const int g = grp[r], c = cls(g);
+                int32_t *q = rec.data() + (size_t)r * (W + 2);
+                q[0] = g;
+                q[1] = h->env_inst[g * W];
+                for (int b = 0; b < W; b++) q[2 + b] = (int32_t)h->env_off16[g * W + b];
+                if (r == 0 || cls(grp[r - 1]) != c) bg.ranges[c][0] = r;
+                bg.ranges[c][1] = r + 1;
+            }
+            if (int rc = dev_alloc(h, &bg.dev, rec.size(), false)) return rc;
+            JSS_CUDA(h, cudaMemcpy(bg.dev, rec.data(), rec.size() * 4, cudaMemcpyHostToDevice));
+            JSS_CUDA(h, cudaStreamSynchronize(nullptr));   // a caller's non-blocking stream does not wait for it
+        }
+        it = h->beam_groups.emplace(W, bg).first;
+    }
+    if (!it->second.err.empty()) return fail(h, JSS_ERR_INVALID, "%s", it->second.err.c_str());
+    out = &it->second;
+    return JSS_OK;
+}
+
+// jss_beam_step's shared-memory layout: the instance tables without the suffix sums, the observation staging per warp
+// (which env_check_no_op's table shares), then the beam region of width W with one buffer of blocks of the batch maxima
+JssSmemLayout beam_step_layout(const jss_t *h) {
+    JssSmemLayout sl = h->sl_env;
+    sl.off_warp0 = sl.off_rem;
+    return sl;
+}
+
+}  // namespace
+
+int jss_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, float *score_dev, int32_t *parent_out_dev,
+                  int32_t *action_out_dev, int32_t *bad_out_dev, void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    if (bad_ptr(logits_dev) || bad_ptr(score_dev) || bad_ptr(parent_out_dev) || bad_ptr(action_out_dev) ||
+        bad_ptr(bad_out_dev) || width < 1 || width > JSS_MAX_BEAM_WIDTH || ld < (int64_t)h->p.jobs_max + 1)
+        return fail(h, JSS_ERR_INVALID, "jss_beam_step: bad arguments (logits %p, score %p, parent_out %p, action_out "
+                    "%p and bad_out %p must be non-NULL and 4-byte aligned, 1 <= width %d <= %d, ld %lld >= jobs_max + 1 "
+                    "= %d)", (const void *)logits_dev, (void *)score_dev, (void *)parent_out_dev,
+                    (void *)action_out_dev, (void *)bad_out_dev, width, JSS_MAX_BEAM_WIDTH, (long long)ld,
+                    h->p.jobs_max + 1);
+    const jss_handle::BeamGroups *bg = nullptr;
+    if ((rc = beam_groups(h, width, bg))) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = refresh_obs(h, st))) return rc;            // the untouched rows must be current, as after any call
+    JssLaunch a{};
+    a.mode = JSS_MODE_BEAM_STEP;
+    a.stage = JSS_STAGE_OPS;
+    a.beam_width = width;
+    a.beam_groups = bg->dev;
+    a.logits = logits_dev;
+    a.logits_ld = ld;
+    a.log_prob_out = score_dev;
+    a.parent_out = parent_out_dev;
+    a.job_out = action_out_dev;
+    a.bad_out = bad_out_dev;
+    if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
+    const JssSmemLayout sl = beam_step_layout(h);
+    const size_t smem = smem_bytes(sl) + jss_beam_smem(nullptr, width, jss_block_geom(h->p.jobs_max, h->p.machines_max).words,
+                                                       nullptr, false, 1);
+    for (int c = 0; c < JSS_LANE_CLASSES; c++) {         // one launch per lane class present
+        a.tile_begin = bg->ranges[c][0];
+        a.tile_end = bg->ranges[c][1];
+        const int n_groups = a.tile_end - a.tile_begin;
+        if (n_groups <= 0) continue;
+        const JssKernel k = env_kernels<JSS_MODE_BEAM_STEP>[c];
+        int per_sm = 0;
+        if ((rc = ctas_per_sm(h, k, smem, per_sm))) return rc;
+        JSS_LAUNCH(k, std::min(n_groups, h->sm_count * per_sm), JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
+        JSS_CUDA(h, cudaGetLastError());
+        h->launches += 1;
+    }
+    return JSS_OK;
 }
 
 namespace {

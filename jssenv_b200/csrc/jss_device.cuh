@@ -1544,7 +1544,7 @@ JSS_HD constexpr bool jss_mode_samples(int mode) {
            mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION || mode == JSS_MODE_ORDER_LOG_PROB ||
            mode == JSS_MODE_ORDER_LOG_PROB_GRAD;
 }
-template <int KJ>
+template <int KJ, bool ROW = false>
 JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ]);
 // Env `env`'s next decision under an operation order `ord` (row stride machines_max; jss_order_log_prob): that of
 // env_priority_action on the table -ord, the legal job whose current operation has the smallest entry, ties to the
@@ -1686,7 +1686,9 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
 // with the loads, reductions and fast exp / log of env_priority_sample_action in the same order, so that lp of the job
 // it draws equals its logp bit for bit.  Kept apart from it so that its code (and the sampling kernels') stays as it
 // is.  At least one job must be legal; returns false for a bad row (the bad-table rule of env_priority_sample_action).
-template <int KJ>
+// ROW (jss_beam_step): x_j is column j of env `env`'s logit row (a.logits, row stride a.logits_ld) in place of the table
+// entry of job j's current operation; everything else is the same.
+template <int KJ, bool ROW>
 JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ]) {
     const float *row = a.logits + (int64_t)env * a.logits_ld;
     bool bad = false;                                    // a legal entry is NaN or +inf
@@ -1696,7 +1698,8 @@ JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, i
     for (int i = 0; i < KJ; i++) {
         x[i] = 0.0f;
         if ((s.lb >> i) & 1u) {
-            x[i] = row[(int64_t)(KJ * lane + i) * a.prio_ld_job + (int64_t)s.todo[i] * a.prio_ld_op];
+            x[i] = ROW ? row[KJ * lane + i]
+                       : row[(int64_t)(KJ * lane + i) * a.prio_ld_job + (int64_t)s.todo[i] * a.prio_ld_op];
             bad = bad || !(x[i] < JSS_F32_INF);
             xkey = max(xkey, jss_f32_key(x[i]));
         }
@@ -1727,7 +1730,8 @@ JSS_DEV uint64_t jss_beam_key(uint32_t score_key, int parent, int job) {
 // The beam region of the CTA's shared memory for width W and state blocks of `bw` words (jss_block_geom of the batch
 // maxima): [blocks: 2][W][bw] int32 | [cand: W][W] u64 | [sel: W] u64 | [score: 2][W] f32 | [cnt: W] i32 | [bad] i32,
 // and for the stochastic beam search (swor) then [cscore: W][W] f32 | [key: 2][W] f32, the candidates' scores and the
-// slots' keys.  jss_beam_search and jss_sample_without_replacement size it with the same function.
+// slots' keys.  jss_beam_search and jss_sample_without_replacement size it with the same function; jss_beam_step with
+// one buffer of blocks (nbuf = 1: the parents; the children go straight to their slots' blocks in global memory).
 struct JssBeamSmem {
     int32_t *blocks;
     uint64_t *cand, *sel;
@@ -1735,8 +1739,8 @@ struct JssBeamSmem {
     int32_t *cnt, *bad;
     float *cscore, *key;
 };
-JSS_HD inline size_t jss_beam_smem(char *base, int W, int bw, JssBeamSmem *b, bool swor = false) {
-    const size_t o_cand = (size_t)2 * W * bw * 4, o_sel = o_cand + (size_t)8 * W * W, o_score = o_sel + (size_t)8 * W;
+JSS_HD inline size_t jss_beam_smem(char *base, int W, int bw, JssBeamSmem *b, bool swor = false, int nbuf = 2) {
+    const size_t o_cand = (size_t)nbuf * W * bw * 4, o_sel = o_cand + (size_t)8 * W * W, o_score = o_sel + (size_t)8 * W;
     const size_t o_cnt = o_score + (size_t)8 * W, o_bad = o_cnt + (size_t)4 * W, end = (o_bad + 4 + 15) & ~(size_t)15;
     const size_t o_key = end + (size_t)4 * W * W, end_swor = (o_key + (size_t)8 * W + 15) & ~(size_t)15;
     if (b) {
@@ -1780,6 +1784,60 @@ JSS_DEV void jss_beam_order(const JssParams &p, const uint16_t *trace, int W, in
         for (int i = 0; i < KJ; i++)
             if (KJ * lane + i == j) { ord[(size_t)j * p.machines_max + (M - 1 - seen[i])] = r; seen[i]++; }
     }
+}
+
+// The pieces of a beam round that jss_beam_search, jss_sample_without_replacement and jss_beam_step share.
+// The W argmax passes of the expansion of the beam in slot b: its `taken` best candidates in key order (key[i]: owned
+// job i's key, 0 for none; the passes clear them) go to bs.cand[b W ..].  SWOR: bs.cscore gets their scores sc + lp.
+template <int KJ, bool SWOR>
+JSS_DEV void jss_beam_passes(const JssBeamSmem &bs, uint32_t (&key)[KJ], const float (&lp)[KJ], float sc, int b, int W,
+                             int lane, int taken) {
+    for (int q = 0; q < taken; q++) {
+        uint32_t lk = 0u;
+        int lj = 1 << 20;
+#pragma unroll
+        for (int i = 0; i < KJ; i++)
+            if (key[i] > lk) { lk = key[i]; lj = KJ * lane + i; }
+        const uint32_t best = __reduce_max_sync(JSS_FULL, lk);
+        const int j = (int)__reduce_min_sync(JSS_FULL, (unsigned)(lk == best ? lj : 1 << 20));
+#pragma unroll
+        for (int i = 0; i < KJ; i++)
+            if (KJ * lane + i == j) key[i] = 0u;
+        if (lane == 0) bs.cand[b * W + q] = jss_beam_key(best, b, j);
+        if (SWOR) {
+            float cj = 0.0f;
+#pragma unroll
+            for (int i = 0; i < KJ; i++)
+                if (KJ * lane + i == j) cj = sc + lp[i];
+            cj = __shfl_sync(JSS_FULL, cj, j / KJ);
+            if (lane == 0) bs.cscore[b * W + q] = cj;
+        }
+    }
+}
+
+// Selection, by the whole CTA: each kept candidate of the n slots' sorted lists (bs.cnt[b] of them) is ranked against
+// the others, and rank < W becomes new slot rank in bs.sel (SWOR: its score goes to buffer cur ^ 1 of bs.score).
+// Returns the number of candidates.  The caller synchronises the CTA before and after.
+template <bool SWOR>
+JSS_DEV int jss_beam_rank(const JssBeamSmem &bs, int n, int W, int cur) {
+    int total = 0;
+    for (int b = 0; b < n; b++) total += bs.cnt[b];
+    for (int e = (int)threadIdx.x; e < n * W; e += (int)blockDim.x) {
+        const int b = e / W;
+        if (e - b * W >= bs.cnt[b]) continue;
+        const uint64_t k = bs.cand[e];
+        int rank = 0;
+        for (int b2 = 0; b2 < n; b2++) {                 // each list is sorted, best first
+            const uint64_t *c2 = bs.cand + b2 * W;
+            const int n2 = bs.cnt[b2];
+            for (int q = 0; q < n2 && c2[q] > k; q++) rank++;
+        }
+        if (rank < W) {
+            bs.sel[rank] = k;
+            if (SWOR) bs.score[(cur ^ 1) * W + rank] = bs.cscore[e];
+        }
+    }
+    return total;
 }
 
 // One env searched by the whole CTA (`root`: its state block, never written).  The beams are state blocks in shared
@@ -1882,48 +1940,12 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
                     }
                 }
                 taken = min(W, (int)__reduce_add_sync(JSS_FULL, (unsigned)nc));
-                for (int q = 0; q < taken; q++) {
-                    uint32_t lk = 0u;
-                    int lj = 1 << 20;
-#pragma unroll
-                    for (int i = 0; i < KJ; i++)
-                        if (key[i] > lk) { lk = key[i]; lj = KJ * lane + i; }
-                    const uint32_t best = __reduce_max_sync(JSS_FULL, lk);
-                    const int j = (int)__reduce_min_sync(JSS_FULL, (unsigned)(lk == best ? lj : 1 << 20));
-#pragma unroll
-                    for (int i = 0; i < KJ; i++)
-                        if (KJ * lane + i == j) key[i] = 0u;
-                    if (lane == 0) bs.cand[b * W + q] = jss_beam_key(best, b, j);
-                    if (SWOR) {
-                        float cj = 0.0f;
-#pragma unroll
-                        for (int i = 0; i < KJ; i++)
-                            if (KJ * lane + i == j) cj = sc + lp[i];
-                        cj = __shfl_sync(JSS_FULL, cj, j / KJ);
-                        if (lane == 0) bs.cscore[b * W + q] = cj;
-                    }
-                }
+                jss_beam_passes<KJ, SWOR>(bs, key, lp, sc, b, W, lane, taken);
             }
             if (lane == 0) bs.cnt[b] = taken;
         }
         __syncthreads();
-        int total = 0;                                   // 2. select
-        for (int b = 0; b < n; b++) total += bs.cnt[b];
-        for (int e = (int)threadIdx.x; e < n * W; e += (int)blockDim.x) {
-            const int b = e / W;
-            if (e - b * W >= bs.cnt[b]) continue;
-            const uint64_t k = bs.cand[e];
-            int rank = 0;
-            for (int b2 = 0; b2 < n; b2++) {             // each list is sorted, best first
-                const uint64_t *c2 = bs.cand + b2 * W;
-                const int n2 = bs.cnt[b2];
-                for (int q = 0; q < n2 && c2[q] > k; q++) rank++;
-            }
-            if (rank < W) {
-                bs.sel[rank] = k;
-                if (SWOR) bs.score[(cur ^ 1) * W + rank] = bs.cscore[e];
-            }
-        }
+        const int total = jss_beam_rank<SWOR>(bs, n, W, cur);   // 2. select
         __syncthreads();
         const int nn = min(W, total), nxt = cur ^ 1;
         for (int b = warp; b < nn; b += JSS_WARPS_PER_CTA) {   // 3. step the kept children
@@ -1984,6 +2006,109 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
     // the best slot: smallest makespan, ties to the lowest slot (t < 2^24)
     const int best = any ? (int)(__reduce_min_sync(JSS_FULL, t >= 0 ? ((uint32_t)t << 5) | (uint32_t)b : ~0u) & 31u) : -1;
     jss_beam_order<KJ>(p, trace, W, R, J, M, lane, best, a.order_out + (size_t)env * p.jobs_max * p.machines_max);
+}
+
+// ---- one beam-search round per group of W envs from per-beam logit rows (jss_beam_step) ----------------------------
+// The whole CTA works on group g (record `rec`: g, its instance, its W slots' block offsets), slot b = env g W + b.  A
+// slot is live iff its score (a.log_prob_out) is finite.
+//   0. the scores and the live slots' blocks (the parents, as at entry) go to shared memory.  Without a live, not-done
+//      slot the group is untouched: parent b, job -1, bad 0, and nothing else is written;
+//   1. warp w expands the slots b = w, w + 8, ...: a live, not-done slot with a legal job takes the log-probabilities
+//      of its row (env_table_logp<KJ, true>) and keeps its best children, keyed as env_beam_search keys them, by the
+//      argmax passes (jss_beam_passes); a bad row sets bad;
+//   2. the CTA ranks the candidates (jss_beam_rank);
+//   3. warp w steps new slot b = w, w + 8, ... < nn from its parent's block, takes the forced no-ops while no
+//      job is legal and the no-op is, and writes the slot's block, its observation, mask and scalar record whole (the
+//      raw reward of its last step) and its score, parent and job; slots nn .. W-1 get -inf, -1, -1.
+// Every step is env_step<KJ, false>: no statistics, solution, auto-reset or RNG.
+template <int KJ>
+JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstView &iv, const int32_t *rec, int warp,
+                           int lane, float *scratch, char *bsm) {
+    constexpr uint32_t LM = jss_legal_mask<KJ>();
+    const int W = a.beam_width, bw = jss_block_geom(p.jobs_max, p.machines_max).words;
+    const int J = jss_J(iv), nw = iv.si->block_words;
+    const int g = rec[0], e0 = g * W;
+    const uint32_t *off = reinterpret_cast<const uint32_t *>(rec + 2);
+    int *hz = reinterpret_cast<int *>(scratch);
+    JssBeamSmem bs;
+    jss_beam_smem(bsm, W, bw, &bs, false, 1);
+    const auto live = [](float x) { return x > -JSS_F32_INF && x < JSS_F32_INF; };
+    __syncthreads();                                     // the previous group's last reads of the region are done
+    for (int b = (int)threadIdx.x; b < W; b += (int)blockDim.x) bs.score[b] = a.log_prob_out[e0 + b];
+    if (threadIdx.x == 0) bs.bad[0] = 0;
+    __syncthreads();
+    for (int k = (int)threadIdx.x; k < W * (nw / 4); k += (int)blockDim.x) {   // 0. the live slots' blocks
+        const int b = k / (nw / 4), q = k - b * (nw / 4);
+        if (live(bs.score[b]))
+            reinterpret_cast<int4 *>(bs.blocks + (size_t)b * bw)[q] =
+                reinterpret_cast<const int4 *>(p.state + (size_t)off[b] * 4)[q];
+    }
+    __syncthreads();
+    bool moves = false;                                  // CTA-uniform: every thread reads the same words
+    for (int b = 0; b < W; b++)
+        moves = moves || (live(bs.score[b]) && !(bs.blocks[(size_t)b * bw + nw - 4 + JSS_HDR_FLAGS] & JSS_FLAG_DONE));
+    if (!moves) {
+        for (int b = (int)threadIdx.x; b < W; b += (int)blockDim.x) { a.parent_out[e0 + b] = b; a.job_out[e0 + b] = -1; }
+        if (threadIdx.x == 0) a.bad_out[g] = 0;
+        return;
+    }
+    EnvRegs<KJ> s;
+    for (int b = warp; b < W; b += JSS_WARPS_PER_CTA) {   // 1. expand
+        const float sc = bs.score[b];
+        int taken = 0;
+        if (live(sc)) {
+            env_load<KJ>(iv, bs.blocks + (size_t)b * bw, lane, s);
+            s.flags = jss_uniform(s.flags);
+            if (!(s.flags & JSS_FLAG_DONE) && __any_sync(JSS_FULL, (s.lb & LM) != 0u)) {
+                float lp[KJ];
+                if (env_table_logp<KJ, true>(a, s, e0 + b, lane, lp)) {
+                    uint32_t key[KJ];                    // 0: not a candidate, or already taken
+                    int nc = 0;
+#pragma unroll
+                    for (int i = 0; i < KJ; i++) {
+                        const float cs = sc + lp[i];
+                        key[i] = ((s.lb >> i) & 1u) && cs > -JSS_F32_INF ? jss_f32_key(cs + 0.0f) : 0u;
+                        nc += key[i] != 0u;
+                    }
+                    taken = min(W, (int)__reduce_add_sync(JSS_FULL, (unsigned)nc));
+                    jss_beam_passes<KJ, false>(bs, key, lp, sc, b, W, lane, taken);
+                } else if (lane == 0) {
+                    bs.bad[0] = 1;
+                }
+            }
+        }
+        if (lane == 0) bs.cnt[b] = taken;
+    }
+    __syncthreads();
+    const int nn = min(W, jss_beam_rank<false>(bs, W, W, 0));   // 2. select
+    __syncthreads();
+    for (int b = warp; b < nn; b += JSS_WARPS_PER_CTA) {   // 3. step the kept children into their slots
+        const int env = e0 + b;
+        const uint64_t k = bs.sel[b];
+        const uint32_t pj = ~(uint32_t)k;
+        env_load<KJ>(iv, bs.blocks + (size_t)(pj >> 8) * bw, lane, s);
+        s.flags = jss_uniform(s.flags);
+        int raw;
+        bool ok = env_step<KJ, false>(p, iv, s, env, lane, (int)(pj & 255u), raw, hz);
+        s.flags = jss_uniform(s.flags);
+        while (ok && !__any_sync(JSS_FULL, (s.lb & LM) != 0u) && (s.flags & JSS_FLAG_NOOP_LEGAL)) {   // forced no-ops
+            ok = env_step<KJ, false>(p, iv, s, env, lane, J, raw, hz);
+            s.flags = jss_uniform(s.flags);
+        }
+        env_store<KJ>(iv, p.state + (size_t)off[b] * 4, lane, s);
+        env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
+        if (lane == 0) {
+            a.log_prob_out[env] = ok ? jss_key_f32((uint32_t)(k >> 32)) : JSS_F32_NAN;
+            a.parent_out[env] = (int)(pj >> 8);
+            a.job_out[env] = (int)(pj & 255u);
+        }
+    }
+    for (int b = nn + (int)threadIdx.x; b < W; b += (int)blockDim.x) {   // empty slots: their blocks left stale
+        a.log_prob_out[e0 + b] = -JSS_F32_INF;
+        a.parent_out[e0 + b] = -1;
+        a.job_out[e0 + b] = -1;
+    }
+    if (threadIdx.x == 0) a.bad_out[g] = bs.bad[0];
 }
 
 template <int KJ, int MODE>
@@ -2104,6 +2229,8 @@ constexpr int JSS_BEAM_SEARCH_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
 constexpr int JSS_SWOR_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
 constexpr int JSS_ORDER_LOG_PROB_MIN_CTAS[JSS_LANE_CLASSES] = {6, 4, 4, 2};
 constexpr int JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 1};
+// The beam round of jss_beam_step likewise (CUDA 12.9, sm_90a; DESIGN.md section 4).
+constexpr int JSS_BEAM_STEP_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
     return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
@@ -2116,6 +2243,7 @@ JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
          : mode == JSS_MODE_SWOR ? JSS_SWOR_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_ORDER_LOG_PROB ? JSS_ORDER_LOG_PROB_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_ORDER_LOG_PROB_GRAD ? JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_BEAM_STEP ? JSS_BEAM_STEP_MIN_CTAS[jss_lane_class(32 * KJ)]
          : 1;
 }
 
@@ -2149,6 +2277,25 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
             jss_iv_shape(iv);
             env_beam_search<KJ, MODE == JSS_MODE_SWOR>(p, a, iv, env, p.state + (size_t)t.off16 * 4, warp, lane,
                                                        reinterpret_cast<int *>(scratch), bsm);
+        }
+        return;
+    }
+    if (MODE == JSS_MODE_BEAM_STEP) {
+        // work item = one group record, CTA-strided; the per-warp regions are the observation staging (emission), and
+        // the beam region follows them
+        char *bsm = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;
+        int staged = -1;
+        for (int item = a.tile_begin + (int)blockIdx.x; item < a.tile_end; item += (int)gridDim.x) {
+            const int32_t *rec = a.beam_groups + (size_t)item * (a.beam_width + 2);
+            const int inst = jss_uniform(rec[1]);
+            if (inst != staged) {                        // CTA-uniform
+                __syncthreads();
+                jss_stage_instance(p, p.inst[inst], c, JSS_STAGE_OPS);
+                staged = inst;
+                __syncthreads();
+            }
+            jss_iv_shape(iv);
+            env_beam_step<KJ>(p, a, iv, rec, warp, lane, scratch, bsm);
         }
         return;
     }

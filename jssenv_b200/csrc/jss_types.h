@@ -175,7 +175,8 @@ struct JssLaunch {           // per-launch arguments
         int32_t greedy;      // steps from a row (a.logits): 0 categorical draw, 1 epsilon-greedy decode
         int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env; jss_order_log_prob (_grad):
                              // K, the orders per env
-        int32_t beam_width;  // jss_beam_search, jss_sample_without_replacement: W, the beams kept per env
+        int32_t beam_width;  // jss_beam_search, jss_sample_without_replacement: W, the beams kept per env;
+                             // jss_beam_step: W, the envs per group
     };
     int32_t coin_mode, n_steps, write_obs;   // jss_lookahead (_priority): n_steps is S, the work items each tile's
                                              // candidates are spread over (launch_all); jss_sample_episodes: the
@@ -205,6 +206,8 @@ struct JssLaunch {           // per-launch arguments
         const int32_t *actions;  // step; jss_sample_episodes_solution: the sample each env replays (< 0: none)
         const float *weights;    // jss_sample_episodes_grad: sample s of env i weighs weights[i * samples_ld + s]
         uint16_t *beam_trace;    // jss_beam_search with an order: per CTA, W backpointers per round (NULL: no order)
+        const int32_t *beam_groups;   // jss_beam_step: per group [group, instance, W block offsets in 16-byte units],
+                                      // grouped by lane class; a launch takes records [tile_begin, tile_end)
     };
     union {
         int32_t *actions_out;    // policy; jss_lookahead: env i's value of action a at actions_out + i * logits_ld + a
@@ -212,6 +215,7 @@ struct JssLaunch {           // per-launch arguments
                                  // makespan at actions_out + i * samples_ld + s
         int32_t *solution_out;   // jss_sample_episodes_solution: [N][jobs_max][machines_max] start times
                                  // (jss_beam_search: slot b's makespan at actions_out + i * samples_ld + b)
+        int32_t *parent_out;     // jss_beam_step: [N] each slot's parent slot
     };
     union {
         const uint8_t *env_mask; // reset / import
@@ -224,10 +228,13 @@ struct JssLaunch {           // per-launch arguments
     // each env's log-probability with respect to its table entries (may be NULL)
     // jss_beam_search: order_out is the [N][jobs_max][machines_max] order of each env's best slot (may be NULL), and
     // slot b's score goes to log_prob_out + i * samples_ld + b
+    // jss_beam_step: slot b of group g has score log_prob_out[g W + b] (read and written), parent parent_out, job
+    // job_out, and group g's bad-row bit goes to bad_out[g]
     union {
         float *traj_obs;
         float *grad_out;
         int32_t *order_out;
+        int32_t *job_out;
     };
     uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
     // jss_sample_without_replacement: slot b's score goes to log_prob_out and its key to key_out + i * samples_ld + b,
@@ -235,6 +242,7 @@ struct JssLaunch {           // per-launch arguments
     union {
         uint8_t *wire;       // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
         float *key_out;
+        int32_t *bad_out;
     };
     int32_t wire_stride;
     JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
@@ -276,5 +284,7 @@ struct JssLaunch {           // per-launch arguments
                                          // table, the envs untouched (jss_order_log_prob)
 #define JSS_MODE_ORDER_LOG_PROB_GRAD 18  // its weighted gradient, added into the caller's chunks
                                          // (jss_order_log_prob_grad)
+#define JSS_MODE_BEAM_STEP 19            // one beam-search round per group of W envs from per-beam logit rows, the
+                                         // children stepped into the group's envs (jss_beam_step)
 
 #define JSS_WARPS_PER_CTA 8

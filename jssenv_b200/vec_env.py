@@ -631,6 +631,42 @@ class JssVecEnv:
             out["order"] = ord_
         return out
 
+    def beam_step(self, logits, width: int, score, parent_out=None, action_out=None):
+        """One round of beam search for a policy that reads the observation at every decision (jss_beam_step, one
+        launch per lane class): the envs form groups of `width` consecutive envs, one search each, env g*width + b
+        holding slot b of group g; every env of a group must run the same instance.  `score` is the (N,) float32 device
+        tensor of the slots' scores, updated in place; a slot is live iff its score is finite (a search starts at
+        [0, -inf, ..., -inf] per group).  `logits` (N, >= J+1) gives each slot's row, taken as step_logits() takes it (a
+        tensor that requires grad is read detached); only a live, not-done slot's legal columns are read.  Every live,
+        not-done slot's legal jobs are candidates scored by its score plus the job's log-softmax over its legal columns
+        (as beam_search() computes it); the `width` best per group (score descending, then parent slot, then job) are
+        stepped into the group's slots, each then taking the no-op while no job is legal and the no-op is.  A group
+        without a live, not-done slot is left untouched.  No statistics, solution, auto-reset or RNG.  Returns
+        ``(parent, action, bad)``: int32 (N,) tensors of each slot's parent slot and job (-1 / -1 for an empty slot,
+        b / -1 in an untouched group; `parent_out` / `action_out` when given), and int32 (N / width,) bad, 1 where a
+        beam of the group met a bad row (NaN / +inf at a legal job, or all legal jobs -inf).  ObsBeamSearch
+        (jssenv_b200.beam) drives whole searches with it."""
+        import torch
+        n = self.num_envs
+        if not 1 <= int(width) <= N.MAX_BEAM_WIDTH or n % int(width):
+            raise ValueError(f"beam_step: width must be in 1..{N.MAX_BEAM_WIDTH} and divide {n}, got {width!r}")
+        width = int(width)
+        x, ld = self._logits_arg(logits.detach() if isinstance(logits, torch.Tensor) else logits, "beam_step")
+        if parent_out is None:
+            parent_out = torch.empty(n, dtype=torch.int32, device=self.device)
+        if action_out is None:
+            action_out = torch.empty(n, dtype=torch.int32, device=self.device)
+        for name, t, dt in (("score", score, torch.float32), ("parent_out", parent_out, torch.int32),
+                            ("action_out", action_out, torch.int32)):
+            if (not isinstance(t, torch.Tensor) or t.dtype != dt or tuple(t.shape) != (n,) or not t.is_contiguous()
+                    or t.device != x.device):
+                raise ValueError(f"beam_step: {name} must be a contiguous {dt} tensor of shape ({n},) on {x.device}")
+        bad = torch.empty(n // width, dtype=torch.int32, device=self.device)
+        rc = self._L.jss_beam_step(self._h, x.data_ptr(), int(ld), width, score.data_ptr(), parent_out.data_ptr(),
+                                   action_out.data_ptr(), bad.data_ptr(), self._stream())
+        N.check(self._h, rc, "jss_beam_step")
+        return parent_out, action_out, bad
+
     def sample_without_replacement(self, logits, k: int, order: bool = False):
         """Draw `k` distinct episodes per env without replacement from the logit table `logits` by stochastic beam
         search (Kool et al., 2019), each from the env's current state, in one launch per lane class
