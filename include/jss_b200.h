@@ -606,6 +606,33 @@ int jss_sample_without_replacement(jss_t *h, const float *logits_dev, int64_t ld
 int jss_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, float *score_dev, int32_t *parent_out_dev,
                   int32_t *action_out_dev, int32_t *bad_out_dev, void *stream);
 
+/* One round of stochastic beam search (Kool, van Hoof, Welling, ICML 2019) for a policy that reads the observation at
+ * every decision: the per-round form of jss_sample_without_replacement(), as jss_beam_step() is of jss_beam_search().
+ * Run over a whole search, each group's W slots end as W distinct episodes drawn without replacement from the policy.
+ *   Everything is as in jss_beam_step(): groups, live slots, rows, bad rows, the forced no-ops, untouched groups,
+ *     parent_out_dev / action_out_dev / bad_out_dev and what a written slot's state and rows equal.  On top of that:
+ *   Keys: key_dev, caller-owned fp32 [N], is read and written like score_dev (a search starts with key = [0, -inf, ...,
+ *     -inf] per group).  score_dev carries each slot's log-probability under the rows, key_dev its perturbed one.
+ *   Noise: group g hashes h = jss_hash3(seed, env_id_base / width + g, step_index), and candidate j of the beam in
+ *     slot b gets G_j = (score_b + logp_j) + g_j, g_j the Gumbel noise of h at index b * 256 + j.  With Z = max G,
+ *     the candidate at Z (lowest job on ties) gets key T_b, every other one min(T_b, T_b - max(v, 0) - log1p(e^-|v|)),
+ *     v = T_b - G_j + log(1 - e^(G_j - Z)): jss_sample_without_replacement()'s arithmetic in its order.  The W best
+ *     candidates by key (descending, then parent slot, then job) become the new slots, each with its score and key; an
+ *     empty slot gets -inf in both, a failed step NaN in the score.
+ *   Rows gathered from a table at each slot's todo, with step_index c + r in round r, give
+ *     jss_sample_without_replacement() of that table at counter c on a G-env batch with env_id_base / width bit for
+ *     bit (its log_prob is the score here).  Group ids make sharding free: shards with env_id_base = r * N equal the
+ *     unsharded batch.
+ *   Returns JSS_ERR_INVALID for everything jss_beam_step() rejects, a NULL or not 4-byte-aligned key_dev, and
+ *     env_id_base not a multiple of width; JSS_ERR_STATE before jss_assign().
+ * Measured on an H100 SXM 80 GB HBM3 at a 700 W power limit with a linear policy on real_obs in torch (median of three
+ * rounds): ta80 at G = 256, W = 16 from reset 269 ms per search (135 us per round, policy included) against 220 ms for
+ * jss_beam_step() and 190 ms for one jss_step_logits() per round on the same N*W envs; ta01 at G = 4 096, W = 8 41.1
+ * against 35.1 and 29.4 ms (DESIGN.md section 4). */
+int jss_stochastic_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, uint64_t seed,
+                             uint64_t step_index, float *score_dev, float *key_dev, int32_t *parent_out_dev,
+                             int32_t *action_out_dev, int32_t *bad_out_dev, void *stream);
+
 /* The teacher-forced log-likelihood of k given operation orders per env under a caller's logit table, each from the
  * env's current state, in one launch per lane class present, leaving the envs untouched.
  *   order_dev: device int32 [N][k][jobs_max][machines_max].  Order s of env i stands for the episode that

@@ -81,6 +81,7 @@ SIGNATURES = {
     "jss_sample_without_replacement": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int, _VP, _VP,
                                                _VP, c_int64, _VP, _VP]),
     "jss_beam_step": (c_int, [_VP, _VP, c_int64, c_int, _VP, _VP, _VP, _VP, _VP]),
+    "jss_stochastic_beam_step": (c_int, [_VP, _VP, c_int64, c_int, c_uint64, c_uint64, _VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_order_log_prob": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, _VP, c_int64, _VP]),
     "jss_order_log_prob_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, c_int64, c_int, _VP,
                                         _VP]),

@@ -1149,20 +1149,20 @@ namespace {
 // jss_beam_step's group records for width W, built once per handle and width: per group [g, instance, the W slots'
 // block offsets in 16-byte units] (blocks are in tile order, and a group need not align with tiles), grouped by lane
 // class and, within one, by instance, so that a CTA restages the instance tables rarely.  Leaves `out` null with the
-// reason in the handle's error if the width does not divide N or a group mixes instances.
-int beam_groups(jss_t *h, int W, const jss_handle::BeamGroups *&out) {
+// reason in the handle's error (after `who`) if the width does not divide N or a group mixes instances.
+int beam_groups(jss_t *h, const char *who, int W, const jss_handle::BeamGroups *&out) {
     out = nullptr;
     auto it = h->beam_groups.find(W);
     if (it == h->beam_groups.end()) {
         jss_handle::BeamGroups bg;
         const int N = h->n_envs, G = N / W;
         if (N % W) {
-            bg.err = "jss_beam_step: width " + std::to_string(W) + " does not divide the " + std::to_string(N) + " envs";
+            bg.err = "width " + std::to_string(W) + " does not divide the " + std::to_string(N) + " envs";
         } else {
             for (int g = 0; g < G && bg.err.empty(); g++)
                 for (int b = 1; b < W; b++)
                     if (h->env_inst[g * W + b] != h->env_inst[g * W]) {
-                        bg.err = "jss_beam_step: group " + std::to_string(g) + " (envs " + std::to_string(g * W) + " .. " +
+                        bg.err = "group " + std::to_string(g) + " (envs " + std::to_string(g * W) + " .. " +
                                  std::to_string(g * W + W - 1) + ") mixes instances";
                         break;
                     }
@@ -1191,7 +1191,7 @@ int beam_groups(jss_t *h, int W, const jss_handle::BeamGroups *&out) {
         }
         it = h->beam_groups.emplace(W, bg).first;
     }
-    if (!it->second.err.empty()) return fail(h, JSS_ERR_INVALID, "%s", it->second.err.c_str());
+    if (!it->second.err.empty()) return fail(h, JSS_ERR_INVALID, "%s: %s", who, it->second.err.c_str());
     out = &it->second;
     return JSS_OK;
 }
@@ -1204,25 +1204,29 @@ JssSmemLayout beam_step_layout(const jss_t *h) {
     return sl;
 }
 
-}  // namespace
-
-int jss_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, float *score_dev, int32_t *parent_out_dev,
-                  int32_t *action_out_dev, int32_t *bad_out_dev, void *stream) {
-    int rc = check_ready(h, stream);
-    if (rc) return rc;
+// jss_beam_step and jss_stochastic_beam_step (key_dev non-NULL): the checks, the group records and one launch per lane
+// class present
+int beam_step_launch(jss_t *h, const char *who, const float *logits_dev, int64_t ld, int width, uint64_t seed,
+                     uint64_t step_index, float *score_dev, float *key_dev, int32_t *parent_out_dev,
+                     int32_t *action_out_dev, int32_t *bad_out_dev, void *stream) {
+    const bool swor = key_dev != nullptr;
     if (bad_ptr(logits_dev) || bad_ptr(score_dev) || bad_ptr(parent_out_dev) || bad_ptr(action_out_dev) ||
         bad_ptr(bad_out_dev) || width < 1 || width > JSS_MAX_BEAM_WIDTH || ld < (int64_t)h->p.jobs_max + 1)
-        return fail(h, JSS_ERR_INVALID, "jss_beam_step: bad arguments (logits %p, score %p, parent_out %p, action_out "
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (logits %p, score %p, parent_out %p, action_out "
                     "%p and bad_out %p must be non-NULL and 4-byte aligned, 1 <= width %d <= %d, ld %lld >= jobs_max + 1 "
-                    "= %d)", (const void *)logits_dev, (void *)score_dev, (void *)parent_out_dev,
+                    "= %d)", who, (const void *)logits_dev, (void *)score_dev, (void *)parent_out_dev,
                     (void *)action_out_dev, (void *)bad_out_dev, width, JSS_MAX_BEAM_WIDTH, (long long)ld,
                     h->p.jobs_max + 1);
+    if (swor && h->env_id_base % (uint64_t)width)
+        return fail(h, JSS_ERR_INVALID, "%s: env_id_base %llu is not a multiple of width %d (group ids are "
+                    "env_id_base / width + g)", who, (unsigned long long)h->env_id_base, width);
+    int rc;
     const jss_handle::BeamGroups *bg = nullptr;
-    if ((rc = beam_groups(h, width, bg))) return rc;
+    if ((rc = beam_groups(h, who, width, bg))) return rc;
     const cudaStream_t st = (cudaStream_t)stream;
     if ((rc = refresh_obs(h, st))) return rc;            // the untouched rows must be current, as after any call
     JssLaunch a{};
-    a.mode = JSS_MODE_BEAM_STEP;
+    a.mode = swor ? JSS_MODE_STOCHASTIC_BEAM_STEP : JSS_MODE_BEAM_STEP;
     a.stage = JSS_STAGE_OPS;
     a.beam_width = width;
     a.beam_groups = bg->dev;
@@ -1232,16 +1236,21 @@ int jss_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, floa
     a.parent_out = parent_out_dev;
     a.job_out = action_out_dev;
     a.bad_out = bad_out_dev;
+    if (swor) {
+        a.key_io = key_dev;
+        a.hash_key = jss_fold32(seed);                   // jss_hash3 reads the seed only through its fold
+        a.sample_step_index = step_index;
+    }
     if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
     const JssSmemLayout sl = beam_step_layout(h);
     const size_t smem = smem_bytes(sl) + jss_beam_smem(nullptr, width, jss_block_geom(h->p.jobs_max, h->p.machines_max).words,
-                                                       nullptr, false, 1);
+                                                       nullptr, swor, 1);
     for (int c = 0; c < JSS_LANE_CLASSES; c++) {         // one launch per lane class present
         a.tile_begin = bg->ranges[c][0];
         a.tile_end = bg->ranges[c][1];
         const int n_groups = a.tile_end - a.tile_begin;
         if (n_groups <= 0) continue;
-        const JssKernel k = env_kernels<JSS_MODE_BEAM_STEP>[c];
+        const JssKernel k = swor ? env_kernels<JSS_MODE_STOCHASTIC_BEAM_STEP>[c] : env_kernels<JSS_MODE_BEAM_STEP>[c];
         int per_sm = 0;
         if ((rc = ctas_per_sm(h, k, smem, per_sm))) return rc;
         JSS_LAUNCH(k, std::min(n_groups, h->sm_count * per_sm), JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
@@ -1249,6 +1258,28 @@ int jss_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, floa
         h->launches += 1;
     }
     return JSS_OK;
+}
+
+}  // namespace
+
+int jss_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, float *score_dev, int32_t *parent_out_dev,
+                  int32_t *action_out_dev, int32_t *bad_out_dev, void *stream) {
+    const int rc = check_ready(h, stream);
+    if (rc) return rc;
+    return beam_step_launch(h, "jss_beam_step", logits_dev, ld, width, 0, 0, score_dev, nullptr, parent_out_dev,
+                            action_out_dev, bad_out_dev, stream);
+}
+
+int jss_stochastic_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int width, uint64_t seed,
+                             uint64_t step_index, float *score_dev, float *key_dev, int32_t *parent_out_dev,
+                             int32_t *action_out_dev, int32_t *bad_out_dev, void *stream) {
+    const int rc = check_ready(h, stream);
+    if (rc) return rc;
+    if (bad_ptr(key_dev))
+        return fail(h, JSS_ERR_INVALID, "jss_stochastic_beam_step: bad arguments (key %p must be non-NULL and 4-byte "
+                    "aligned)", (void *)key_dev);
+    return beam_step_launch(h, "jss_stochastic_beam_step", logits_dev, ld, width, seed, step_index, score_dev, key_dev,
+                            parent_out_dev, action_out_dev, bad_out_dev, stream);
 }
 
 namespace {

@@ -2021,7 +2021,12 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
 //      job is legal and the no-op is, and writes the slot's block, its observation, mask and scalar record whole (the
 //      raw reward of its last step) and its score, parent and job; slots nn .. W-1 get -inf, -1, -1.
 // Every step is env_step<KJ, false>: no statistics, solution, auto-reset or RNG.
-template <int KJ>
+// SWOR (jss_stochastic_beam_step): the round of env_beam_search<KJ, true>.  Each slot also carries a key T (a.key_io,
+// read with the scores); candidate j of the beam in slot b gets G_j, Z and its key exactly as there, with the noise
+// jss_hash_env(h, b * 256 + j), h = jss_hash3(seed, env_id_base / W + g, step_index) (the group's global id); the
+// selection ranks the keys, and a kept child's score comes with the selection (bs.score[W ..]), its key from it.  The
+// per-candidate key stays inline here as in env_beam_search: shared, it changed that kernel's register assignment.
+template <int KJ, bool SWOR>
 JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstView &iv, const int32_t *rec, int warp,
                            int lane, float *scratch, char *bsm) {
     constexpr uint32_t LM = jss_legal_mask<KJ>();
@@ -2031,10 +2036,13 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
     const uint32_t *off = reinterpret_cast<const uint32_t *>(rec + 2);
     int *hz = reinterpret_cast<int *>(scratch);
     JssBeamSmem bs;
-    jss_beam_smem(bsm, W, bw, &bs, false, 1);
+    jss_beam_smem(bsm, W, bw, &bs, SWOR, 1);
     const auto live = [](float x) { return x > -JSS_F32_INF && x < JSS_F32_INF; };
     __syncthreads();                                     // the previous group's last reads of the region are done
-    for (int b = (int)threadIdx.x; b < W; b += (int)blockDim.x) bs.score[b] = a.log_prob_out[e0 + b];
+    for (int b = (int)threadIdx.x; b < W; b += (int)blockDim.x) {
+        bs.score[b] = a.log_prob_out[e0 + b];
+        if (SWOR) bs.key[b] = a.key_io[e0 + b];
+    }
     if (threadIdx.x == 0) bs.bad[0] = 0;
     __syncthreads();
     for (int k = (int)threadIdx.x; k < W * (nw / 4); k += (int)blockDim.x) {   // 0. the live slots' blocks
@@ -2053,6 +2061,8 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
         return;
     }
     EnvRegs<KJ> s;
+    const uint32_t hr = SWOR ? jss_hash_env(jss_hash_key_folded(a.hash_key, a.sample_step_index),
+                                            p.env_id_base / (uint64_t)W + (uint64_t)g) : 0u;
     for (int b = warp; b < W; b += JSS_WARPS_PER_CTA) {   // 1. expand
         const float sc = bs.score[b];
         int taken = 0;
@@ -2070,8 +2080,33 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
                         key[i] = ((s.lb >> i) & 1u) && cs > -JSS_F32_INF ? jss_f32_key(cs + 0.0f) : 0u;
                         nc += key[i] != 0u;
                     }
+                    if (SWOR) {                          // the perturbed values G, Z and the keys in their place
+                        const float T = bs.key[b];
+                        float gv[KJ];
+                        uint32_t zk = 0u;
+                        int zj = 1 << 20;
+#pragma unroll
+                        for (int i = 0; i < KJ; i++) {
+                            gv[i] = (sc + lp[i]) + jss_gumbel(jss_hash_env(hr, (uint64_t)(b * 256 + KJ * lane + i)));
+                            const uint32_t k = jss_f32_key(gv[i] + 0.0f);
+                            if (key[i] != 0u && k > zk) { zk = k; zj = KJ * lane + i; }
+                        }
+                        const uint32_t zbest = __reduce_max_sync(JSS_FULL, zk);
+                        zj = (int)__reduce_min_sync(JSS_FULL, (unsigned)(zk == zbest ? zj : 1 << 20));
+                        const float Z = jss_key_f32(zbest);
+#pragma unroll
+                        for (int i = 0; i < KJ; i++) {
+                            if (key[i] == 0u) continue;
+                            float kv = T;
+                            if (KJ * lane + i != zj) {
+                                const float v = T - gv[i] + jss_log1mexp(gv[i] - Z);
+                                kv = fminf(T, T - fmaxf(v, 0.0f) - log1pf(expf(-fabsf(v))));
+                            }
+                            key[i] = jss_f32_key(kv + 0.0f);
+                        }
+                    }
                     taken = min(W, (int)__reduce_add_sync(JSS_FULL, (unsigned)nc));
-                    jss_beam_passes<KJ, false>(bs, key, lp, sc, b, W, lane, taken);
+                    jss_beam_passes<KJ, SWOR>(bs, key, lp, sc, b, W, lane, taken);
                 } else if (lane == 0) {
                     bs.bad[0] = 1;
                 }
@@ -2080,7 +2115,7 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
         if (lane == 0) bs.cnt[b] = taken;
     }
     __syncthreads();
-    const int nn = min(W, jss_beam_rank<false>(bs, W, W, 0));   // 2. select
+    const int nn = min(W, jss_beam_rank<SWOR>(bs, W, W, 0));   // 2. select (SWOR: the scores to bs.score[W ..])
     __syncthreads();
     for (int b = warp; b < nn; b += JSS_WARPS_PER_CTA) {   // 3. step the kept children into their slots
         const int env = e0 + b;
@@ -2098,13 +2133,19 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
         env_store<KJ>(iv, p.state + (size_t)off[b] * 4, lane, s);
         env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
         if (lane == 0) {
-            a.log_prob_out[env] = ok ? jss_key_f32((uint32_t)(k >> 32)) : JSS_F32_NAN;
+            if (SWOR) {                                  // the score came with the selection
+                a.log_prob_out[env] = ok ? bs.score[W + b] : JSS_F32_NAN;
+                a.key_io[env] = jss_key_f32((uint32_t)(k >> 32));
+            } else {
+                a.log_prob_out[env] = ok ? jss_key_f32((uint32_t)(k >> 32)) : JSS_F32_NAN;
+            }
             a.parent_out[env] = (int)(pj >> 8);
             a.job_out[env] = (int)(pj & 255u);
         }
     }
     for (int b = nn + (int)threadIdx.x; b < W; b += (int)blockDim.x) {   // empty slots: their blocks left stale
         a.log_prob_out[e0 + b] = -JSS_F32_INF;
+        if (SWOR) a.key_io[e0 + b] = -JSS_F32_INF;
         a.parent_out[e0 + b] = -1;
         a.job_out[e0 + b] = -1;
     }
@@ -2229,8 +2270,9 @@ constexpr int JSS_BEAM_SEARCH_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
 constexpr int JSS_SWOR_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
 constexpr int JSS_ORDER_LOG_PROB_MIN_CTAS[JSS_LANE_CLASSES] = {6, 4, 4, 2};
 constexpr int JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 1};
-// The beam round of jss_beam_step likewise (CUDA 12.9, sm_90a; DESIGN.md section 4).
+// The beam round of jss_beam_step likewise (CUDA 12.9, sm_90a; DESIGN.md section 4), and its stochastic form.
 constexpr int JSS_BEAM_STEP_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
+constexpr int JSS_STOCHASTIC_BEAM_STEP_MIN_CTAS[JSS_LANE_CLASSES] = {3, 3, 2, 1};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
     return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
@@ -2244,6 +2286,7 @@ JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
          : mode == JSS_MODE_ORDER_LOG_PROB ? JSS_ORDER_LOG_PROB_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_ORDER_LOG_PROB_GRAD ? JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_BEAM_STEP ? JSS_BEAM_STEP_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_STOCHASTIC_BEAM_STEP ? JSS_STOCHASTIC_BEAM_STEP_MIN_CTAS[jss_lane_class(32 * KJ)]
          : 1;
 }
 
@@ -2280,7 +2323,7 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
         }
         return;
     }
-    if (MODE == JSS_MODE_BEAM_STEP) {
+    if (MODE == JSS_MODE_BEAM_STEP || MODE == JSS_MODE_STOCHASTIC_BEAM_STEP) {
         // work item = one group record, CTA-strided; the per-warp regions are the observation staging (emission), and
         // the beam region follows them
         char *bsm = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;
@@ -2295,7 +2338,7 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
                 __syncthreads();
             }
             jss_iv_shape(iv);
-            env_beam_step<KJ>(p, a, iv, rec, warp, lane, scratch, bsm);
+            env_beam_step<KJ, MODE == JSS_MODE_STOCHASTIC_BEAM_STEP>(p, a, iv, rec, warp, lane, scratch, bsm);
         }
         return;
     }

@@ -176,7 +176,7 @@ struct JssLaunch {           // per-launch arguments
         int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env; jss_order_log_prob (_grad):
                              // K, the orders per env
         int32_t beam_width;  // jss_beam_search, jss_sample_without_replacement: W, the beams kept per env;
-                             // jss_beam_step: W, the envs per group
+                             // jss_beam_step, jss_stochastic_beam_step: W, the envs per group
     };
     int32_t coin_mode, n_steps, write_obs;   // jss_lookahead (_priority): n_steps is S, the work items each tile's
                                              // candidates are spread over (launch_all); jss_sample_episodes: the
@@ -197,6 +197,7 @@ struct JssLaunch {           // per-launch arguments
     union {
         double cr_factor;    // CriticalRatio due_date_factor (dispatching.py:337-349); reference default 1.5
         uint64_t sample_step_index;   // jss_rollout_priority_sample: the RNG counter of the env's first decision
+                                      // (jss_stochastic_beam_step: of the round)
         int64_t values_ld;   // jss_lookahead_priority: env i's value of action a at actions_out + i * values_ld + a
                              // (logits_ld is the table's env stride there)
         const int32_t *order_in;   // jss_order_log_prob (_grad): order s of env i at order_in + (i * n_samples + s) *
@@ -236,7 +237,12 @@ struct JssLaunch {           // per-launch arguments
         int32_t *order_out;
         int32_t *job_out;
     };
-    uint8_t *traj_mask; int32_t *traj_scalars; int32_t *traj_actions;
+    // jss_stochastic_beam_step: as jss_beam_step, and slot b of group g has key key_io[g W + b] (read and written)
+    union {
+        uint8_t *traj_mask;
+        float *key_io;
+    };
+    int32_t *traj_scalars; int32_t *traj_actions;
     // jss_sample_without_replacement: slot b's score goes to log_prob_out and its key to key_out + i * samples_ld + b,
     // and order_out is the [N][W][jobs_max][machines_max] order of every slot (may be NULL)
     union {
@@ -286,5 +292,7 @@ struct JssLaunch {           // per-launch arguments
                                          // (jss_order_log_prob_grad)
 #define JSS_MODE_BEAM_STEP 19            // one beam-search round per group of W envs from per-beam logit rows, the
                                          // children stepped into the group's envs (jss_beam_step)
+#define JSS_MODE_STOCHASTIC_BEAM_STEP 20 // the same perturbed by top-down Gumbel noise, the beams ranked by key
+                                         // (jss_stochastic_beam_step)
 
 #define JSS_WARPS_PER_CTA 8

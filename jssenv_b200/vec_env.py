@@ -646,25 +646,50 @@ class JssVecEnv:
         b / -1 in an untouched group; `parent_out` / `action_out` when given), and int32 (N / width,) bad, 1 where a
         beam of the group met a bad row (NaN / +inf at a legal job, or all legal jobs -inf).  ObsBeamSearch
         (jssenv_b200.beam) drives whole searches with it."""
+        return self._beam_step("beam_step", logits, width, score, None, None, parent_out, action_out)
+
+    def stochastic_beam_step(self, logits, width: int, score, key, step_index: int, parent_out=None, action_out=None):
+        """One round of stochastic beam search (Kool et al., 2019) for a policy that reads the observation at every
+        decision (jss_stochastic_beam_step, one launch per lane class): beam_step() with each candidate's score
+        perturbed by top-down Gumbel noise and the `width` best per group ranked by that perturbed log-probability, the
+        key.  `key` is the (N,) float32 device tensor of the slots' keys, updated in place like `score` (a search starts
+        at key [0, -inf, ..., -inf] per group); `score` stays each slot's log-probability under its rows.  The noise of
+        group g is drawn from ``self.seed``, the group's global id env_id_base / width + g (env_id_base must be a
+        multiple of width) and the explicit RNG counter `step_index`, one per round; the env's own counter does not
+        move.  Over a whole search (ObsBeamSearch(stochastic=True)) the slots of a group are distinct episodes drawn
+        without replacement from the policy.  Returns ``(parent, action, bad)`` as beam_step()."""
+        return self._beam_step("stochastic_beam_step", logits, width, score, key, int(step_index), parent_out,
+                               action_out)
+
+    def _beam_step(self, who, logits, width, score, key, step_index, parent_out, action_out):
+        """The checked native call of beam_step (key None) and stochastic_beam_step."""
         import torch
         n = self.num_envs
         if not 1 <= int(width) <= N.MAX_BEAM_WIDTH or n % int(width):
-            raise ValueError(f"beam_step: width must be in 1..{N.MAX_BEAM_WIDTH} and divide {n}, got {width!r}")
+            raise ValueError(f"{who}: width must be in 1..{N.MAX_BEAM_WIDTH} and divide {n}, got {width!r}")
         width = int(width)
-        x, ld = self._logits_arg(logits.detach() if isinstance(logits, torch.Tensor) else logits, "beam_step")
+        if key is not None and self.env_id_base % width:
+            raise ValueError(f"{who}: env_id_base {self.env_id_base} must be a multiple of width {width}")
+        x, ld = self._logits_arg(logits.detach() if isinstance(logits, torch.Tensor) else logits, who)
         if parent_out is None:
             parent_out = torch.empty(n, dtype=torch.int32, device=self.device)
         if action_out is None:
             action_out = torch.empty(n, dtype=torch.int32, device=self.device)
-        for name, t, dt in (("score", score, torch.float32), ("parent_out", parent_out, torch.int32),
-                            ("action_out", action_out, torch.int32)):
+        bufs = (("score", score, torch.float32),) + ((("key", key, torch.float32),) if key is not None else ()) + (
+            ("parent_out", parent_out, torch.int32), ("action_out", action_out, torch.int32))
+        for name, t, dt in bufs:
             if (not isinstance(t, torch.Tensor) or t.dtype != dt or tuple(t.shape) != (n,) or not t.is_contiguous()
                     or t.device != x.device):
-                raise ValueError(f"beam_step: {name} must be a contiguous {dt} tensor of shape ({n},) on {x.device}")
+                raise ValueError(f"{who}: {name} must be a contiguous {dt} tensor of shape ({n},) on {x.device}")
         bad = torch.empty(n // width, dtype=torch.int32, device=self.device)
-        rc = self._L.jss_beam_step(self._h, x.data_ptr(), int(ld), width, score.data_ptr(), parent_out.data_ptr(),
-                                   action_out.data_ptr(), bad.data_ptr(), self._stream())
-        N.check(self._h, rc, "jss_beam_step")
+        if key is None:
+            rc = self._L.jss_beam_step(self._h, x.data_ptr(), int(ld), width, score.data_ptr(), parent_out.data_ptr(),
+                                       action_out.data_ptr(), bad.data_ptr(), self._stream())
+        else:
+            rc = self._L.jss_stochastic_beam_step(self._h, x.data_ptr(), int(ld), width, self.seed, step_index,
+                                                  score.data_ptr(), key.data_ptr(), parent_out.data_ptr(),
+                                                  action_out.data_ptr(), bad.data_ptr(), self._stream())
+        N.check(self._h, rc, "jss_" + who)
         return parent_out, action_out, bad
 
     def sample_without_replacement(self, logits, k: int, order: bool = False):
