@@ -659,6 +659,45 @@ int jss_order_log_prob_grad(jss_t *h, const float *logits_dev, int64_t ld_env, i
                             const int32_t *order_dev, int64_t k, const float *weights_dev, int64_t ld, int split,
                             float *grad_out_dev, void *stream);
 
+/* Local search on given operation orders: each of the k orders per env improved by steepest descent on the critical
+ * path (the N1 neighbourhood of van Laarhoven, Aarts and Lenstra, 1992: swaps of two adjacent operations of a critical
+ * machine block), each from the env's current state, in one launch per lane class present, leaving the envs untouched.
+ * No RNG, no logit table.  For each env i and order s (order_dev: device int32 [N][k][jobs_max][machines_max]):
+ *   1. Replay: order O stands for the episode jss_order_log_prob() / jss_rollout_priority(-O) runs from env i's state:
+ *      the legal job whose current operation has the smallest entry (compared as fp32 of -entry), ties to the lowest
+ *      job, the no-op only when no job is legal; at most 2*J_i*M_i + 1 decisions.  The replay records for each
+ *      operation it allocates its round (0, 1, ... counting job allocations only) and its start time.
+ *   2. Canonical order: R(O)[j][k] is the round of operation (j, k), -1 for operations started before the call.
+ *      Replaying R(O) reproduces the episode exactly.  The descent starts from R(O).
+ *   3. Chain, on the current canonical schedule, over the in-call operations only (end = start + duration): start at
+ *      the operation that ends at the makespan (the largest round if several; none: the chain is empty).  At operation
+ *      o with start s, let p_m be the operation on o's machine with the largest round below o's and p_j o's job
+ *      predecessor if it is in call.  If p_m ends at s, record the pair (p_m, o) and step to p_m; else if p_j ends at s,
+ *      step to p_j; else stop.  Neighbour c is the c-th recorded pair, counted from the makespan end.
+ *   4. Neighbour of pair (u, v): R with the entries of u and v swapped, valued by the makespan of its replay.
+ *   5. Move: the neighbour of smallest makespan (lowest c on ties), accepted only if strictly below the current
+ *      makespan; the current order becomes its canonical order.  Stops at a local optimum or after max_moves moves.
+ *   Outputs (device int32, row stride ld >= k, 64-bit index arithmetic): makespan_out_dev[i*ld + s] the final makespan,
+ *     start_makespan_out_dev[i*ld + s] the input's, moves_out_dev[i*ld + s] the accepted moves, and
+ *     order_out_dev[i][s][j][k] the final canonical order in jss_beam_search()'s format (entries past J_i / M_i are not
+ *     written).  An env done at entry, and an input whose replay does not end done (an imported state that errs, or
+ *     nothing legal), read -1 / -1 / 0 and -1 in every order entry; a neighbour whose replay does not end done is never
+ *     accepted.  order_out_dev may equal order_dev (in place); no other two buffers may overlap.
+ *   No side effects: those of jss_lookahead().  The call reads only the state blocks and neither needs nor triggers
+ *     jss_refresh_obs().  The results do not depend on the grid, the batch order or sharding.
+ *   Returns JSS_ERR_INVALID for a NULL or not 4-byte-aligned pointer, k < 1, ld < k, max_moves < 0 or an overlap other
+ *     than in place; JSS_ERR_UNSUPPORTED for k >= 2^31; JSS_ERR_STATE before jss_assign().
+ * Memory: one CTA per (env, order), with the canonical order, its start times and the chain's pairs in shared memory
+ * (24 KB for ta80, 96 KB for 256 x 32).  Bytes per neighbour decision: none beyond the state block loaded once per
+ * neighbour (L2) and the shared-memory tables.  Measured on an H100 SXM 80 GB HBM3 at a 700 W power limit (per-env
+ * random tables, at most 3 moves, median of three rounds): ta80 at N = 256 from the best beam_search(W = 16) order
+ * 167.9 ms per call against 1 330 ms for the host loop of canonical replay, start-time replay, chain walk and
+ * jss_order_log_prob() on the padded neighbours per move; ta80 at N = 256, k = 16 1 919 against 19 962 ms; ta01 at
+ * N = 4 096 16.3 against 1 276 ms (DESIGN.md section 4). */
+int jss_improve_orders(jss_t *h, const int32_t *order_dev, int64_t k, int max_moves, int32_t *order_out_dev,
+                       int32_t *makespan_out_dev, int32_t *start_makespan_out_dev, int32_t *moves_out_dev, int64_t ld,
+                       void *stream);
+
 /* Host-buffer form of step(): copies actions H2D, steps, copies the results D2H with
  * contiguous DMA, synchronises.  Any output pointer may be NULL.  Host layouts equal the
  * device layouts: mask_host [N][mask_stride] bytes (row i: bytes 0..J_i), obs_host

@@ -85,6 +85,7 @@ SIGNATURES = {
     "jss_order_log_prob": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, _VP, c_int64, _VP]),
     "jss_order_log_prob_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, c_int64, c_int, _VP,
                                         _VP]),
+    "jss_improve_orders": (c_int, [_VP, _VP, c_int64, c_int, _VP, _VP, _VP, _VP, c_int64, _VP]),
     "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_step_begin": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_wait": (c_int, [_VP, c_int]),

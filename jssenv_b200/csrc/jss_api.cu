@@ -1343,6 +1343,63 @@ int jss_order_log_prob_grad(jss_t *h, const float *logits_dev, int64_t ld_env, i
     return launch_all(h, a, (cudaStream_t)stream);
 }
 
+int jss_improve_orders(jss_t *h, const int32_t *order_dev, int64_t k, int max_moves, int32_t *order_out_dev,
+                       int32_t *makespan_out_dev, int32_t *start_makespan_out_dev, int32_t *moves_out_dev, int64_t ld,
+                       void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    const char *who = "jss_improve_orders";
+    if (bad_ptr(order_dev) || bad_ptr(order_out_dev) || bad_ptr(makespan_out_dev) || bad_ptr(start_makespan_out_dev) ||
+        bad_ptr(moves_out_dev) || k < 1 || ld < k || max_moves < 0)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (order %p, order_out %p, makespan_out %p, start_makespan_out "
+                    "%p and moves_out %p must be non-NULL and 4-byte aligned, k %lld >= 1, ld %lld >= k, max_moves %d "
+                    ">= 0)", who, (const void *)order_dev, (void *)order_out_dev, (void *)makespan_out_dev,
+                    (void *)start_makespan_out_dev, (void *)moves_out_dev, (long long)k, (long long)ld, max_moves);
+    if (k > INT32_MAX)
+        return fail(h, JSS_ERR_UNSUPPORTED, "%s: k must stay below 2^31", who);
+    // the byte ranges the call reads or writes; only order_out == order may share one
+    const uint64_t N = (uint64_t)h->n_envs, ords = N * (uint64_t)k * h->p.jobs_max * h->p.machines_max * 4,
+                   rows = ((N - 1) * (uint64_t)ld + (uint64_t)k) * 4;
+    const struct { const void *p; uint64_t bytes; } span[5] = {{order_dev, ords}, {order_out_dev, ords},
+        {makespan_out_dev, rows}, {start_makespan_out_dev, rows}, {moves_out_dev, rows}};
+    for (int x = 0; x < 5; x++)
+        for (int y = x + 1; y < 5; y++) {
+            const uintptr_t px = (uintptr_t)span[x].p, py = (uintptr_t)span[y].p;
+            if (x == 0 && y == 1 && px == py) continue;  // in place
+            if (px < py + span[y].bytes && py < px + span[x].bytes)
+                return fail(h, JSS_ERR_INVALID, "%s: bad arguments (buffers %d and %d overlap; only order_out == order "
+                            "may)", who, x, y);
+        }
+    JssLaunch a{};
+    a.mode = JSS_MODE_IMPROVE_ORDERS;
+    a.stage = JSS_STAGE_OPS;
+    a.order_in = order_dev;
+    a.n_samples = (int)k;
+    a.samples_ld = ld;
+    a.n_steps = max_moves;
+    a.order_out = order_out_dev;
+    a.actions_out = makespan_out_dev;
+    a.start_out = start_makespan_out_dev;
+    a.moves_out = moves_out_dev;
+    if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
+    const JssSmemLayout sl = beam_layout(h);
+    const size_t smem = smem_bytes(sl) + jss_improve_smem(nullptr, h->p.jobs_max, h->p.machines_max, nullptr);
+    for (int c = 0; c < JSS_LANE_CLASSES; c++) {         // one launch per lane class present
+        a.tile_begin = h->class_tiles[c][0];
+        a.tile_end = h->class_tiles[c][1];
+        const int64_t n_items = (int64_t)(a.tile_end - a.tile_begin) * JSS_WARPS_PER_CTA * k;
+        if (n_items <= 0) continue;
+        const JssKernel kern = env_kernels<JSS_MODE_IMPROVE_ORDERS>[c];
+        int per_sm = 0;
+        if ((rc = ctas_per_sm(h, kern, smem, per_sm))) return rc;
+        const int grid = (int)std::min<int64_t>(n_items, (int64_t)h->sm_count * per_sm);
+        JSS_LAUNCH(kern, grid, JSS_WARPS_PER_CTA * 32, smem, (cudaStream_t)stream, h->p, a, sl);
+        JSS_CUDA(h, cudaGetLastError());
+        h->launches += 1;
+    }
+    return JSS_OK;
+}
+
 int jss_step_host(jss_t *h, const int32_t *actions_host, uint8_t *mask_host, float *obs_host,
                   int32_t *scalars_host, void *stream) {
     int rc = check_ready(h, stream);

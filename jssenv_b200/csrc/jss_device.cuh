@@ -1552,9 +1552,11 @@ JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, i
 // and the order's log-probability agree bit for bit), and each owned slot's p_i = exp(lp_i) (0 for a job that is not
 // legal).  Returns as env_priority_sample_action does: the no-op, logp and p left 0, when no job is legal and it is;
 // JSS_INF for a bad table row; JSS_ACTION_SKIP when nothing is legal.
-template <int KJ>
+// SWAP (jss_improve_orders): the entries at ord index sw.x and sw.y read as sw.z and sw.w (an index < 0 matches
+// nothing), and the decision is returned without reading a table (logp and p stay 0).
+template <int KJ, bool SWAP = false>
 JSS_DEV int env_order_action(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
-                             const int32_t *ord, int mstride, float &logp, float (&pr)[KJ]) {
+                             const int32_t *ord, int mstride, float &logp, float (&pr)[KJ], int4 sw = int4()) {
     constexpr uint32_t LM = jss_legal_mask<KJ>();
     logp = 0.0f;
 #pragma unroll
@@ -1563,8 +1565,13 @@ JSS_DEV int env_order_action(const JssLaunch &a, const InstView &iv, const EnvRe
         return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
     int act = JSS_INF;
     env_legal_argmax<KJ>(s, lane, jss_J(iv), false, [&](int i, int j) {
+        if constexpr (SWAP) {
+            const int q = j * mstride + jss_sel<KJ>(s.todo, i);
+            return -(float)(q == sw.x ? sw.z : q == sw.y ? sw.w : ord[q]);
+        }
         return -(float)ord[(size_t)j * mstride + jss_sel<KJ>(s.todo, i)];
     }, act);
+    if (SWAP) return act;
     float lp[KJ];
     if (!env_table_logp<KJ>(a, s, env, lane, lp)) return JSS_INF;
     float la = 0.0f;
@@ -2152,6 +2159,173 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
     if (threadIdx.x == 0) a.bad_out[g] = bs.bad[0];
 }
 
+// ---- critical-path descent on operation orders, the envs untouched (jss_improve_orders) ---------------------------
+// The improvement region of the CTA's shared memory for the batch maxima jmax x mmax (row stride mmax throughout):
+// [ord: jmax][mmax] i32 | [start: jmax][mmax] i32 | [pairs: jmax * mmax] u32 | [best: 8] u64 | [ctl: 4] i32.  ord is
+// the current canonical order, start its operations' start times, pairs the chain's (u << 16 | v) operation pairs,
+// best each warp's best neighbour (makespan << 32 | c) and ctl[0] the current makespan, ctl[1] the number of pairs.
+struct JssImproveSmem {
+    int32_t *ord, *start;
+    uint32_t *pairs;
+    uint64_t *best;
+    int32_t *ctl;
+};
+JSS_HD inline size_t jss_improve_smem(char *base, int jmax, int mmax, JssImproveSmem *b) {
+    const size_t n = (size_t)jmax * mmax * 4, o_best = (3 * n + 15) & ~(size_t)15;
+    const size_t o_ctl = o_best + 8 * JSS_WARPS_PER_CTA;
+    if (b) {
+        b->ord = reinterpret_cast<int32_t *>(base);
+        b->start = reinterpret_cast<int32_t *>(base + n);
+        b->pairs = reinterpret_cast<uint32_t *>(base + 2 * n);
+        b->best = reinterpret_cast<uint64_t *>(base + o_best);
+        b->ctl = reinterpret_cast<int32_t *>(base + o_ctl);
+    }
+    return o_ctl + 16;
+}
+
+// One replay of the env whose state block is `root` under an operation order: env_order_action's decisions on `ord`
+// (row stride machines_max) with the entries at indices sw.x / sw.y read as sw.z / sw.w, each step with
+// env_step<KJ, false>, at most 2 J M + 1 decisions.  Returns the end time if the episode ends done, else -1 (an env done
+// at entry, nothing legal, a step that leaves the env unchanged, the bound).  It stops as soon as t reaches `limit`:
+// such an episode cannot end below it.  REC: the round of each allocated operation (job allocations counted from 0)
+// goes to rec_ord and its start time to rec_start.  rec_ord may be `ord`: an entry is read only while its operation
+// is its job's current one, and written once that operation is allocated.
+template <int KJ, bool REC>
+JSS_DEV int env_improve_replay(const JssParams &p, const JssLaunch &a, const InstView &iv, const int32_t *root,
+                               int lane, const int32_t *ord, int4 sw, int limit, int32_t *rec_ord, int32_t *rec_start,
+                               int *hz) {
+    const int J = jss_J(iv), ms = p.machines_max, bound = 2 * J * jss_M(iv) + 1;
+    EnvRegs<KJ> s;
+    env_load<KJ>(iv, root, lane, s);
+    s.flags = jss_uniform(s.flags);
+    if (s.flags & JSS_FLAG_DONE) return -1;
+    int round = 0;
+    for (int d = 0; d < bound && !(s.flags & JSS_FLAG_DONE) && s.t < limit; d++) {
+        float logp, pr[KJ];
+        const int act = jss_uniform(env_order_action<KJ, true>(a, iv, s, 0, lane, ord, ms, logp, pr, sw));
+        if (act == JSS_ACTION_SKIP) return -1;
+        if (REC && act < J) {
+#pragma unroll
+            for (int i = 0; i < KJ; i++)
+                if (KJ * lane + i == act) rec_ord[act * ms + s.todo[i]] = round;
+        }
+        int r;
+        const bool changed = env_step<KJ, false, false, REC>(p, iv, s, 0, lane, act, r, hz, rec_start);
+        s.flags = jss_uniform(s.flags);
+        if (!changed) return -1;
+        round += act < J ? 1 : 0;
+    }
+    return (s.flags & JSS_FLAG_DONE) ? s.t : -1;
+}
+
+// The chain of the canonical schedule (ord, start; row stride machines_max) that ends at makespan T, walked by one
+// warp: from the in-call operation (ord >= 0) that ends at T with the largest round, step to the in-call operation on
+// the same machine with the largest round below it if that one ends at the current start (recording the pair), else
+// to the job predecessor if it is in call and ends there, else stop.  Writes the pairs in walk order and returns their
+// number.  Keys (round + 1) << 13 | index fit 27 bits: rounds and indices are below 256 * 32.
+template <int KJ>
+JSS_DEV int jss_improve_chain(const JssParams &p, const InstView &iv, const int32_t *ord, const int32_t *start,
+                              uint32_t *pairs, int T, int lane) {
+    const int J = jss_J(iv), M = jss_M(iv), ms = p.machines_max;
+    const auto end = [&](int q) { const int j = q / ms; return start[q] + jss_op_d(iv.ops[j * M + q - j * ms]); };
+    const auto key = [&](int q) { return ((uint32_t)(ord[q] + 1) << 13) | (uint32_t)q; };
+    __syncwarp();                                        // the replay's lanes wrote ord and start
+    uint32_t at = 0u;
+    for (int j = lane; j < J; j += 32)
+        for (int k = 0; k < M; k++)
+            if (ord[j * ms + k] >= 0 && end(j * ms + k) == T) at = max(at, key(j * ms + k));
+    at = __reduce_max_sync(JSS_FULL, at);
+    int n = 0;
+    while (at != 0u) {
+        const int q = (int)(at & 8191u), r = (int)(at >> 13) - 1, j = q / ms, k = q - j * ms, s0 = start[q];
+        const uint32_t m = jss_op_m(iv.ops[j * M + k]);
+        uint32_t pm = 0u;                                // the machine predecessor
+        for (int jj = lane; jj < J; jj += 32)
+            for (int kk = 0; kk < M; kk++) {
+                const int rr = ord[jj * ms + kk];
+                if (rr >= 0 && rr < r && jss_op_m(iv.ops[jj * M + kk]) == m) pm = max(pm, key(jj * ms + kk));
+            }
+        pm = __reduce_max_sync(JSS_FULL, pm);
+        at = 0u;
+        if (pm != 0u && end((int)(pm & 8191u)) == s0) {
+            if (lane == 0) pairs[n] = (pm & 8191u) << 16 | (uint32_t)q;
+            n++;
+            at = pm;
+        } else if (k > 0 && ord[q - 1] >= 0 && end(q - 1) == s0) {
+            at = key(q - 1);
+        }
+    }
+    return n;
+}
+
+// Order `smp` of env `env` (a.order_in, [N][k][jobs_max][machines_max]) improved by steepest descent on the critical
+// path, by the whole CTA (`root`: the env's state block, never written).  Warp 0 replays the input recording its
+// canonical order R and start times into shared memory, and walks the chain; then per move warp w replays the
+// neighbours c = w, w + 8, ... (pair c's two entries of R swapped at lookup), the CTA takes the smallest makespan
+// (lowest c on ties) and, if it is below the current one, warp 0 replays that neighbour recording its canonical order
+// in place and walks its chain.  At most a.n_steps moves.  Outputs: the final order (-1 everywhere unless the input
+// ends done), makespan, the input's makespan and the moves, at row env * a.samples_ld + smp.
+template <int KJ>
+JSS_DEV void env_improve_order(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int smp,
+                               const int32_t *root, int warp, int lane, int *hz, char *ism) {
+    const int J = jss_J(iv), M = jss_M(iv), ms = p.machines_max;
+    JssImproveSmem is;
+    jss_improve_smem(ism, p.jobs_max, ms, &is);
+    const size_t o_off = ((size_t)env * a.n_samples + smp) * p.jobs_max * ms;
+    const int64_t row = (int64_t)env * a.samples_ld + smp;
+    const int4 none = make_int4(-1, -1, 0, 0);
+    __syncthreads();                                     // the previous item's last reads of the region are done
+    if (warp == 0) {
+        for (int q = lane; q < J * ms; q += 32) is.ord[q] = -1;   // the operations started before the call
+        __syncwarp();
+        const int t = env_improve_replay<KJ, true>(p, a, iv, root, lane, a.order_in + o_off, none, JSS_INF, is.ord,
+                                                   is.start, hz);
+        const int n = t >= 0 ? jss_improve_chain<KJ>(p, iv, is.ord, is.start, is.pairs, t, lane) : 0;
+        if (lane == 0) { is.ctl[0] = t; is.ctl[1] = n; }
+    }
+    __syncthreads();
+    const int t0 = is.ctl[0];
+    int cur = t0, moves = 0;
+    while (cur >= 0 && moves < a.n_steps) {
+        const int n = is.ctl[1];
+        uint64_t best = ~0ull;
+        for (int c = warp; c < n; c += JSS_WARPS_PER_CTA) {
+            const uint32_t pr = is.pairs[c];
+            const int u = (int)(pr >> 16), v = (int)(pr & 0xffffu);
+            const int t = env_improve_replay<KJ, false>(p, a, iv, root, lane, is.ord,
+                                                        make_int4(u, v, is.ord[v], is.ord[u]), cur, nullptr, nullptr, hz);
+            if (t >= 0 && t < cur) best = min(best, (uint64_t)t << 32 | (uint32_t)c);
+        }
+        if (lane == 0) is.best[warp] = best;
+        __syncthreads();
+        best = ~0ull;
+        for (int w = 0; w < JSS_WARPS_PER_CTA; w++) best = min(best, is.best[w]);
+        if (best == ~0ull) break;                        // CTA-uniform: a local optimum
+        if (warp == 0) {
+            const uint32_t pr = is.pairs[(uint32_t)best];
+            const int u = (int)(pr >> 16), v = (int)(pr & 0xffffu);
+            const int t = env_improve_replay<KJ, true>(p, a, iv, root, lane, is.ord,
+                                                       make_int4(u, v, is.ord[v], is.ord[u]), JSS_INF, is.ord,
+                                                       is.start, hz);
+            const int n2 = jss_improve_chain<KJ>(p, iv, is.ord, is.start, is.pairs, t, lane);
+            if (lane == 0) is.ctl[1] = n2;
+        }
+        cur = (int)(best >> 32);
+        moves++;
+        __syncthreads();
+    }
+    int32_t *out = a.order_out + o_off;
+    for (int q = (int)threadIdx.x; q < J * M; q += (int)blockDim.x) {
+        const int j = q / M, k = q - j * M;
+        out[(size_t)j * ms + k] = t0 >= 0 ? is.ord[j * ms + k] : -1;
+    }
+    if (threadIdx.x == 0) {
+        a.actions_out[row] = cur;
+        a.start_out[row] = t0;
+        a.moves_out[row] = moves;
+    }
+}
+
 template <int KJ, int MODE>
 JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
                              int lane, float *scratch) {
@@ -2273,6 +2447,9 @@ constexpr int JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 1};
 // The beam round of jss_beam_step likewise (CUDA 12.9, sm_90a; DESIGN.md section 4), and its stochastic form.
 constexpr int JSS_BEAM_STEP_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
 constexpr int JSS_STOCHASTIC_BEAM_STEP_MIN_CTAS[JSS_LANE_CLASSES] = {3, 3, 2, 1};
+// The critical-path descent likewise: 32 / 40 / 60 / 116 registers (CUDA 12.9, sm_90a); 8 is the SM's limit, and one
+// CTA more spills with 8 jobs per lane.  Its shared memory (three [J][M] tables) bounds the resident CTAs at large J M.
+constexpr int JSS_IMPROVE_ORDERS_MIN_CTAS[JSS_LANE_CLASSES] = {8, 6, 4, 2};
 JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
     return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
@@ -2287,6 +2464,7 @@ JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
          : mode == JSS_MODE_ORDER_LOG_PROB_GRAD ? JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_BEAM_STEP ? JSS_BEAM_STEP_MIN_CTAS[jss_lane_class(32 * KJ)]
          : mode == JSS_MODE_STOCHASTIC_BEAM_STEP ? JSS_STOCHASTIC_BEAM_STEP_MIN_CTAS[jss_lane_class(32 * KJ)]
+         : mode == JSS_MODE_IMPROVE_ORDERS ? JSS_IMPROVE_ORDERS_MIN_CTAS[jss_lane_class(32 * KJ)]
          : 1;
 }
 
@@ -2339,6 +2517,30 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
             }
             jss_iv_shape(iv);
             env_beam_step<KJ, MODE == JSS_MODE_STOCHASTIC_BEAM_STEP>(p, a, iv, rec, warp, lane, scratch, bsm);
+        }
+        return;
+    }
+    if (MODE == JSS_MODE_IMPROVE_ORDERS) {
+        // work item = one (env, order): env slot e = item / K of the class's tiles, order item % K, CTA-strided; the
+        // per-warp regions hold only env_check_no_op's table, and the improvement region follows them
+        char *ism = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;
+        const int64_t K = a.n_samples, n_items = (int64_t)(a.tile_end - a.tile_begin) * JSS_WARPS_PER_CTA * K;
+        int staged = -1;
+        for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
+            const int64_t e = item / K;
+            const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, a.tile_begin + (int)(e / JSS_WARPS_PER_CTA),
+                                           (int)(e % JSS_WARPS_PER_CTA));
+            const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
+            if (env < 0) continue;                       // CTA-uniform
+            if (inst != staged) {
+                __syncthreads();
+                jss_stage_instance(p, p.inst[inst], c, JSS_STAGE_OPS);
+                staged = inst;
+                __syncthreads();
+            }
+            jss_iv_shape(iv);
+            env_improve_order<KJ>(p, a, iv, env, (int)(item - e * K), p.state + (size_t)t.off16 * 4, warp, lane,
+                                  reinterpret_cast<int *>(scratch), ism);
         }
         return;
     }

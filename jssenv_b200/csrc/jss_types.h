@@ -173,8 +173,8 @@ struct JssLaunch {           // per-launch arguments
     union {
         int32_t rule;
         int32_t greedy;      // steps from a row (a.logits): 0 categorical draw, 1 epsilon-greedy decode
-        int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env; jss_order_log_prob (_grad):
-                             // K, the orders per env
+        int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env; jss_order_log_prob (_grad),
+                             // jss_improve_orders: K, the orders per env
         int32_t beam_width;  // jss_beam_search, jss_sample_without_replacement: W, the beams kept per env;
                              // jss_beam_step, jss_stochastic_beam_step: W, the envs per group
     };
@@ -200,8 +200,8 @@ struct JssLaunch {           // per-launch arguments
                                       // (jss_stochastic_beam_step: of the round)
         int64_t values_ld;   // jss_lookahead_priority: env i's value of action a at actions_out + i * values_ld + a
                              // (logits_ld is the table's env stride there)
-        const int32_t *order_in;   // jss_order_log_prob (_grad): order s of env i at order_in + (i * n_samples + s) *
-                                   // jobs_max * machines_max
+        const int32_t *order_in;   // jss_order_log_prob (_grad), jss_improve_orders: order s of env i at order_in +
+                                   // (i * n_samples + s) * jobs_max * machines_max
     };
     union {
         const int32_t *actions;  // step; jss_sample_episodes_solution: the sample each env replays (< 0: none)
@@ -238,9 +238,13 @@ struct JssLaunch {           // per-launch arguments
         int32_t *job_out;
     };
     // jss_stochastic_beam_step: as jss_beam_step, and slot b of group g has key key_io[g W + b] (read and written)
+    // jss_improve_orders: order s of env i goes to order_out + (i * n_samples + s) * jobs_max * machines_max, its
+    // makespan to actions_out, the input's to start_out and the accepted moves to moves_out, each at i * samples_ld + s;
+    // n_steps is the move limit
     union {
         uint8_t *traj_mask;
         float *key_io;
+        int32_t *moves_out;
     };
     int32_t *traj_scalars; int32_t *traj_actions;
     // jss_sample_without_replacement: slot b's score goes to log_prob_out and its key to key_out + i * samples_ld + b,
@@ -249,6 +253,7 @@ struct JssLaunch {           // per-launch arguments
         uint8_t *wire;       // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
         float *key_out;
         int32_t *bad_out;
+        int32_t *start_out;
     };
     int32_t wire_stride;
     JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
@@ -294,5 +299,7 @@ struct JssLaunch {           // per-launch arguments
                                          // children stepped into the group's envs (jss_beam_step)
 #define JSS_MODE_STOCHASTIC_BEAM_STEP 20 // the same perturbed by top-down Gumbel noise, the beams ranked by key
                                          // (jss_stochastic_beam_step)
+#define JSS_MODE_IMPROVE_ORDERS 21       // operation orders improved by steepest descent on the critical path, one
+                                         // (env, order) per CTA, the envs untouched (jss_improve_orders)
 
 #define JSS_WARPS_PER_CTA 8

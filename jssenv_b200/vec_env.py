@@ -773,6 +773,51 @@ class JssVecEnv:
             log_prob, makespan, _ = run(x)
         return (log_prob[:, 0], makespan[:, 0]) if single else (log_prob, makespan)
 
+    def improve_orders(self, order, max_moves: Optional[int] = None):
+        """Improve given operation orders by steepest descent on the critical path, each from the env's current state,
+        in one launch per lane class (jss_improve_orders), leaving the envs untouched.  `order` is (N, J, M) or
+        (N, k, J, M) integer, as order_log_prob() takes it: order s of env i stands for the episode
+        rollout_priority(-order[i, s]) runs from this state (the orders of beam_search() and
+        sample_without_replacement() replay their beams).  Each order is first replaced by its canonical form, the
+        round at which its replay allocates each operation; then each move replays every swap of two adjacent
+        operations of a machine block on the critical path (N1 of van Laarhoven, Aarts and Lenstra, 1992) and takes
+        the one of smallest makespan (the first on the path from its end on ties) if it is strictly better, until none
+        is or after `max_moves` moves (None: no limit).  Neighbours are valued by this env's own replay, so every
+        returned order is an episode of it.  No RNG, no table.  Returns a dict of device tensors, shaped like the input
+        without (J, M): ``"makespan"`` and ``"start_makespan"`` int32, the final and the input's makespan,
+        ``"moves"`` int32, the accepted moves, and ``"order"`` int32 like the input, the final canonical order (-1 /
+        -1 / 0 and -1 everywhere for an env done now or an input whose replay does not end done); for (N, k, J, M)
+        input also ``"best"`` (N,) int64, the lowest s of smallest makespan, -1 if none.  The improved order is an
+        imitation target: ``order_log_prob(logits, out["order"])`` is its differentiable log-likelihood."""
+        import torch
+        n, J, M = self.num_envs, self.jobs, self.machines
+        o = torch.as_tensor(order, device=self.device)
+        single = o.dim() == 3
+        if (o.dim() not in (3, 4) or o.shape[0] != n or tuple(o.shape[-2:]) != (J, M) or o.is_floating_point()
+                or o.is_complex() or o.dtype == torch.bool or (o.dim() == 4 and o.shape[1] < 1)):
+            raise ValueError(f"improve_orders: order must be an integer tensor of shape ({n}, {J}, {M}) or "
+                             f"({n}, k, {J}, {M}), got {tuple(o.shape)} {o.dtype}")
+        if max_moves is None:
+            max_moves = 2 ** 31 - 1
+        elif isinstance(max_moves, bool) or not isinstance(max_moves, (int, np.integer)) or not 0 <= max_moves < 2 ** 31:
+            raise ValueError(f"improve_orders: max_moves must be None or an integer in [0, 2^31), got {max_moves!r}")
+        o = o.reshape(n, -1, J, M).to(torch.int32).contiguous()
+        k = o.shape[1]
+        out = {"order": torch.full_like(o, -1)}
+        for name in ("makespan", "start_makespan", "moves"):
+            out[name] = torch.empty((n, k), dtype=torch.int32, device=self.device)
+        rc = self._L.jss_improve_orders(self._h, o.data_ptr(), k, int(max_moves), out["order"].data_ptr(),
+                                        out["makespan"].data_ptr(), out["start_makespan"].data_ptr(),
+                                        out["moves"].data_ptr(), k, self._stream())
+        N.check(self._h, rc, "jss_improve_orders")
+        if single:
+            return {name: t[:, 0] for name, t in out.items()}
+        ms = out["makespan"]
+        ended = ms >= 0
+        best = torch.where(ended, ms, torch.iinfo(torch.int32).max).argmin(1)
+        out["best"] = torch.where(ended.any(1), best, -1)
+        return out
+
     def _order_log_prob(self, x, order):
         """The native call of order_log_prob on a checked table `x` and (N, k, J, M) contiguous int32 orders:
         (log_prob, makespan, order)."""
