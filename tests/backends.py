@@ -23,8 +23,8 @@ def native_test(emu=(), gpu=(), names=None):
     return declare
 
 
-def _bind(fn, backend):
-    cases = fn.native_cases[backend]
+def _bind(fn, backend, cases=None, schedule=None, suffix=""):
+    cases = fn.native_cases[backend] if cases is None else cases
     sig = inspect.signature(fn)
     fixed = cases if isinstance(cases, dict) else {}
     own = [p for p in sig.parameters.values()
@@ -33,10 +33,10 @@ def _bind(fn, backend):
     def test(**params):
         from jssenv_b200 import JssVecEnv
         given = {"make_env": JssVecEnv, "backend": backend, **fixed, **params}
-        with use_emulation() if backend == "emu" else contextlib.nullcontext():
+        with use_emulation(schedule) if backend == "emu" else contextlib.nullcontext():
             fn(**{a: given[a] for a in sig.parameters if a in given})
 
-    test.__name__ = test.__qualname__ = fn.native_names.get(backend, f"test_{backend}_{fn.__name__}")
+    test.__name__ = test.__qualname__ = fn.native_names.get(backend, f"test_{backend}_{fn.__name__}") + suffix
     test.__doc__ = fn.__doc__
     test.__signature__ = sig.replace(parameters=own)      # pytest reads the test's parameters from here
     if isinstance(cases, list):
@@ -44,10 +44,16 @@ def _bind(fn, backend):
     return pytest.mark.gpu(test) if backend == "gpu" else test
 
 
-def collect(namespace, source, *backends):
-    """Binds every test `source` (a module or a namespace) declares into `namespace`, for each of `backends`."""
+def collect(namespace, source, *backends, only=None, schedule=None, suffix=""):
+    """Binds every test `source` (a module or a namespace) declares into `namespace`, for each of `backends`.
+
+    `only` binds just the declarations it names: a dict from name to the parameter sets to bind (in native_test's
+    form) or None for the declared ones.  `schedule` runs the emu tests under use_emulation(schedule), and `suffix`
+    is appended to the tests' names."""
     for fn in list(vars(source).values() if inspect.ismodule(source) else source.values()):
+        if only is not None and getattr(fn, "__name__", None) not in only:
+            continue
         for backend in backends:
             if getattr(fn, "native_cases", {}).get(backend) is not None:
-                test = _bind(fn, backend)
+                test = _bind(fn, backend, None if only is None else only[fn.__name__], schedule, suffix)
                 namespace[test.__name__] = test

@@ -45,6 +45,7 @@ static inline float4 make_float4(float a, float b, float c, float d) { return fl
 namespace emu {
 extern thread_local dim3 threadIdx_, blockIdx_, blockDim_, gridDim_;
 extern void *smem_ptr;
+extern int poison;   // -1, or the byte every block's dynamic shared memory and every cudaMalloc start as
 enum Op { OP_SHFL = 1, OP_SHFL_XOR, OP_SHFL_UP, OP_BALLOT, OP_RED_MIN, OP_RED_MAX, OP_RED_ADD, OP_RED_OR, OP_SYNCWARP, OP_SYNCTHREADS };
 uint64_t collective(int op, unsigned mask, uint64_t value, int arg);
 void launch_impl(void (*entry)(void *), void *args, dim3 grid, dim3 block, size_t smem);
@@ -118,7 +119,12 @@ static inline const char *cudaGetErrorString(cudaError_t) { return "emu"; }
 static inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return 0; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { p->major = 9; p->minor = 0; p->multiProcessorCount = 2; return 0; }
 static inline cudaError_t cudaSetDevice(int) { return 0; }
-static inline cudaError_t cudaMalloc(void **p, size_t n) { *p = aligned_alloc(256, (n + 255) / 256 * 256); return *p ? 0 : 2; }
+static inline cudaError_t cudaMalloc(void **p, size_t n) {
+    const size_t bytes = (n + 255) / 256 * 256;
+    *p = aligned_alloc(256, bytes);
+    if (*p && emu::poison >= 0) memset(*p, emu::poison, bytes);   // device memory is not zeroed on allocation
+    return *p ? 0 : 2;
+}
 static inline cudaError_t cudaFree(void *p) { free(p); return 0; }
 static inline cudaError_t cudaFreeHost(void *p) { free(p); return 0; }
 enum { cudaHostAllocMapped = 2, cudaHostAllocPortable = 1 };

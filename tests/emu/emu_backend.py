@@ -12,7 +12,7 @@ EMU_LIB = os.path.join(HERE, "libjss_emu.so")
 
 
 def build(force=False):
-    srcs = [os.path.join(HERE, f) for f in ("cuda_shim.h", "emu_runtime.cpp")]
+    srcs = [os.path.join(HERE, f) for f in ("cuda_shim.h", "emu_runtime.cpp", "emu_selftest.cpp", "build_emu.sh")]
     csrc = os.path.join(HERE, "..", "..", "jssenv_b200", "csrc")
     srcs += [os.path.join(csrc, f) for f in os.listdir(csrc)]
     srcs.append(os.path.join(HERE, "..", "..", "include", "jss_b200.h"))
@@ -32,7 +32,10 @@ class EmuBackend:
     def library(self):
         if self._lib is None:
             build()
-            self._lib = _native._declare(ctypes.CDLL(EMU_LIB))
+            lib = _native._declare(ctypes.CDLL(EMU_LIB))
+            lib.jss_emu_set_schedule.restype = ctypes.c_int
+            lib.jss_emu_set_schedule.argtypes = [ctypes.c_int, ctypes.c_uint64, ctypes.c_int]
+            self._lib = lib
         return self._lib
 
     def torch_device(self, index):
@@ -50,14 +53,39 @@ class EmuBackend:
         pass
 
 
+ASCENDING, DESCENDING, SHUFFLED = 0, 1, 2
+DEFAULT_SCHEDULE = (ASCENDING, 0, -1)
+
+
 class use_emulation:
-    """Context manager / pytest helper: `with use_emulation(): env = JssVecEnv(...)`."""
+    """Context manager / pytest helper: `with use_emulation(): env = JssVecEnv(...)`.
+
+    `schedule=(order, seed, poison)` runs the emulated kernels under another legal schedule until the block exits (see
+    README.md): order ASCENDING (the default), DESCENDING or SHUFFLED (seeded by `seed`) for the threads of a block and
+    the blocks of a launch; poison -1 (the default) or a byte every block's shared memory and every cudaMalloc
+    allocation start as.  The default schedule is restored on exit."""
+
+    def __init__(self, schedule=None):
+        self._schedule = schedule
 
     def __enter__(self):
         self._saved = _native.backend
         _native.backend = EmuBackend()
+        if self._schedule is not None:
+            try:
+                self._set(self._schedule)
+            except BaseException:
+                _native.backend = self._saved
+                raise
         return _native.backend
 
     def __exit__(self, *exc):
+        if self._schedule is not None:
+            self._set(DEFAULT_SCHEDULE)
         _native.backend = self._saved
         return False
+
+    @staticmethod
+    def _set(schedule):
+        if _native.backend.library().jss_emu_set_schedule(*schedule) != 0:
+            raise ValueError(f"bad emulation schedule {schedule!r}")

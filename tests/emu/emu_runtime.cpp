@@ -2,6 +2,8 @@
 // Every CUDA thread of the running block is a fiber on its own stack; fibers run
 // until they reach a collective, the scheduler resolves a warp's collective once
 // all 32 lanes have arrived with the same operation (strict: anything else aborts).
+// jss_emu_set_schedule() picks the order in which ready fibers and blocks run and what
+// shared and device memory hold before anything writes them (see README.md).
 #include <setjmp.h>
 #include <stdio.h>
 #include <sys/mman.h>
@@ -15,6 +17,7 @@ namespace emu {
 
 thread_local dim3 threadIdx_, blockIdx_, blockDim_, gridDim_;
 void *smem_ptr = nullptr;
+int poison = -1;
 
 namespace {
 enum { READY = 0, WAITING = 1, DONE = 2 };
@@ -37,6 +40,24 @@ ucontext_t sched_ctx;
 void (*g_entry)(void *) = nullptr;
 void *g_args = nullptr;
 std::vector<char> smem_buf;
+enum { ASCENDING = 0, DESCENDING = 1, SHUFFLED = 2 };
+int sched_order = ASCENDING;
+uint64_t sched_rng = 0;
+
+uint64_t next_random() {   // splitmix64
+    uint64_t z = (sched_rng += 0x9e3779b97f4a7c15ull);
+    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+    return z ^ (z >> 31);
+}
+
+// 0..n-1 in the order of the current schedule; a shuffle is drawn afresh on every call
+void schedule_order(std::vector<int> &seq, int n) {
+    seq.resize(n);
+    for (int i = 0; i < n; i++) seq[i] = sched_order == DESCENDING ? n - 1 - i : i;
+    if (sched_order == SHUFFLED)
+        for (int i = n - 1; i > 0; i--) std::swap(seq[i], seq[next_random() % (uint64_t)(i + 1)]);
+}
 
 [[noreturn]] void die(const char *msg, int warp = -1) {
     fprintf(stderr, "[jss emu] FATAL: %s (block %u warp %d)\n", msg, blockIdx_.x, warp);
@@ -122,8 +143,11 @@ void launch_impl(void (*entry)(void *), void *args, dim3 grid, dim3 block, size_
     smem_ptr = (void *)(((uintptr_t)smem_buf.data() + 15) & ~(uintptr_t)15);
     g_entry = entry; g_args = args;
     blockDim_ = block; gridDim_ = grid;
-    for (unsigned b = 0; b < grid.x; b++) {
-        blockIdx_ = dim3(b, 1, 1);
+    std::vector<int> blocks, seq;
+    schedule_order(blocks, (int)grid.x);
+    for (int b : blocks) {
+        blockIdx_ = dim3((unsigned)b, 1, 1);
+        if (poison >= 0) memset(smem_buf.data(), poison, smem_buf.size());   // a CTA starts with garbage
         for (int i = 0; i < nt; i++) {
             Fiber &f = fibers[i];
             f.started = false; f.state = READY;
@@ -135,7 +159,8 @@ void launch_impl(void (*entry)(void *), void *args, dim3 grid, dim3 block, size_
         }
         for (;;) {
             bool progress = false;
-            for (int i = 0; i < nt; i++)
+            schedule_order(seq, nt);
+            for (int i : seq)
                 if (fibers[i].state == READY) { run_fiber(i); progress = true; }
             int done = 0, at_bar = 0;
             for (int i = 0; i < nt; i++) {
@@ -166,3 +191,15 @@ void launch_impl(void (*entry)(void *), void *args, dim3 grid, dim3 block, size_
 }
 
 }  // namespace emu
+
+// order: 0 ascending threads and blocks (the default), 1 descending, 2 a shuffle seeded by `seed`, redrawn on every
+// scheduling pass and every launch.  poison: -1 zero-fills dynamic shared memory once per launch (the default), a
+// byte value fills it at the start of every block and fills every cudaMalloc allocation.  Returns 0, or -1 if an
+// argument is out of range (nothing changes then).
+extern "C" int jss_emu_set_schedule(int order, uint64_t seed, int poison) {
+    if (order < emu::ASCENDING || order > emu::SHUFFLED || poison < -1 || poison > 255) return -1;
+    emu::sched_order = order;
+    emu::sched_rng = seed;
+    emu::poison = poison;
+    return 0;
+}
