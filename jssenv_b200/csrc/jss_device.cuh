@@ -60,10 +60,20 @@ struct EnvRegs {
     int t;             // current_time_step
     uint32_t flags;
     int ep_steps, ep_return;
-    // bit i: the step changed job slot i's row of real_obs (set conservatively; read only by the uniform step kernels'
-    // stores, which write back just the 32-byte sectors of the row that hold a marked job)
+    // What the step changed of job slot i, for the uniform step kernels' stores, which write back just the 32-byte
+    // sectors of the row and of the state block that hold a marked job: bit JSS_DIRTY_W0 + i / W1 + i / W2 + i its
+    // word in the block's region w0 / w1 / w2, bit JSS_DIRTY_LEGAL + i its legal bit (column 0 of its row, not in the
+    // job record).  Its row changed iff one of the first two or the last is set (env_dirty_rows).
     uint32_t dirty;
 };
+#define JSS_DIRTY_W0 0
+#define JSS_DIRTY_W1 8
+#define JSS_DIRTY_W2 16
+#define JSS_DIRTY_LEGAL 24
+template <int KJ>
+JSS_DEV uint32_t env_dirty_rows(const EnvRegs<KJ> &s) {
+    return (s.dirty >> JSS_DIRTY_W0) | (s.dirty >> JSS_DIRTY_W1) | (s.dirty >> JSS_DIRTY_LEGAL);
+}
 
 // ---- warp-uniformity hints -----------------------------------------------------------
 // ptxas proves a warp converged only while every branch on the way depends on values it KNOWS to be warp-uniform
@@ -408,7 +418,7 @@ JSS_DEV void env_reset_regs(const InstView &iv, EnvRegs<KJ> &s, int lane) {
 }
 
 // ---- increase_time_step (jss_env.py:495-637); returns hole_planning ---------------
-// TRACK: mark in s.dirty the jobs whose rows the advance changes (the uniform step kernels' dirty-row stores)
+// TRACK: mark in s.dirty the job records the advance changes (the uniform step kernels' dirty-sector stores)
 template <int KJ, bool TRACK = false>
 JSS_DEV int env_advance(const InstView &iv, EnvRegs<KJ> &s, int lane) {
     // next event = smallest positive machine countdown (the sorted event list of
@@ -430,10 +440,17 @@ JSS_DEV int env_advance(const InstView &iv, EnvRegs<KJ> &s, int lane) {
         const bool running = was > 0;
         const bool finished = running && left <= 0;
         const bool waiting = !running && s.todo[i] < M;
-        if (TRACK) s.dirty |= (running || waiting) ? 1u << i : 0u;   // every unfinished job's row changes
         s.tufco[i] = left > 0 ? left : 0;                 // == max(0, was - diff); 0 stays 0
         const int slack = diff - was;                     // idle part of the step for a job finishing now
-        s.total_idle[i] += finished ? slack : (waiting ? diff : 0);
+        const int idle = finished ? slack : (waiting ? diff : 0);
+        s.total_idle[i] += idle;
+        // w0 (tufco, and todo / col4 when finishing) of every running job, w1 (the idle times) of every waiting or
+        // finishing one, and w2 only where total_idle >> 8 changed, i.e. where adding idle >= 0 carried out of the low
+        // byte (then the low byte is now below idle): most advances leave it alone
+        if (TRACK)
+            s.dirty |= (running ? 1u << (JSS_DIRTY_W0 + i) : 0u) |
+                       (waiting || finished ? 1u << (JSS_DIRTY_W1 + i) : 0u) |
+                       ((s.total_idle[i] & 0xff) < idle ? 1u << (JSS_DIRTY_W2 + i) : 0u);
         s.idle_last[i] = finished ? slack : s.idle_last[i] + (waiting ? diff : 0);
         s.todo[i] += finished ? 1 : 0;
         {   // next op of a job that just finished one: unconditional clamped lookup + selects (no branch)
@@ -586,31 +603,17 @@ struct JssOut {
 };
 JSS_DEV JssOut jss_out_default(const JssParams &p) { return JssOut{p.obs, p.mask, p.scalars}; }
 
-// ---- observation / mask / reward (jss_env.py:102-134, 483-493) ---------------------
-// The staged row (n16 16-byte chunks) leaves by the warp's own 16-byte stores, but only the chunks in a 32-byte sector
-// (absolute addresses: a row may start 16 bytes into one) that holds a job s.dirty marks: a sector is written whole or
-// not at all.  This relies on real_obs holding, at the step's entry, the observation of the state block it loaded
-// (jss_b200.h).  Bit k of word w of `sec`: sector 32 w + k counted from the one that holds dst[0].
-template <int KJ>
-JSS_DEV void env_store_dirty_row(const EnvRegs<KJ> &s, float *dst, const float *staged, int n16, int lane) {
-    constexpr int NW = (16 + 28 * 32 * KJ + 31) / 32 / 32 + 1;   // words for the largest row of the lane class
-    const int lead = (int)((uintptr_t)dst & 31u);
-    const int r0 = lead + 28 * KJ * lane;                    // this lane's first row byte, from dst's first sector
-    uint32_t loc = 0u;                                       // its jobs' sectors, from sector r0 >> 5 on
-#pragma unroll
-    for (int i = 0; i < KJ; i++) {
-        const int a = ((r0 & 31) + 28 * i) >> 5, b = ((r0 & 31) + 28 * i + 27) >> 5;
-        if (s.dirty & (1u << i)) loc |= (2u << b) - (1u << a);
-    }
-    const uint64_t v = (uint64_t)loc << ((r0 >> 5) & 31);
-    uint32_t sec[NW];
-#pragma unroll
-    for (int w = 0; w < NW; w++)
-        sec[w] = __reduce_or_sync(JSS_FULL, (r0 >> 10) == w ? (uint32_t)v : (r0 >> 10) + 1 == w ? (uint32_t)(v >> 32) : 0u);
+// ---- dirty-sector stores of the uniform step kernels ---------------------------------------------
+// The staged bytes (n16 16-byte chunks) leave by the warp's own 16-byte stores, but only the chunks in a 32-byte sector
+// whose bit `sec` sets (absolute addresses: dst may start 16 bytes into a sector): a sector is written whole or not at
+// all.  Bit k of word w of `sec`: sector 32 w + k counted from the one that holds dst[0].  NW words cover every sector
+// and NIT rounds of 32 chunks every chunk of the largest n16 the caller passes.
+template <int NW, int NIT>
+JSS_DEV void jss_store_sectors(void *dst, const void *staged, int n16, const uint32_t (&sec)[NW], int lane) {
     // chunk k = lane + 32 it lies in sector 16 it + x: bit 16 (it & 1) + x of word it / 2 (or of the next word)
-    const int x = (lead + 16 * lane) >> 5;
+    const int x = ((int)((uintptr_t)dst & 31u) + 16 * lane) >> 5;
 #pragma unroll
-    for (int it = 0; it < (56 * KJ + 31) / 32; it++) {   // 7 J / 4 <= 56 KJ chunks
+    for (int it = 0; it < NIT; it++) {
         const int k = lane + 32 * it, b = 16 * (it & 1) + x;
         const uint32_t m = b < 32 ? sec[it / 2] : sec[it / 2 + 1 < NW ? it / 2 + 1 : NW - 1];
         if (k < n16 && ((m >> (b & 31)) & 1u))
@@ -618,6 +621,74 @@ JSS_DEV void env_store_dirty_row(const EnvRegs<KJ> &s, float *dst, const float *
     }
     __syncwarp();
 }
+
+// The staged observation row: the sectors that hold a job whose row changed (env_dirty_rows).  This relies on real_obs
+// holding, at the step's entry, the observation of the state block it loaded (jss_b200.h).
+template <int KJ>
+JSS_DEV void env_store_dirty_row(const EnvRegs<KJ> &s, float *dst, const float *staged, int n16, int lane) {
+    constexpr int NW = (16 + 28 * 32 * KJ + 31) / 32 / 32 + 1;   // words for the largest row of the lane class
+    const uint32_t rows = env_dirty_rows<KJ>(s);
+    const int lead = (int)((uintptr_t)dst & 31u);
+    const int r0 = lead + 28 * KJ * lane;                    // this lane's first row byte, from dst's first sector
+    uint32_t loc = 0u;                                       // its jobs' sectors, from sector r0 >> 5 on
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        const int a = ((r0 & 31) + 28 * i) >> 5, b = ((r0 & 31) + 28 * i + 27) >> 5;
+        if (rows & (1u << i)) loc |= (2u << b) - (1u << a);
+    }
+    const uint64_t v = (uint64_t)loc << ((r0 >> 5) & 31);
+    uint32_t sec[NW];
+#pragma unroll
+    for (int w = 0; w < NW; w++)
+        sec[w] = __reduce_or_sync(JSS_FULL, (r0 >> 10) == w ? (uint32_t)v : (r0 >> 10) + 1 == w ? (uint32_t)(v >> 32) : 0u);
+    jss_store_sectors<NW, (56 * KJ + 31) / 32>(dst, staged, n16, sec, lane);   // 7 J / 4 <= 56 KJ chunks
+}
+
+// 16-byte chunks of the lane class's largest state block (J = 32 KJ, M = 32: jss_block_geom)
+template <int KJ>
+JSS_DEV constexpr int jss_block16_max() { return (80 * KJ + 36 + 2 * jss_lane_slots(KJ)) / 4; }
+
+// The staged state block: the sectors that hold a job record word s.dirty marks, every sector of the tail (tuam, the
+// job bits and the header change at almost every step; its first sector may hold the end of w2) and the block's first
+// sector.  The first and the last sector (in the tail) may be shared with the neighbouring blocks: storing this block's
+// half of them always keeps such a sector whole in L2 when the neighbour does the same.  This relies on the block in
+// HBM being, until the store, the block the step loaded.
+template <int KJ>
+JSS_DEV void env_store_dirty_block(const InstView &iv, const EnvRegs<KJ> &s, int32_t *dst, const int32_t *staged,
+                                   int lane) {
+    constexpr int N16 = jss_block16_max<KJ>(), NW = (16 * N16 + 16 + 1023) / 1024;
+    const int lead = (int)((uintptr_t)dst & 31u);
+    const int Jc = iv.si->Jcap;
+    uint32_t loc[NW];                                        // this lane's changed sectors
+#pragma unroll
+    for (int w = 0; w < NW; w++) loc[w] = 0u;
+    const auto mark = [&](int byte, uint32_t changed) {     // the sector of block byte `byte`, if `changed`
+        const int g = (lead + byte) >> 5;
+#pragma unroll
+        for (int w = 0; w < NW; w++) loc[w] |= (changed != 0u && (g >> 5) == w) ? 1u << (g & 31) : 0u;
+    };
+    if (KJ * lane < jss_J(iv)) {
+        // a lane's slice of w0 / w1 is 4 KJ bytes, of w2 2 KJ: each 16-byte piece of it lies in one sector
+        constexpr int P = KJ > 4 ? KJ / 4 : 1, JP = KJ / P;
+        constexpr uint32_t PM = (1u << JP) - 1u;
+#pragma unroll
+        for (int q = 0; q < P; q++) {
+            mark(4 * (KJ * lane + JP * q), (s.dirty >> (JSS_DIRTY_W0 + JP * q)) & PM);
+            mark(4 * (Jc + KJ * lane + JP * q), (s.dirty >> (JSS_DIRTY_W1 + JP * q)) & PM);
+        }
+        mark(8 * Jc + 2 * KJ * lane, (s.dirty >> JSS_DIRTY_W2) & jss_legal_mask<KJ>());
+    }
+    const int t0 = (lead + 4 * iv.si->tail) >> 5;            // the tail's first sector
+    uint32_t sec[NW];
+#pragma unroll
+    for (int w = 0; w < NW; w++) {
+        const int sh = t0 - 32 * w;
+        sec[w] = __reduce_or_sync(JSS_FULL, loc[w]) | (w == 0 ? 1u : 0u) | (sh <= 0 ? ~0u : sh < 32 ? ~0u << sh : 0u);
+    }
+    jss_store_sectors<NW, (N16 + 31) / 32>(dst, staged, iv.si->block_words >> 2, sec, lane);
+}
+
+// ---- observation / mask / reward (jss_env.py:102-134, 483-493) ---------------------
 
 template <int KJ, bool BULK = false, bool DIRTY = false>
 JSS_DEV void env_emit_obs(const JssParams &p, const JssOut &out, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
@@ -664,15 +735,17 @@ JSS_DEV void env_emit_obs(const JssParams &p, const JssOut &out, const InstView 
         __syncwarp();
         if (lane == 0) {
             if (st_bytes) jss_bulk_store(st_dst, st_sa, st_bytes);
-            if (!DIRTY && (n & 3) == 0 && (p.jobs_max & 3) == 0) jss_bulk_store(dst, scratch_sa, (uint32_t)n * 4u);
+            if ((n & 3) == 0 && (p.jobs_max & 3) == 0) jss_bulk_store(dst, scratch_sa, (uint32_t)n * 4u);
             jss_bulk_commit();           // ONE group for both copies (an empty group is legal)
         }
-        if ((n & 3) == 0 && (p.jobs_max & 3) == 0) {
-            if (DIRTY) env_store_dirty_row<KJ>(s, dst, scratch, n >> 2, lane);
+        if ((n & 3) == 0 && (p.jobs_max & 3) == 0)
             return;                      // the caller waits (wait_group.read) before reusing the staging buffers
-        }
     } else {
         __syncwarp();
+        if (DIRTY && (n & 3) == 0 && (p.jobs_max & 3) == 0) {
+            env_store_dirty_row<KJ>(s, dst, scratch, n >> 2, lane);
+            return;
+        }
     }
     // ... and stream the J*7 floats of the env out with fully coalesced stores
     int done_elems = 0;
@@ -788,7 +861,7 @@ JSS_DEV bool env_step(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, in
         s.tuam = ((uint32_t)lane == m_a) ? gain : s.tuam;            // :446
 #pragma unroll
         for (int i = 0; i < KJ; i++) s.tufco[i] = (lane == la && i == ia) ? gain : s.tufco[i];   // :447
-        if (TRACK && lane == la) s.dirty |= 1u << ia;
+        if (TRACK && lane == la) s.dirty |= 1u << (JSS_DIRTY_W0 + ia);
         if (BOOKKEEP && p.solution && lane == la)                     // :454
             p.solution[((size_t)env * p.jobs_max + action) * p.machines_max + jss_sel<KJ>(s.todo, ia)] = s.t;
         if (SOL_OUT && lane == la)
@@ -2602,7 +2675,7 @@ JSS_DEV void jss_pdl_wait() {}
 // Persistent CTAs (grid = SMs x resident CTAs), one warp per env of a tile.  Per warp in shared
 // memory: an mbarrier, a state-block buffer that receives the NEXT env's block by cp.async.bulk
 // while the current env is simulated, and the staging buffers (new state block, observation rows)
-// that leave by bulk store.
+// that leave by bulk store (DIRTY kernels: by the warp's own stores of the changed sectors).
 // SAMPLE = 1 / 2 additionally picks every env's NEXT action (masked-uniform sampler / any dispatching
 // rule) from the freshly computed state, so a policy-driven loop is one launch per step.
 // SAMPLE = 3 takes the env's action from the caller's policy logits BEFORE the step (jss_step_logits): the next env's
@@ -2625,8 +2698,8 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
                             const JssWarpSmem &w, int warp, int lane, int tile, int tile_end, int tile_step, int &staged,
                             uint32_t &phase) {
     constexpr bool ROW = jss_step_takes_row(SAMPLE), RECORD = jss_step_records(SAMPLE);
-    // a uniform batch stepped by its actions or a rule stores only the changed sectors of a row (a row step, whose
-    // kernel also prefetches the row, has not been measured with it)
+    // a uniform batch stepped by its actions or a rule stores only the changed sectors of a row and of a state block,
+    // with the warp's own stores (a row step, whose kernel also prefetches the row, has not been measured with it)
     constexpr bool DIRTY = UNI && !ROW;
     int env_next = -1, act_next = 0;
     // start the bulk load of the state block of this warp's env of tile `next` and fetch its action (a row: start the
@@ -2686,9 +2759,12 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
         prefetch(tile + tile_step);
         if (env < 0) continue;
         int raw = 0;
-        // the previous env's observation must have left the staging buffer (also aliased by hz)
-        if (lane == 0) jss_bulk_store_wait_read();
-        __syncwarp();
+        // the previous env's observation must have left the staging buffer (also aliased by hz); the dirty-sector
+        // stores leave it before they return
+        if (!DIRTY) {
+            if (lane == 0) jss_bulk_store_wait_read();
+            __syncwarp();
+        }
         // every lane holds the same flags word (one address, loaded by all lanes): say so -- ptxas already sees that
         // for the action and the time, a shuffle of those is folded away
         if (jss_hint_flags<KJ, UNI>()) s.flags = jss_uniform(s.flags);
@@ -2697,7 +2773,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
         const bool changed =
             env_step<KJ, true, DIRTY>(p, iv, s, env, lane, action, raw, reinterpret_cast<int *>(w.scratch));
         if (jss_hint_flags<KJ, UNI>()) s.flags = jss_uniform(s.flags);   // the no-op test returns from inside lane-dependent code
-        if (DIRTY) s.dirty |= (s.lb ^ lb_in) & jss_legal_mask<KJ>();   // a job's legal bit is column 0 of its row
+        if (DIRTY) s.dirty |= ((s.lb ^ lb_in) & jss_legal_mask<KJ>()) << JSS_DIRTY_LEGAL;
         if (SAMPLE == 1 || SAMPLE == 2) {
             const uint32_t h = jss_hash_env(a.hash_key, p.env_id_base + (uint64_t)env);   // == jss_hash3(seed, genv, step_index)
             const int nxt = env_select_action<KJ, SAMPLE == 1>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor);
@@ -2719,11 +2795,18 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
             if (changed || s.flags != flags_in) env_emit_scalars<KJ>(jss_out_default(p), iv, s, env, lane, raw);
             env_emit_mask<KJ>(p, slot, iv, s, env, lane, noop);
             env_emit_scalars<KJ>(slot, iv, s, env, lane, raw);
+        } else if (changed && DIRTY) {
+            // new state -> shared staging -> the warp's own stores of the changed sectors of the block and the row
+            // (the block last: the emit's __syncwarp covers both staging buffers, and the job registers are dead then)
+            env_store_to<KJ>(iv, w.state_out, lane, s);
+            env_emit_all<KJ, false, true>(p, iv, s, env, lane, w.scratch, raw);
+            env_store_dirty_block<KJ>(iv, s, p.state + (size_t)jss_tile(p, a, UNI, tile, warp).off16 * 4, w.state_out,
+                                      lane);
         } else if (changed) {
             // new state -> shared staging -> one bulk store (every word of the block is rewritten)
             env_store_to<KJ>(iv, w.state_out, lane, s);
             const JssTileWarp t = jss_tile(p, a, UNI, tile, warp);
-            env_emit_all<KJ, true, DIRTY>(p, iv, s, env, lane, w.scratch, raw, w.scratch_sa,
+            env_emit_all<KJ, true>(p, iv, s, env, lane, w.scratch, raw, w.scratch_sa,
                                    p.state + (size_t)t.off16 * 4, w.state_out_sa, t.blk16 * 16u);
         } else if (s.flags != flags_in) {
             env_store_flags_only<KJ>(p, iv, p.state + (size_t)jss_tile(p, a, UNI, tile, warp).off16 * 4, s, env, lane);

@@ -9,7 +9,10 @@ diffed at ABSOLUTE 32-byte sector granularity: a sector is dirty when one of its
 and per region (obs, w0, w1, w2, tail): the bytes written today (every changed env rewrites its whole row and block),
 the bytes written when only dirty sectors are stored (the tail -- tuam, job bits, header -- always), and the number of
 contiguous dirty runs (one bulk store each).  The block tail is counted as always written, so its header fields that
-export_state() does not return (episode steps and return) need not be re-encoded.
+export_state() does not return (episode steps and return) need not be re-encoded.  `state_block_sector_store` is what the
+uniform step kernels store of a block: every sector that holds a changed byte of w0 / w1 / w2, every sector of the
+tail and the block's first sector, each with the block's bytes in it; `per_env_step_total` sets it against whole
+blocks with the changed row sectors (`dirty_rows`) and with whole rows (`today`).
 
   python tools/count_step_bytes.py [--envs N] [--steps S] [--instance ta80]
 """
@@ -131,6 +134,7 @@ def main():
         tail_bytes = g["size"] - g["tail"]
         tot = {k: 0.0 for k in ("obs", "w0", "w1", "w2")}
         full_runs = {"obs": 0.0, "block": 0.0}
+        block_store = 0.0
         blk0, obs0 = snap()
         for _ in range(args.steps):
             *_, acts = env.step_sample(acts, "RANDOM")
@@ -144,6 +148,13 @@ def main():
             ns = bm.shape[1]
             s0 = np.arange(ns)[None, :] * SECTOR - blead[:, None]
             bm_t = bm | (s0 + SECTOR > g["tail"]) & (s0 < g["size"])
+            # the sector store: bm covers the job records only, so widen it to the whole block first
+            nsb = (int(blead.max()) + g["size"] + SECTOR - 1) // SECTOR
+            sb = np.arange(nsb)[None, :] * SECTOR - blead[:, None]
+            stored = np.zeros((n, nsb), bool)
+            stored[:, :ns] = bm
+            stored |= (sb + SECTOR > g["tail"]) & (sb < g["size"]) | (sb <= 0)
+            block_store += sector_bytes(stored, blead, 0, g["size"]).sum()
             full_runs["obs"] += runs(om).sum()
             full_runs["block"] += runs(bm_t).sum()
             blk0, obs0 = blk1, obs1
@@ -156,14 +167,19 @@ def main():
         read = g["size"] + 4
         w_today = sum(today.values()) + other - 4
         w_dirty = sum(dirty.values()) + other - 4
+        w_rows = per["obs"] + g["size"] + other - 4
+        w_store = per["obs"] + block_store / es + other - 4
         print(json.dumps({
             "workload": f"{args.instance} N={n} masked-random auto-reset, pre-rolled (i*7919) mod {TA80_EPISODE}, "
                         f"{args.steps} steps, host emulation",
             "bytes_written_today": today, "bytes_written_dirty_sectors": {k: round(v, 1) for k, v in dirty.items()},
-            "state_block_read": g["size"],
+            "state_block_read": g["size"], "state_block_sector_store": round(block_store / es, 1),
             "per_env_step_total": {"today": w_today + read, "dirty_sectors": round(w_dirty + read, 1),
                                    "saving": round(w_today - w_dirty, 1),
-                                   "saving_frac": round((w_today - w_dirty) / (w_today + read), 4)},
+                                   "saving_frac": round((w_today - w_dirty) / (w_today + read), 4),
+                                   "dirty_rows": round(w_rows + read, 1),
+                                   "dirty_rows_and_block_sectors": round(w_store + read, 1),
+                                   "block_saving_frac": round((w_rows - w_store) / (w_rows + read), 4)},
             "mean_runs_per_env_step": {k: round(v / es, 2) for k, v in full_runs.items()},
         }, indent=1))
 
