@@ -28,6 +28,7 @@ static cudaError_t jss_launch_pdl(void (*kern)(KArgs...), int grid, int block, s
 #endif
 
 #include <algorithm>
+#include <array>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
@@ -173,9 +174,13 @@ int ctas_per_sm(jss_t *h, Kern kern, size_t smem, int &per_sm) {
 }
 
 typedef void (*JssKernel)(JssParams, JssLaunch, JssSmemLayout);
-template <int MODE>   // by lane class
-const JssKernel env_kernels[JSS_LANE_CLASSES] = {jss_env_kernel<1, MODE>, jss_env_kernel<2, MODE>,
-                                                 jss_env_kernel<4, MODE>, jss_env_kernel<8, MODE>};
+// the generic kernel by mode and lane class: the instantiation JSS_MODES[mode].kernel
+template <size_t... MODE>
+std::array<std::array<JssKernel, JSS_LANE_CLASSES>, sizeof...(MODE)> env_kernel_table(std::index_sequence<MODE...>) {
+    return {{{jss_env_kernel<1, JSS_MODES[MODE].kernel>, jss_env_kernel<2, JSS_MODES[MODE].kernel>,
+              jss_env_kernel<4, JSS_MODES[MODE].kernel>, jss_env_kernel<8, JSS_MODES[MODE].kernel>}...}};
+}
+const auto env_kernels = env_kernel_table(std::make_index_sequence<JSS_NUM_MODES>());
 template <int SAMPLE>
 const JssKernel step_kernels[JSS_LANE_CLASSES] = {jss_step_kernel<1, SAMPLE>, jss_step_kernel<2, SAMPLE>,
                                                   jss_step_kernel<4, SAMPLE>, jss_step_kernel<8, SAMPLE>};
@@ -222,28 +227,40 @@ int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
     return JSS_OK;
 }
 
-int launch_all(jss_t *h, JssLaunch a, cudaStream_t st);
+// ranges: the records of each lane class if not its tiles (jss_beam_step's group records)
+int launch_all(jss_t *h, JssLaunch a, cudaStream_t st, const int32_t (*ranges)[2] = nullptr);
 
-// jss_beam_search's shared-memory layout: the instance tables without the suffix sums, env_check_no_op's 32-word
-// table per warp, then the beam region of width W (jss_beam_smem) with blocks of the batch maxima
-JssSmemLayout beam_layout(const jss_t *h) {
+// the shared-memory layout of a launch of a.mode (JSS_SMEM_*), and in `smem` its size: the CTA's region behind the
+// per-warp regions depends on the width or the batch maxima
+JssSmemLayout mode_layout(const jss_t *h, const JssLaunch &a, size_t &smem) {
+    const JssMode &m = JSS_MODES[a.mode];
+    const int bw = jss_block_geom(h->p.jobs_max, h->p.machines_max).words;
     JssSmemLayout sl = h->sl_env;
-    sl.off_warp0 = sl.off_rem;
-    sl.warp_stride = 32 * 4;
+    if (m.smem != JSS_SMEM_ENV) sl.off_warp0 = sl.off_rem;                      // no suffix sums
+    if (m.smem == JSS_SMEM_BEAM || m.smem == JSS_SMEM_IMPROVE) sl.warp_stride = 32 * 4;   // env_check_no_op's table
+    smem = smem_bytes(sl);
+    if (m.smem == JSS_SMEM_BEAM) smem += jss_beam_smem(nullptr, a.beam_width, bw, nullptr, m.keys);
+    if (m.smem == JSS_SMEM_BEAM_STEP) smem += jss_beam_smem(nullptr, a.beam_width, bw, nullptr, m.keys, 1);
+    if (m.smem == JSS_SMEM_IMPROVE) smem += jss_improve_smem(nullptr, h->p.jobs_max, h->p.machines_max, nullptr);
     return sl;
 }
-size_t beam_smem(const jss_t *h, int W, bool swor) {
-    return smem_bytes(beam_layout(h)) +
-           jss_beam_smem(nullptr, W, jss_block_geom(h->p.jobs_max, h->p.machines_max).words, nullptr, swor);
-}
-// the persistent grid of lane class c's beam search launch (swor: the stochastic one): one work item per env, at most
-// the resident CTAs
-int beam_grid(jss_t *h, int c, int W, bool swor, int &grid) {
-    const int n_items = (h->class_tiles[c][1] - h->class_tiles[c][0]) * JSS_WARPS_PER_CTA;
+
+// the grid of lane class c's launch of a.mode over the tiles (or records) [a.tile_begin, a.tile_end) at `smem` bytes
+// (JSS_GRID_*); a launch that spreads its tiles' candidates or samples also gets its split S in a.n_steps
+int mode_grid(jss_t *h, JssLaunch &a, int c, size_t smem, int &grid) {
+    const JssMode &m = JSS_MODES[a.mode];
+    const int n = a.tile_end - a.tile_begin;
     int per_sm = 0;
-    const JssKernel k = swor ? env_kernels<JSS_MODE_SWOR>[c] : env_kernels<JSS_MODE_BEAM_SEARCH>[c];
-    if (int rc = ctas_per_sm(h, k, beam_smem(h, W, swor), per_sm)) return rc;
-    grid = std::min(n_items, h->sm_count * per_sm);
+    if (int rc = ctas_per_sm(h, env_kernels[a.mode][c], smem, per_sm)) return rc;
+    const int slots = h->sm_count * per_sm;
+    if (m.grid == JSS_GRID_SPREAD_J || m.grid == JSS_GRID_SPREAD_K) {
+        const int most = m.grid == JSS_GRID_SPREAD_J ? std::min(h->p.jobs_max, 32 << c) + 1 : a.n_samples;
+        a.n_steps = n >= slots ? 1 : std::min(most, (slots + n - 1) / n);
+    }
+    const int64_t items = m.item == JSS_ITEM_SPLIT ? (int64_t)n * a.n_steps
+                        : m.item == JSS_ITEM_ENV ? (int64_t)n * JSS_WARPS_PER_CTA
+                        : m.item == JSS_ITEM_ORDER ? (int64_t)n * JSS_WARPS_PER_CTA * a.n_samples : n;
+    grid = (int)(m.grid == JSS_GRID_ALL ? items : std::min<int64_t>(items, slots));
     return JSS_OK;
 }
 
@@ -257,69 +274,25 @@ int refresh_obs(jss_t *h, cudaStream_t st) {
     return JSS_OK;
 }
 
-int launch_all(jss_t *h, JssLaunch a, cudaStream_t st) {
-    // every launch that may read or partly rewrite real_obs brings it up to date first, so each entry point keeps its
-    // meaning after a recording step (a plain step rewrites only the envs it changes)
-    const bool recording = a.mode == JSS_MODE_STEP && a.traj_obs;
-    const bool lookahead = a.mode == JSS_MODE_LOOKAHEAD || a.mode == JSS_MODE_LOOKAHEAD_PRIORITY;
-    const bool samples = jss_mode_samples(a.mode), swor = a.mode == JSS_MODE_SWOR;
-    const bool beam = a.mode == JSS_MODE_BEAM_SEARCH || swor;
-    if (!recording && a.mode != JSS_MODE_EXPORT && a.mode != JSS_MODE_POLICY && a.mode != JSS_MODE_REFRESH &&
-        !lookahead && !samples && !beam)                 // these read only state blocks and write the caller's buffers
+// a plain step: the fused step kernel; every other mode: the generic kernel, one launch per lane class present
+int launch_all(jss_t *h, JssLaunch a, cudaStream_t st, const int32_t (*ranges)[2]) {
+    const JssMode &m = JSS_MODES[a.mode];
+    if (m.refresh == JSS_REFRESH_YES || (m.refresh == JSS_REFRESH_UNLESS_RECORDING && !a.traj_obs))
         if (int rc = refresh_obs(h, st)) return rc;
     if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
     if (a.mode == JSS_MODE_STEP && !a.export_after) return launch_step(h, a, st);   // one launch, whatever the mix of lane classes
-    // the generic kernel: MODE = JSS_MODE_RESET also serves export, import, pack, refresh and exporting steps
-    const JssKernel *kerns = a.mode == JSS_MODE_POLICY ? env_kernels<JSS_MODE_POLICY>
-                           : a.mode == JSS_MODE_ROLLOUT ? env_kernels<JSS_MODE_ROLLOUT>
-                           : a.mode == JSS_MODE_PRIORITY ? env_kernels<JSS_MODE_PRIORITY>
-                           : a.mode == JSS_MODE_PRIORITY_SAMPLE ? env_kernels<JSS_MODE_PRIORITY_SAMPLE>
-                           : a.mode == JSS_MODE_LOOKAHEAD ? env_kernels<JSS_MODE_LOOKAHEAD>
-                           : a.mode == JSS_MODE_LOOKAHEAD_PRIORITY ? env_kernels<JSS_MODE_LOOKAHEAD_PRIORITY>
-                           : a.mode == JSS_MODE_SAMPLE_EPISODES ? env_kernels<JSS_MODE_SAMPLE_EPISODES>
-                           : a.mode == JSS_MODE_SAMPLE_EPISODES_GRAD ? env_kernels<JSS_MODE_SAMPLE_EPISODES_GRAD>
-                           : a.mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION ? env_kernels<JSS_MODE_SAMPLE_EPISODES_SOLUTION>
-                           : a.mode == JSS_MODE_ORDER_LOG_PROB ? env_kernels<JSS_MODE_ORDER_LOG_PROB>
-                           : a.mode == JSS_MODE_ORDER_LOG_PROB_GRAD ? env_kernels<JSS_MODE_ORDER_LOG_PROB_GRAD>
-                           : swor ? env_kernels<JSS_MODE_SWOR>
-                           : beam ? env_kernels<JSS_MODE_BEAM_SEARCH>
-                           : env_kernels<JSS_MODE_RESET>;
-    // what the launch reads: a rollout or lookahead every table; a policy what its rule reads, ops / len (+ suffix sums for MWR / LWR
-    // / CR), and the masked-uniform sampler no table at all (only J); the other modes ops / len (the lookahead over a
-    // priority table too: the caller's table replaces the suffix sums)
-    a.stage = a.mode == JSS_MODE_ROLLOUT || a.mode == JSS_MODE_LOOKAHEAD ? JSS_STAGE_ALL
-            : a.mode != JSS_MODE_POLICY ? JSS_STAGE_OPS
+    a.stage = m.stage != JSS_STAGE_BY_RULE ? m.stage
             : a.rule == JSS_RULE_RANDOM ? 0 : jss_rule_wants_rem(a.rule) ? JSS_STAGE_ALL : JSS_STAGE_OPS;
-    const JssSmemLayout sl = beam ? beam_layout(h) : h->sl_env;
-    const size_t smem = beam ? beam_smem(h, a.beam_width, swor) : smem_bytes(sl);
-    for (int c = 0; c < JSS_LANE_CLASSES; c++) {   // one launch per lane class present
-        a.tile_begin = h->class_tiles[c][0];
-        a.tile_end = h->class_tiles[c][1];
-        const int n_tiles = a.tile_end - a.tile_begin;
-        if (n_tiles <= 0) continue;
-        int per_sm = 0, rc = ctas_per_sm(h, kerns[c], smem, per_sm);
-        if (rc) return rc;
-        // policy kernels touch ~50 B per env: latency-bound, so give every tile its own CTA
-        // instead of a persistent loop with a dependent load per iteration
-        const int slots = h->sm_count * per_sm;
-        int grid = (a.mode == JSS_MODE_POLICY) ? n_tiles : std::min(n_tiles, slots);
-        if (lookahead) {
-            // spread each tile's candidates over S work items when the tiles alone leave resident CTA slots empty:
-            // S = 1 once they fill the SMs, up to the class's J + 1 (one candidate per item) for a small batch
-            const int jc = std::min(h->p.jobs_max, 32 << c);
-            a.n_steps = n_tiles >= slots ? 1 : std::min(jc + 1, (slots + n_tiles - 1) / n_tiles);
-            grid = std::min(n_tiles * a.n_steps, slots);
-        } else if (samples) {
-            // the draws (and the order likelihoods): each tile's K samples spread over S work items in the same way, up
-            // to S = K; the gradients keep the caller's split (one work item per chunk), the solution replay one work
-            // item per tile
-            if (a.mode == JSS_MODE_SAMPLE_EPISODES || a.mode == JSS_MODE_ORDER_LOG_PROB)
-                a.n_steps = n_tiles >= slots ? 1 : std::min(a.n_samples, (slots + n_tiles - 1) / n_tiles);
-            grid = (int)std::min<int64_t>((int64_t)n_tiles * a.n_steps, slots);
-        } else if (beam) {
-            if (int rc = beam_grid(h, c, a.beam_width, swor, grid)) return rc;   // the grid the trace is sized for
-        }
-        JSS_LAUNCH(kerns[c], grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
+    size_t smem = 0;
+    const JssSmemLayout sl = mode_layout(h, a, smem);
+    if (!ranges) ranges = h->class_tiles;
+    for (int c = 0; c < JSS_LANE_CLASSES; c++) {
+        a.tile_begin = ranges[c][0];
+        a.tile_end = ranges[c][1];
+        if (a.tile_end <= a.tile_begin) continue;
+        int grid = 0;
+        if (int rc = mode_grid(h, a, c, smem, grid)) return rc;
+        JSS_LAUNCH(env_kernels[a.mode][c], grid, JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
         JSS_CUDA(h, cudaGetLastError());
         h->launches += 1;
     }
@@ -980,15 +953,20 @@ bool bad_ptr(const void *ptr) { return !ptr || ((uintptr_t)ptr & 3u); }
 
 // a.beam_trace for a (stochastic) beam search of width W that writes orders: W backpointers per round (at most
 // jobs_max * machines_max rounds) for each CTA of the largest grid, owned by the handle and grown as needed
-int beam_trace(jss_t *h, int width, bool swor, JssLaunch &a) {
+int beam_trace(jss_t *h, JssLaunch &a) {
+    JssLaunch g = a;
+    size_t smem = 0;
+    mode_layout(h, g, smem);
     int grid_max = 0;
     for (int c = 0; c < JSS_LANE_CLASSES; c++) {
-        if (h->class_tiles[c][1] <= h->class_tiles[c][0]) continue;
+        g.tile_begin = h->class_tiles[c][0];
+        g.tile_end = h->class_tiles[c][1];
+        if (g.tile_end <= g.tile_begin) continue;
         int grid = 0;
-        if (int rc = beam_grid(h, c, width, swor, grid)) return rc;
+        if (int rc = mode_grid(h, g, c, smem, grid)) return rc;
         grid_max = std::max(grid_max, grid);
     }
-    const size_t need = (size_t)grid_max * width * h->p.jobs_max * h->p.machines_max * sizeof(uint16_t);
+    const size_t need = (size_t)grid_max * a.beam_width * h->p.jobs_max * h->p.machines_max * sizeof(uint16_t);
     if (need > h->beam_trace_bytes) {
         if (h->beam_trace) {                             // cudaFree waits for the launches that may still use it
             JSS_CUDA(h, cudaFree(h->beam_trace));
@@ -1110,7 +1088,7 @@ int jss_beam_search(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t l
     a.log_prob_out = score_out_dev;
     a.samples_ld = ld;
     a.order_out = order_out_dev;
-    if (order_out_dev && (rc = beam_trace(h, width, false, a))) return rc;
+    if (order_out_dev && (rc = beam_trace(h, a))) return rc;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 
@@ -1140,7 +1118,7 @@ int jss_sample_without_replacement(jss_t *h, const float *logits_dev, int64_t ld
     a.key_out = key_out_dev;
     a.samples_ld = ld;
     a.order_out = order_out_dev;
-    if (order_out_dev && (rc = beam_trace(h, width, true, a))) return rc;
+    if (order_out_dev && (rc = beam_trace(h, a))) return rc;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 
@@ -1196,16 +1174,7 @@ int beam_groups(jss_t *h, const char *who, int W, const jss_handle::BeamGroups *
     return JSS_OK;
 }
 
-// jss_beam_step's shared-memory layout: the instance tables without the suffix sums, the observation staging per warp
-// (which env_check_no_op's table shares), then the beam region of width W with one buffer of blocks of the batch maxima
-JssSmemLayout beam_step_layout(const jss_t *h) {
-    JssSmemLayout sl = h->sl_env;
-    sl.off_warp0 = sl.off_rem;
-    return sl;
-}
-
-// jss_beam_step and jss_stochastic_beam_step (key_dev non-NULL): the checks, the group records and one launch per lane
-// class present
+// jss_beam_step and jss_stochastic_beam_step (key_dev non-NULL): the checks and the group records
 int beam_step_launch(jss_t *h, const char *who, const float *logits_dev, int64_t ld, int width, uint64_t seed,
                      uint64_t step_index, float *score_dev, float *key_dev, int32_t *parent_out_dev,
                      int32_t *action_out_dev, int32_t *bad_out_dev, void *stream) {
@@ -1223,11 +1192,8 @@ int beam_step_launch(jss_t *h, const char *who, const float *logits_dev, int64_t
     int rc;
     const jss_handle::BeamGroups *bg = nullptr;
     if ((rc = beam_groups(h, who, width, bg))) return rc;
-    const cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = refresh_obs(h, st))) return rc;            // the untouched rows must be current, as after any call
     JssLaunch a{};
     a.mode = swor ? JSS_MODE_STOCHASTIC_BEAM_STEP : JSS_MODE_BEAM_STEP;
-    a.stage = JSS_STAGE_OPS;
     a.beam_width = width;
     a.beam_groups = bg->dev;
     a.logits = logits_dev;
@@ -1241,23 +1207,7 @@ int beam_step_launch(jss_t *h, const char *who, const float *logits_dev, int64_t
         a.hash_key = jss_fold32(seed);                   // jss_hash3 reads the seed only through its fold
         a.sample_step_index = step_index;
     }
-    if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
-    const JssSmemLayout sl = beam_step_layout(h);
-    const size_t smem = smem_bytes(sl) + jss_beam_smem(nullptr, width, jss_block_geom(h->p.jobs_max, h->p.machines_max).words,
-                                                       nullptr, swor, 1);
-    for (int c = 0; c < JSS_LANE_CLASSES; c++) {         // one launch per lane class present
-        a.tile_begin = bg->ranges[c][0];
-        a.tile_end = bg->ranges[c][1];
-        const int n_groups = a.tile_end - a.tile_begin;
-        if (n_groups <= 0) continue;
-        const JssKernel k = swor ? env_kernels<JSS_MODE_STOCHASTIC_BEAM_STEP>[c] : env_kernels<JSS_MODE_BEAM_STEP>[c];
-        int per_sm = 0;
-        if ((rc = ctas_per_sm(h, k, smem, per_sm))) return rc;
-        JSS_LAUNCH(k, std::min(n_groups, h->sm_count * per_sm), JSS_WARPS_PER_CTA * 32, smem, st, h->p, a, sl);
-        JSS_CUDA(h, cudaGetLastError());
-        h->launches += 1;
-    }
-    return JSS_OK;
+    return launch_all(h, a, (cudaStream_t)stream, bg->ranges);
 }
 
 }  // namespace
@@ -1372,7 +1322,6 @@ int jss_improve_orders(jss_t *h, const int32_t *order_dev, int64_t k, int max_mo
         }
     JssLaunch a{};
     a.mode = JSS_MODE_IMPROVE_ORDERS;
-    a.stage = JSS_STAGE_OPS;
     a.order_in = order_dev;
     a.n_samples = (int)k;
     a.samples_ld = ld;
@@ -1381,23 +1330,7 @@ int jss_improve_orders(jss_t *h, const int32_t *order_dev, int64_t k, int max_mo
     a.actions_out = makespan_out_dev;
     a.start_out = start_makespan_out_dev;
     a.moves_out = moves_out_dev;
-    if (h->p.uniform_inst >= 0) a.uni = h->insts[h->p.uniform_inst];
-    const JssSmemLayout sl = beam_layout(h);
-    const size_t smem = smem_bytes(sl) + jss_improve_smem(nullptr, h->p.jobs_max, h->p.machines_max, nullptr);
-    for (int c = 0; c < JSS_LANE_CLASSES; c++) {         // one launch per lane class present
-        a.tile_begin = h->class_tiles[c][0];
-        a.tile_end = h->class_tiles[c][1];
-        const int64_t n_items = (int64_t)(a.tile_end - a.tile_begin) * JSS_WARPS_PER_CTA * k;
-        if (n_items <= 0) continue;
-        const JssKernel kern = env_kernels<JSS_MODE_IMPROVE_ORDERS>[c];
-        int per_sm = 0;
-        if ((rc = ctas_per_sm(h, kern, smem, per_sm))) return rc;
-        const int grid = (int)std::min<int64_t>(n_items, (int64_t)h->sm_count * per_sm);
-        JSS_LAUNCH(kern, grid, JSS_WARPS_PER_CTA * 32, smem, (cudaStream_t)stream, h->p, a, sl);
-        JSS_CUDA(h, cudaGetLastError());
-        h->launches += 1;
-    }
-    return JSS_OK;
+    return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_step_host(jss_t *h, const int32_t *actions_host, uint8_t *mask_host, float *obs_host,

@@ -25,6 +25,7 @@
 #pragma once
 #include <stdint.h>
 #include <string.h>
+#include <type_traits>
 
 #include "../../include/jss_b200.h"
 #include "jss_rng.h"
@@ -1370,6 +1371,19 @@ JSS_DEV void jss_stage_instance(const JssParams &p, const JssInst &d, const JssC
     }
 }
 
+// a CTA-uniform work item of instance `inst`: stage its tables (`what`) unless `staged` is that instance already, then
+// refresh iv's J / M; returns the instance staged now
+JSS_DEV int jss_restage(const JssParams &p, const JssCtaSmem &c, InstView &iv, int inst, int staged, int what) {
+    if (inst != staged) {
+        __syncthreads();
+        jss_stage_instance(p, p.inst[inst], c, what);
+        staged = inst;
+        __syncthreads();
+    }
+    jss_iv_shape(iv);
+    return staged;
+}
+
 template <int KJ, bool BULK = false, bool DIRTY = false>
 JSS_DEV void env_emit_all(const JssParams &p, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
                           float *scratch, int raw, jss_saddr_t scratch_sa = jss_saddr_t(), void *st_dst = nullptr,
@@ -2490,60 +2504,131 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
     }
 }
 
-// Resident CTAs per SM the generic kernel is built for: one, except in the priority loop, which carries none of the
-// rules' code and keeps each env on chip for a whole episode, so that more warps per SM hide its latency.
-// The sampling loop likewise: the largest count per lane class that builds without a stack frame or spills (one CTA
-// more spills in every class).
-constexpr int JSS_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 3, 2};
-constexpr int JSS_PRIORITY_SAMPLE_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 2};
-// The lookahead loop likewise (the rules' code, but no output emission).
-constexpr int JSS_LOOKAHEAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 4, 3, 2};
-// The lookahead over a priority table likewise (the table's argmax in place of the rules): 31 / 48 / 56 / 80 registers
-// (CUDA 12.9, sm_90a); one CTA more spills in the classes with 2, 4 and 8 jobs per lane, and 8 is the SM's limit.
-constexpr int JSS_LOOKAHEAD_PRIORITY_MIN_CTAS[JSS_LANE_CLASSES] = {8, 5, 4, 3};
-// The sampled episodes likewise, per mode (CUDA 12.9, sm_90a): the draws at 32 / 32 / 39 / 72 registers, their replay
-// with the gradient adds at 56 / 64 / 64 / 122, the solution replay at 40 / 48 / 40 / 72.  ptxas is not monotonic
-// here: the draws with 4 jobs per lane spill at 5 CTAs but not at 6, and spill again at 7.
-constexpr int JSS_SAMPLE_EPISODES_MIN_CTAS[JSS_LANE_CLASSES] = {8, 8, 6, 3};
-constexpr int JSS_SAMPLE_EPISODES_GRAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 4, 4, 2};
-constexpr int JSS_SAMPLE_EPISODES_SOLUTION_MIN_CTAS[JSS_LANE_CLASSES] = {6, 5, 6, 3};
-// The beam search likewise: 60 / 75 / 113 / 175 registers (CUDA 12.9, sm_90a); one CTA more spills in the classes with
-// 2, 4 and 8 jobs per lane.  Its shared memory (2 W state blocks) bounds the resident CTAs at large W anyway.
-constexpr int JSS_BEAM_SEARCH_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
-// The stochastic beam search likewise: 64 / 75 / 113 / 176 registers (CUDA 12.9, sm_90a).  The order likelihood at
-// 40 / 62 / 64 / 92 registers, its gradient at 64 / 72 / 64 / 143; one CTA more spills in every class of the
-// likelihood but the one with 1 job per lane (untried at 7), and in the classes with 2 and 8 jobs per lane of the
-// gradient.
-constexpr int JSS_SWOR_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
-constexpr int JSS_ORDER_LOG_PROB_MIN_CTAS[JSS_LANE_CLASSES] = {6, 4, 4, 2};
-constexpr int JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 4, 1};
-// The beam round of jss_beam_step likewise (CUDA 12.9, sm_90a; DESIGN.md section 4), and its stochastic form.
-constexpr int JSS_BEAM_STEP_MIN_CTAS[JSS_LANE_CLASSES] = {4, 3, 2, 1};
-constexpr int JSS_STOCHASTIC_BEAM_STEP_MIN_CTAS[JSS_LANE_CLASSES] = {3, 3, 2, 1};
-// The critical-path descent likewise: 32 / 40 / 60 / 116 registers (CUDA 12.9, sm_90a); 8 is the SM's limit, and one
-// CTA more spills with 8 jobs per lane.  Its shared memory (three [J][M] tables) bounds the resident CTAs at large J M.
-constexpr int JSS_IMPROVE_ORDERS_MIN_CTAS[JSS_LANE_CLASSES] = {8, 6, 4, 2};
-JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) {
-    return mode == JSS_MODE_PRIORITY ? JSS_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_PRIORITY_SAMPLE ? JSS_PRIORITY_SAMPLE_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_LOOKAHEAD ? JSS_LOOKAHEAD_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_LOOKAHEAD_PRIORITY ? JSS_LOOKAHEAD_PRIORITY_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_SAMPLE_EPISODES ? JSS_SAMPLE_EPISODES_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_SAMPLE_EPISODES_GRAD ? JSS_SAMPLE_EPISODES_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION ? JSS_SAMPLE_EPISODES_SOLUTION_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_BEAM_SEARCH ? JSS_BEAM_SEARCH_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_SWOR ? JSS_SWOR_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_ORDER_LOG_PROB ? JSS_ORDER_LOG_PROB_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_ORDER_LOG_PROB_GRAD ? JSS_ORDER_LOG_PROB_GRAD_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_BEAM_STEP ? JSS_BEAM_STEP_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_STOCHASTIC_BEAM_STEP ? JSS_STOCHASTIC_BEAM_STEP_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : mode == JSS_MODE_IMPROVE_ORDERS ? JSS_IMPROVE_ORDERS_MIN_CTAS[jss_lane_class(32 * KJ)]
-         : 1;
+// ---- the modes of the generic kernel: one row each (JSS_MODES) ---------------------------------------------------
+// What one work item of jss_env_kernel's CTA-strided loop is; launch_all counts the items of a class by the same rule.
+#define JSS_ITEM_WARP 0    // a tile, one env per warp (the items are the class's tiles themselves)
+#define JSS_ITEM_SPLIT 1   // (tile, s), s < S = a.n_steps: warp w takes env w of the tile and share s of its candidates
+                           // or samples; a tile's S items are adjacent and share its instance
+#define JSS_ITEM_ENV 2     // one env of the class's tiles per CTA
+#define JSS_ITEM_ORDER 3   // one (env, order) per CTA: env slot item / K of the class's tiles, order item % K
+                           // (K = a.n_samples; 64-bit items)
+#define JSS_ITEM_GROUP 4   // one group record of a.beam_groups per CTA (the items are the class's records themselves)
+// The grid of a launch over `items` work items with `slots` resident CTAs.
+#define JSS_GRID_ALL 0        // one CTA per item: a policy touches ~50 B per env and is latency-bound, so every tile
+                              // gets its own CTA instead of a persistent loop with a dependent load per iteration
+#define JSS_GRID_RESIDENT 1   // min(items, slots)
+#define JSS_GRID_SPREAD_J 2   // the same, with each tile's candidates spread over S items while the tiles alone leave
+                              // slots empty: S = 1 once they fill them, up to the class's J + 1 for a small batch
+#define JSS_GRID_SPREAD_K 3   // the same, up to S = K samples per tile
+// The host stages what the rule reads: ops / len, + the suffix sums for MWR / LWR / CR, no table for the masked-uniform
+// sampler (it reads only J)
+#define JSS_STAGE_BY_RULE (-1)
+// Shared-memory layout families (jss_api.cu): [instance tables][8 per-warp regions][the CTA's region]
+#define JSS_SMEM_ENV 0         // every table; per warp the observation staging, which env_check_no_op's table shares
+#define JSS_SMEM_BEAM 1        // no suffix sums; per warp env_check_no_op's table; two buffers of W beams (jss_beam_smem)
+#define JSS_SMEM_BEAM_STEP 2   // no suffix sums; per warp the observation staging; one buffer of W beams
+#define JSS_SMEM_IMPROVE 3     // no suffix sums; per warp env_check_no_op's table; the improvement region
+                               // (jss_improve_smem)
+// Whether launch_all first rewrites a real_obs that a recording step left stale: a mode that may read or partly
+// rewrite real_obs does; one that reads only the state blocks and writes the caller's buffers does not.
+#define JSS_REFRESH_NO 0
+#define JSS_REFRESH_YES 1
+#define JSS_REFRESH_UNLESS_RECORDING 2   // a step recording into the caller's slot (a.traj_obs) does not
+struct JssMode {
+    int kernel;                       // the JSS_MODE_* whose jss_env_kernel instantiation runs the mode
+    int min_ctas[JSS_LANE_CLASSES];   // resident CTAs per SM that kernel is built for, by lane class (launch bound)
+    int item, grid, stage, smem;      // JSS_ITEM_*, JSS_GRID_*, JSS_STAGE_*, JSS_SMEM_*
+    bool keys;                        // beam layouts: every slot also carries a Gumbel key
+    int refresh;                      // JSS_REFRESH_*
+};
+// Resident CTAs: one, except in the loops that keep an env on chip for a whole episode or rollout, so that more warps
+// per SM hide their latency: there the largest count per lane class that builds without a stack frame or spills
+// (ptxas registers by class, CUDA 12.9, sm_90a).
+constexpr JssMode JSS_MODES[] = {
+    // RESET also runs a step that exports (facade), export, import, pack and refresh
+    {JSS_MODE_RESET, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false, JSS_REFRESH_YES},
+    {JSS_MODE_RESET, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_UNLESS_RECORDING},                                                                       // STEP
+    {JSS_MODE_ROLLOUT, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_ALL, JSS_SMEM_ENV, false,
+     JSS_REFRESH_YES},
+    {JSS_MODE_POLICY, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_ALL, JSS_STAGE_BY_RULE, JSS_SMEM_ENV, false, JSS_REFRESH_NO},
+    {JSS_MODE_RESET, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},                                                                                     // EXPORT
+    {JSS_MODE_RESET, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_YES},                                                                                    // IMPORT
+    {JSS_MODE_RESET, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_YES},                                                                                    // PACK
+    {JSS_MODE_RESET, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},                                                                                     // REFRESH
+    // the priority loop carries none of the rules' code; its sampling form: one CTA more spills in every class
+    {JSS_MODE_PRIORITY, {4, 3, 3, 2}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_YES},
+    {JSS_MODE_PRIORITY_SAMPLE, {4, 3, 4, 2}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_YES},
+    // the lookahead loop: the rules' code, but no output emission; over a priority table (the table's argmax in place
+    // of the rules) 31 / 48 / 56 / 80 registers, one CTA more spills in the classes with 2, 4 and 8 jobs per lane, and 8
+    // is the SM's limit
+    {JSS_MODE_LOOKAHEAD, {4, 4, 3, 2}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_J, JSS_STAGE_ALL, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},
+    {JSS_MODE_LOOKAHEAD_PRIORITY, {8, 5, 4, 3}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_J, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},
+    // the sampled episodes: the draws at 32 / 32 / 39 / 72 registers, their replay with the gradient adds (the caller's
+    // split) at 56 / 64 / 64 / 122, the solution replay (S = 1) at 40 / 48 / 40 / 72.  ptxas is not monotonic here: the
+    // draws with 4 jobs per lane spill at 5 CTAs but not at 6, and spill again at 7.
+    {JSS_MODE_SAMPLE_EPISODES, {8, 8, 6, 3}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_K, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},
+    {JSS_MODE_SAMPLE_EPISODES_GRAD, {4, 4, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV,
+     false, JSS_REFRESH_NO},
+    {JSS_MODE_SAMPLE_EPISODES_SOLUTION, {6, 5, 6, 3}, JSS_ITEM_SPLIT, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV,
+     false, JSS_REFRESH_NO},
+    // the beam search: 60 / 75 / 113 / 175 registers, one CTA more spills in the classes with 2, 4 and 8 jobs per lane;
+    // its shared memory (2 W state blocks) bounds the resident CTAs at large W anyway.  The stochastic one: 64 / 75 /
+    // 113 / 176 registers.
+    {JSS_MODE_BEAM_SEARCH, {4, 3, 2, 1}, JSS_ITEM_ENV, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_BEAM, false,
+     JSS_REFRESH_NO},
+    {JSS_MODE_SWOR, {4, 3, 2, 1}, JSS_ITEM_ENV, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_BEAM, true, JSS_REFRESH_NO},
+    // the order likelihood at 40 / 62 / 64 / 92 registers, its gradient at 64 / 72 / 64 / 143; one CTA more spills in
+    // every class of the likelihood but the one with 1 job per lane (untried at 7), and in the classes with 2 and 8 jobs
+    // per lane of the gradient
+    {JSS_MODE_ORDER_LOG_PROB, {6, 4, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_K, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},
+    {JSS_MODE_ORDER_LOG_PROB_GRAD, {4, 3, 4, 1}, JSS_ITEM_SPLIT, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},
+    // the beam round of jss_beam_step (DESIGN.md section 4), and its stochastic form
+    {JSS_MODE_BEAM_STEP, {4, 3, 2, 1}, JSS_ITEM_GROUP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_BEAM_STEP, false,
+     JSS_REFRESH_YES},
+    {JSS_MODE_STOCHASTIC_BEAM_STEP, {3, 3, 2, 1}, JSS_ITEM_GROUP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_BEAM_STEP,
+     true, JSS_REFRESH_YES},
+    // the critical-path descent: 32 / 40 / 60 / 116 registers; 8 is the SM's limit, and one CTA more spills with 8 jobs
+    // per lane.  Its shared memory (three [J][M] tables) bounds the resident CTAs at large J M.
+    {JSS_MODE_IMPROVE_ORDERS, {8, 6, 4, 2}, JSS_ITEM_ORDER, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_IMPROVE, false,
+     JSS_REFRESH_NO},
+};
+static_assert(sizeof(JSS_MODES) / sizeof(JSS_MODES[0]) == JSS_NUM_MODES, "one row per JSS_MODE_*");
+// a mode that another mode's kernel runs has that kernel's loop, tables, layout and launch bound
+constexpr bool jss_modes_agree() {
+    for (const JssMode &m : JSS_MODES) {
+        const JssMode &k = JSS_MODES[m.kernel];
+        bool same = k.kernel == m.kernel && k.item == m.item && k.stage == m.stage && k.smem == m.smem && k.keys == m.keys;
+        for (int c = 0; c < JSS_LANE_CLASSES; c++) same = same && k.min_ctas[c] == m.min_ctas[c];
+        if (!same) return false;
+    }
+    return true;
 }
+static_assert(jss_modes_agree(), "JSS_MODES: a row disagrees with the row of the kernel that runs it");
+JSS_HD constexpr int jss_env_min_ctas(int KJ, int mode) { return JSS_MODES[mode].min_ctas[jss_lane_class(32 * KJ)]; }
 
+// One launch of a mode over the work items of one lane class, CTA-strided: [a.tile_begin, a.tile_end) where the items
+// are the tiles or group records themselves, else [0, n) decoded by the mode's item shape.  An item restages the
+// instance tables when its instance changes, then runs the mode's body.  An empty warp slot is skipped before staging
+// where an item is one env (CTA-uniform), after it where a tile's warps share the item.
 template <int KJ, int MODE>
 __global__ void __launch_bounds__(JSS_WARPS_PER_CTA * 32, jss_env_min_ctas(KJ, MODE))
 jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
+    constexpr JssMode M = JSS_MODES[MODE];
+    constexpr bool BY_INDEX = M.item == JSS_ITEM_WARP || M.item == JSS_ITEM_GROUP;
+    constexpr bool PER_WARP = M.item == JSS_ITEM_WARP || M.item == JSS_ITEM_SPLIT;
+    using Item = std::conditional_t<M.item == JSS_ITEM_ORDER, int64_t, int>;
     JSS_SMEM_DECL(jss_smem);
     char *sm = reinterpret_cast<char *>(jss_smem);
     JssCtaSmem c;
@@ -2551,110 +2636,43 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     jss_cta_carve(sl, sm, c, iv);
     const int warp = jss_warp_index(), lane = threadIdx.x & 31;
     float *scratch = reinterpret_cast<float *>(sm + sl.off_warp0 + warp * sl.warp_stride);
-    if (MODE == JSS_MODE_BEAM_SEARCH || MODE == JSS_MODE_SWOR) {
-        // work item = one env (tile, warp slot), CTA-strided; the per-warp regions hold only env_check_no_op's table,
-        // and the beam region follows them
-        char *bsm = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;
-        const int n_items = (a.tile_end - a.tile_begin) * JSS_WARPS_PER_CTA;
-        int staged = -1;
-        for (int item = (int)blockIdx.x; item < n_items; item += (int)gridDim.x) {
-            const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, a.tile_begin + item / JSS_WARPS_PER_CTA,
-                                           item % JSS_WARPS_PER_CTA);
-            const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
-            if (env < 0) continue;                       // CTA-uniform
-            if (inst != staged) {
-                __syncthreads();
-                jss_stage_instance(p, p.inst[inst], c, JSS_STAGE_OPS);
-                staged = inst;
-                __syncthreads();
-            }
-            jss_iv_shape(iv);
-            env_beam_search<KJ, MODE == JSS_MODE_SWOR>(p, a, iv, env, p.state + (size_t)t.off16 * 4, warp, lane,
-                                                       reinterpret_cast<int *>(scratch), bsm);
-        }
-        return;
-    }
-    if (MODE == JSS_MODE_BEAM_STEP || MODE == JSS_MODE_STOCHASTIC_BEAM_STEP) {
-        // work item = one group record, CTA-strided; the per-warp regions are the observation staging (emission), and
-        // the beam region follows them
-        char *bsm = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;
-        int staged = -1;
-        for (int item = a.tile_begin + (int)blockIdx.x; item < a.tile_end; item += (int)gridDim.x) {
-            const int32_t *rec = a.beam_groups + (size_t)item * (a.beam_width + 2);
-            const int inst = jss_uniform(rec[1]);
-            if (inst != staged) {                        // CTA-uniform
-                __syncthreads();
-                jss_stage_instance(p, p.inst[inst], c, JSS_STAGE_OPS);
-                staged = inst;
-                __syncthreads();
-            }
-            jss_iv_shape(iv);
-            env_beam_step<KJ, MODE == JSS_MODE_STOCHASTIC_BEAM_STEP>(p, a, iv, rec, warp, lane, scratch, bsm);
-        }
-        return;
-    }
-    if (MODE == JSS_MODE_IMPROVE_ORDERS) {
-        // work item = one (env, order): env slot e = item / K of the class's tiles, order item % K, CTA-strided; the
-        // per-warp regions hold only env_check_no_op's table, and the improvement region follows them
-        char *ism = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;
-        const int64_t K = a.n_samples, n_items = (int64_t)(a.tile_end - a.tile_begin) * JSS_WARPS_PER_CTA * K;
-        int staged = -1;
-        for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
-            const int64_t e = item / K;
-            const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, a.tile_begin + (int)(e / JSS_WARPS_PER_CTA),
-                                           (int)(e % JSS_WARPS_PER_CTA));
-            const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
-            if (env < 0) continue;                       // CTA-uniform
-            if (inst != staged) {
-                __syncthreads();
-                jss_stage_instance(p, p.inst[inst], c, JSS_STAGE_OPS);
-                staged = inst;
-                __syncthreads();
-            }
-            jss_iv_shape(iv);
-            env_improve_order<KJ>(p, a, iv, env, (int)(item - e * K), p.state + (size_t)t.off16 * 4, warp, lane,
-                                  reinterpret_cast<int *>(scratch), ism);
-        }
-        return;
-    }
-    if (MODE == JSS_MODE_LOOKAHEAD || MODE == JSS_MODE_LOOKAHEAD_PRIORITY || jss_mode_samples(MODE)) {
-        // work items (tile, sp), sp = 0 .. S-1, CTA-strided; a tile's S items are adjacent and share its instance.  The
-        // rules read every table; the priority table replaces the suffix sums, so that lookahead stages ops / len only
-        // (and so do the sampled episodes)
-        constexpr bool PRIO = MODE != JSS_MODE_LOOKAHEAD;
-        const int S = a.n_steps, n_items = (a.tile_end - a.tile_begin) * S;
-        int staged = -1;
-        for (int item = (int)blockIdx.x; item < n_items; item += (int)gridDim.x) {
-            const int tile = a.tile_begin + item / S;
-            const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, tile, warp);
-            const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
-            if (inst != staged) {                        // CTA-uniform
-                __syncthreads();
-                jss_stage_instance(p, p.inst[inst], c, PRIO ? JSS_STAGE_OPS : JSS_STAGE_ALL);
-                staged = inst;
-                __syncthreads();
-            }
-            jss_iv_shape(iv);
-            if (env < 0) continue;
-            if (jss_mode_samples(MODE)) env_sample_episodes<KJ, MODE>(p, a, iv, env, tile, warp, lane, item % S, scratch);
-            else env_lookahead<KJ, PRIO>(p, a, iv, env, tile, warp, lane, item % S, scratch);
-        }
-        return;
-    }
-    // a constant where MODE fixes the tables (the values launch_all sets): only a policy kernel branches on a.stage
-    const int stage = MODE == JSS_MODE_POLICY ? a.stage : MODE == JSS_MODE_ROLLOUT ? JSS_STAGE_ALL : JSS_STAGE_OPS;
+    char *region = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;   // the CTA's beam / improvement region
+    const Item K = M.item == JSS_ITEM_ORDER ? (Item)a.n_samples : 1;           // items per env slot
+    const Item per_tile = M.item == JSS_ITEM_SPLIT ? (Item)a.n_steps : (Item)JSS_WARPS_PER_CTA * K;
+    const Item n_items = (Item)(a.tile_end - a.tile_begin) * per_tile;        // the decoded shapes' items
+    const int stage = M.stage == JSS_STAGE_BY_RULE ? a.stage : M.stage;   // a policy's tables depend on its rule
     int staged = -1;
-    for (int tile = a.tile_begin + (int)blockIdx.x; tile < a.tile_end; tile += (int)gridDim.x) {
-        const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, tile, warp);
-        const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
-        if (inst != staged) {                            // CTA-uniform
-            __syncthreads();
-            jss_stage_instance(p, p.inst[inst], c, stage);
-            staged = inst;
-            __syncthreads();
+    for (Item item = (BY_INDEX ? a.tile_begin : 0) + (Item)blockIdx.x; item < (BY_INDEX ? (Item)a.tile_end : n_items);
+         item += (Item)gridDim.x) {
+        if constexpr (M.item == JSS_ITEM_GROUP) {
+            const int32_t *rec = a.beam_groups + (size_t)item * (a.beam_width + 2);
+            staged = jss_restage(p, c, iv, jss_uniform(rec[1]), staged, M.stage);
+            env_beam_step<KJ, M.keys>(p, a, iv, rec, warp, lane, scratch, region);
+        } else {
+            // SPLIT: tile item / S, share item % S; ENV / ORDER: env slot e = item / K of the class's tiles, order item % K
+            const Item e = PER_WARP ? item : item / K;
+            const int tile = M.item == JSS_ITEM_WARP ? (int)item
+                           : M.item == JSS_ITEM_SPLIT ? a.tile_begin + (int)(item / per_tile)
+                                                      : a.tile_begin + (int)(e / JSS_WARPS_PER_CTA);
+            const int slot = PER_WARP ? warp : (int)(e % JSS_WARPS_PER_CTA);
+            const JssTileWarp t = jss_tile(p, a, p.uniform_inst >= 0, tile, slot);
+            const int inst = jss_uniform(t.inst), env = jss_uniform(t.env);
+            if (!PER_WARP && env < 0) continue;
+            staged = jss_restage(p, c, iv, inst, staged, stage);
+            if (env < 0) continue;
+            const int32_t *blk = p.state + (size_t)t.off16 * 4;
+            const int sub = M.item == JSS_ITEM_SPLIT ? (int)(item % per_tile) : (int)(item - e * K);
+            if constexpr (M.item == JSS_ITEM_WARP)
+                jss_process_env<KJ, MODE>(p, a, iv, env, tile, warp, lane, scratch);
+            else if constexpr (M.item == JSS_ITEM_ENV)
+                env_beam_search<KJ, M.keys>(p, a, iv, env, blk, warp, lane, reinterpret_cast<int *>(scratch), region);
+            else if constexpr (M.item == JSS_ITEM_ORDER)
+                env_improve_order<KJ>(p, a, iv, env, sub, blk, warp, lane, reinterpret_cast<int *>(scratch), region);
+            else if constexpr (jss_mode_samples(MODE))
+                env_sample_episodes<KJ, MODE>(p, a, iv, env, tile, warp, lane, sub, scratch);
+            else
+                env_lookahead<KJ, MODE == JSS_MODE_LOOKAHEAD_PRIORITY>(p, a, iv, env, tile, warp, lane, sub, scratch);
         }
-        jss_iv_shape(iv);
-        if (env >= 0) jss_process_env<KJ, MODE>(p, a, iv, env, tile, warp, lane, scratch);
     }
 }
 
@@ -2723,16 +2741,8 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
     };
     prefetch(tile);
     for (; tile < tile_end; tile += tile_step) {
-        if (!UNI) {
-            const int inst = jss_tile(p, a, UNI, tile, warp).inst;
-            if (inst != staged) {                        // CTA-uniform
-                __syncthreads();
-                jss_stage_instance(p, p.inst[inst], c, SAMPLE == 2 ? a.stage : JSS_STAGE_OPS);
-                staged = inst;
-                __syncthreads();
-            }
-            jss_iv_shape(iv);
-        }
+        if (!UNI)
+            staged = jss_restage(p, c, iv, jss_tile(p, a, UNI, tile, warp).inst, staged, SAMPLE == 2 ? a.stage : JSS_STAGE_OPS);
         const int env = UNI ? env_next : jss_uniform(env_next);
         int action = act_next;
         EnvRegs<KJ> s;

@@ -301,5 +301,6 @@ struct JssLaunch {           // per-launch arguments
                                          // (jss_stochastic_beam_step)
 #define JSS_MODE_IMPROVE_ORDERS 21       // operation orders improved by steepest descent on the critical path, one
                                          // (env, order) per CTA, the envs untouched (jss_improve_orders)
+#define JSS_NUM_MODES 22                 // the rows of JSS_MODES (jss_device.cuh)
 
 #define JSS_WARPS_PER_CTA 8
