@@ -202,7 +202,7 @@ JssKernel step_kernel(const jss_t *h) {
 int launch_step(jss_t *h, JssLaunch a, cudaStream_t st) {
     // SAMPLE: 0 none, 1 masked-uniform sampler, 2 dispatching rule, 3 action drawn from policy logits before the step,
     // 4 the same draw with the outputs recorded into the caller's slot, 5 / 6 epsilon-greedy decode of the row (as 3 / 4)
-    const int sample = a.logits ? (a.greedy ? 5 : 3) + (a.traj_obs ? 1 : 0)
+    const int sample = a.rows ? (a.greedy ? 5 : 3) + (a.traj_obs ? 1 : 0)
                      : a.actions_out == nullptr ? 0 : (a.rule == JSS_RULE_RANDOM ? 1 : 2);
     static JssKernel (*const by_sample[])(const jss_t *) = {step_kernel<0>, step_kernel<1>, step_kernel<2>,
                                                             step_kernel<3>, step_kernel<4>, step_kernel<5>,
@@ -246,7 +246,7 @@ JssSmemLayout mode_layout(const jss_t *h, const JssLaunch &a, size_t &smem) {
 }
 
 // the grid of lane class c's launch of a.mode over the tiles (or records) [a.tile_begin, a.tile_end) at `smem` bytes
-// (JSS_GRID_*); a launch that spreads its tiles' candidates or samples also gets its split S in a.n_steps
+// (JSS_GRID_*); a launch that spreads its tiles' candidates or samples also gets its split S in a.split
 int mode_grid(jss_t *h, JssLaunch &a, int c, size_t smem, int &grid) {
     const JssMode &m = JSS_MODES[a.mode];
     const int n = a.tile_end - a.tile_begin;
@@ -255,9 +255,9 @@ int mode_grid(jss_t *h, JssLaunch &a, int c, size_t smem, int &grid) {
     const int slots = h->sm_count * per_sm;
     if (m.grid == JSS_GRID_SPREAD_J || m.grid == JSS_GRID_SPREAD_K) {
         const int most = m.grid == JSS_GRID_SPREAD_J ? std::min(h->p.jobs_max, 32 << c) + 1 : a.n_samples;
-        a.n_steps = n >= slots ? 1 : std::min(most, (slots + n - 1) / n);
+        a.split = n >= slots ? 1 : std::min(most, (slots + n - 1) / n);
     }
-    const int64_t items = m.item == JSS_ITEM_SPLIT ? (int64_t)n * a.n_steps
+    const int64_t items = m.item == JSS_ITEM_SPLIT ? (int64_t)n * a.split
                         : m.item == JSS_ITEM_ENV ? (int64_t)n * JSS_WARPS_PER_CTA
                         : m.item == JSS_ITEM_ORDER ? (int64_t)n * JSS_WARPS_PER_CTA * a.n_samples : n;
     grid = (int)(m.grid == JSS_GRID_ALL ? items : std::min<int64_t>(items, slots));
@@ -302,6 +302,17 @@ int launch_all(jss_t *h, JssLaunch a, cudaStream_t st, const int32_t (*ranges)[2
 // the action choice of jss_policy / jss_step_sample / jss_rollout / jss_rollout_traj
 bool valid_rule_coin(int rule, int coin_mode) {
     return rule >= 0 && rule < JSS_NUM_RULES && (coin_mode == JSS_COIN_DEVICE || coin_mode == JSS_COIN_NEVER);
+}
+
+bool bad_ptr(const void *ptr) { return !ptr || ((uintptr_t)ptr & 3u); }
+
+// a caller's (N, J, M) table into t: non-NULL, 4-byte aligned, strides >= 0
+int table_arg(jss_t *h, const char *who, const float *ptr, int64_t ld_env, int64_t ld_job, int64_t ld_op, JssTable &t) {
+    if (bad_ptr(ptr) || ld_env < 0 || ld_job < 0 || ld_op < 0)
+        return fail(h, JSS_ERR_INVALID, "%s: bad table (%p must be non-NULL and 4-byte aligned, strides %lld / %lld / "
+                    "%lld >= 0)", who, (const void *)ptr, (long long)ld_env, (long long)ld_job, (long long)ld_op);
+    t = JssTable{ptr, ld_env, ld_job, ld_op};
+    return JSS_OK;
 }
 
 int check_ready(jss_t *h) {
@@ -724,13 +735,13 @@ int jss_step_sample(jss_t *h, const int32_t *actions_dev, int rule, int coin_mod
                     uint64_t step_index, int32_t *next_actions_dev, void *stream) {
     int rc = check_ready(h, stream);
     if (rc) return rc;
-    if (!actions_dev || !next_actions_dev || !valid_rule_coin(rule, coin_mode))
+    if (!actions_dev || bad_ptr(next_actions_dev) || !valid_rule_coin(rule, coin_mode))
         return fail(h, JSS_ERR_INVALID, "jss_step_sample: bad arguments (rule %d, coin %d)", rule, coin_mode);
     JssLaunch a{};
     a.mode = JSS_MODE_STEP;
     a.actions = actions_dev;
     a.actions_out = next_actions_dev;
-    a.rule = rule; a.coin_mode = coin_mode; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
+    a.rule = rule; a.coin_mode = coin_mode; a.cr_factor = h->cr_factor;
     a.hash_key = jss_hash_key(seed, step_index);
     return launch_all(h, a, (cudaStream_t)stream);
 }
@@ -739,13 +750,13 @@ namespace {
 // the checks and the launch arguments jss_step_logits and jss_step_logits_record share
 int logits_launch(jss_t *h, const char *what, const float *logits_dev, int64_t ld, uint64_t seed, uint64_t step_index,
                   int32_t *actions_out_dev, float *log_prob_out_dev, JssLaunch &a) {
-    if (!logits_dev || !actions_out_dev || ld < (int64_t)h->p.jobs_max + 1)
+    if (!logits_dev || bad_ptr(actions_out_dev) || ld < (int64_t)h->p.jobs_max + 1)
         return fail(h, JSS_ERR_INVALID, "%s: bad arguments (logits %p, actions_out %p, ld %lld < jobs_max + 1 = %d)", what,
                     (const void *)logits_dev, (void *)actions_out_dev, (long long)ld, h->p.jobs_max + 1);
     a = JssLaunch{};
     a.mode = JSS_MODE_STEP;
-    a.logits = logits_dev;
-    a.logits_ld = ld;
+    a.rows = logits_dev;
+    a.rows_ld = ld;
     a.actions_out = actions_out_dev;
     a.log_prob_out = log_prob_out_dev;
     a.hash_key = jss_hash_key(seed, step_index);
@@ -833,7 +844,7 @@ int jss_policy(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_i
                void *stream) {
     int rc = check_ready(h, stream);
     if (rc) return rc;
-    if (!actions_dev || !valid_rule_coin(rule, coin_mode))
+    if (bad_ptr(actions_dev) || !valid_rule_coin(rule, coin_mode))
         return fail(h, JSS_ERR_INVALID, "jss_policy: bad arguments (rule %d, coin %d)", rule, coin_mode);
     JssLaunch a{};
     a.mode = JSS_MODE_POLICY;
@@ -872,17 +883,14 @@ int jss_rollout_traj(jss_t *h, int rule, uint64_t seed, uint64_t step_index, int
 
 int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op, int n_steps,
                          void *stream) {
+    const char *who = "jss_rollout_priority";
     int rc = check_ready(h, stream);
     if (rc) return rc;
-    if (!prio_dev || ((uintptr_t)prio_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || n_steps < 0)
-        return fail(h, JSS_ERR_INVALID, "jss_rollout_priority: bad arguments (prio %p must be 4-byte aligned, strides "
-                    "%lld / %lld / %lld >= 0, n_steps %d >= 0)", (const void *)prio_dev, (long long)ld_env,
-                    (long long)ld_job, (long long)ld_op, n_steps);
-    if (n_steps == 0) return JSS_OK;
     JssLaunch a{};
+    if ((rc = table_arg(h, who, prio_dev, ld_env, ld_job, ld_op, a.table))) return rc;
+    if (n_steps < 0) return fail(h, JSS_ERR_INVALID, "%s: bad arguments (n_steps %d >= 0)", who, n_steps);
+    if (n_steps == 0) return JSS_OK;
     a.mode = JSS_MODE_PRIORITY;
-    a.logits = prio_dev;
-    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
     a.n_steps = n_steps;
     return launch_all(h, a, (cudaStream_t)stream);
 }
@@ -890,21 +898,18 @@ int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_
 int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                                 uint64_t seed, uint64_t step_index, int n_steps, float *log_prob_out_dev,
                                 float *grad_out_dev, void *stream) {
+    const char *who = "jss_rollout_priority_sample";
     int rc = check_ready(h, stream);
     if (rc) return rc;
-    if (!logits_dev || ((uintptr_t)logits_dev & 3u) || !log_prob_out_dev || ((uintptr_t)log_prob_out_dev & 3u) ||
-        ((uintptr_t)grad_out_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || n_steps < 0)
-        return fail(h, JSS_ERR_INVALID, "jss_rollout_priority_sample: bad arguments (logits %p and log_prob_out %p must "
-                    "be non-NULL, logits, log_prob_out and grad_out %p 4-byte aligned, strides %lld / %lld / %lld >= 0, "
-                    "n_steps %d >= 0)", (const void *)logits_dev, (void *)log_prob_out_dev, (void *)grad_out_dev,
-                    (long long)ld_env, (long long)ld_job, (long long)ld_op, n_steps);
-    if (n_steps == 0) return JSS_OK;
     JssLaunch a{};
+    if ((rc = table_arg(h, who, logits_dev, ld_env, ld_job, ld_op, a.table))) return rc;
+    if (bad_ptr(log_prob_out_dev) || ((uintptr_t)grad_out_dev & 3u) || n_steps < 0)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (log_prob_out %p must be non-NULL, it and grad_out %p "
+                    "4-byte aligned, n_steps %d >= 0)", who, (void *)log_prob_out_dev, (void *)grad_out_dev, n_steps);
+    if (n_steps == 0) return JSS_OK;
     a.mode = JSS_MODE_PRIORITY_SAMPLE;
-    a.logits = logits_dev;
-    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
-    a.hash_key = jss_fold32(seed);                       // jss_hash3 reads the seed only through its fold
-    a.sample_step_index = step_index;
+    a.seed_folded = jss_fold32(seed);                    // jss_hash3 reads the seed only through its fold
+    a.sample_counter = step_index;
     a.n_steps = n_steps;
     a.log_prob_out = log_prob_out_dev;
     a.grad_out = grad_out_dev;
@@ -915,41 +920,35 @@ int jss_lookahead(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t ste
                   int64_t ld, void *stream) {
     int rc = check_ready(h, stream);
     if (rc) return rc;
-    if (!valid_rule_coin(rule, coin_mode) || !makespan_out_dev || ((uintptr_t)makespan_out_dev & 3u) ||
-        ld < (int64_t)h->p.jobs_max + 1)
+    if (!valid_rule_coin(rule, coin_mode) || bad_ptr(makespan_out_dev) || ld < (int64_t)h->p.jobs_max + 1)
         return fail(h, JSS_ERR_INVALID, "jss_lookahead: bad arguments (rule %d, coin %d, makespan_out %p must be "
                     "4-byte aligned, ld %lld >= jobs_max + 1 = %d)", rule, coin_mode, (void *)makespan_out_dev,
                     (long long)ld, h->p.jobs_max + 1);
     JssLaunch a{};
     a.mode = JSS_MODE_LOOKAHEAD;
     a.rule = rule; a.coin_mode = coin_mode; a.seed = seed; a.step_index = step_index; a.cr_factor = h->cr_factor;
-    a.actions_out = makespan_out_dev;
-    a.logits_ld = ld;
+    a.values_out = makespan_out_dev;
+    a.out_ld = ld;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_lookahead_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                            int32_t *makespan_out_dev, int64_t ld, void *stream) {
+    const char *who = "jss_lookahead_priority";
     int rc = check_ready(h, stream);
     if (rc) return rc;
-    if (!prio_dev || ((uintptr_t)prio_dev & 3u) || ld_env < 0 || ld_job < 0 || ld_op < 0 || !makespan_out_dev ||
-        ((uintptr_t)makespan_out_dev & 3u) || ld < (int64_t)h->p.jobs_max + 1)
-        return fail(h, JSS_ERR_INVALID, "jss_lookahead_priority: bad arguments (prio %p and makespan_out %p must be "
-                    "4-byte aligned, strides %lld / %lld / %lld >= 0, ld %lld >= jobs_max + 1 = %d)",
-                    (const void *)prio_dev, (void *)makespan_out_dev, (long long)ld_env, (long long)ld_job,
-                    (long long)ld_op, (long long)ld, h->p.jobs_max + 1);
     JssLaunch a{};
+    if ((rc = table_arg(h, who, prio_dev, ld_env, ld_job, ld_op, a.table))) return rc;
+    if (bad_ptr(makespan_out_dev) || ld < (int64_t)h->p.jobs_max + 1)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p must be non-NULL and 4-byte aligned, ld "
+                    "%lld >= jobs_max + 1 = %d)", who, (void *)makespan_out_dev, (long long)ld, h->p.jobs_max + 1);
     a.mode = JSS_MODE_LOOKAHEAD_PRIORITY;
-    a.logits = prio_dev;
-    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
-    a.actions_out = makespan_out_dev;
-    a.values_ld = ld;
+    a.values_out = makespan_out_dev;
+    a.out_ld = ld;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 
 namespace {
-
-bool bad_ptr(const void *ptr) { return !ptr || ((uintptr_t)ptr & 3u); }
 
 // a.beam_trace for a (stochastic) beam search of width W that writes orders: W backpointers per round (at most
 // jobs_max * machines_max rounds) for each CTA of the largest grid, owned by the handle and grown as needed
@@ -986,9 +985,7 @@ int beam_trace(jss_t *h, JssLaunch &a) {
 // and counter; k and ld where the call has them (has_k)
 int sample_episodes_args(jss_t *h, const char *who, const float *logits, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                          uint64_t seed, uint64_t step_index, bool has_k, int64_t k, int64_t ld, JssLaunch &a) {
-    if (bad_ptr(logits) || ld_env < 0 || ld_job < 0 || ld_op < 0)
-        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (logits %p must be 4-byte aligned, strides %lld / %lld / "
-                    "%lld >= 0)", who, (const void *)logits, (long long)ld_env, (long long)ld_job, (long long)ld_op);
+    if (int rc = table_arg(h, who, logits, ld_env, ld_job, ld_op, a.table)) return rc;
     if (has_k) {
         const uint64_t bound = 2ull * (uint64_t)h->p.jobs_max * (uint64_t)h->p.machines_max + 1;
         if (k < 1 || ld < k || (uint64_t)k > UINT64_MAX / bound)
@@ -996,13 +993,11 @@ int sample_episodes_args(jss_t *h, const char *who, const float *logits, int64_t
                         "ld %lld >= k)", who, (long long)k, (long long)ld);
         if (k > INT32_MAX)
             return fail(h, JSS_ERR_UNSUPPORTED, "%s: k must stay below 2^31", who);
+        a.n_samples = (int)k;
+        a.out_ld = ld;
     }
-    a.logits = logits;
-    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
-    a.hash_key = jss_fold32(seed);                       // jss_hash3 reads the seed only through its fold
-    a.sample_step_index = step_index;
-    a.n_samples = (int)k;
-    a.samples_ld = ld;
+    a.seed_folded = jss_fold32(seed);                    // jss_hash3 reads the seed only through its fold
+    a.sample_counter = step_index;
     return JSS_OK;
 }
 
@@ -1021,7 +1016,7 @@ int jss_sample_episodes(jss_t *h, const float *logits_dev, int64_t ld_env, int64
     a.mode = JSS_MODE_SAMPLE_EPISODES;
     if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
         return rc;
-    a.actions_out = makespan_out_dev;
+    a.makespan_out = makespan_out_dev;
     a.log_prob_out = log_prob_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);
 }
@@ -1043,7 +1038,7 @@ int jss_sample_episodes_grad(jss_t *h, const float *logits_dev, int64_t ld_env, 
     if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
         return rc;
     a.weights = weights_dev;
-    a.n_steps = split;
+    a.split = split;
     a.grad_out = grad_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);
 }
@@ -1061,32 +1056,30 @@ int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_e
     a.mode = JSS_MODE_SAMPLE_EPISODES_SOLUTION;
     if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, false, 0, 0, a)))
         return rc;
-    a.actions = sample_dev;
+    a.sample_in = sample_dev;
     a.solution_out = solution_out_dev;
-    a.n_steps = 1;
+    a.split = 1;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 
 int jss_beam_search(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op, int width,
                     int32_t *makespan_out_dev, float *score_out_dev, int64_t ld, int32_t *order_out_dev, void *stream) {
+    const char *who = "jss_beam_search";
     int rc = check_ready(h, stream);
     if (rc) return rc;
-    if (bad_ptr(logits_dev) || ld_env < 0 || ld_job < 0 || ld_op < 0 || bad_ptr(makespan_out_dev) ||
-        bad_ptr(score_out_dev) || ((uintptr_t)order_out_dev & 3u) || width < 1 || width > JSS_MAX_BEAM_WIDTH ||
-        ld < width)
-        return fail(h, JSS_ERR_INVALID, "jss_beam_search: bad arguments (logits %p, makespan_out %p and score_out %p "
-                    "must be non-NULL, they and order_out %p 4-byte aligned, strides %lld / %lld / %lld >= 0, "
-                    "1 <= width %d <= %d, ld %lld >= width)", (const void *)logits_dev, (void *)makespan_out_dev,
-                    (void *)score_out_dev, (void *)order_out_dev, (long long)ld_env, (long long)ld_job,
-                    (long long)ld_op, width, JSS_MAX_BEAM_WIDTH, (long long)ld);
     JssLaunch a{};
+    if ((rc = table_arg(h, who, logits_dev, ld_env, ld_job, ld_op, a.table))) return rc;
+    if (bad_ptr(makespan_out_dev) || bad_ptr(score_out_dev) || ((uintptr_t)order_out_dev & 3u) || width < 1 ||
+        width > JSS_MAX_BEAM_WIDTH || ld < width)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p and score_out %p must be non-NULL, they "
+                    "and order_out %p 4-byte aligned, 1 <= width %d <= %d, ld %lld >= width)", who,
+                    (void *)makespan_out_dev, (void *)score_out_dev, (void *)order_out_dev, width, JSS_MAX_BEAM_WIDTH,
+                    (long long)ld);
     a.mode = JSS_MODE_BEAM_SEARCH;
-    a.logits = logits_dev;
-    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
     a.beam_width = width;
-    a.actions_out = makespan_out_dev;
-    a.log_prob_out = score_out_dev;
-    a.samples_ld = ld;
+    a.makespan_out = makespan_out_dev;
+    a.score_out = score_out_dev;
+    a.out_ld = ld;
     a.order_out = order_out_dev;
     if (order_out_dev && (rc = beam_trace(h, a))) return rc;
     return launch_all(h, a, (cudaStream_t)stream);
@@ -1096,27 +1089,25 @@ int jss_sample_without_replacement(jss_t *h, const float *logits_dev, int64_t ld
                                    uint64_t seed, uint64_t step_index, int width, int32_t *makespan_out_dev,
                                    float *log_prob_out_dev, float *key_out_dev, int64_t ld, int32_t *order_out_dev,
                                    void *stream) {
+    const char *who = "jss_sample_without_replacement";
     int rc = check_ready(h, stream);
     if (rc) return rc;
-    if (bad_ptr(logits_dev) || ld_env < 0 || ld_job < 0 || ld_op < 0 || bad_ptr(makespan_out_dev) ||
-        bad_ptr(log_prob_out_dev) || bad_ptr(key_out_dev) || ((uintptr_t)order_out_dev & 3u) || width < 1 ||
-        width > JSS_MAX_BEAM_WIDTH || ld < width)
-        return fail(h, JSS_ERR_INVALID, "jss_sample_without_replacement: bad arguments (logits %p, makespan_out %p, "
-                    "log_prob_out %p and key_out %p must be non-NULL, they and order_out %p 4-byte aligned, strides "
-                    "%lld / %lld / %lld >= 0, 1 <= width %d <= %d, ld %lld >= width)", (const void *)logits_dev,
-                    (void *)makespan_out_dev, (void *)log_prob_out_dev, (void *)key_out_dev, (void *)order_out_dev,
-                    (long long)ld_env, (long long)ld_job, (long long)ld_op, width, JSS_MAX_BEAM_WIDTH, (long long)ld);
     JssLaunch a{};
+    if ((rc = table_arg(h, who, logits_dev, ld_env, ld_job, ld_op, a.table))) return rc;
+    if (bad_ptr(makespan_out_dev) || bad_ptr(log_prob_out_dev) || bad_ptr(key_out_dev) ||
+        ((uintptr_t)order_out_dev & 3u) || width < 1 || width > JSS_MAX_BEAM_WIDTH || ld < width)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p, log_prob_out %p and key_out %p must be "
+                    "non-NULL, they and order_out %p 4-byte aligned, 1 <= width %d <= %d, ld %lld >= width)", who,
+                    (void *)makespan_out_dev, (void *)log_prob_out_dev, (void *)key_out_dev, (void *)order_out_dev,
+                    width, JSS_MAX_BEAM_WIDTH, (long long)ld);
     a.mode = JSS_MODE_SWOR;
-    a.logits = logits_dev;
-    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
-    a.hash_key = jss_fold32(seed);                       // jss_hash3 reads the seed only through its fold
-    a.sample_step_index = step_index;
+    a.seed_folded = jss_fold32(seed);                    // jss_hash3 reads the seed only through its fold
+    a.sample_counter = step_index;
     a.beam_width = width;
-    a.actions_out = makespan_out_dev;
+    a.makespan_out = makespan_out_dev;
     a.log_prob_out = log_prob_out_dev;
     a.key_out = key_out_dev;
-    a.samples_ld = ld;
+    a.out_ld = ld;
     a.order_out = order_out_dev;
     if (order_out_dev && (rc = beam_trace(h, a))) return rc;
     return launch_all(h, a, (cudaStream_t)stream);
@@ -1196,16 +1187,16 @@ int beam_step_launch(jss_t *h, const char *who, const float *logits_dev, int64_t
     a.mode = swor ? JSS_MODE_STOCHASTIC_BEAM_STEP : JSS_MODE_BEAM_STEP;
     a.beam_width = width;
     a.beam_groups = bg->dev;
-    a.logits = logits_dev;
-    a.logits_ld = ld;
-    a.log_prob_out = score_dev;
+    a.rows = logits_dev;
+    a.rows_ld = ld;
+    a.score_io = score_dev;
     a.parent_out = parent_out_dev;
     a.job_out = action_out_dev;
     a.bad_out = bad_out_dev;
     if (swor) {
         a.key_io = key_dev;
-        a.hash_key = jss_fold32(seed);                   // jss_hash3 reads the seed only through its fold
-        a.sample_step_index = step_index;
+        a.seed_folded = jss_fold32(seed);                // jss_hash3 reads the seed only through its fold
+        a.sample_counter = step_index;
     }
     return launch_all(h, a, (cudaStream_t)stream, bg->ranges);
 }
@@ -1234,23 +1225,25 @@ int jss_stochastic_beam_step(jss_t *h, const float *logits_dev, int64_t ld, int 
 
 namespace {
 
+// K operation orders per env, and the row stride of the per-order outputs
+int orders_arg(jss_t *h, const char *who, const int32_t *order, int64_t k, int64_t ld, JssLaunch &a) {
+    if (bad_ptr(order) || k < 1 || ld < k)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (order %p must be non-NULL and 4-byte aligned, k %lld >= 1, "
+                    "ld %lld >= k)", who, (const void *)order, (long long)k, (long long)ld);
+    if (k > INT32_MAX)
+        return fail(h, JSS_ERR_UNSUPPORTED, "%s: k must stay below 2^31", who);
+    a.order_in = order;
+    a.n_samples = (int)k;
+    a.out_ld = ld;
+    return JSS_OK;
+}
+
 // the arguments jss_order_log_prob and its gradient share: the table as jss_rollout_priority_sample takes it, k orders
 // per env, and ld
 int order_log_prob_args(jss_t *h, const char *who, const float *logits, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                         const int32_t *order, int64_t k, int64_t ld, JssLaunch &a) {
-    if (bad_ptr(logits) || ld_env < 0 || ld_job < 0 || ld_op < 0 || bad_ptr(order) || k < 1 || ld < k)
-        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (logits %p and order %p must be non-NULL and 4-byte "
-                    "aligned, strides %lld / %lld / %lld >= 0, k %lld >= 1, ld %lld >= k)", who, (const void *)logits,
-                    (const void *)order, (long long)ld_env, (long long)ld_job, (long long)ld_op, (long long)k,
-                    (long long)ld);
-    if (k > INT32_MAX)
-        return fail(h, JSS_ERR_UNSUPPORTED, "%s: k must stay below 2^31", who);
-    a.logits = logits;
-    a.logits_ld = ld_env; a.prio_ld_job = ld_job; a.prio_ld_op = ld_op;
-    a.order_in = order;
-    a.n_samples = (int)k;
-    a.samples_ld = ld;
-    return JSS_OK;
+    if (int rc = table_arg(h, who, logits, ld_env, ld_job, ld_op, a.table)) return rc;
+    return orders_arg(h, who, order, k, ld, a);
 }
 
 }  // namespace
@@ -1267,7 +1260,7 @@ int jss_order_log_prob(jss_t *h, const float *logits_dev, int64_t ld_env, int64_
     JssLaunch a{};
     a.mode = JSS_MODE_ORDER_LOG_PROB;
     if ((rc = order_log_prob_args(h, who, logits_dev, ld_env, ld_job, ld_op, order_dev, k, ld, a))) return rc;
-    a.actions_out = makespan_out_dev;
+    a.makespan_out = makespan_out_dev;
     a.log_prob_out = log_prob_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);
 }
@@ -1288,7 +1281,7 @@ int jss_order_log_prob_grad(jss_t *h, const float *logits_dev, int64_t ld_env, i
     a.mode = JSS_MODE_ORDER_LOG_PROB_GRAD;
     if ((rc = order_log_prob_args(h, who, logits_dev, ld_env, ld_job, ld_op, order_dev, k, ld, a))) return rc;
     a.weights = weights_dev;
-    a.n_steps = split;
+    a.split = split;
     a.grad_out = grad_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);
 }
@@ -1299,14 +1292,13 @@ int jss_improve_orders(jss_t *h, const int32_t *order_dev, int64_t k, int max_mo
     int rc = check_ready(h, stream);
     if (rc) return rc;
     const char *who = "jss_improve_orders";
-    if (bad_ptr(order_dev) || bad_ptr(order_out_dev) || bad_ptr(makespan_out_dev) || bad_ptr(start_makespan_out_dev) ||
-        bad_ptr(moves_out_dev) || k < 1 || ld < k || max_moves < 0)
-        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (order %p, order_out %p, makespan_out %p, start_makespan_out "
-                    "%p and moves_out %p must be non-NULL and 4-byte aligned, k %lld >= 1, ld %lld >= k, max_moves %d "
-                    ">= 0)", who, (const void *)order_dev, (void *)order_out_dev, (void *)makespan_out_dev,
-                    (void *)start_makespan_out_dev, (void *)moves_out_dev, (long long)k, (long long)ld, max_moves);
-    if (k > INT32_MAX)
-        return fail(h, JSS_ERR_UNSUPPORTED, "%s: k must stay below 2^31", who);
+    if (bad_ptr(order_out_dev) || bad_ptr(makespan_out_dev) || bad_ptr(start_makespan_out_dev) ||
+        bad_ptr(moves_out_dev) || max_moves < 0)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (order_out %p, makespan_out %p, start_makespan_out %p and "
+                    "moves_out %p must be non-NULL and 4-byte aligned, max_moves %d >= 0)", who, (void *)order_out_dev,
+                    (void *)makespan_out_dev, (void *)start_makespan_out_dev, (void *)moves_out_dev, max_moves);
+    JssLaunch a{};
+    if ((rc = orders_arg(h, who, order_dev, k, ld, a))) return rc;
     // the byte ranges the call reads or writes; only order_out == order may share one
     const uint64_t N = (uint64_t)h->n_envs, ords = N * (uint64_t)k * h->p.jobs_max * h->p.machines_max * 4,
                    rows = ((N - 1) * (uint64_t)ld + (uint64_t)k) * 4;
@@ -1320,14 +1312,10 @@ int jss_improve_orders(jss_t *h, const int32_t *order_dev, int64_t k, int max_mo
                 return fail(h, JSS_ERR_INVALID, "%s: bad arguments (buffers %d and %d overlap; only order_out == order "
                             "may)", who, x, y);
         }
-    JssLaunch a{};
     a.mode = JSS_MODE_IMPROVE_ORDERS;
-    a.order_in = order_dev;
-    a.n_samples = (int)k;
-    a.samples_ld = ld;
-    a.n_steps = max_moves;
+    a.max_moves = max_moves;
     a.order_out = order_out_dev;
-    a.actions_out = makespan_out_dev;
+    a.makespan_out = makespan_out_dev;
     a.start_out = start_makespan_out_dev;
     a.moves_out = moves_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);

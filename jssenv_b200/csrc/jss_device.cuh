@@ -1155,19 +1155,25 @@ JSS_DEV int env_greedy_scores(const InstView &iv, const EnvRegs<KJ> &s, int lane
 }
 
 // ---- caller's priority table (jss_rollout_priority) -------------------------------------------------------------
-// Env `env`'s next action under its priority table (a.logits, strides a.logits_ld / prio_ld_job / prio_ld_op): the
-// legal job whose current operation has the largest priority, by env_legal_argmax without the no-op; the no-op only
-// when no job is legal and it is.  Each lane loads the entries of its own legal jobs' current operations, nothing
-// else.  Returns JSS_INF for bad priorities and JSS_ACTION_SKIP when nothing is legal (an imported state).
+// Env `env`'s part of a caller's table, hoisted out of the job loops, and its entry for operation k of job j
+JSS_DEV const float *jss_table_row(const JssTable &t, int env) { return t.p + (int64_t)env * t.ld_env; }
+JSS_DEV float jss_table_at(const JssTable &t, const float *row, int j, int k) {
+    return row[(int64_t)j * t.ld_job + (int64_t)k * t.ld_op];
+}
+
+// Env `env`'s next action under its priority table (a.table): the legal job whose current operation has the largest
+// priority, by env_legal_argmax without the no-op; the no-op only when no job is legal and it is.  Each lane loads the
+// entries of its own legal jobs' current operations, nothing else.  Returns JSS_INF for bad priorities and
+// JSS_ACTION_SKIP when nothing is legal (an imported state).
 template <int KJ>
 JSS_DEV int env_priority_action(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane) {
     constexpr uint32_t LM = jss_legal_mask<KJ>();
     if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u))
         return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
-    const float *row = a.logits + (int64_t)env * a.logits_ld;
+    const float *row = jss_table_row(a.table, env);
     int g = JSS_INF;
     env_legal_argmax<KJ>(s, lane, jss_J(iv), false, [&](int i, int j) {
-        return row[(int64_t)j * a.prio_ld_job + (int64_t)jss_sel<KJ>(s.todo, i) * a.prio_ld_op];
+        return jss_table_at(a.table, row, j, jss_sel<KJ>(s.todo, i));
     }, g);
     return g;
 }
@@ -1189,7 +1195,7 @@ JSS_DEV int env_priority_sample_action(const JssLaunch &a, const InstView &iv, c
     for (int i = 0; i < KJ; i++) pr[i] = 0.0f;
     if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u))
         return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
-    const float *row = a.logits + (int64_t)env * a.logits_ld;
+    const float *row = jss_table_row(a.table, env);
     bool bad = false;                                    // a legal entry is NaN or +inf
     uint32_t xkey = 0u;                                  // 0: below every candidate's key
     float x[KJ];
@@ -1197,7 +1203,7 @@ JSS_DEV int env_priority_sample_action(const JssLaunch &a, const InstView &iv, c
     for (int i = 0; i < KJ; i++) {
         x[i] = 0.0f;
         if ((s.lb >> i) & 1u) {
-            x[i] = row[(int64_t)(KJ * lane + i) * a.prio_ld_job + (int64_t)s.todo[i] * a.prio_ld_op];
+            x[i] = jss_table_at(a.table, row, KJ * lane + i, s.todo[i]);
             bad = bad || !(x[i] < JSS_F32_INF);
             xkey = max(xkey, jss_f32_key(x[i]));
         }
@@ -1316,9 +1322,20 @@ struct JssSmemLayout {
     int32_t off_scratch;    // step kernels: [mbarrier 16 B][state-in block][scratch][state-out block]; else 0
     int32_t off_logits;     // step kernels that take a row: [logits row, J + 1 floats] behind state-out; else 0
 };
-static_assert(sizeof(JssParams) == 248 && sizeof(JssLaunch) == 240 && sizeof(JssSmemLayout) == 32 &&
+static_assert(sizeof(JssParams) == 248 && sizeof(JssLaunch) == 472 && sizeof(JssSmemLayout) == 32 &&
               sizeof(JssTile) == 16 && sizeof(JssCtaRange) == 32,
               "ptxas allocates the kernels' registers by the parameter offsets (JssParams::pad0_): measure a change");
+// the same for the fields of JssLaunch that the fused step kernels read
+static_assert(offsetof(JssLaunch, tile_begin) == 0 && offsetof(JssLaunch, tile_end) == 4 &&
+              offsetof(JssLaunch, rule) == 12 && offsetof(JssLaunch, coin_mode) == 16 &&
+              offsetof(JssLaunch, explore_t) == 32 && offsetof(JssLaunch, hash_key) == 48 &&
+              offsetof(JssLaunch, stage) == 52 && offsetof(JssLaunch, cr_factor) == 56 &&
+              offsetof(JssLaunch, actions) == 64 && offsetof(JssLaunch, actions_out) == 72 &&
+              offsetof(JssLaunch, traj_obs) == 88 && offsetof(JssLaunch, traj_mask) == 96 &&
+              offsetof(JssLaunch, traj_scalars) == 104 && offsetof(JssLaunch, uni) == 132 &&
+              offsetof(JssLaunch, rows) == 216 && offsetof(JssLaunch, log_prob_out) == 224 &&
+              offsetof(JssLaunch, rows_ld) == 232,
+              "ptxas allocates the step kernels' registers by the parameter offsets: measure a change");
 
 struct JssCtaSmem {         // the CTA-shared part
     JssInst *si;
@@ -1449,7 +1466,7 @@ JSS_DEV void env_priority_rollout(const JssParams &p, const JssLaunch &a, const 
 }
 
 // jss_rollout_priority_sample: the loop of env_priority_rollout with the draws of env_priority_sample_action, decision
-// d with h = jss_hash3(seed, global env id, sample_step_index + d).  Besides its outputs: log_prob_out[env], the sum of
+// d with h = jss_hash3(seed, global env id, sample_counter + d).  Besides its outputs: log_prob_out[env], the sum of
 // the decisions' log-probabilities in decision order (NaN if a decision of this call left the env unchanged with the
 // error bit), and, with grad_out, the gradient G of that sum with respect to the env's table entries,
 // G[j][k] = sum over the decisions t where job j is legal at operation k of (1[j drawn at t] - p_t(j)).  A job is legal
@@ -1483,7 +1500,7 @@ JSS_DEV void env_priority_sample_rollout(const JssParams &p, const JssLaunch &a,
 #pragma unroll
     for (int i = 0; i < KJ; i++) acc[i] = 0.0f;
     for (int k = 0; k < a.n_steps && !(s.flags & JSS_FLAG_DONE); k++) {
-        const uint32_t h = jss_hash_env(jss_hash_key_folded(a.hash_key, a.sample_step_index + (uint64_t)k), genv);
+        const uint32_t h = jss_hash_env(jss_hash_key_folded(a.seed_folded, a.sample_counter + (uint64_t)k), genv);
         float logp, pr[KJ];
         const int act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
         if (act == JSS_ACTION_SKIP) break;               // nothing legal: no decision changes the env
@@ -1557,25 +1574,26 @@ JSS_DEV JssTileWarp jss_tile(const JssParams &p, const JssLaunch &a, bool uni, i
 }
 
 // ---- one-step lookahead over a dispatching rule or a priority table (jss_lookahead, jss_lookahead_priority) -----
-// Work item (tile, sp) of a launch split S ways (a.n_steps): warp `warp` values its env of the tile at the candidates
+// Work item (tile, sp) of a launch split S ways (a.split): warp `warp` values its env of the tile at the candidates
 // c = sp, sp + S, ... <= J.  Each candidate is simulated in registers from the env's state block, which the call never
 // writes: load, step c, then the rule's decisions d = 0, 1, ... (RNG counter step_index + d, so every candidate of an
 // env sees the same numbers) until done, at most 2 J M + 1 of them, every step with env_step<KJ, false>.  Lane 0 stores
 // the end time, or -1 for an illegal candidate, an env done at entry, and a rollout that stops before done (the rule
 // finds nothing legal, a step leaves the env unchanged with the error bit, or the bound trips).  The block is reloaded
-// for each candidate (unchanged and L2-resident) instead of kept as a second register copy of the root state.
+// for each candidate (unchanged and L2-resident) instead of kept as a second register copy of the root state.  The
+// values go to a.values_out.
 // PRIO (jss_lookahead_priority): the decisions after the candidate are env_priority_action's on the caller's table
-// (a.logits, its env stride a.logits_ld; the values' row stride is a.values_ld), no RNG; a bad table at a decision
-// (JSS_INF) stops that candidate's rollout, which then reads -1, and touches nothing else.
+// (a.table), no RNG; a bad table at a decision (JSS_INF) stops that candidate's rollout, which then reads -1, and
+// touches nothing else.
 template <int KJ, bool PRIO>
 JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
                            int lane, int sp, float *scratch) {
     const int32_t *blk = p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4;
-    int32_t *out = a.actions_out + (int64_t)env * (PRIO ? a.values_ld : a.logits_ld);
+    int32_t *out = a.values_out + (int64_t)env * a.out_ld;
     const uint64_t genv = p.env_id_base + (uint64_t)env;
     const int J = jss_J(iv), bound = 2 * J * jss_M(iv) + 1;
     int *hz = reinterpret_cast<int *>(scratch);
-    for (int c = sp; c <= J; c += a.n_steps) {
+    for (int c = sp; c <= J; c += a.split) {
         EnvRegs<KJ> s;
         env_load<KJ>(iv, blk, lane, s);
         s.flags = jss_uniform(s.flags);
@@ -1608,13 +1626,13 @@ JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstVie
 // ---- K episodes per env drawn from a logit table, the envs untouched (jss_sample_episodes, _grad, _solution) -----
 // Sample s of env `env` is jss_rollout_priority_sample's loop run in registers from the env's state block, which the
 // call never writes: at most B = 2 jobs_max machines_max + 1 decisions of env_priority_sample_action, decision d at RNG
-// counter a.sample_step_index + s B + d, each step with env_step<KJ, false>.  It ends done, errs (a bad table, or a
+// counter a.sample_counter + s B + d, each step with env_step<KJ, false>.  It ends done, errs (a bad table, or a
 // step that leaves the env unchanged: log-probability NaN) or stops (nothing legal, or the bound).  The block is
 // reloaded for each sample, as the lookahead reloads it for each candidate.
-// JSS_MODE_SAMPLE_EPISODES: work item (tile, sp) of a launch split S ways (a.n_steps) takes the samples s = sp, sp + S,
-//   ... < K and stores each one's makespan (-1 unless done) and log-probability at column s of the env's rows (row
-//   stride a.samples_ld); an env done at entry gets -1 and 0 in each of those columns.
-// JSS_MODE_SAMPLE_EPISODES_GRAD: work item (tile, c), c < split (a.n_steps), takes the samples s = c, c + split, ... in
+// JSS_MODE_SAMPLE_EPISODES: work item (tile, sp) of a launch split S ways (a.split) takes the samples s = sp, sp + S,
+//   ... < K and stores each one's makespan (-1 unless done) and log-probability at column s of the env's rows of
+//   a.makespan_out and a.log_prob_out; an env done at entry gets -1 and 0 in each of those columns.
+// JSS_MODE_SAMPLE_EPISODES_GRAD: work item (tile, c), c < a.split, takes the samples s = c, c + split, ... in
 //   increasing s and adds w_s G_s into chunk c of a.grad_out with env_priority_sample_rollout's accumulator: w_s (1 -
 //   acc) at a drawn operation, w_s (0 - acc) at each job's first undrawn one at the end.  Each entry is read and written
 //   only by the lane that owns its job, in program order, so a chunk's sums do not depend on the schedule.  A sample
@@ -1622,7 +1640,7 @@ JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstVie
 //   sample err after its first draw (a no-op is drawn only from an imported state, at decision 0, before any add), so
 //   an env with either has each sample first run without adds to find out.  Samples with w_s == 0 and envs done at
 //   entry are skipped.
-// JSS_MODE_SAMPLE_EPISODES_SOLUTION: one work item per tile; env i replays sample a.actions[i] (none if < 0) and writes
+// JSS_MODE_SAMPLE_EPISODES_SOLUTION: one work item per tile; env i replays sample a.sample_in[i] (none if < 0) and writes
 //   the start time of each operation it starts into a.solution_out.
 // JSS_MODE_ORDER_LOG_PROB / _GRAD: the loop of JSS_MODE_SAMPLE_EPISODES / _GRAD with the decisions of env_order_action
 //   on order s of the env (a.order_in) in place of the draws; no RNG.
@@ -1635,7 +1653,7 @@ template <int KJ, bool ROW = false>
 JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ]);
 // Env `env`'s next decision under an operation order `ord` (row stride machines_max; jss_order_log_prob): that of
 // env_priority_action on the table -ord, the legal job whose current operation has the smallest entry, ties to the
-// lowest job.  Writes logp, its log-probability under the logit table a.logits by env_table_logp (so that a beam's score
+// lowest job.  Writes logp, its log-probability under the logit table a.table by env_table_logp (so that a beam's score
 // and the order's log-probability agree bit for bit), and each owned slot's p_i = exp(lp_i) (0 for a job that is not
 // legal).  Returns as env_priority_sample_action does: the no-op, logp and p left 0, when no job is legal and it is;
 // JSS_INF for a bad table row; JSS_ACTION_SKIP when nothing is legal.
@@ -1679,27 +1697,27 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
     const int32_t *blk = p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4;
     const uint64_t genv = p.env_id_base + (uint64_t)env;
     const int J = jss_J(iv), M = jss_M(iv), bound = 2 * p.jobs_max * p.machines_max + 1;
-    const int64_t row = (int64_t)env * a.samples_ld;
+    const int64_t row = (int64_t)env * a.out_ld;
     int *hz = reinterpret_cast<int *>(scratch);
     EnvRegs<KJ> s;
     env_load<KJ>(iv, blk, lane, s);
     s.flags = jss_uniform(s.flags);
-    int first = sp, end = a.n_samples, stride = a.n_steps;
+    int first = sp, end = a.n_samples, stride = a.split;
     if (SOL) {
-        first = jss_uniform(a.actions[env]);
+        first = jss_uniform(a.sample_in[env]);
         end = first + 1; stride = 1;
         if (first < 0) return;
     }
     if (s.flags & JSS_FLAG_DONE) {
         if (!GRAD && !SOL && lane == 0)
-            for (int k = first; k < end; k += stride) { a.actions_out[row + k] = -1; a.log_prob_out[row + k] = 0.0f; }
+            for (int k = first; k < end; k += stride) { a.makespan_out[row + k] = -1; a.log_prob_out[row + k] = 0.0f; }
         return;
     }
     float *grad = nullptr;
     bool check = false;                                  // GRAD: a sample may err after an add
     if (GRAD) {
         grad = a.grad_out + ((size_t)sp * p.n_envs + env) * p.jobs_max * p.machines_max;
-        const float *tab = a.logits + (int64_t)env * a.logits_ld;
+        const float *tab = jss_table_row(a.table, env);
         bool clean = true;
 #pragma unroll 1
         for (int i = 0; i < KJ; i++) {
@@ -1707,7 +1725,7 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
             if (j >= J) break;
             clean = clean && !(((s.lb >> i) & 1u) && jss_sel<KJ>(s.op, i) == JSS_OP_NONE);
             for (int k = 0; k < M; k++) {
-                const float x = tab[(int64_t)j * a.prio_ld_job + (int64_t)k * a.prio_ld_op];
+                const float x = jss_table_at(a.table, tab, j, k);
                 clean = clean && x > -JSS_F32_INF && x < JSS_F32_INF;
             }
         }
@@ -1719,7 +1737,7 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
             w = __int_as_float(jss_uniform(__float_as_int(a.weights[row + smp])));
             if (w == 0.0f) continue;
         }
-        const uint64_t c0 = a.sample_step_index + (uint64_t)smp * (uint64_t)bound;
+        const uint64_t c0 = a.sample_counter + (uint64_t)smp * (uint64_t)bound;
         const int32_t *ord = ORD ? a.order_in + ((size_t)env * a.n_samples + smp) * p.jobs_max * p.machines_max : nullptr;
         // GRAD: pass 0 (only where `check`) finds out whether the sample errs, pass 1 adds
         for (int pass = (GRAD && !check) ? 1 : 0; pass < (GRAD ? 2 : 1); pass++) {
@@ -1736,7 +1754,7 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
                 if (ORD) {
                     act = jss_uniform(env_order_action<KJ>(a, iv, s, env, lane, ord, p.machines_max, logp, pr));
                 } else {
-                    const uint32_t h = jss_hash_env(jss_hash_key_folded(a.hash_key, c0 + (uint64_t)d), genv);
+                    const uint32_t h = jss_hash_env(jss_hash_key_folded(a.seed_folded, c0 + (uint64_t)d), genv);
                     act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
                 }
                 if (act == JSS_ACTION_SKIP) break;       // nothing legal: no decision changes the env
@@ -1760,7 +1778,7 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
                 lp += logp;
             }
             if (!GRAD && !SOL && lane == 0) {
-                a.actions_out[row + smp] = (s.flags & JSS_FLAG_DONE) ? s.t : -1;
+                a.makespan_out[row + smp] = (s.flags & JSS_FLAG_DONE) ? s.t : -1;
                 a.log_prob_out[row + smp] = err ? JSS_F32_NAN : lp;
             }
             if (err) break;                              // GRAD: no adds, or none yet (decision 0 of pass 1)
@@ -1780,11 +1798,11 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
 // with the loads, reductions and fast exp / log of env_priority_sample_action in the same order, so that lp of the job
 // it draws equals its logp bit for bit.  Kept apart from it so that its code (and the sampling kernels') stays as it
 // is.  At least one job must be legal; returns false for a bad row (the bad-table rule of env_priority_sample_action).
-// ROW (jss_beam_step): x_j is column j of env `env`'s logit row (a.logits, row stride a.logits_ld) in place of the table
-// entry of job j's current operation; everything else is the same.
+// ROW (jss_beam_step): x_j is column j of env `env`'s logit row (a.rows) in place of the table entry of job j's current
+// operation; everything else is the same.
 template <int KJ, bool ROW>
 JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ]) {
-    const float *row = a.logits + (int64_t)env * a.logits_ld;
+    const float *row = ROW ? a.rows + (int64_t)env * a.rows_ld : jss_table_row(a.table, env);
     bool bad = false;                                    // a legal entry is NaN or +inf
     uint32_t xkey = 0u;                                  // 0: below every candidate's key
     float x[KJ];
@@ -1792,8 +1810,7 @@ JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, i
     for (int i = 0; i < KJ; i++) {
         x[i] = 0.0f;
         if ((s.lb >> i) & 1u) {
-            x[i] = ROW ? row[KJ * lane + i]
-                       : row[(int64_t)(KJ * lane + i) * a.prio_ld_job + (int64_t)s.todo[i] * a.prio_ld_op];
+            x[i] = ROW ? row[KJ * lane + i] : jss_table_at(a.table, row, KJ * lane + i, s.todo[i]);
             bad = bad || !(x[i] < JSS_F32_INF);
             xkey = max(xkey, jss_f32_key(x[i]));
         }
@@ -1978,7 +1995,7 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
     const int R = done0 ? 0 : (int)__reduce_add_sync(JSS_FULL, (unsigned)left);
     int n = 1, cur = 0;                                  // live slots, and the buffer that holds them
     for (int r = 0; r < R && n > 0; r++) {
-        const uint32_t hr = SWOR ? jss_hash_env(jss_hash_key_folded(a.hash_key, a.sample_step_index + (uint64_t)r),
+        const uint32_t hr = SWOR ? jss_hash_env(jss_hash_key_folded(a.seed_folded, a.sample_counter + (uint64_t)r),
                                                 p.env_id_base + (uint64_t)env) : 0u;
         for (int b = warp; b < n; b += JSS_WARPS_PER_CTA) {   // 1. expand
             int32_t *blk = slot(cur, b);
@@ -2092,9 +2109,9 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
     if (done0) sc = ky = 0.0f;
     else if (!any && bs.bad[0]) sc = ky = JSS_F32_NAN;
     if (b < W) {
-        a.actions_out[(int64_t)env * a.samples_ld + b] = t;
-        a.log_prob_out[(int64_t)env * a.samples_ld + b] = sc;
-        if (SWOR) a.key_out[(int64_t)env * a.samples_ld + b] = ky;
+        a.makespan_out[(int64_t)env * a.out_ld + b] = t;
+        (SWOR ? a.log_prob_out : a.score_out)[(int64_t)env * a.out_ld + b] = sc;
+        if (SWOR) a.key_out[(int64_t)env * a.out_ld + b] = ky;
     }
     if (SWOR || !a.order_out) return;
     // the best slot: smallest makespan, ties to the lowest slot (t < 2^24)
@@ -2104,7 +2121,7 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
 
 // ---- one beam-search round per group of W envs from per-beam logit rows (jss_beam_step) ----------------------------
 // The whole CTA works on group g (record `rec`: g, its instance, its W slots' block offsets), slot b = env g W + b.  A
-// slot is live iff its score (a.log_prob_out) is finite.
+// slot is live iff its score (a.score_io) is finite.
 //   0. the scores and the live slots' blocks (the parents, as at entry) go to shared memory.  Without a live, not-done
 //      slot the group is untouched: parent b, job -1, bad 0, and nothing else is written;
 //   1. warp w expands the slots b = w, w + 8, ...: a live, not-done slot with a legal job takes the log-probabilities
@@ -2134,7 +2151,7 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
     const auto live = [](float x) { return x > -JSS_F32_INF && x < JSS_F32_INF; };
     __syncthreads();                                     // the previous group's last reads of the region are done
     for (int b = (int)threadIdx.x; b < W; b += (int)blockDim.x) {
-        bs.score[b] = a.log_prob_out[e0 + b];
+        bs.score[b] = a.score_io[e0 + b];
         if (SWOR) bs.key[b] = a.key_io[e0 + b];
     }
     if (threadIdx.x == 0) bs.bad[0] = 0;
@@ -2155,7 +2172,7 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
         return;
     }
     EnvRegs<KJ> s;
-    const uint32_t hr = SWOR ? jss_hash_env(jss_hash_key_folded(a.hash_key, a.sample_step_index),
+    const uint32_t hr = SWOR ? jss_hash_env(jss_hash_key_folded(a.seed_folded, a.sample_counter),
                                             p.env_id_base / (uint64_t)W + (uint64_t)g) : 0u;
     for (int b = warp; b < W; b += JSS_WARPS_PER_CTA) {   // 1. expand
         const float sc = bs.score[b];
@@ -2228,17 +2245,17 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
         env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
         if (lane == 0) {
             if (SWOR) {                                  // the score came with the selection
-                a.log_prob_out[env] = ok ? bs.score[W + b] : JSS_F32_NAN;
+                a.score_io[env] = ok ? bs.score[W + b] : JSS_F32_NAN;
                 a.key_io[env] = jss_key_f32((uint32_t)(k >> 32));
             } else {
-                a.log_prob_out[env] = ok ? jss_key_f32((uint32_t)(k >> 32)) : JSS_F32_NAN;
+                a.score_io[env] = ok ? jss_key_f32((uint32_t)(k >> 32)) : JSS_F32_NAN;
             }
             a.parent_out[env] = (int)(pj >> 8);
             a.job_out[env] = (int)(pj & 255u);
         }
     }
     for (int b = nn + (int)threadIdx.x; b < W; b += (int)blockDim.x) {   // empty slots: their blocks left stale
-        a.log_prob_out[e0 + b] = -JSS_F32_INF;
+        a.score_io[e0 + b] = -JSS_F32_INF;
         if (SWOR) a.key_io[e0 + b] = -JSS_F32_INF;
         a.parent_out[e0 + b] = -1;
         a.job_out[e0 + b] = -1;
@@ -2350,8 +2367,8 @@ JSS_DEV int jss_improve_chain(const JssParams &p, const InstView &iv, const int3
 // canonical order R and start times into shared memory, and walks the chain; then per move warp w replays the
 // neighbours c = w, w + 8, ... (pair c's two entries of R swapped at lookup), the CTA takes the smallest makespan
 // (lowest c on ties) and, if it is below the current one, warp 0 replays that neighbour recording its canonical order
-// in place and walks its chain.  At most a.n_steps moves.  Outputs: the final order (-1 everywhere unless the input
-// ends done), makespan, the input's makespan and the moves, at row env * a.samples_ld + smp.
+// in place and walks its chain.  At most a.max_moves moves.  Outputs: the final order (-1 everywhere unless the input
+// ends done) to a.order_out, and makespan, the input's makespan and the moves at column smp of the env's rows.
 template <int KJ>
 JSS_DEV void env_improve_order(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int smp,
                                const int32_t *root, int warp, int lane, int *hz, char *ism) {
@@ -2359,7 +2376,7 @@ JSS_DEV void env_improve_order(const JssParams &p, const JssLaunch &a, const Ins
     JssImproveSmem is;
     jss_improve_smem(ism, p.jobs_max, ms, &is);
     const size_t o_off = ((size_t)env * a.n_samples + smp) * p.jobs_max * ms;
-    const int64_t row = (int64_t)env * a.samples_ld + smp;
+    const int64_t row = (int64_t)env * a.out_ld + smp;
     const int4 none = make_int4(-1, -1, 0, 0);
     __syncthreads();                                     // the previous item's last reads of the region are done
     if (warp == 0) {
@@ -2373,7 +2390,7 @@ JSS_DEV void env_improve_order(const JssParams &p, const JssLaunch &a, const Ins
     __syncthreads();
     const int t0 = is.ctl[0];
     int cur = t0, moves = 0;
-    while (cur >= 0 && moves < a.n_steps) {
+    while (cur >= 0 && moves < a.max_moves) {
         const int n = is.ctl[1];
         uint64_t best = ~0ull;
         for (int c = warp; c < n; c += JSS_WARPS_PER_CTA) {
@@ -2407,7 +2424,7 @@ JSS_DEV void env_improve_order(const JssParams &p, const JssLaunch &a, const Ins
         out[(size_t)j * ms + k] = t0 >= 0 ? is.ord[j * ms + k] : -1;
     }
     if (threadIdx.x == 0) {
-        a.actions_out[row] = cur;
+        a.makespan_out[row] = cur;
         a.start_out[row] = t0;
         a.moves_out[row] = moves;
     }
@@ -2507,7 +2524,7 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
 // ---- the modes of the generic kernel: one row each (JSS_MODES) ---------------------------------------------------
 // What one work item of jss_env_kernel's CTA-strided loop is; launch_all counts the items of a class by the same rule.
 #define JSS_ITEM_WARP 0    // a tile, one env per warp (the items are the class's tiles themselves)
-#define JSS_ITEM_SPLIT 1   // (tile, s), s < S = a.n_steps: warp w takes env w of the tile and share s of its candidates
+#define JSS_ITEM_SPLIT 1   // (tile, s), s < S = a.split: warp w takes env w of the tile and share s of its candidates
                            // or samples; a tile's S items are adjacent and share its instance
 #define JSS_ITEM_ENV 2     // one env of the class's tiles per CTA
 #define JSS_ITEM_ORDER 3   // one (env, order) per CTA: env slot item / K of the class's tiles, order item % K
@@ -2638,7 +2655,7 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
     float *scratch = reinterpret_cast<float *>(sm + sl.off_warp0 + warp * sl.warp_stride);
     char *region = sm + sl.off_warp0 + JSS_WARPS_PER_CTA * sl.warp_stride;   // the CTA's beam / improvement region
     const Item K = M.item == JSS_ITEM_ORDER ? (Item)a.n_samples : 1;           // items per env slot
-    const Item per_tile = M.item == JSS_ITEM_SPLIT ? (Item)a.n_steps : (Item)JSS_WARPS_PER_CTA * K;
+    const Item per_tile = M.item == JSS_ITEM_SPLIT ? (Item)a.split : (Item)JSS_WARPS_PER_CTA * K;
     const Item n_items = (Item)(a.tile_end - a.tile_begin) * per_tile;        // the decoded shapes' items
     const int stage = M.stage == JSS_STAGE_BY_RULE ? a.stage : M.stage;   // a policy's tables depend on its rule
     int staged = -1;
@@ -2702,7 +2719,7 @@ JSS_DEV void jss_pdl_wait() {}
 // rollout slot (a.traj_obs) instead of real_obs, the mask and the scalar record to the slot and the env's buffers, and
 // an env the step left unchanged is emitted into the slot as well.
 // SAMPLE = 5 / 6 are SAMPLE = 3 / 4 with the epsilon-greedy decode of the row (jss_step_greedy / _record).
-JSS_HD constexpr bool jss_step_takes_row(int sample) { return sample >= 3; }   // the action comes from a row (a.logits)
+JSS_HD constexpr bool jss_step_takes_row(int sample) { return sample >= 3; }   // the action comes from a row (a.rows)
 JSS_HD constexpr bool jss_step_records(int sample) { return sample == 4 || sample == 6; }   // into the caller's slot
 struct JssWarpSmem {        // per-warp shared-memory regions of the step kernels
     int32_t *state_in, *state_out;
@@ -2731,7 +2748,7 @@ JSS_DEV void jss_step_tiles(const JssParams &p, const JssLaunch &a, InstView &iv
             if (lane == 0) jss_bulk_load(w.state_sa, p.state + (size_t)t.off16 * 4, t.blk16 * 16u, w.mbar);
             if (ROW) {
                 const int J = UNI ? a.uni.J : p.inst[t.inst].J;
-                const float *src = a.logits + (size_t)env_next * (size_t)a.logits_ld;
+                const float *src = a.rows + (size_t)env_next * (size_t)a.rows_ld;
                 for (int k = lane; k <= J; k += 32) jss_cp_async4(w.logits_sa + 4u * (uint32_t)k, src + k);
                 jss_cp_async_commit();
             } else {

@@ -167,103 +167,72 @@ struct JssParams {
     uint8_t *x_legal, *x_blocked;
 };
 
-struct JssLaunch {           // per-launch arguments
-    int32_t tile_begin, tile_end;
+// A caller's (N, J, M) float table: env i's entry for operation k of job j is at p + i ld_env + j ld_job + k ld_op
+// (jss_table_row, jss_table_at).  Priorities or logits, whichever the mode reads.
+struct JssTable {
+    const float *p;
+    int64_t ld_env, ld_job, ld_op;
+};
+
+// Per-launch arguments.  Each field holds one thing in every mode that reads it; an entry point sets its mode's fields
+// and leaves the rest zero.  Row i of a per-env output starts at i * out_ld.  The fields up to rows_ld include all
+// that the fused step kernels read, at byte offsets that jss_device.cuh pins.
+struct JssLaunch {
+    int32_t tile_begin, tile_end;   // the tiles (jss_beam_step: the group records) of one launch, set by launch_all
     int32_t mode;            // JSS_MODE_*
-    union {
-        int32_t rule;
-        int32_t greedy;      // steps from a row (a.logits): 0 categorical draw, 1 epsilon-greedy decode
-        int32_t n_samples;   // jss_sample_episodes (_grad): K, the episodes drawn per env; jss_order_log_prob (_grad),
-                             // jss_improve_orders: K, the orders per env
-        int32_t beam_width;  // jss_beam_search, jss_sample_without_replacement: W, the beams kept per env;
-                             // jss_beam_step, jss_stochastic_beam_step: W, the envs per group
-    };
-    int32_t coin_mode, n_steps, write_obs;   // jss_lookahead (_priority): n_steps is S, the work items each tile's
-                                             // candidates are spread over (launch_all); jss_sample_episodes: the
-                                             // work items each tile's samples are spread over (_grad: the chunks)
-    int32_t export_after;    // step through the generic kernel: also decode the new state into the x_* arrays (facade)
-    union {
-        uint64_t seed;
-        uint64_t explore_t;  // epsilon-greedy decode: an env explores iff jss_hash_env(h_env, 0) < explore_t, 0 .. 2^32
-        int64_t prio_ld_job; // jss_rollout_priority: element stride between jobs of the priority table
-    };
-    union {
-        uint64_t step_index;
-        int64_t prio_ld_op;  // jss_rollout_priority: element stride between operations of a job
-    };
-    uint32_t hash_key;       // jss_hash_key(seed, step_index), folded once per launch on the host (fused step + sampler);
-                             // jss_rollout_priority_sample: jss_fold32(seed), all of the seed that jss_hash3 reads
+    int32_t rule;            // JSS_RULE_*: jss_step_sample, jss_policy, jss_rollout (_traj), jss_lookahead
+    int32_t coin_mode;       // JSS_COIN_*: the same entry points
+    int32_t n_steps;         // the decision budget per env: jss_rollout (_traj), jss_rollout_priority (_sample)
+    int32_t write_obs;       // jss_rollout (_traj): emit the observation of every step that changes the env
+    int32_t export_after;    // jss_step_export: also decode the new state into the x_* arrays (facade)
+    uint64_t explore_t;      // jss_step_greedy (_record): explore iff jss_hash_env(h_env, 0) < explore_t (<= 2^32)
+    uint64_t step_index;     // jss_hash3's counter: jss_policy, jss_rollout (_traj), jss_lookahead
+    uint32_t hash_key;       // jss_hash_key(seed, step_index): jss_step_sample, jss_step_logits / _greedy (_record)
     int32_t stage;           // JSS_STAGE_*: the instance tables the launch stages in shared memory (launch_all)
-    union {
-        double cr_factor;    // CriticalRatio due_date_factor (dispatching.py:337-349); reference default 1.5
-        uint64_t sample_step_index;   // jss_rollout_priority_sample: the RNG counter of the env's first decision
-                                      // (jss_stochastic_beam_step: of the round)
-        int64_t values_ld;   // jss_lookahead_priority: env i's value of action a at actions_out + i * values_ld + a
-                             // (logits_ld is the table's env stride there)
-        const int32_t *order_in;   // jss_order_log_prob (_grad), jss_improve_orders: order s of env i at order_in +
-                                   // (i * n_samples + s) * jobs_max * machines_max
-    };
-    union {
-        const int32_t *actions;  // step; jss_sample_episodes_solution: the sample each env replays (< 0: none)
-        const float *weights;    // jss_sample_episodes_grad: sample s of env i weighs weights[i * samples_ld + s]
-        uint16_t *beam_trace;    // jss_beam_search with an order: per CTA, W backpointers per round (NULL: no order)
-        const int32_t *beam_groups;   // jss_beam_step: per group [group, instance, W block offsets in 16-byte units],
-                                      // grouped by lane class; a launch takes records [tile_begin, tile_end)
-    };
-    union {
-        int32_t *actions_out;    // policy; jss_lookahead: env i's value of action a at actions_out + i * logits_ld + a
-                                 // (jss_lookahead_priority: + i * values_ld + a); jss_sample_episodes: sample s's
-                                 // makespan at actions_out + i * samples_ld + s
-        int32_t *solution_out;   // jss_sample_episodes_solution: [N][jobs_max][machines_max] start times
-                                 // (jss_beam_search: slot b's makespan at actions_out + i * samples_ld + b)
-        int32_t *parent_out;     // jss_beam_step: [N] each slot's parent slot
-    };
-    union {
-        const uint8_t *env_mask; // reset / import
-        int64_t samples_ld;      // jss_sample_episodes (_grad): row stride of the per-sample outputs / weights;
-                                 // jss_beam_search: of the per-slot outputs
-    };
-    // rollout with trajectory recording: outputs of step k of env e go to slot k * n_envs + e of these buffers;
-    // jss_step_logits_record / jss_step_greedy_record: env e's observation, mask and scalar record go to row e of
-    // traj_obs / mask / scalars.  jss_rollout_priority_sample: grad_out is the [N][jobs_max][machines_max] gradient of
-    // each env's log-probability with respect to its table entries (may be NULL)
-    // jss_beam_search: order_out is the [N][jobs_max][machines_max] order of each env's best slot (may be NULL), and
-    // slot b's score goes to log_prob_out + i * samples_ld + b
-    // jss_beam_step: slot b of group g has score log_prob_out[g W + b] (read and written), parent parent_out, job
-    // job_out, and group g's bad-row bit goes to bad_out[g]
-    union {
-        float *traj_obs;
-        float *grad_out;
-        int32_t *order_out;
-        int32_t *job_out;
-    };
-    // jss_stochastic_beam_step: as jss_beam_step, and slot b of group g has key key_io[g W + b] (read and written)
-    // jss_improve_orders: order s of env i goes to order_out + (i * n_samples + s) * jobs_max * machines_max, its
-    // makespan to actions_out, the input's to start_out and the accepted moves to moves_out, each at i * samples_ld + s;
-    // n_steps is the move limit
-    union {
-        uint8_t *traj_mask;
-        float *key_io;
-        int32_t *moves_out;
-    };
-    int32_t *traj_scalars; int32_t *traj_actions;
-    // jss_sample_without_replacement: slot b's score goes to log_prob_out and its key to key_out + i * samples_ld + b,
-    // and order_out is the [N][W][jobs_max][machines_max] order of every slot (may be NULL)
-    union {
-        uint8_t *wire;       // pack: [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job)
-        float *key_out;
-        int32_t *bad_out;
-        int32_t *start_out;
-    };
+    double cr_factor;        // CriticalRatio due_date_factor (dispatching.py:337-349): the entry points that take a rule
+    const int32_t *actions;  // [N] the actions a step takes: jss_step (_export), jss_step_sample
+    int32_t *actions_out;    // [N] the chosen or next actions: jss_policy, jss_step_sample, jss_step_logits / _greedy
+    const uint8_t *env_mask; // [N] the envs a reset or import touches (NULL: all): jss_reset, jss_import_state
+    float *traj_obs;         // the caller's slot: jss_rollout_traj (step k of env e at k * n_envs + e), the _record steps
+    uint8_t *traj_mask;      // (env e at row e)
+    int32_t *traj_scalars;
+    int32_t *traj_actions;   // jss_rollout_traj (may be NULL)
+    uint8_t *wire;           // [N][wire_stride] packed observation rows (JSS_WIRE_JOB_BYTES per job): pack
     int32_t wire_stride;
-    JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size)
-    // jss_step_logits / jss_step_greedy: env i's logits (scores) at logits + i * logits_ld; the chosen actions go to
-    // actions_out, their log-probabilities to log_prob_out (may be NULL).  jss_rollout_priority (_sample): env i's
-    // priority (logit) of operation k of job j at logits + i * logits_ld + j * prio_ld_job + k * prio_ld_op; _sample
-    // writes env i's episode log-probability to log_prob_out[i]
-    const float *logits;
-    float *log_prob_out;
-    int64_t logits_ld;
+    JssInst uni;             // the single instance of a uniform batch (step kernel scalars, tile block size): launch_all
+    const float *rows;       // env i's row at rows + i * rows_ld: jss_step_logits / _greedy (_record), jss_beam_step
+    float *log_prob_out;     // log-probabilities: the row steps (may be NULL) and the sampling and order modes
+    int64_t rows_ld;
+    int32_t greedy;          // a row step decodes epsilon-greedily instead of drawing: jss_step_greedy (_record)
+    int32_t split;           // S, the work items a tile's candidates or samples are spread over: mode_grid or the caller
+    int32_t n_samples;       // K, the samples or orders per env: jss_sample_episodes, jss_order_log_prob (_grad), ...
+    int32_t beam_width;      // W, the beams per env (beam search, SWOR) or the envs per group (the beam steps)
+    int32_t max_moves;       // the moves each order may take: jss_improve_orders
+    uint32_t seed_folded;    // jss_fold32(seed), hashed with sample_counter + d: the table samplers, the stochastic
+                             // beam step
+    uint64_t seed;           // jss_hash3's seed: jss_policy, jss_rollout (_traj), jss_lookahead
+    uint64_t sample_counter; // the RNG counter of an env's first draw (jss_stochastic_beam_step: of the round)
+    int64_t out_ld;          // the row stride of every per-env output row, and of the weights
+    JssTable table;          // the caller's table: the priority, sampling, beam-search and order modes
+    const int32_t *order_in;     // [N][K][jobs_max][machines_max] orders: jss_order_log_prob (_grad), jss_improve_orders
+    const int32_t *sample_in;    // [N] the sample each env replays (< 0: none): jss_sample_episodes_solution
+    const float *weights;        // row i: each sample's weight: the _grad modes
+    uint16_t *beam_trace;        // per CTA, W backpointers per round: the beam searches that write orders (NULL: none)
+    const int32_t *beam_groups;  // per group [g, instance, W block offsets in 16-byte units], by lane class: beam steps
+    int32_t *values_out;     // row i: each action's value: jss_lookahead (_priority)
+    int32_t *makespan_out;   // row i: each sample's, slot's or order's makespan
+    float *score_out;        // row i: each slot's score: jss_beam_search
+    float *key_out;          // row i: each slot's key: jss_sample_without_replacement
+    int32_t *start_out;      // row i: each input order's makespan: jss_improve_orders
+    int32_t *moves_out;      // row i: each order's accepted moves: jss_improve_orders
+    int32_t *order_out;      // [jobs_max][machines_max] per order written: the beam searches (may be NULL), improve
+    int32_t *solution_out;   // [N][jobs_max][machines_max] start times: jss_sample_episodes_solution
+    float *grad_out;         // [N][jobs_max][machines_max] per chunk: jss_rollout_priority_sample (may be NULL), _grad
+    float *score_io;         // [N] each slot's score, read and written: the beam steps (slot b of group g: env g W + b)
+    float *key_io;           // [N] each slot's key, read and written: jss_stochastic_beam_step
+    int32_t *parent_out;     // [N] each slot's parent slot: the beam steps
+    int32_t *job_out;        // [N] each slot's job: the beam steps
+    int32_t *bad_out;        // [N / W] each group's bad-row bit: the beam steps
 };
 
 #define JSS_MODE_RESET 0

@@ -47,6 +47,21 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
+def _table_args(v):
+    """The pointer and the three element strides of a table view (JssVecEnv._table_view), as the entry points take
+    them.  The caller keeps `v` alive across the call: it may be a converted copy."""
+    return (v.data_ptr(), *(int(s) for s in v.stride()))
+
+
+def _best_slot(makespan):
+    """Per row of an (N, k) int32 makespan tensor, the lowest column of smallest makespan among those that ended
+    (>= 0), -1 if none: (N,) int64."""
+    import torch
+    ended = makespan >= 0
+    best = torch.where(ended, makespan, torch.iinfo(torch.int32).max).argmin(1)
+    return torch.where(ended.any(1), best, -1)
+
+
 def _host_buffer(shape, dtype):
     """Host staging buffer, page-locked where the backend can pin (DMA target, device-mapped writes); a backend that
     does not declare ``pin_memory`` gets ordinary pageable memory."""
@@ -476,8 +491,7 @@ class JssVecEnv:
         v = self._table_view(self._table_arg(priorities, "rollout_priority", "priorities"))
         if n_steps is None:
             n_steps = 2 * J * M + 1
-        rc = self._L.jss_rollout_priority(self._h, v.data_ptr(), *(int(s) for s in v.stride()), int(n_steps),
-                                          self._stream())
+        rc = self._L.jss_rollout_priority(self._h, *_table_args(v), int(n_steps), self._stream())
         N.check(self._h, rc, "jss_rollout_priority")
         return self._obs(), self.reward, self.done, self._truncated, {}
 
@@ -507,9 +521,8 @@ class JssVecEnv:
         import torch
         v = self._table_view(x)
         log_prob = torch.empty(self.num_envs, dtype=torch.float32, device=self.device)
-        rc = self._L.jss_rollout_priority_sample(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
-                                                 self._step_index, n_steps, log_prob.data_ptr(), _ptr(grad_out),
-                                                 self._stream())
+        rc = self._L.jss_rollout_priority_sample(self._h, *_table_args(v), self.seed, self._step_index, n_steps,
+                                                 log_prob.data_ptr(), _ptr(grad_out), self._stream())
         N.check(self._h, rc, "jss_rollout_priority_sample")
         self._step_index += n_steps
         return log_prob
@@ -549,8 +562,7 @@ class JssVecEnv:
         advance."""
         v = self._table_view(self._table_arg(priorities, "lookahead_priority", "priorities"))
         out = self._values_out(out, "lookahead_priority")
-        rc = self._L.jss_lookahead_priority(self._h, v.data_ptr(), *(int(s) for s in v.stride()), out.data_ptr(),
-                                            int(out.shape[1]), self._stream())
+        rc = self._L.jss_lookahead_priority(self._h, *_table_args(v), out.data_ptr(), int(out.shape[1]), self._stream())
         N.check(self._h, rc, "jss_lookahead_priority")
         return out
 
@@ -577,17 +589,15 @@ class JssVecEnv:
         else:
             makespan, log_prob = self._sample_episodes(x, k, step_index)
         self._step_index += k * (2 * J * M + 1)
-        ended = makespan >= 0
-        best = torch.where(ended, makespan, torch.iinfo(torch.int32).max).argmin(1)
-        best = torch.where(ended.any(1), best, -1)
+        best = _best_slot(makespan)
         out = {"makespan": makespan, "log_prob": log_prob, "best": best}
         if solution:
             sol = (self.solution.clone() if self.solution is not None
                    else torch.full((self.num_envs, J, M), -1, dtype=torch.int32, device=self.device))
             v = self._table_view(x)
             b32 = best.to(torch.int32)
-            rc = self._L.jss_sample_episodes_solution(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
-                                                      step_index, b32.data_ptr(), sol.data_ptr(), self._stream())
+            rc = self._L.jss_sample_episodes_solution(self._h, *_table_args(v), self.seed, step_index, b32.data_ptr(),
+                                                      sol.data_ptr(), self._stream())
             N.check(self._h, rc, "jss_sample_episodes_solution")
             out["solution"] = sol
         return out
@@ -620,13 +630,10 @@ class JssVecEnv:
         score = torch.empty((self.num_envs, width), dtype=torch.float32, device=self.device)
         ord_ = (torch.full((self.num_envs, self.jobs, self.machines), -1, dtype=torch.int32, device=self.device)
                 if order else None)
-        rc = self._L.jss_beam_search(self._h, v.data_ptr(), *(int(s) for s in v.stride()), width,
-                                     makespan.data_ptr(), score.data_ptr(), width, _ptr(ord_), self._stream())
+        rc = self._L.jss_beam_search(self._h, *_table_args(v), width, makespan.data_ptr(), score.data_ptr(), width,
+                                     _ptr(ord_), self._stream())
         N.check(self._h, rc, "jss_beam_search")
-        ended = makespan >= 0
-        best = torch.where(ended, makespan, torch.iinfo(torch.int32).max).argmin(1)
-        best = torch.where(ended.any(1), best, -1)
-        out = {"makespan": makespan, "score": score, "best": best}
+        out = {"makespan": makespan, "score": score, "best": _best_slot(makespan)}
         if order:
             out["order"] = ord_
         return out
@@ -721,10 +728,7 @@ class JssVecEnv:
         else:
             log_prob, makespan, key, ord_ = run(x)
         self._step_index += self.jobs * self.machines
-        ended = makespan >= 0
-        best = torch.where(ended, makespan, torch.iinfo(torch.int32).max).argmin(1)
-        best = torch.where(ended.any(1), best, -1)
-        out = {"makespan": makespan, "log_prob": log_prob, "key": key, "best": best}
+        out = {"makespan": makespan, "log_prob": log_prob, "key": key, "best": _best_slot(makespan)}
         if order:
             out["order"] = ord_
         return out
@@ -740,9 +744,9 @@ class JssVecEnv:
         key = torch.empty((n, k), dtype=torch.float32, device=self.device)
         ord_ = (torch.full((n, k, self.jobs, self.machines), -1, dtype=torch.int32, device=self.device)
                 if order else None)
-        rc = self._L.jss_sample_without_replacement(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
-                                                    step_index, k, makespan.data_ptr(), log_prob.data_ptr(),
-                                                    key.data_ptr(), k, _ptr(ord_), self._stream())
+        rc = self._L.jss_sample_without_replacement(self._h, *_table_args(v), self.seed, step_index, k,
+                                                    makespan.data_ptr(), log_prob.data_ptr(), key.data_ptr(), k,
+                                                    _ptr(ord_), self._stream())
         N.check(self._h, rc, "jss_sample_without_replacement")
         return log_prob, makespan, key, ord_
 
@@ -758,14 +762,7 @@ class JssVecEnv:
         to it (jss_order_log_prob_grad); the envs must not be stepped or reset between this call and the backward."""
         import torch
         x = self._table_arg(logits, "order_log_prob", "logits")
-        n, J, M = self.num_envs, self.jobs, self.machines
-        o = torch.as_tensor(order, device=self.device)
-        single = o.dim() == 3
-        if (o.dim() not in (3, 4) or o.shape[0] != n or tuple(o.shape[-2:]) != (J, M) or o.is_floating_point()
-                or o.is_complex() or o.dtype == torch.bool or (o.dim() == 4 and o.shape[1] < 1)):
-            raise ValueError(f"order_log_prob: order must be an integer tensor of shape ({n}, {J}, {M}) or "
-                             f"({n}, k, {J}, {M}), got {tuple(o.shape)} {o.dtype}")
-        o = o.reshape(n, -1, J, M).to(torch.int32).contiguous()
+        o, single = self._orders_arg(order, "order_log_prob")
         run = functools.partial(self._order_log_prob, order=o)
         if x.requires_grad and torch.is_grad_enabled():
             log_prob, makespan, _ = _order_log_prob_fn().apply(x, self, run)
@@ -790,18 +787,12 @@ class JssVecEnv:
         input also ``"best"`` (N,) int64, the lowest s of smallest makespan, -1 if none.  The improved order is an
         imitation target: ``order_log_prob(logits, out["order"])`` is its differentiable log-likelihood."""
         import torch
-        n, J, M = self.num_envs, self.jobs, self.machines
-        o = torch.as_tensor(order, device=self.device)
-        single = o.dim() == 3
-        if (o.dim() not in (3, 4) or o.shape[0] != n or tuple(o.shape[-2:]) != (J, M) or o.is_floating_point()
-                or o.is_complex() or o.dtype == torch.bool or (o.dim() == 4 and o.shape[1] < 1)):
-            raise ValueError(f"improve_orders: order must be an integer tensor of shape ({n}, {J}, {M}) or "
-                             f"({n}, k, {J}, {M}), got {tuple(o.shape)} {o.dtype}")
+        n = self.num_envs
+        o, single = self._orders_arg(order, "improve_orders")
         if max_moves is None:
             max_moves = 2 ** 31 - 1
         elif isinstance(max_moves, bool) or not isinstance(max_moves, (int, np.integer)) or not 0 <= max_moves < 2 ** 31:
             raise ValueError(f"improve_orders: max_moves must be None or an integer in [0, 2^31), got {max_moves!r}")
-        o = o.reshape(n, -1, J, M).to(torch.int32).contiguous()
         k = o.shape[1]
         out = {"order": torch.full_like(o, -1)}
         for name in ("makespan", "start_makespan", "moves"):
@@ -812,10 +803,7 @@ class JssVecEnv:
         N.check(self._h, rc, "jss_improve_orders")
         if single:
             return {name: t[:, 0] for name, t in out.items()}
-        ms = out["makespan"]
-        ended = ms >= 0
-        best = torch.where(ended, ms, torch.iinfo(torch.int32).max).argmin(1)
-        out["best"] = torch.where(ended.any(1), best, -1)
+        out["best"] = _best_slot(out["makespan"])
         return out
 
     def _order_log_prob(self, x, order):
@@ -826,8 +814,8 @@ class JssVecEnv:
         k = order.shape[1]
         makespan = torch.empty((self.num_envs, k), dtype=torch.int32, device=self.device)
         log_prob = torch.empty((self.num_envs, k), dtype=torch.float32, device=self.device)
-        rc = self._L.jss_order_log_prob(self._h, v.data_ptr(), *(int(s) for s in v.stride()), order.data_ptr(), k,
-                                        makespan.data_ptr(), log_prob.data_ptr(), k, self._stream())
+        rc = self._L.jss_order_log_prob(self._h, *_table_args(v), order.data_ptr(), k, makespan.data_ptr(),
+                                        log_prob.data_ptr(), k, self._stream())
         N.check(self._h, rc, "jss_order_log_prob")
         return log_prob, makespan, order
 
@@ -839,8 +827,8 @@ class JssVecEnv:
         k = order.shape[1]
         w = weights.detach().to(torch.float32).contiguous()
         grad = torch.zeros((split, self.num_envs, self.jobs, self.machines), dtype=torch.float32, device=self.device)
-        rc = self._L.jss_order_log_prob_grad(self._h, v.data_ptr(), *(int(s) for s in v.stride()), order.data_ptr(),
-                                             k, w.data_ptr(), k, int(split), grad.data_ptr(), self._stream())
+        rc = self._L.jss_order_log_prob_grad(self._h, *_table_args(v), order.data_ptr(), k, w.data_ptr(), k, int(split),
+                                             grad.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_order_log_prob_grad")
         return grad
 
@@ -851,8 +839,8 @@ class JssVecEnv:
         v = self._table_view(x)
         makespan = torch.empty((self.num_envs, k), dtype=torch.int32, device=self.device)
         log_prob = torch.empty((self.num_envs, k), dtype=torch.float32, device=self.device)
-        rc = self._L.jss_sample_episodes(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed, step_index,
-                                         k, makespan.data_ptr(), log_prob.data_ptr(), k, self._stream())
+        rc = self._L.jss_sample_episodes(self._h, *_table_args(v), self.seed, step_index, k, makespan.data_ptr(),
+                                         log_prob.data_ptr(), k, self._stream())
         N.check(self._h, rc, "jss_sample_episodes")
         return makespan, log_prob
 
@@ -863,9 +851,8 @@ class JssVecEnv:
         v = self._table_view(x)
         w = weights.detach().to(torch.float32).contiguous()
         grad = torch.zeros((split, self.num_envs, self.jobs, self.machines), dtype=torch.float32, device=self.device)
-        rc = self._L.jss_sample_episodes_grad(self._h, v.data_ptr(), *(int(s) for s in v.stride()), self.seed,
-                                              step_index, k, w.data_ptr(), k, int(split), grad.data_ptr(),
-                                              self._stream())
+        rc = self._L.jss_sample_episodes_grad(self._h, *_table_args(v), self.seed, step_index, k, w.data_ptr(), k,
+                                              int(split), grad.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_sample_episodes_grad")
         return grad
 
@@ -892,6 +879,18 @@ class JssVecEnv:
         if v.dtype != torch.float32:
             v = v.to(torch.float32)
         return v.expand(self.num_envs, self.jobs, self.machines)
+
+    def _orders_arg(self, order, who: str):
+        """Operation orders, (N, J, M) or (N, k, J, M) integer, as an (N, k, J, M) contiguous int32 tensor on the env's
+        device, and whether they came without the k dimension."""
+        import torch
+        n, J, M = self.num_envs, self.jobs, self.machines
+        o = torch.as_tensor(order, device=self.device)
+        if (o.dim() not in (3, 4) or o.shape[0] != n or tuple(o.shape[-2:]) != (J, M) or o.is_floating_point()
+                or o.is_complex() or o.dtype == torch.bool or (o.dim() == 4 and o.shape[1] < 1)):
+            raise ValueError(f"{who}: order must be an integer tensor of shape ({n}, {J}, {M}) or "
+                             f"({n}, k, {J}, {M}), got {tuple(o.shape)} {o.dtype}")
+        return o.reshape(n, -1, J, M).to(torch.int32).contiguous(), o.dim() == 3
 
     def _values_out(self, out, who: str):
         """The (N, >= J+1) contiguous int32 device table a lookahead writes: `out` once checked, else a fresh (N, J+1)
