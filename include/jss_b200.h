@@ -493,6 +493,39 @@ int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_e
                                  uint64_t seed, uint64_t step_index, const int32_t *sample_dev,
                                  int32_t *solution_out_dev, void *stream);
 
+/* jss_lookahead() with k episodes drawn from a caller's logit table after each candidate: every legal action of every
+ * env valued by k sampled rollouts to the end of its episode, in one launch per lane class present, changing nothing
+ * but the caller's values.  These are the action values Q(s, a) of the table's stochastic policy that a rollout
+ * policy-improvement step (argmin of the mean or best-of-k), a soft improvement target exp(-Q / tau) or a per-action
+ * baseline needs, without a twin batch and an import, a step and a jss_sample_episodes() per candidate.
+ *   Table: that of jss_rollout_priority_sample(), entry logits_dev[i*ld_env + j*ld_job + k*ld_op].
+ *   Candidates: those of jss_lookahead(), the set bits of env i's action_mask row, each taken whatever its logit.
+ *   Value: with B = 2*J*M + 1 (J and M the batch maxima, the B of jss_sample_episodes()), makespan_out_dev[i*ld + a*k +
+ *     s] is the current_time_step at which env i's episode ends if it takes a now and then draws at most B decisions,
+ *     decision d at RNG counter step_index + s*B + d, exactly as sample s of jss_sample_episodes() draws them.
+ *     Equivalently: a twin batch (same instances, seed and env_id_base, auto-reset off, env i in the same state)
+ *     stepped with a and then run with jss_sample_episodes(logits, seed, step_index, k) has column s of its makespan
+ *     equal to makespan_out[i][a*k + s]; where the step alone ends the episode, every s holds that end time.  Common
+ *     random numbers: every candidate of an env uses the same counters, so differences between candidates reflect the
+ *     action, not the noise.
+ *   -1 is written for every pair of an illegal column 0..J_i, every pair of an env done at entry, a candidate step that
+ *     leaves the env unchanged with the error bit, and a sample that stops before done: nothing legal, a bad table at
+ *     one of its decisions (the bad-row rule of jss_rollout_priority_sample(); no error bit is set), or the bound.
+ *     Entries (J_i+1)*k .. ld-1 are not written.  How each env's pairs are spread over work items is the library's
+ *     choice and changes no output.
+ *   No side effects: those of jss_lookahead().  The call reads only the state blocks and neither needs nor triggers
+ *     jss_refresh_obs().
+ *   Returns JSS_ERR_INVALID for a NULL or not 4-byte-aligned pointer, a negative stride, k < 1, k*B past 2^64 or
+ *     ld < (jobs_max + 1)*k, JSS_ERR_UNSUPPORTED for k >= 2^31 or tiles*(jobs_max + 1)*k >= 2^31 (tiles: at most one
+ *     per 8 envs of an instance), and JSS_ERR_STATE before jss_assign().
+ * Cost: about one jss_sample_episodes() sample per (legal candidate, s) pair.  Measured on an H100 SXM 80 GB HBM3 at a
+ * 700 W power limit (seeded per-env table, median of three rounds): ta80 at N = 256, k = 16 from reset 831.8 ms per
+ * call against 889.8 ms for import_state + jss_step + jss_sample_episodes per candidate column; after 500 random
+ * decisions 83.0 against 701.4 ms; ta01 at N = 4 096, k = 8 53.9 against 68.6 ms (DESIGN.md section 4). */
+int jss_lookahead_sample(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                         uint64_t seed, uint64_t step_index, int64_t k, int32_t *makespan_out_dev, int64_t ld,
+                         void *stream);
+
 /* Beam search over a caller's logit table, in one launch per lane class present, leaving the envs untouched: the W
  * most likely schedules per env under the table's softmax policy, keeping W partial schedules per env on chip (one CTA
  * per env, the beams' state blocks in shared memory).  Deterministic: no RNG, no seed.

@@ -72,6 +72,8 @@ SIGNATURES = {
                                             _VP]),
     "jss_lookahead": (c_int, [_VP, c_int, c_int, c_uint64, c_uint64, _VP, c_int64, _VP]),
     "jss_lookahead_priority": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP]),
+    "jss_lookahead_sample": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, c_int64,
+                                     _VP]),
     "jss_sample_episodes": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, _VP, c_int64,
                                     _VP]),
     "jss_sample_episodes_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, c_int64,

@@ -257,6 +257,11 @@ int mode_grid(jss_t *h, JssLaunch &a, int c, size_t smem, int &grid) {
         const int most = m.grid == JSS_GRID_SPREAD_J ? std::min(h->p.jobs_max, 32 << c) + 1 : a.n_samples;
         a.split = n >= slots ? 1 : std::min(most, (slots + n - 1) / n);
     }
+    if (m.grid == JSS_GRID_SPREAD_JK) {   // rounded down: a tile's many pairs make every item long, and a CTA that
+                                          // took a second one would double the launch
+        const int64_t most = (int64_t)(std::min(h->p.jobs_max, 32 << c) + 1) * a.n_samples;
+        a.split = n >= slots ? 1 : (int)std::min<int64_t>(most, slots / n);
+    }
     const int64_t items = m.item == JSS_ITEM_SPLIT ? (int64_t)n * a.split
                         : m.item == JSS_ITEM_ENV ? (int64_t)n * JSS_WARPS_PER_CTA
                         : m.item == JSS_ITEM_ORDER ? (int64_t)n * JSS_WARPS_PER_CTA * a.n_samples : n;
@@ -1059,6 +1064,28 @@ int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_e
     a.sample_in = sample_dev;
     a.solution_out = solution_out_dev;
     a.split = 1;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int jss_lookahead_sample(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                         uint64_t seed, uint64_t step_index, int64_t k, int32_t *makespan_out_dev, int64_t ld,
+                         void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    const char *who = "jss_lookahead_sample";
+    JssLaunch a{};
+    a.mode = JSS_MODE_LOOKAHEAD_SAMPLE;
+    if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
+        return rc;
+    const int64_t row = (int64_t)(h->p.jobs_max + 1) * k;   // k < 2^31 here
+    if (bad_ptr(makespan_out_dev) || ld < row)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p must be non-NULL and 4-byte aligned, ld "
+                    "%lld >= (jobs_max + 1) * k = %lld)", who, (void *)makespan_out_dev, (long long)ld,
+                    (long long)row);
+    // a tile's split reaches (jobs_max + 1) k at most: its work items, and an env's pairs, stay below 2^31
+    if ((int64_t)h->n_tiles * row > INT32_MAX)
+        return fail(h, JSS_ERR_UNSUPPORTED, "%s: tiles * (jobs_max + 1) * k must stay below 2^31", who);
+    a.values_out = makespan_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);
 }
 

@@ -1573,27 +1573,37 @@ JSS_DEV JssTileWarp jss_tile(const JssParams &p, const JssLaunch &a, bool uni, i
     return t;
 }
 
-// ---- one-step lookahead over a dispatching rule or a priority table (jss_lookahead, jss_lookahead_priority) -----
-// Work item (tile, sp) of a launch split S ways (a.split): warp `warp` values its env of the tile at the candidates
-// c = sp, sp + S, ... <= J.  Each candidate is simulated in registers from the env's state block, which the call never
-// writes: load, step c, then the rule's decisions d = 0, 1, ... (RNG counter step_index + d, so every candidate of an
-// env sees the same numbers) until done, at most 2 J M + 1 of them, every step with env_step<KJ, false>.  Lane 0 stores
-// the end time, or -1 for an illegal candidate, an env done at entry, and a rollout that stops before done (the rule
-// finds nothing legal, a step leaves the env unchanged with the error bit, or the bound trips).  The block is reloaded
-// for each candidate (unchanged and L2-resident) instead of kept as a second register copy of the root state.  The
-// values go to a.values_out.
-// PRIO (jss_lookahead_priority): the decisions after the candidate are env_priority_action's on the caller's table
-// (a.table), no RNG; a bad table at a decision (JSS_INF) stops that candidate's rollout, which then reads -1, and
-// touches nothing else.
-template <int KJ, bool PRIO>
+// ---- one-step lookahead over a rule, a priority table or a logit table (jss_lookahead, _priority, _sample) -------
+// Work item (tile, sp) of a launch split S ways (a.split): warp `warp` values its env of the tile at the (candidate,
+// sample) pairs q = sp, sp + S, ... < (J + 1) K, candidate c = q / K and sample s = q % K (K = 1 but for the sampled
+// kind, so that the other two loop over the candidates c = sp, sp + S, ... <= J).  Each pair is simulated in registers
+// from the env's state block, which the call never writes: load, step c, then the kind's decisions d = 0, 1, ... until
+// done, every step with env_step<KJ, false>.  Lane 0 stores the end time at column q of the env's row of a.values_out,
+// or -1 for an illegal candidate, an env done at entry, and a rollout that stops before done (nothing is legal, a step
+// leaves the env unchanged with the error bit, a bad table entry, or the bound trips).  The block is reloaded for each
+// pair (unchanged and L2-resident) instead of kept as a second register copy of the root state.
+// JSS_LOOK_RULE (jss_lookahead): the rule's decisions, RNG counter step_index + d, at most 2 J M + 1 of them.
+// JSS_LOOK_TABLE (jss_lookahead_priority): env_priority_action's on the caller's table (a.table), no RNG, at most
+//   2 J M + 1.  A bad table at a decision (JSS_INF) stops that candidate's rollout and touches nothing else.
+// JSS_LOOK_SAMPLE (jss_lookahead_sample): env_priority_sample_action's draws on the caller's logit table, K =
+//   a.n_samples, decision d of sample s at RNG counter sample_counter + s B + d, B = 2 jobs_max machines_max + 1, as
+//   env_sample_episodes draws them, and at most B of them.  Every candidate of an env sees the same numbers.
+#define JSS_LOOK_RULE 0
+#define JSS_LOOK_TABLE 1
+#define JSS_LOOK_SAMPLE 2
+template <int KJ, int KIND>
 JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile, int warp,
                            int lane, int sp, float *scratch) {
+    constexpr bool SAMPLE = KIND == JSS_LOOK_SAMPLE;
     const int32_t *blk = p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4;
     int32_t *out = a.values_out + (int64_t)env * a.out_ld;
     const uint64_t genv = p.env_id_base + (uint64_t)env;
-    const int J = jss_J(iv), bound = 2 * J * jss_M(iv) + 1;
+    const int J = jss_J(iv), bound = SAMPLE ? 2 * p.jobs_max * p.machines_max + 1 : 2 * J * jss_M(iv) + 1;
+    const int K = SAMPLE ? a.n_samples : 1, pairs = (J + 1) * K;   // below 2^31: jss_lookahead_sample checks it
     int *hz = reinterpret_cast<int *>(scratch);
-    for (int c = sp; c <= J; c += a.split) {
+    for (int q = sp; SAMPLE ? q < pairs : q <= J; q += a.split) {
+        const int c = SAMPLE ? q / K : q, smp = SAMPLE ? q % K : 0;
+        const uint64_t c0 = a.sample_counter + (uint64_t)smp * (uint64_t)bound;
         EnvRegs<KJ> s;
         env_load<KJ>(iv, blk, lane, s);
         s.flags = jss_uniform(s.flags);
@@ -1607,19 +1617,23 @@ JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstVie
             s.flags = jss_uniform(s.flags);
             for (int d = 0; ok && !(s.flags & JSS_FLAG_DONE) && d < bound; d++) {
                 int act;
-                if (PRIO) {
+                if (KIND == JSS_LOOK_TABLE) {
                     act = jss_uniform(env_priority_action<KJ>(a, iv, s, env, lane));
+                } else if (SAMPLE) {
+                    const uint32_t h = jss_hash_env(jss_hash_key_folded(a.seed_folded, c0 + (uint64_t)d), genv);
+                    float logp, pr[KJ];
+                    act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
                 } else {
                     const uint32_t h = jss_hash3(a.seed, genv, a.step_index + (uint64_t)d);
                     act = jss_uniform(env_select_action<KJ>(iv, s, lane, a.rule, a.coin_mode, h, a.cr_factor));
                 }
-                ok = act != JSS_ACTION_SKIP && !(PRIO && act == JSS_INF) &&
+                ok = act != JSS_ACTION_SKIP && !(KIND != JSS_LOOK_RULE && act == JSS_INF) &&
                      env_step<KJ, false>(p, iv, s, env, lane, act, r, hz);
                 s.flags = jss_uniform(s.flags);
             }
             if (s.flags & JSS_FLAG_DONE) t = s.t;
         }
-        if (lane == 0) out[c] = t;
+        if (lane == 0) out[q] = t;
     }
 }
 
@@ -2537,6 +2551,8 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
 #define JSS_GRID_SPREAD_J 2   // the same, with each tile's candidates spread over S items while the tiles alone leave
                               // slots empty: S = 1 once they fill them, up to the class's J + 1 for a small batch
 #define JSS_GRID_SPREAD_K 3   // the same, up to S = K samples per tile
+#define JSS_GRID_SPREAD_JK 4  // the same, up to S = (the class's J + 1) K (candidate, sample) pairs per tile, with
+                              // S = slots / tiles rounded down, so that every item runs in the first wave
 // The host stages what the rule reads: ops / len, + the suffix sums for MWR / LWR / CR, no table for the masked-uniform
 // sampler (it reads only J)
 #define JSS_STAGE_BY_RULE (-1)
@@ -2620,6 +2636,10 @@ constexpr JssMode JSS_MODES[] = {
     // per lane.  Its shared memory (three [J][M] tables) bounds the resident CTAs at large J M.
     {JSS_MODE_IMPROVE_ORDERS, {8, 6, 4, 2}, JSS_ITEM_ORDER, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_IMPROVE, false,
      JSS_REFRESH_NO},
+    // the sampled lookahead: the lookahead loop with the draws of the sampled episodes, 25 / 31 / 56 / 91 registers; 8
+    // is the SM's limit, and one CTA more spills with 8 jobs per lane, as do 5 and 6 with 4
+    {JSS_MODE_LOOKAHEAD_SAMPLE, {8, 8, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_JK, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},
 };
 static_assert(sizeof(JSS_MODES) / sizeof(JSS_MODES[0]) == JSS_NUM_MODES, "one row per JSS_MODE_*");
 // a mode that another mode's kernel runs has that kernel's loop, tables, layout and launch bound
@@ -2688,7 +2708,9 @@ jss_env_kernel(const JssParams p, const JssLaunch a, const JssSmemLayout sl) {
             else if constexpr (jss_mode_samples(MODE))
                 env_sample_episodes<KJ, MODE>(p, a, iv, env, tile, warp, lane, sub, scratch);
             else
-                env_lookahead<KJ, MODE == JSS_MODE_LOOKAHEAD_PRIORITY>(p, a, iv, env, tile, warp, lane, sub, scratch);
+                env_lookahead<KJ, MODE == JSS_MODE_LOOKAHEAD_PRIORITY ? JSS_LOOK_TABLE
+                                  : MODE == JSS_MODE_LOOKAHEAD_SAMPLE ? JSS_LOOK_SAMPLE : JSS_LOOK_RULE>(
+                    p, a, iv, env, tile, warp, lane, sub, scratch);
         }
     }
 }

@@ -219,7 +219,7 @@ struct JssLaunch {
     const float *weights;        // row i: each sample's weight: the _grad modes
     uint16_t *beam_trace;        // per CTA, W backpointers per round: the beam searches that write orders (NULL: none)
     const int32_t *beam_groups;  // per group [g, instance, W block offsets in 16-byte units], by lane class: beam steps
-    int32_t *values_out;     // row i: each action's value: jss_lookahead (_priority)
+    int32_t *values_out;     // row i: each action's value: jss_lookahead (_priority; _sample: K per action)
     int32_t *makespan_out;   // row i: each sample's, slot's or order's makespan
     float *score_out;        // row i: each slot's score: jss_beam_search
     float *key_out;          // row i: each slot's key: jss_sample_without_replacement
@@ -270,6 +270,8 @@ struct JssLaunch {
                                          // (jss_stochastic_beam_step)
 #define JSS_MODE_IMPROVE_ORDERS 21       // operation orders improved by steepest descent on the critical path, one
                                          // (env, order) per CTA, the envs untouched (jss_improve_orders)
-#define JSS_NUM_MODES 22                 // the rows of JSS_MODES (jss_device.cuh)
+#define JSS_MODE_LOOKAHEAD_SAMPLE 22     // each legal action's makespans under K episodes drawn from a logit table
+                                         // after it, the envs untouched (jss_lookahead_sample)
+#define JSS_NUM_MODES 23                 // the rows of JSS_MODES (jss_device.cuh)
 
 #define JSS_WARPS_PER_CTA 8

@@ -566,6 +566,44 @@ class JssVecEnv:
         N.check(self._h, rc, "jss_lookahead_priority")
         return out
 
+    def lookahead_sample(self, logits, k: int, out=None):
+        """Value every legal action by `k` episodes drawn from the logit table `logits` after it, in one launch per lane
+        class (jss_lookahead_sample), leaving the envs untouched: the action values Q(s, a) of the table's stochastic
+        policy.  With B = 2*J*M + 1, ``"makespan"[i, a, s]`` is the makespan env i reaches if it takes action a now and
+        then draws as sample s of sample_episodes(logits, k) would (decision d at RNG counter ``self._step_index +
+        s*B + d``), or its end time at once if a ends the episode; -1 for an action that is not legal (the no-op
+        unless it is), every action of a done env, and a sample that stops before done, such as one that meets a bad
+        entry (no error bit is set).  Every action of an env uses the same counters (common random numbers), so
+        differences between actions reflect the action, not the noise.  `logits` is taken as by
+        rollout_priority_sample(); a table that requires grad is read detached (the values have no gradient).  `out`:
+        a contiguous int32 (N, J+1, k) device tensor; by default a fresh one filled with -1, so that the columns past
+        an env's J_i read -1 too (the call writes only columns 0..J_i).  Returns a dict of device tensors: ``"makespan"``
+        (`out`); ``"mean"`` (N, J+1) float32, the mean over the samples that ended (computed in float64), NaN where
+        none did; ``"min"`` (N, J+1) int32, their best, -1 where none did.  The RNG counter advances by k*B."""
+        import torch
+        n, J, M = self.num_envs, self.jobs, self.machines
+        v = self._table_view(self._table_arg(logits, "lookahead_sample", "logits"))
+        if int(k) < 1:
+            raise ValueError(f"lookahead_sample: k must be at least 1, got {k!r}")
+        k = int(k)
+        if out is None:
+            out = torch.full((n, J + 1, k), -1, dtype=torch.int32, device=self.device)
+        elif (not isinstance(out, torch.Tensor) or out.dtype != torch.int32 or tuple(out.shape) != (n, J + 1, k)
+              or not out.is_contiguous() or out.device != self.device):
+            raise ValueError(f"lookahead_sample: out must be a contiguous int32 tensor of shape ({n}, {J + 1}, {k}) "
+                             f"on the env's device")
+        rc = self._L.jss_lookahead_sample(self._h, *_table_args(v), self.seed, self._step_index, k, out.data_ptr(),
+                                          (J + 1) * k, self._stream())
+        N.check(self._h, rc, "jss_lookahead_sample")
+        self._step_index += k * (2 * J * M + 1)
+        ended = out >= 0
+        count = ended.sum(2)
+        total = torch.where(ended, out, 0).sum(2, dtype=torch.float64)
+        mean = torch.where(count > 0, total / count, torch.nan).to(torch.float32)
+        best = torch.where(ended, out, torch.iinfo(torch.int32).max).amin(2)
+        best = torch.where(count > 0, best, -1)
+        return {"makespan": out, "mean": mean, "min": best}
+
     def sample_episodes(self, logits, k: int, solution: bool = False):
         """Draw `k` whole episodes per env from the logit table `logits`, each from the env's current state, in one
         launch per lane class (jss_sample_episodes), leaving the envs untouched.  With B = 2*J*M + 1, sample s of env i
