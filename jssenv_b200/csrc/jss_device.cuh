@@ -1436,73 +1436,88 @@ JSS_DEV void env_store_rollout_end(const JssParams &p, const InstView &iv, int32
     }
 }
 
+// slot i's first operation not drawn yet: todo, or todo + 1 while the drawn operation todo runs (tufco > 0)
+template <int KJ>
+JSS_DEV int env_undrawn(const EnvRegs<KJ> &s, int i) { return s.todo[i] + (s.tufco[i] > 0 ? 1 : 0); }
+
+// The gradient of a sampled episode's log-probability with respect to its env's table entries, into `grad` (one row of
+// stride ms per job): G[j][k] = sum over the decisions t where job j is legal at operation k of (1[j drawn at t] -
+// p_t(j)).  A job is legal only at its current operation, which it leaves only after being drawn there, so each owned
+// slot adds up its p_t in a register and puts 1 - acc when drawn (draw), and 0 - acc at its first undrawn operation at
+// the end (finish, +0 for a job never legal): one 4-byte access per decision, and the table of gradients is never read
+// but by the adds.  Every access to a job's row comes from the lane that owns the job, so program order orders them.
+// ADD (the replays of jss_sample_episodes_grad): a put adds w times the value; else it stores the value.
+template <int KJ, bool ADD>
+struct JssGradAcc {
+    float *grad;
+    int ms;
+    float w;
+    float acc[KJ];
+    JSS_DEV void put(int j, int k, float v) {
+        float *q = grad + (size_t)j * ms + k;
+        if (ADD) *q += w * v;
+        else *q = v;
+    }
+    // job `act` (< J) drawn, the owned slots' probabilities pr
+    JSS_DEV void draw(const EnvRegs<KJ> &s, int lane, int act, const float (&pr)[KJ]) {
+#pragma unroll
+        for (int i = 0; i < KJ; i++) {
+            acc[i] += pr[i];
+            if (KJ * lane + i == act) {
+                put(act, s.todo[i], 1.0f - acc[i]);
+                acc[i] = 0.0f;
+            }
+        }
+    }
+    JSS_DEV void finish(const EnvRegs<KJ> &s, int lane, int J, int M) {
+#pragma unroll
+        for (int i = 0; i < KJ; i++) {
+            const int j = KJ * lane + i, k0 = env_undrawn<KJ>(s, i);
+            if (j < J && k0 < M) put(j, k0, 0.0f - acc[i]);
+        }
+    }
+};
+
 // jss_rollout_priority: decisions (env_priority_action) until the episode ends, at most a.n_steps, without reset; a
 // done env is left as it is.  Bad priorities set the sticky error bit and end the env's call in its state before that
 // decision.  The outputs are written once at the end and equal what the jss_step_greedy calls the loop replaces leave:
 // the whole block and every output if a decision changed the env, else the flags and a zero-reward record if they
 // changed (the rollout's store covers only the first case, which its rules never leave).
-template <int KJ>
+// SAMPLE (jss_rollout_priority_sample): the draws of env_priority_sample_action, decision d with h = jss_hash3(seed,
+// global env id, sample_counter + d).  Besides those outputs: log_prob_out[env], the sum of the decisions'
+// log-probabilities in decision order (NaN if a decision of this call left the env unchanged with the error bit), and,
+// with grad_out, the gradient of that sum with respect to the env's table entries (JssGradAcc).  The operations drawn
+// before the call get 0, the first undrawn one at the end -acc and the later ones 0; an env that errs gets 0
+// everywhere, so that a caller who masks it out gets no NaN in a backward pass.
+template <int KJ, bool SAMPLE>
 JSS_DEV void env_priority_rollout(const JssParams &p, const JssLaunch &a, const InstView &iv, EnvRegs<KJ> &s, int32_t *blk,
                                   int env, int lane, float *scratch) {
-    const uint32_t flags_in = s.flags;
-    bool dirty = false;
-    int raw = 0;                                         // the raw reward in the scalar record
-    for (int k = 0; k < a.n_steps && !(s.flags & JSS_FLAG_DONE); k++) {
-        const int act = jss_uniform(env_priority_action<KJ>(a, iv, s, env, lane));
-        if (act == JSS_ACTION_SKIP) break;               // nothing legal: no decision changes the env
-        const uint32_t flags_before = s.flags;
-        int r = 0;
-        bool changed = false;
-        if (act == JSS_INF) s.flags |= JSS_FLAG_ERROR;
-        else changed = env_step<KJ>(p, iv, s, env, lane, act, r, reinterpret_cast<int *>(scratch));
-        s.flags = jss_uniform(s.flags);
-        if (changed) { raw = r; dirty = true; continue; }
-        // unchanged, with the error bit (bad priorities, or a no-op without a pending event): every later decision
-        // would find the same state.  A new bit comes with a zero-reward record (env_store_flags_only).
-        if (s.flags != flags_before) raw = 0;
-        break;
-    }
-    env_store_rollout_end<KJ>(p, iv, blk, s, env, lane, scratch, dirty, raw, flags_in);
-}
-
-// jss_rollout_priority_sample: the loop of env_priority_rollout with the draws of env_priority_sample_action, decision
-// d with h = jss_hash3(seed, global env id, sample_counter + d).  Besides its outputs: log_prob_out[env], the sum of
-// the decisions' log-probabilities in decision order (NaN if a decision of this call left the env unchanged with the
-// error bit), and, with grad_out, the gradient G of that sum with respect to the env's table entries,
-// G[j][k] = sum over the decisions t where job j is legal at operation k of (1[j drawn at t] - p_t(j)).  A job is legal
-// only at its current operation, which it leaves only after being drawn there, so each owned slot adds up its p_t in a
-// register and stores 1 - acc when drawn: one 4-byte store per decision, and the table of gradients is never read.  The
-// operations drawn before the call get 0, the first undrawn one at the end -acc and the later ones 0; an env that errs
-// gets 0
-// everywhere, so that a caller who masks it out gets no NaN in a backward pass.  Every store to a job's row comes from
-// the lane that owns the job, so program order orders them.
-template <int KJ>
-JSS_DEV void env_priority_sample_rollout(const JssParams &p, const JssLaunch &a, const InstView &iv, EnvRegs<KJ> &s,
-                                         int32_t *blk, int env, int lane, float *scratch) {
     const int J = jss_J(iv), M = jss_M(iv);
-    float *grad = a.grad_out ? a.grad_out + (size_t)env * p.jobs_max * p.machines_max : nullptr;
+    JssGradAcc<KJ, false> g{SAMPLE && a.grad_out ? a.grad_out + (size_t)env * p.jobs_max * p.machines_max : nullptr,
+                            p.machines_max, 1.0f, {}};
     const auto zero_ops = [&](int i, int k0, int k1) {   // operations k0 .. k1-1 of owned slot i
-        float *g = grad + (size_t)(KJ * lane + i) * p.machines_max;
-        for (int k = k0; k < k1; k++) g[k] = 0.0f;
+        for (int k = k0; k < k1; k++) g.put(KJ * lane + i, k, 0.0f);
     };
-    // slot i's first operation not drawn yet: todo, or todo + 1 while the drawn operation todo runs (tufco > 0)
-    const auto undrawn = [&](int i) { return s.todo[i] + (s.tufco[i] > 0 ? 1 : 0); };
-    if (grad) {
+    if (g.grad) {
 #pragma unroll
         for (int i = 0; i < KJ; i++)
-            if (KJ * lane + i < J) zero_ops(i, 0, (s.flags & JSS_FLAG_DONE) ? M : undrawn(i));
+            if (KJ * lane + i < J) zero_ops(i, 0, (s.flags & JSS_FLAG_DONE) ? M : env_undrawn<KJ>(s, i));
     }
     const uint64_t genv = p.env_id_base + (uint64_t)env;
     const uint32_t flags_in = s.flags;
-    bool dirty = false, err = false;
+    bool dirty = false;
     int raw = 0;                                         // the raw reward in the scalar record
-    float lp = 0.0f, acc[KJ];
-#pragma unroll
-    for (int i = 0; i < KJ; i++) acc[i] = 0.0f;
+    bool err = false;
+    float lp = 0.0f;
     for (int k = 0; k < a.n_steps && !(s.flags & JSS_FLAG_DONE); k++) {
-        const uint32_t h = jss_hash_env(jss_hash_key_folded(a.seed_folded, a.sample_counter + (uint64_t)k), genv);
-        float logp, pr[KJ];
-        const int act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
+        float logp = 0.0f, pr[KJ];
+        int act;
+        if (SAMPLE) {
+            const uint32_t h = jss_hash_env(jss_hash_key_folded(a.seed_folded, a.sample_counter + (uint64_t)k), genv);
+            act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
+        } else {
+            act = jss_uniform(env_priority_action<KJ>(a, iv, s, env, lane));
+        }
         if (act == JSS_ACTION_SKIP) break;               // nothing legal: no decision changes the env
         const uint32_t flags_before = s.flags;
         int r = 0;
@@ -1510,39 +1525,27 @@ JSS_DEV void env_priority_sample_rollout(const JssParams &p, const JssLaunch &a,
         if (act == JSS_INF) {
             s.flags |= JSS_FLAG_ERROR;
         } else {
-            if (grad && act < J) {                       // a job drawn (act == J, the no-op, has no p_t)
-#pragma unroll
-                for (int i = 0; i < KJ; i++) {
-                    acc[i] += pr[i];
-                    if (KJ * lane + i == act) {
-                        grad[(size_t)act * p.machines_max + s.todo[i]] = 1.0f - acc[i];
-                        acc[i] = 0.0f;
-                    }
-                }
-            }
+            if (g.grad && act < J) g.draw(s, lane, act, pr);   // a job drawn (act == J, the no-op, has no p_t)
             changed = env_step<KJ>(p, iv, s, env, lane, act, r, reinterpret_cast<int *>(scratch));
         }
         s.flags = jss_uniform(s.flags);
         if (changed) { lp += logp; raw = r; dirty = true; continue; }
-        // unchanged, with the error bit: as in env_priority_rollout, and the call's log-probability is NaN
+        // unchanged, with the error bit (bad priorities, or a no-op without a pending event): every later decision
+        // would find the same state.  A new bit comes with a zero-reward record (env_store_flags_only); the call's
+        // log-probability is NaN.
         err = true;
         if (s.flags != flags_before) raw = 0;
         break;
     }
-    if (grad) {
+    if (SAMPLE) {
+        if (g.grad) {
+            if (!err) g.finish(s, lane, J, M);
 #pragma unroll
-        for (int i = 0; i < KJ; i++) {
-            if (KJ * lane + i >= J) continue;
-            const int k0 = undrawn(i);
-            if (err) {
-                zero_ops(i, 0, M);
-            } else if (k0 < M) {
-                grad[(size_t)(KJ * lane + i) * p.machines_max + k0] = 0.0f - acc[i];   // +0 when never legal
-                zero_ops(i, k0 + 1, M);
-            }
+            for (int i = 0; i < KJ; i++)
+                if (KJ * lane + i < J) zero_ops(i, err ? 0 : env_undrawn<KJ>(s, i) + 1, M);
         }
+        if (lane == 0) a.log_prob_out[env] = err ? JSS_F32_NAN : lp;
     }
-    if (lane == 0) a.log_prob_out[env] = err ? JSS_F32_NAN : lp;
     env_store_rollout_end<KJ>(p, iv, blk, s, env, lane, scratch, dirty, raw, flags_in);
 }
 
@@ -1647,8 +1650,8 @@ JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstVie
 //   ... < K and stores each one's makespan (-1 unless done) and log-probability at column s of the env's rows of
 //   a.makespan_out and a.log_prob_out; an env done at entry gets -1 and 0 in each of those columns.
 // JSS_MODE_SAMPLE_EPISODES_GRAD: work item (tile, c), c < a.split, takes the samples s = c, c + split, ... in
-//   increasing s and adds w_s G_s into chunk c of a.grad_out with env_priority_sample_rollout's accumulator: w_s (1 -
-//   acc) at a drawn operation, w_s (0 - acc) at each job's first undrawn one at the end.  Each entry is read and written
+//   increasing s and adds w_s G_s into chunk c of a.grad_out with JssGradAcc<KJ, true>: w_s (1 - acc) at a drawn
+//   operation, w_s (0 - acc) at each job's first undrawn one at the end.  Each entry is read and written
 //   only by the lane that owns its job, in program order, so a chunk's sums do not depend on the schedule.  A sample
 //   that errs adds nothing.  Only a non-finite table entry or an imported legal job without an operation can make a
 //   sample err after its first draw (a no-op is drawn only from an imported state, at decision 0, before any add), so
@@ -1727,10 +1730,10 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
             for (int k = first; k < end; k += stride) { a.makespan_out[row + k] = -1; a.log_prob_out[row + k] = 0.0f; }
         return;
     }
-    float *grad = nullptr;
+    JssGradAcc<KJ, true> g{GRAD ? a.grad_out + ((size_t)sp * p.n_envs + env) * p.jobs_max * p.machines_max : nullptr,
+                           p.machines_max, 0.0f, {}};
     bool check = false;                                  // GRAD: a sample may err after an add
     if (GRAD) {
-        grad = a.grad_out + ((size_t)sp * p.n_envs + env) * p.jobs_max * p.machines_max;
         const float *tab = jss_table_row(a.table, env);
         bool clean = true;
 #pragma unroll 1
@@ -1758,10 +1761,11 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
             const bool add = GRAD && pass == 1;
             env_load<KJ>(iv, blk, lane, s);
             s.flags = jss_uniform(s.flags);
-            bool err = false;
-            float lp = 0.0f, acc[KJ];
+            g.w = w;
 #pragma unroll
-            for (int i = 0; i < KJ; i++) acc[i] = 0.0f;
+            for (int i = 0; i < KJ; i++) g.acc[i] = 0.0f;
+            bool err = false;
+            float lp = 0.0f;
             for (int d = 0; d < bound && !(s.flags & JSS_FLAG_DONE); d++) {
                 float logp, pr[KJ];
                 int act;
@@ -1775,16 +1779,7 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
                 int r;
                 bool changed = false;
                 if (act != JSS_INF) {
-                    if (add && act < J) {                // a job drawn (the no-op has no p_t)
-#pragma unroll
-                        for (int i = 0; i < KJ; i++) {
-                            acc[i] += pr[i];
-                            if (KJ * lane + i == act) {
-                                grad[(size_t)act * p.machines_max + s.todo[i]] += w * (1.0f - acc[i]);
-                                acc[i] = 0.0f;
-                            }
-                        }
-                    }
+                    if (add && act < J) g.draw(s, lane, act, pr);   // a job drawn (the no-op has no p_t)
                     changed = env_step<KJ, false, false, SOL>(p, iv, s, env, lane, act, r, hz, a.solution_out);
                 }
                 s.flags = jss_uniform(s.flags);
@@ -1796,13 +1791,7 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
                 a.log_prob_out[row + smp] = err ? JSS_F32_NAN : lp;
             }
             if (err) break;                              // GRAD: no adds, or none yet (decision 0 of pass 1)
-            if (add) {
-#pragma unroll
-                for (int i = 0; i < KJ; i++) {
-                    const int j = KJ * lane + i, k0 = s.todo[i] + (s.tufco[i] > 0 ? 1 : 0);
-                    if (j < J && k0 < M) grad[(size_t)j * p.machines_max + k0] += w * (0.0f - acc[i]);
-                }
-            }
+            if (add) g.finish(s, lane, J, M);
         }
     }
 }
@@ -1810,8 +1799,9 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
 // ---- beam search over a logit table, the envs untouched (jss_beam_search) -----------------------------------------
 // Each owned legal job's log-probability under the table, lp[i] = (x - mx) - log(sum exp(x - mx)) over the legal jobs,
 // with the loads, reductions and fast exp / log of env_priority_sample_action in the same order, so that lp of the job
-// it draws equals its logp bit for bit.  Kept apart from it so that its code (and the sampling kernels') stays as it
-// is.  At least one job must be legal; returns false for a bad row (the bad-table rule of env_priority_sample_action).
+// it draws equals its logp bit for bit.  Kept apart from it: with one softmax shared by the two and one loop shared
+// by the rollouts and the sampled-episode replays, those calls ran 1-4 % slower on an H100 (DESIGN.md section 4).
+// At least one job must be legal; returns false for a bad row (the bad-table rule of env_priority_sample_action).
 // ROW (jss_beam_step): x_j is column j of env `env`'s logit row (a.rows) in place of the table entry of job j's current
 // operation; everything else is the same.
 template <int KJ, bool ROW>
@@ -1912,11 +1902,65 @@ JSS_DEV void jss_beam_order(const JssParams &p, const uint16_t *trace, int W, in
 }
 
 // The pieces of a beam round that jss_beam_search, jss_sample_without_replacement and jss_beam_step share.
-// The W argmax passes of the expansion of the beam in slot b: its `taken` best candidates in key order (key[i]: owned
-// job i's key, 0 for none; the passes clear them) go to bs.cand[b W ..].  SWOR: bs.cscore gets their scores sc + lp.
-template <int KJ, bool SWOR>
-JSS_DEV void jss_beam_passes(const JssBeamSmem &bs, uint32_t (&key)[KJ], const float (&lp)[KJ], float sc, int b, int W,
-                             int lane, int taken) {
+// The forced no-ops of a beam: while no job is legal and the no-op is, take it (env_step<KJ, false>; raw: the last
+// one's raw reward).  Returns the number taken, or -1 if one leaves the env unchanged.
+template <int KJ>
+JSS_DEV int env_forced_noops(const JssParams &p, const InstView &iv, EnvRegs<KJ> &s, int env, int lane, int &raw,
+                             int *hz) {
+    constexpr uint32_t LM = jss_legal_mask<KJ>();
+    int n = 0;
+    for (; !__any_sync(JSS_FULL, (s.lb & LM) != 0u) && (s.flags & JSS_FLAG_NOOP_LEGAL); n++) {
+        const bool ok = env_step<KJ, false>(p, iv, s, env, lane, jss_J(iv), raw, hz);
+        s.flags = jss_uniform(s.flags);
+        if (!ok) return -1;
+    }
+    return n;
+}
+
+// The expansion of the beam in slot b (state s, some job legal, score sc; SWOR: its key T = bs.key[kb] and the
+// round's noise hash hr): the log-probabilities lp of its legal jobs under env `env`'s table or, ROW, logit row
+// (env_table_logp), each candidate's score sc + lp and key (jss_f32_key of score + 0; SWOR: the perturbed values G, Z
+// and the key in its place, env_beam_search), and the beam's best min(W, candidates) children in key order, by W argmax
+// passes, to bs.cand[b W ..] (SWOR: their scores to bs.cscore).  Returns their number, or -1 for a bad row.
+template <int KJ, bool SWOR, bool ROW>
+JSS_DEV int jss_beam_expand(const JssLaunch &a, const JssBeamSmem &bs, const EnvRegs<KJ> &s, int env, int lane, int b,
+                            int W, float sc, int kb, uint32_t hr) {
+    float lp[KJ];
+    if (!env_table_logp<KJ, ROW>(a, s, env, lane, lp)) return -1;
+    uint32_t key[KJ];                                    // 0: not a candidate, or already taken
+    int nc = 0;
+#pragma unroll
+    for (int i = 0; i < KJ; i++) {
+        const float cs = sc + lp[i];
+        key[i] = ((s.lb >> i) & 1u) && cs > -JSS_F32_INF ? jss_f32_key(cs + 0.0f) : 0u;
+        nc += key[i] != 0u;
+    }
+    if (SWOR) {                                          // the perturbed values G, Z and the keys in their place
+        const float T = bs.key[kb];
+        float g[KJ];
+        uint32_t zk = 0u;
+        int zj = 1 << 20;
+#pragma unroll
+        for (int i = 0; i < KJ; i++) {
+            g[i] = (sc + lp[i]) + jss_gumbel(jss_hash_env(hr, (uint64_t)(b * 256 + KJ * lane + i)));
+            const uint32_t k = jss_f32_key(g[i] + 0.0f);
+            if (key[i] != 0u && k > zk) { zk = k; zj = KJ * lane + i; }
+        }
+        const uint32_t zbest = __reduce_max_sync(JSS_FULL, zk);
+        zj = (int)__reduce_min_sync(JSS_FULL, (unsigned)(zk == zbest ? zj : 1 << 20));
+        const float Z = jss_key_f32(zbest);
+#pragma unroll
+        for (int i = 0; i < KJ; i++) {
+            if (key[i] == 0u) continue;
+            float kv = T;
+            if (KJ * lane + i != zj) {
+                const float v = T - g[i] + jss_log1mexp(g[i] - Z);
+                kv = fminf(T, T - fmaxf(v, 0.0f) - log1pf(expf(-fabsf(v))));
+            }
+            key[i] = jss_f32_key(kv + 0.0f);
+        }
+    }
+    const int taken = min(W, (int)__reduce_add_sync(JSS_FULL, (unsigned)nc));
     for (int q = 0; q < taken; q++) {
         uint32_t lk = 0u;
         int lj = 1 << 20;
@@ -1938,6 +1982,7 @@ JSS_DEV void jss_beam_passes(const JssBeamSmem &bs, uint32_t (&key)[KJ], const f
             if (lane == 0) bs.cscore[b * W + q] = cj;
         }
     }
+    return taken;
 }
 
 // Selection, by the whole CTA: each kept candidate of the n slots' sorted lists (bs.cnt[b] of them) is ranked against
@@ -1968,8 +2013,8 @@ JSS_DEV int jss_beam_rank(const JssBeamSmem &bs, int n, int W, int cur) {
 // One env searched by the whole CTA (`root`: its state block, never written).  The beams are state blocks in shared
 // memory, double-buffered: round r reads buffer r & 1 and writes the other.  Per round (R rounds, the operations not
 // started at entry; jss_b200.h):
-//   1. warp w expands the beams b = w, w + 8, ...: forced no-ops (stored back in place), the log-probabilities of the
-//      legal jobs (env_table_logp), and the beam's best min(W, candidates) children in key order, by W argmax passes;
+//   1. warp w expands the beams b = w, w + 8, ...: forced no-ops (env_forced_noops, stored back in place; a beam that
+//      then has no legal job has no children), then jss_beam_expand on the table;
 //   2. the CTA ranks every candidate against the others' sorted lists; rank < W becomes slot rank;
 //   3. warp w loads the parent block of each of its new slots, steps the job with env_step<KJ, false> and stores the
 //      result in the other buffer; lane 0 records the backpointer parent << 8 | job in the trace (a.beam_trace).
@@ -2016,56 +2061,19 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
             env_load<KJ>(iv, blk, lane, s);
             s.flags = jss_uniform(s.flags);
             const float sc = bs.score[cur * W + b];
-            bool ok = sc == sc, moved = false;           // NaN: the step into this slot failed (an imported state)
-            while (ok && !__any_sync(JSS_FULL, (s.lb & LM) != 0u)) {   // forced no-ops
-                int raw;
-                ok = (s.flags & JSS_FLAG_NOOP_LEGAL) && env_step<KJ, false>(p, iv, s, env, lane, J, raw, hz);
-                s.flags = jss_uniform(s.flags);
-                moved = true;
-            }
-            if (ok && moved) env_store<KJ>(iv, blk, lane, s);
             int taken = 0;
-            float lp[KJ];
-            if (ok && !env_table_logp<KJ>(a, s, env, lane, lp)) {
-                ok = false;
-                if (lane == 0) bs.bad[0] = 1;
-            }
-            if (ok) {
-                uint32_t key[KJ];                        // 0: not a candidate, or already taken
-                int nc = 0;
-#pragma unroll
-                for (int i = 0; i < KJ; i++) {
-                    const float cs = sc + lp[i];
-                    key[i] = ((s.lb >> i) & 1u) && cs > -JSS_F32_INF ? jss_f32_key(cs + 0.0f) : 0u;
-                    nc += key[i] != 0u;
-                }
-                if (SWOR) {                              // the perturbed values G, Z and the keys in their place
-                    const float T = bs.key[cur * W + b];
-                    float g[KJ];
-                    uint32_t zk = 0u;
-                    int zj = 1 << 20;
-#pragma unroll
-                    for (int i = 0; i < KJ; i++) {
-                        g[i] = (sc + lp[i]) + jss_gumbel(jss_hash_env(hr, (uint64_t)(b * 256 + KJ * lane + i)));
-                        const uint32_t k = jss_f32_key(g[i] + 0.0f);
-                        if (key[i] != 0u && k > zk) { zk = k; zj = KJ * lane + i; }
-                    }
-                    const uint32_t zbest = __reduce_max_sync(JSS_FULL, zk);
-                    zj = (int)__reduce_min_sync(JSS_FULL, (unsigned)(zk == zbest ? zj : 1 << 20));
-                    const float Z = jss_key_f32(zbest);
-#pragma unroll
-                    for (int i = 0; i < KJ; i++) {
-                        if (key[i] == 0u) continue;
-                        float kv = T;
-                        if (KJ * lane + i != zj) {
-                            const float v = T - g[i] + jss_log1mexp(g[i] - Z);
-                            kv = fminf(T, T - fmaxf(v, 0.0f) - log1pf(expf(-fabsf(v))));
-                        }
-                        key[i] = jss_f32_key(kv + 0.0f);
+            if (sc == sc) {                              // NaN: the step into this slot failed (an imported state)
+                int raw;
+                const int noops = env_forced_noops<KJ>(p, iv, s, env, lane, raw, hz);
+                const bool ok = noops >= 0 && __any_sync(JSS_FULL, (s.lb & LM) != 0u);
+                if (ok && noops > 0) env_store<KJ>(iv, blk, lane, s);
+                if (ok) {
+                    taken = jss_beam_expand<KJ, SWOR, false>(a, bs, s, env, lane, b, W, sc, cur * W + b, hr);
+                    if (taken < 0) {
+                        taken = 0;
+                        if (lane == 0) bs.bad[0] = 1;
                     }
                 }
-                taken = min(W, (int)__reduce_add_sync(JSS_FULL, (unsigned)nc));
-                jss_beam_passes<KJ, SWOR>(bs, key, lp, sc, b, W, lane, taken);
             }
             if (lane == 0) bs.cnt[b] = taken;
         }
@@ -2138,25 +2146,23 @@ JSS_DEV void env_beam_search(const JssParams &p, const JssLaunch &a, const InstV
 // slot is live iff its score (a.score_io) is finite.
 //   0. the scores and the live slots' blocks (the parents, as at entry) go to shared memory.  Without a live, not-done
 //      slot the group is untouched: parent b, job -1, bad 0, and nothing else is written;
-//   1. warp w expands the slots b = w, w + 8, ...: a live, not-done slot with a legal job takes the log-probabilities
-//      of its row (env_table_logp<KJ, true>) and keeps its best children, keyed as env_beam_search keys them, by the
-//      argmax passes (jss_beam_passes); a bad row sets bad;
+//   1. warp w expands the slots b = w, w + 8, ...: a live, not-done slot with a legal job by jss_beam_expand on its
+//      logit row; a bad row sets bad;
 //   2. the CTA ranks the candidates (jss_beam_rank);
-//   3. warp w steps new slot b = w, w + 8, ... < nn from its parent's block, takes the forced no-ops while no
-//      job is legal and the no-op is, and writes the slot's block, its observation, mask and scalar record whole (the
+//   3. warp w steps new slot b = w, w + 8, ... < nn from its parent's block, takes the forced no-ops
+//      (env_forced_noops), and writes the slot's block, its observation, mask and scalar record whole (the
 //      raw reward of its last step) and its score, parent and job; slots nn .. W-1 get -inf, -1, -1.
 // Every step is env_step<KJ, false>: no statistics, solution, auto-reset or RNG.
 // SWOR (jss_stochastic_beam_step): the round of env_beam_search<KJ, true>.  Each slot also carries a key T (a.key_io,
 // read with the scores); candidate j of the beam in slot b gets G_j, Z and its key exactly as there, with the noise
 // jss_hash_env(h, b * 256 + j), h = jss_hash3(seed, env_id_base / W + g, step_index) (the group's global id); the
-// selection ranks the keys, and a kept child's score comes with the selection (bs.score[W ..]), its key from it.  The
-// per-candidate key stays inline here as in env_beam_search: shared, it changed that kernel's register assignment.
+// selection ranks the keys, and a kept child's score comes with the selection (bs.score[W ..]), its key from it.
 template <int KJ, bool SWOR>
 JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstView &iv, const int32_t *rec, int warp,
                            int lane, float *scratch, char *bsm) {
     constexpr uint32_t LM = jss_legal_mask<KJ>();
     const int W = a.beam_width, bw = jss_block_geom(p.jobs_max, p.machines_max).words;
-    const int J = jss_J(iv), nw = iv.si->block_words;
+    const int nw = iv.si->block_words;
     const int g = rec[0], e0 = g * W;
     const uint32_t *off = reinterpret_cast<const uint32_t *>(rec + 2);
     int *hz = reinterpret_cast<int *>(scratch);
@@ -2195,45 +2201,10 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
             env_load<KJ>(iv, bs.blocks + (size_t)b * bw, lane, s);
             s.flags = jss_uniform(s.flags);
             if (!(s.flags & JSS_FLAG_DONE) && __any_sync(JSS_FULL, (s.lb & LM) != 0u)) {
-                float lp[KJ];
-                if (env_table_logp<KJ, true>(a, s, e0 + b, lane, lp)) {
-                    uint32_t key[KJ];                    // 0: not a candidate, or already taken
-                    int nc = 0;
-#pragma unroll
-                    for (int i = 0; i < KJ; i++) {
-                        const float cs = sc + lp[i];
-                        key[i] = ((s.lb >> i) & 1u) && cs > -JSS_F32_INF ? jss_f32_key(cs + 0.0f) : 0u;
-                        nc += key[i] != 0u;
-                    }
-                    if (SWOR) {                          // the perturbed values G, Z and the keys in their place
-                        const float T = bs.key[b];
-                        float gv[KJ];
-                        uint32_t zk = 0u;
-                        int zj = 1 << 20;
-#pragma unroll
-                        for (int i = 0; i < KJ; i++) {
-                            gv[i] = (sc + lp[i]) + jss_gumbel(jss_hash_env(hr, (uint64_t)(b * 256 + KJ * lane + i)));
-                            const uint32_t k = jss_f32_key(gv[i] + 0.0f);
-                            if (key[i] != 0u && k > zk) { zk = k; zj = KJ * lane + i; }
-                        }
-                        const uint32_t zbest = __reduce_max_sync(JSS_FULL, zk);
-                        zj = (int)__reduce_min_sync(JSS_FULL, (unsigned)(zk == zbest ? zj : 1 << 20));
-                        const float Z = jss_key_f32(zbest);
-#pragma unroll
-                        for (int i = 0; i < KJ; i++) {
-                            if (key[i] == 0u) continue;
-                            float kv = T;
-                            if (KJ * lane + i != zj) {
-                                const float v = T - gv[i] + jss_log1mexp(gv[i] - Z);
-                                kv = fminf(T, T - fmaxf(v, 0.0f) - log1pf(expf(-fabsf(v))));
-                            }
-                            key[i] = jss_f32_key(kv + 0.0f);
-                        }
-                    }
-                    taken = min(W, (int)__reduce_add_sync(JSS_FULL, (unsigned)nc));
-                    jss_beam_passes<KJ, SWOR>(bs, key, lp, sc, b, W, lane, taken);
-                } else if (lane == 0) {
-                    bs.bad[0] = 1;
+                taken = jss_beam_expand<KJ, SWOR, true>(a, bs, s, e0 + b, lane, b, W, sc, b, hr);
+                if (taken < 0) {
+                    taken = 0;
+                    if (lane == 0) bs.bad[0] = 1;
                 }
             }
         }
@@ -2251,10 +2222,7 @@ JSS_DEV void env_beam_step(const JssParams &p, const JssLaunch &a, const InstVie
         int raw;
         bool ok = env_step<KJ, false>(p, iv, s, env, lane, (int)(pj & 255u), raw, hz);
         s.flags = jss_uniform(s.flags);
-        while (ok && !__any_sync(JSS_FULL, (s.lb & LM) != 0u) && (s.flags & JSS_FLAG_NOOP_LEGAL)) {   // forced no-ops
-            ok = env_step<KJ, false>(p, iv, s, env, lane, J, raw, hz);
-            s.flags = jss_uniform(s.flags);
-        }
+        ok = ok && env_forced_noops<KJ>(p, iv, s, env, lane, raw, hz) >= 0;
         env_store<KJ>(iv, p.state + (size_t)off[b] * 4, lane, s);
         env_emit_all<KJ>(p, iv, s, env, lane, scratch, raw);
         if (lane == 0) {
@@ -2480,9 +2448,8 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
     if (mode == JSS_MODE_EXPORT) { env_export<KJ>(p, iv, s, env, lane); return; }
     if (mode == JSS_MODE_PACK) { env_pack<KJ>(a, iv, s, env, lane, scratch); return; }
     if (mode == JSS_MODE_REFRESH) { env_emit_obs<KJ>(p, jss_out_default(p), iv, s, env, lane, scratch); return; }
-    if (MODE == JSS_MODE_PRIORITY) { env_priority_rollout<KJ>(p, a, iv, s, blk(), env, lane, scratch); return; }
-    if (MODE == JSS_MODE_PRIORITY_SAMPLE) {
-        env_priority_sample_rollout<KJ>(p, a, iv, s, blk(), env, lane, scratch);
+    if (MODE == JSS_MODE_PRIORITY || MODE == JSS_MODE_PRIORITY_SAMPLE) {
+        env_priority_rollout<KJ, MODE == JSS_MODE_PRIORITY_SAMPLE>(p, a, iv, s, blk(), env, lane, scratch);
         return;
     }
     if (mode == JSS_MODE_POLICY) {
@@ -2575,8 +2542,8 @@ struct JssMode {
     int refresh;                      // JSS_REFRESH_*
 };
 // Resident CTAs: one, except in the loops that keep an env on chip for a whole episode or rollout, so that more warps
-// per SM hide their latency: there the largest count per lane class that builds without a stack frame or spills
-// (ptxas registers by class, CUDA 12.9, sm_90a).
+// per SM hide their latency: there a count per lane class that builds without a stack frame or spills.  The notes give
+// the registers by class and where one CTA more spills (ptxas, CUDA 12.9, sm_90a).
 constexpr JssMode JSS_MODES[] = {
     // RESET also runs a step that exports (facade), export, import, pack and refresh
     {JSS_MODE_RESET, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false, JSS_REFRESH_YES},
@@ -2593,51 +2560,52 @@ constexpr JssMode JSS_MODES[] = {
      JSS_REFRESH_YES},                                                                                    // PACK
     {JSS_MODE_RESET, {1, 1, 1, 1}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_NO},                                                                                     // REFRESH
-    // the priority loop carries none of the rules' code; its sampling form: one CTA more spills in every class
+    // the priority loop carries none of the rules' code, 64 / 80 / 80 / 124 registers: one CTA more spills with 1 and 8
+    // jobs per lane, not with 2 or 4; its sampling form at 64 / 80 / 64 / 123: with 1, 4 and 8, not with 2
     {JSS_MODE_PRIORITY, {4, 3, 3, 2}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_YES},
     {JSS_MODE_PRIORITY_SAMPLE, {4, 3, 4, 2}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_YES},
-    // the lookahead loop: the rules' code, but no output emission; over a priority table (the table's argmax in place
-    // of the rules) 31 / 48 / 56 / 80 registers, one CTA more spills in the classes with 2, 4 and 8 jobs per lane, and 8
-    // is the SM's limit
+    // the lookahead loop: the rules' code, but no output emission, 53 / 64 / 78 / 104 registers, one CTA more spills
+    // in every class; over a priority table (the table's argmax in place of the rules) 31 / 48 / 56 / 80 registers, one
+    // CTA more spills in the classes with 2, 4 and 8 jobs per lane, and 8 is the SM's limit
     {JSS_MODE_LOOKAHEAD, {4, 4, 3, 2}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_J, JSS_STAGE_ALL, JSS_SMEM_ENV, false,
      JSS_REFRESH_NO},
     {JSS_MODE_LOOKAHEAD_PRIORITY, {8, 5, 4, 3}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_J, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_NO},
     // the sampled episodes: the draws at 32 / 32 / 39 / 72 registers, their replay with the gradient adds (the caller's
-    // split) at 56 / 64 / 64 / 122, the solution replay (S = 1) at 40 / 48 / 40 / 72.  ptxas is not monotonic here: the
-    // draws with 4 jobs per lane spill at 5 CTAs but not at 6, and spill again at 7.
+    // split) at 59 / 64 / 64 / 120, the solution replay (S = 1) at 40 / 48 / 40 / 72; one CTA more spills in every
+    // class below the SM's limit of 8
     {JSS_MODE_SAMPLE_EPISODES, {8, 8, 6, 3}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_K, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_NO},
     {JSS_MODE_SAMPLE_EPISODES_GRAD, {4, 4, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV,
      false, JSS_REFRESH_NO},
     {JSS_MODE_SAMPLE_EPISODES_SOLUTION, {6, 5, 6, 3}, JSS_ITEM_SPLIT, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV,
      false, JSS_REFRESH_NO},
-    // the beam search: 60 / 75 / 113 / 175 registers, one CTA more spills in the classes with 2, 4 and 8 jobs per lane;
-    // its shared memory (2 W state blocks) bounds the resident CTAs at large W anyway.  The stochastic one: 64 / 75 /
-    // 113 / 176 registers.
+    // the beam search: 62 / 75 / 121 / 173 registers, one CTA more spills in every class; its shared memory (2 W state
+    // blocks) bounds the resident CTAs at large W anyway.  The stochastic one: 60 / 78 / 118 / 175 registers, the
+    // same.
     {JSS_MODE_BEAM_SEARCH, {4, 3, 2, 1}, JSS_ITEM_ENV, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_BEAM, false,
      JSS_REFRESH_NO},
     {JSS_MODE_SWOR, {4, 3, 2, 1}, JSS_ITEM_ENV, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_BEAM, true, JSS_REFRESH_NO},
-    // the order likelihood at 40 / 62 / 64 / 92 registers, its gradient at 64 / 72 / 64 / 143; one CTA more spills in
-    // every class of the likelihood but the one with 1 job per lane (untried at 7), and in the classes with 2 and 8 jobs
-    // per lane of the gradient
+    // the order likelihood at 40 / 62 / 64 / 92 registers, its gradient at 64 / 72 / 64 / 124; one CTA more spills in
+    // every class of the likelihood, and in the classes with 1, 2 and 4 jobs per lane of the gradient (not with 8)
     {JSS_MODE_ORDER_LOG_PROB, {6, 4, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_K, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_NO},
     {JSS_MODE_ORDER_LOG_PROB_GRAD, {4, 3, 4, 1}, JSS_ITEM_SPLIT, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_NO},
-    // the beam round of jss_beam_step (DESIGN.md section 4), and its stochastic form
+    // the beam round of jss_beam_step (DESIGN.md section 4) at 64 / 78 / 128 / 167 registers, and its stochastic form
+    // at 80 / 80 / 128 / 165; one CTA more spills with 1 job per lane in both, not in the other classes
     {JSS_MODE_BEAM_STEP, {4, 3, 2, 1}, JSS_ITEM_GROUP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_BEAM_STEP, false,
      JSS_REFRESH_YES},
     {JSS_MODE_STOCHASTIC_BEAM_STEP, {3, 3, 2, 1}, JSS_ITEM_GROUP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_BEAM_STEP,
      true, JSS_REFRESH_YES},
-    // the critical-path descent: 32 / 40 / 60 / 116 registers; 8 is the SM's limit, and one CTA more spills with 8 jobs
-    // per lane.  Its shared memory (three [J][M] tables) bounds the resident CTAs at large J M.
+    // the critical-path descent: 32 / 40 / 60 / 116 registers; 8 is the SM's limit, and one CTA more spills with 2, 4
+    // and 8 jobs per lane.  Its shared memory (three [J][M] tables) bounds the resident CTAs at large J M.
     {JSS_MODE_IMPROVE_ORDERS, {8, 6, 4, 2}, JSS_ITEM_ORDER, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_IMPROVE, false,
      JSS_REFRESH_NO},
     // the sampled lookahead: the lookahead loop with the draws of the sampled episodes, 25 / 31 / 56 / 91 registers; 8
-    // is the SM's limit, and one CTA more spills with 8 jobs per lane, as do 5 and 6 with 4
+    // is the SM's limit, and one CTA more spills with 4 and 8 jobs per lane
     {JSS_MODE_LOOKAHEAD_SAMPLE, {8, 8, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_JK, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_NO},
 };
