@@ -374,6 +374,27 @@ int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_en
                                 uint64_t seed, uint64_t step_index, int n_steps, float *log_prob_out_dev,
                                 float *grad_out_dev, void *stream);
 
+/* jss_rollout_priority_sample() with each episode's policy entropy, the regulariser of REINFORCE and PPO on a table
+ * policy, and its gradient.  Every draw, state, log_prob_out and grad_out entry, RNG counter advance and error bit is
+ * bit for bit what jss_rollout_priority_sample() gives with the same arguments.
+ *   Entropy of a decision with legal jobs L: with x_j, mx, d_j = x_j - mx, e_j = exp(d_j) and S = sum_{j in L} e_j the
+ *     values the draw computes (fast exp / log), H_t = log S - T / S, T = sum over j in L with e_j > 0 of e_j d_j,
+ *     summed in S's order.  A term with e_j = 0 adds nothing (no 0 * -inf), and a decision with one job of nonzero
+ *     probability gives exactly +0.
+ *   entropy_out_dev (device fp32 [N], required): env i's fp32 sum of H_t over its decisions of this call, in decision
+ *     order; forced no-ops add 0; 0 for an env done at entry or making no decision; NaN wherever log_prob_out is NaN.
+ *   entropy_grad_out_dev (device fp32 [N][jobs_max][machines_max], the layout of grad_out; NULL: none):
+ *     d entropy_out[i] / d (entry of operation k of job j) = sum over the decisions t where j is legal at operation k
+ *     of -p_t(j) (lp_t(j) + H_t), p = e_j / S and lp = d_j - log S (0 where p = 0).  Written where grad_out is, with
+ *     grad_out's zeros: operations finished before the call or never reached, envs done at entry, all-zero rows for an
+ *     env that gets NaN.  Either gradient pointer may be NULL.
+ *   Returns the errors of jss_rollout_priority_sample(), and JSS_ERR_INVALID for a NULL or not 4-byte-aligned
+ *     entropy_out_dev or a misaligned entropy_grad_out_dev. */
+int jss_rollout_priority_sample_entropy(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job,
+                                        int64_t ld_op, uint64_t seed, uint64_t step_index, int n_steps,
+                                        float *log_prob_out_dev, float *entropy_out_dev, float *grad_out_dev,
+                                        float *entropy_grad_out_dev, void *stream);
+
 /* Values every legal action of every env by a dispatching-rule rollout to the end of its episode, in one launch per
  * lane class present, and changes nothing but the caller's table: the reference's copy.deepcopy(env) + step(a) +
  * DispatchingRule.run_episode (dispatching.py:55-75) per legal action.  For the rollout (pilot) method -- take the
@@ -483,6 +504,25 @@ int jss_sample_episodes(jss_t *h, const float *logits_dev, int64_t ld_env, int64
 int jss_sample_episodes_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                              uint64_t seed, uint64_t step_index, int64_t k, const float *weights_dev, int64_t ld,
                              int split, float *grad_out_dev, void *stream);
+
+/* jss_sample_episodes() with each sample's policy entropy: entropy_out_dev[i*ld + s] (device fp32) is what
+ * jss_rollout_priority_sample_entropy() reports for the twin of sample s, bit for bit; 0 for an env done at entry.
+ * makespan_out_dev and log_prob_out_dev are bit for bit jss_sample_episodes()'s.  Returns the errors of
+ * jss_sample_episodes(), entropy_out_dev checked as its outputs are. */
+int jss_sample_episodes_entropy(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                uint64_t seed, uint64_t step_index, int64_t k, int32_t *makespan_out_dev,
+                                float *log_prob_out_dev, float *entropy_out_dev, int64_t ld, void *stream);
+
+/* The backward of jss_sample_episodes_entropy(): one replay of the draws that adds sum_s (weights[i*ld + s] * G_s[i] +
+ * entropy_weights[i*ld + s] * GH_s[i]) into grad_out_dev, G_s and GH_s the grad_out and entropy_grad_out of
+ * jss_rollout_priority_sample_entropy() for the twin of sample s.  Chunking, ownership and determinism are those of
+ * jss_sample_episodes_grad(); a sample adds w G first, so entropy weights of 0 add what jss_sample_episodes_grad()
+ * adds, bit for bit.  Samples with both weights 0 cost nothing.  Returns the errors of jss_sample_episodes_grad(),
+ * entropy_weights_dev checked as weights_dev is. */
+int jss_sample_episodes_entropy_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                     uint64_t seed, uint64_t step_index, int64_t k, const float *weights_dev,
+                                     const float *entropy_weights_dev, int64_t ld, int split, float *grad_out_dev,
+                                     void *stream);
 
 /* The schedule of one sample per env of jss_sample_episodes() (same table, seed and step_index, same state): env i
  * replays sample sample_dev[i] (device int32 [N]; < 0 skips the env) and writes the start time of every operation that
@@ -691,6 +731,24 @@ int jss_order_log_prob(jss_t *h, const float *logits_dev, int64_t ld_env, int64_
 int jss_order_log_prob_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                             const int32_t *order_dev, int64_t k, const float *weights_dev, int64_t ld, int split,
                             float *grad_out_dev, void *stream);
+
+/* jss_order_log_prob() with each order's policy entropy: entropy_out_dev[i*ld + s] (device fp32) is the fp32 sum over
+ * the order's decisions of H_t, computed by the helper of jss_rollout_priority_sample_entropy() on the same values, so
+ * that an order and a sampled episode drawing the same jobs from the same state report the same entropy bit for bit;
+ * forced no-ops add 0, 0 for an env done at entry, NaN where log_prob is NaN.  makespan_out_dev and log_prob_out_dev
+ * are bit for bit jss_order_log_prob()'s.  Returns the errors of jss_order_log_prob(), entropy_out_dev checked as its
+ * outputs are. */
+int jss_order_log_prob_entropy(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                               const int32_t *order_dev, int64_t k, int32_t *makespan_out_dev, float *log_prob_out_dev,
+                               float *entropy_out_dev, int64_t ld, void *stream);
+
+/* The gradient of jss_order_log_prob_entropy(): one replay adding sum_s (weights[i*ld + s] * d log_prob[i][s] / d table
+ * + entropy_weights[i*ld + s] * d entropy[i][s] / d table) into grad_out_dev, as jss_sample_episodes_entropy_grad() adds
+ * it.  Returns the errors of jss_order_log_prob_grad(), entropy_weights_dev checked as weights_dev is. */
+int jss_order_log_prob_entropy_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                    const int32_t *order_dev, int64_t k, const float *weights_dev,
+                                    const float *entropy_weights_dev, int64_t ld, int split, float *grad_out_dev,
+                                    void *stream);
 
 /* Local search on given operation orders: each of the k orders per env improved by steepest descent on the critical
  * path (the N1 neighbourhood of van Laarhoven, Aarts and Lenstra, 1992: swaps of two adjacent operations of a critical

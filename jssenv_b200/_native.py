@@ -70,6 +70,8 @@ SIGNATURES = {
     "jss_rollout_priority": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_int, _VP]),
     "jss_rollout_priority_sample": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int, _VP, _VP,
                                             _VP]),
+    "jss_rollout_priority_sample_entropy": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int,
+                                                    _VP, _VP, _VP, _VP, _VP]),
     "jss_lookahead": (c_int, [_VP, c_int, c_int, c_uint64, c_uint64, _VP, c_int64, _VP]),
     "jss_lookahead_priority": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP]),
     "jss_lookahead_sample": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, c_int64,
@@ -78,6 +80,10 @@ SIGNATURES = {
                                     _VP]),
     "jss_sample_episodes_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, c_int64,
                                          c_int, _VP, _VP]),
+    "jss_sample_episodes_entropy": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP, _VP,
+                                            _VP, c_int64, _VP]),
+    "jss_sample_episodes_entropy_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int64, _VP,
+                                                 _VP, c_int64, c_int, _VP, _VP]),
     "jss_sample_episodes_solution": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, _VP, _VP, _VP]),
     "jss_beam_search": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_int, _VP, _VP, c_int64, _VP, _VP]),
     "jss_sample_without_replacement": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_int, _VP, _VP,
@@ -87,6 +93,10 @@ SIGNATURES = {
     "jss_order_log_prob": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, _VP, c_int64, _VP]),
     "jss_order_log_prob_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, c_int64, c_int, _VP,
                                         _VP]),
+    "jss_order_log_prob_entropy": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, _VP, _VP, c_int64,
+                                           _VP]),
+    "jss_order_log_prob_entropy_grad": (c_int, [_VP, _VP, c_int64, c_int64, c_int64, _VP, c_int64, _VP, _VP, c_int64,
+                                                c_int, _VP, _VP]),
     "jss_improve_orders": (c_int, [_VP, _VP, c_int64, c_int, _VP, _VP, _VP, _VP, c_int64, _VP]),
     "jss_step_host": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "jss_host_step_begin": (c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),

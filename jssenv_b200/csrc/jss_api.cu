@@ -900,10 +900,27 @@ int jss_rollout_priority(jss_t *h, const float *prio_dev, int64_t ld_env, int64_
     return launch_all(h, a, (cudaStream_t)stream);
 }
 
-int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
-                                uint64_t seed, uint64_t step_index, int n_steps, float *log_prob_out_dev,
-                                float *grad_out_dev, void *stream) {
-    const char *who = "jss_rollout_priority_sample";
+namespace {
+
+// the entropy forms take their sibling's arguments and checks, then their own outputs (ent)
+int entropy_out_arg(jss_t *h, const char *who, bool ent, float *entropy_out) {
+    if (ent && bad_ptr(entropy_out))
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (entropy_out %p must be non-NULL and 4-byte aligned)", who,
+                    (void *)entropy_out);
+    return JSS_OK;
+}
+
+int entropy_weights_arg(jss_t *h, const char *who, bool ent, const float *entropy_weights) {
+    if (ent && bad_ptr(entropy_weights))
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (entropy_weights %p must be non-NULL and 4-byte aligned)",
+                    who, (const void *)entropy_weights);
+    return JSS_OK;
+}
+
+int rollout_priority_sample(jss_t *h, const char *who, bool ent, const float *logits_dev, int64_t ld_env,
+                            int64_t ld_job, int64_t ld_op, uint64_t seed, uint64_t step_index, int n_steps,
+                            float *log_prob_out_dev, float *entropy_out_dev, float *grad_out_dev,
+                            float *entropy_grad_out_dev, void *stream) {
     int rc = check_ready(h, stream);
     if (rc) return rc;
     JssLaunch a{};
@@ -911,14 +928,38 @@ int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_en
     if (bad_ptr(log_prob_out_dev) || ((uintptr_t)grad_out_dev & 3u) || n_steps < 0)
         return fail(h, JSS_ERR_INVALID, "%s: bad arguments (log_prob_out %p must be non-NULL, it and grad_out %p "
                     "4-byte aligned, n_steps %d >= 0)", who, (void *)log_prob_out_dev, (void *)grad_out_dev, n_steps);
+    if ((rc = entropy_out_arg(h, who, ent, entropy_out_dev))) return rc;
+    if ((uintptr_t)entropy_grad_out_dev & 3u)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (entropy_grad_out %p must be 4-byte aligned)", who,
+                    (void *)entropy_grad_out_dev);
     if (n_steps == 0) return JSS_OK;
-    a.mode = JSS_MODE_PRIORITY_SAMPLE;
+    a.mode = ent ? JSS_MODE_PRIORITY_SAMPLE_ENT : JSS_MODE_PRIORITY_SAMPLE;
     a.seed_folded = jss_fold32(seed);                    // jss_hash3 reads the seed only through its fold
     a.sample_counter = step_index;
     a.n_steps = n_steps;
     a.log_prob_out = log_prob_out_dev;
     a.grad_out = grad_out_dev;
+    a.entropy_out = entropy_out_dev;
+    a.entropy_grad_out = entropy_grad_out_dev;
     return launch_all(h, a, (cudaStream_t)stream);
+}
+
+}  // namespace
+
+int jss_rollout_priority_sample(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                uint64_t seed, uint64_t step_index, int n_steps, float *log_prob_out_dev,
+                                float *grad_out_dev, void *stream) {
+    return rollout_priority_sample(h, "jss_rollout_priority_sample", false, logits_dev, ld_env, ld_job, ld_op, seed,
+                                   step_index, n_steps, log_prob_out_dev, nullptr, grad_out_dev, nullptr, stream);
+}
+
+int jss_rollout_priority_sample_entropy(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job,
+                                        int64_t ld_op, uint64_t seed, uint64_t step_index, int n_steps,
+                                        float *log_prob_out_dev, float *entropy_out_dev, float *grad_out_dev,
+                                        float *entropy_grad_out_dev, void *stream) {
+    return rollout_priority_sample(h, "jss_rollout_priority_sample_entropy", true, logits_dev, ld_env, ld_job, ld_op,
+                                   seed, step_index, n_steps, log_prob_out_dev, entropy_out_dev, grad_out_dev,
+                                   entropy_grad_out_dev, stream);
 }
 
 int jss_lookahead(jss_t *h, int rule, int coin_mode, uint64_t seed, uint64_t step_index, int32_t *makespan_out_dev,
@@ -1006,46 +1047,77 @@ int sample_episodes_args(jss_t *h, const char *who, const float *logits, int64_t
     return JSS_OK;
 }
 
+int sample_episodes(jss_t *h, const char *who, bool ent, const float *logits_dev, int64_t ld_env, int64_t ld_job,
+                    int64_t ld_op, uint64_t seed, uint64_t step_index, int64_t k, int32_t *makespan_out_dev,
+                    float *log_prob_out_dev, float *entropy_out_dev, int64_t ld, void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    if (bad_ptr(makespan_out_dev) || bad_ptr(log_prob_out_dev))
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p and log_prob_out %p must be 4-byte "
+                    "aligned)", who, (void *)makespan_out_dev, (void *)log_prob_out_dev);
+    if ((rc = entropy_out_arg(h, who, ent, entropy_out_dev))) return rc;
+    JssLaunch a{};
+    a.mode = ent ? JSS_MODE_SAMPLE_EPISODES_ENT : JSS_MODE_SAMPLE_EPISODES;
+    if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
+        return rc;
+    a.makespan_out = makespan_out_dev;
+    a.log_prob_out = log_prob_out_dev;
+    a.entropy_out = entropy_out_dev;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int sample_episodes_grad(jss_t *h, const char *who, bool ent, const float *logits_dev, int64_t ld_env, int64_t ld_job,
+                         int64_t ld_op, uint64_t seed, uint64_t step_index, int64_t k, const float *weights_dev,
+                         const float *entropy_weights_dev, int64_t ld, int split, float *grad_out_dev, void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    if (bad_ptr(weights_dev) || bad_ptr(grad_out_dev) || split < 1 || split > k)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (weights %p and grad_out %p must be 4-byte aligned, "
+                    "1 <= split %d <= k %lld)", who, (const void *)weights_dev, (void *)grad_out_dev, split,
+                    (long long)k);
+    if ((rc = entropy_weights_arg(h, who, ent, entropy_weights_dev))) return rc;
+    if ((int64_t)h->n_tiles * split > INT32_MAX)
+        return fail(h, JSS_ERR_UNSUPPORTED, "%s: split * tiles must stay below 2^31", who);
+    JssLaunch a{};
+    a.mode = ent ? JSS_MODE_SAMPLE_EPISODES_ENT_GRAD : JSS_MODE_SAMPLE_EPISODES_GRAD;
+    if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
+        return rc;
+    a.weights = weights_dev;
+    a.entropy_weights = entropy_weights_dev;
+    a.split = split;
+    a.grad_out = grad_out_dev;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
 }  // namespace
 
 int jss_sample_episodes(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                         uint64_t seed, uint64_t step_index, int64_t k, int32_t *makespan_out_dev,
                         float *log_prob_out_dev, int64_t ld, void *stream) {
-    int rc = check_ready(h, stream);
-    if (rc) return rc;
-    const char *who = "jss_sample_episodes";
-    if (bad_ptr(makespan_out_dev) || bad_ptr(log_prob_out_dev))
-        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p and log_prob_out %p must be 4-byte "
-                    "aligned)", who, (void *)makespan_out_dev, (void *)log_prob_out_dev);
-    JssLaunch a{};
-    a.mode = JSS_MODE_SAMPLE_EPISODES;
-    if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
-        return rc;
-    a.makespan_out = makespan_out_dev;
-    a.log_prob_out = log_prob_out_dev;
-    return launch_all(h, a, (cudaStream_t)stream);
+    return sample_episodes(h, "jss_sample_episodes", false, logits_dev, ld_env, ld_job, ld_op, seed, step_index, k,
+                           makespan_out_dev, log_prob_out_dev, nullptr, ld, stream);
+}
+
+int jss_sample_episodes_entropy(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                uint64_t seed, uint64_t step_index, int64_t k, int32_t *makespan_out_dev,
+                                float *log_prob_out_dev, float *entropy_out_dev, int64_t ld, void *stream) {
+    return sample_episodes(h, "jss_sample_episodes_entropy", true, logits_dev, ld_env, ld_job, ld_op, seed, step_index,
+                           k, makespan_out_dev, log_prob_out_dev, entropy_out_dev, ld, stream);
 }
 
 int jss_sample_episodes_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                              uint64_t seed, uint64_t step_index, int64_t k, const float *weights_dev, int64_t ld,
                              int split, float *grad_out_dev, void *stream) {
-    int rc = check_ready(h, stream);
-    if (rc) return rc;
-    const char *who = "jss_sample_episodes_grad";
-    if (bad_ptr(weights_dev) || bad_ptr(grad_out_dev) || split < 1 || split > k)
-        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (weights %p and grad_out %p must be 4-byte aligned, "
-                    "1 <= split %d <= k %lld)", who, (const void *)weights_dev, (void *)grad_out_dev, split,
-                    (long long)k);
-    if ((int64_t)h->n_tiles * split > INT32_MAX)
-        return fail(h, JSS_ERR_UNSUPPORTED, "%s: split * tiles must stay below 2^31", who);
-    JssLaunch a{};
-    a.mode = JSS_MODE_SAMPLE_EPISODES_GRAD;
-    if ((rc = sample_episodes_args(h, who, logits_dev, ld_env, ld_job, ld_op, seed, step_index, true, k, ld, a)))
-        return rc;
-    a.weights = weights_dev;
-    a.split = split;
-    a.grad_out = grad_out_dev;
-    return launch_all(h, a, (cudaStream_t)stream);
+    return sample_episodes_grad(h, "jss_sample_episodes_grad", false, logits_dev, ld_env, ld_job, ld_op, seed,
+                                step_index, k, weights_dev, nullptr, ld, split, grad_out_dev, stream);
+}
+
+int jss_sample_episodes_entropy_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                     uint64_t seed, uint64_t step_index, int64_t k, const float *weights_dev,
+                                     const float *entropy_weights_dev, int64_t ld, int split, float *grad_out_dev,
+                                     void *stream) {
+    return sample_episodes_grad(h, "jss_sample_episodes_entropy_grad", true, logits_dev, ld_env, ld_job, ld_op, seed,
+                                step_index, k, weights_dev, entropy_weights_dev, ld, split, grad_out_dev, stream);
 }
 
 int jss_sample_episodes_solution(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
@@ -1273,44 +1345,75 @@ int order_log_prob_args(jss_t *h, const char *who, const float *logits, int64_t 
     return orders_arg(h, who, order, k, ld, a);
 }
 
+int order_log_prob(jss_t *h, const char *who, bool ent, const float *logits_dev, int64_t ld_env, int64_t ld_job,
+                   int64_t ld_op, const int32_t *order_dev, int64_t k, int32_t *makespan_out_dev,
+                   float *log_prob_out_dev, float *entropy_out_dev, int64_t ld, void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    if (bad_ptr(makespan_out_dev) || bad_ptr(log_prob_out_dev))
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p and log_prob_out %p must be non-NULL and "
+                    "4-byte aligned)", who, (void *)makespan_out_dev, (void *)log_prob_out_dev);
+    if ((rc = entropy_out_arg(h, who, ent, entropy_out_dev))) return rc;
+    JssLaunch a{};
+    a.mode = ent ? JSS_MODE_ORDER_LOG_PROB_ENT : JSS_MODE_ORDER_LOG_PROB;
+    if ((rc = order_log_prob_args(h, who, logits_dev, ld_env, ld_job, ld_op, order_dev, k, ld, a))) return rc;
+    a.makespan_out = makespan_out_dev;
+    a.log_prob_out = log_prob_out_dev;
+    a.entropy_out = entropy_out_dev;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
+int order_log_prob_grad(jss_t *h, const char *who, bool ent, const float *logits_dev, int64_t ld_env, int64_t ld_job,
+                        int64_t ld_op, const int32_t *order_dev, int64_t k, const float *weights_dev,
+                        const float *entropy_weights_dev, int64_t ld, int split, float *grad_out_dev, void *stream) {
+    int rc = check_ready(h, stream);
+    if (rc) return rc;
+    if (bad_ptr(weights_dev) || bad_ptr(grad_out_dev) || split < 1 || split > k)
+        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (weights %p and grad_out %p must be non-NULL and 4-byte "
+                    "aligned, 1 <= split %d <= k %lld)", who, (const void *)weights_dev, (void *)grad_out_dev, split,
+                    (long long)k);
+    if ((rc = entropy_weights_arg(h, who, ent, entropy_weights_dev))) return rc;
+    if ((int64_t)h->n_tiles * split > INT32_MAX)
+        return fail(h, JSS_ERR_UNSUPPORTED, "%s: split * tiles must stay below 2^31", who);
+    JssLaunch a{};
+    a.mode = ent ? JSS_MODE_ORDER_LOG_PROB_ENT_GRAD : JSS_MODE_ORDER_LOG_PROB_GRAD;
+    if ((rc = order_log_prob_args(h, who, logits_dev, ld_env, ld_job, ld_op, order_dev, k, ld, a))) return rc;
+    a.weights = weights_dev;
+    a.entropy_weights = entropy_weights_dev;
+    a.split = split;
+    a.grad_out = grad_out_dev;
+    return launch_all(h, a, (cudaStream_t)stream);
+}
+
 }  // namespace
 
 int jss_order_log_prob(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                        const int32_t *order_dev, int64_t k, int32_t *makespan_out_dev, float *log_prob_out_dev,
                        int64_t ld, void *stream) {
-    int rc = check_ready(h, stream);
-    if (rc) return rc;
-    const char *who = "jss_order_log_prob";
-    if (bad_ptr(makespan_out_dev) || bad_ptr(log_prob_out_dev))
-        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (makespan_out %p and log_prob_out %p must be non-NULL and "
-                    "4-byte aligned)", who, (void *)makespan_out_dev, (void *)log_prob_out_dev);
-    JssLaunch a{};
-    a.mode = JSS_MODE_ORDER_LOG_PROB;
-    if ((rc = order_log_prob_args(h, who, logits_dev, ld_env, ld_job, ld_op, order_dev, k, ld, a))) return rc;
-    a.makespan_out = makespan_out_dev;
-    a.log_prob_out = log_prob_out_dev;
-    return launch_all(h, a, (cudaStream_t)stream);
+    return order_log_prob(h, "jss_order_log_prob", false, logits_dev, ld_env, ld_job, ld_op, order_dev, k,
+                          makespan_out_dev, log_prob_out_dev, nullptr, ld, stream);
+}
+
+int jss_order_log_prob_entropy(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                               const int32_t *order_dev, int64_t k, int32_t *makespan_out_dev, float *log_prob_out_dev,
+                               float *entropy_out_dev, int64_t ld, void *stream) {
+    return order_log_prob(h, "jss_order_log_prob_entropy", true, logits_dev, ld_env, ld_job, ld_op, order_dev, k,
+                          makespan_out_dev, log_prob_out_dev, entropy_out_dev, ld, stream);
 }
 
 int jss_order_log_prob_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
                             const int32_t *order_dev, int64_t k, const float *weights_dev, int64_t ld, int split,
                             float *grad_out_dev, void *stream) {
-    int rc = check_ready(h, stream);
-    if (rc) return rc;
-    const char *who = "jss_order_log_prob_grad";
-    if (bad_ptr(weights_dev) || bad_ptr(grad_out_dev) || split < 1 || split > k)
-        return fail(h, JSS_ERR_INVALID, "%s: bad arguments (weights %p and grad_out %p must be non-NULL and 4-byte "
-                    "aligned, 1 <= split %d <= k %lld)", who, (const void *)weights_dev, (void *)grad_out_dev, split,
-                    (long long)k);
-    if ((int64_t)h->n_tiles * split > INT32_MAX)
-        return fail(h, JSS_ERR_UNSUPPORTED, "%s: split * tiles must stay below 2^31", who);
-    JssLaunch a{};
-    a.mode = JSS_MODE_ORDER_LOG_PROB_GRAD;
-    if ((rc = order_log_prob_args(h, who, logits_dev, ld_env, ld_job, ld_op, order_dev, k, ld, a))) return rc;
-    a.weights = weights_dev;
-    a.split = split;
-    a.grad_out = grad_out_dev;
-    return launch_all(h, a, (cudaStream_t)stream);
+    return order_log_prob_grad(h, "jss_order_log_prob_grad", false, logits_dev, ld_env, ld_job, ld_op, order_dev, k,
+                               weights_dev, nullptr, ld, split, grad_out_dev, stream);
+}
+
+int jss_order_log_prob_entropy_grad(jss_t *h, const float *logits_dev, int64_t ld_env, int64_t ld_job, int64_t ld_op,
+                                    const int32_t *order_dev, int64_t k, const float *weights_dev,
+                                    const float *entropy_weights_dev, int64_t ld, int split, float *grad_out_dev,
+                                    void *stream) {
+    return order_log_prob_grad(h, "jss_order_log_prob_entropy_grad", true, logits_dev, ld_env, ld_job, ld_op,
+                               order_dev, k, weights_dev, entropy_weights_dev, ld, split, grad_out_dev, stream);
 }
 
 int jss_improve_orders(jss_t *h, const int32_t *order_dev, int64_t k, int max_moves, int32_t *order_out_dev,

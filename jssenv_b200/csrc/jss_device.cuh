@@ -1178,6 +1178,38 @@ JSS_DEV int env_priority_action(const JssLaunch &a, const InstView &iv, const En
     return g;
 }
 
+// The entropy of one decision's softmax over the legal jobs, from each owned slot's d_i = x_i - mx and e_i =
+// jss_fast_exp(d_i) (e_i = 0 for a slot that is not legal), S = sum e_i and ls = jss_fast_log(S) as the decision source
+// formed them: H = ls - T / S, T = sum over e_i > 0 of e_i d_i, summed in S's order (each lane's slots ascending, then
+// the same butterfly).  A term with e_i = 0 (a legal job at -inf, or an exponential that underflows) adds nothing, so
+// 0 * -inf never makes a NaN, and a decision with one job of nonzero probability gives exactly +0.  The one helper both
+// decision sources call, so that an order's entropy and a draw's agree bit for bit.
+template <int KJ>
+JSS_DEV float jss_softmax_entropy(const float (&d)[KJ], const float (&e)[KJ], float sum, float ls) {
+    float t = 0.0f;
+#pragma unroll
+    for (int i = 0; i < KJ; i++)
+        if (e[i] > 0.0f) t += e[i] * d[i];
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) t += __shfl_xor_sync(JSS_FULL, t, off);
+    return ls - t / sum;
+}
+
+// What a decision source reports besides the log-probability when asked for the entropy: H of the decision
+// (jss_softmax_entropy; 0 for a forced no-op) and each owned slot's p_i (lp_i + H), the negated gradient term of H
+// with respect to x_i (0 where p_i = 0, so lp_i = -inf makes no NaN).
+template <int KJ>
+struct JssEnt {
+    float h;
+    float q[KJ];
+};
+template <int KJ>
+JSS_DEV void jss_ent_clear(JssEnt<KJ> *ent) {
+    ent->h = 0.0f;
+#pragma unroll
+    for (int i = 0; i < KJ; i++) ent->q[i] = 0.0f;
+}
+
 // Env `env`'s next decision under its logit table (jss_rollout_priority_sample; the table as in env_priority_action):
 // the Gumbel-max draw of env_sample_logits over the legal jobs, x_j = the entry of job j's current operation.  It
 // equals env_sample_logits on the row x with the no-op column at -inf, bit for bit: the same keys and reductions, and
@@ -1186,13 +1218,15 @@ JSS_DEV int env_priority_action(const JssLaunch &a, const InstView &iv, const En
 // Writes logp = x_a - logsumexp(x) and each owned slot's p_i = softmax(x)_j (0 for a job that is not legal).  Returns
 // the drawn job; the no-op, logp and p left 0, when no job is legal and it is; JSS_INF for a bad table (the bad-row
 // rule of env_sample_logits); JSS_ACTION_SKIP when nothing is legal (an imported state).
-template <int KJ>
+// ENT: also the decision's entropy and gradient terms into *ent (JssEnt; left 0 where logp is left 0).
+template <int KJ, bool ENT = false>
 JSS_DEV int env_priority_sample_action(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
-                                       uint32_t h, float &logp, float (&pr)[KJ]) {
+                                       uint32_t h, float &logp, float (&pr)[KJ], JssEnt<KJ> *ent = nullptr) {
     constexpr uint32_t LM = jss_legal_mask<KJ>();
     logp = 0.0f;
 #pragma unroll
     for (int i = 0; i < KJ; i++) pr[i] = 0.0f;
+    if constexpr (ENT) jss_ent_clear<KJ>(ent);
     if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u))
         return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
     const float *row = jss_table_row(a.table, env);
@@ -1222,6 +1256,7 @@ JSS_DEV int env_priority_sample_action(const JssLaunch &a, const InstView &iv, c
             if (k > skey) { skey = k; sidx = j; sd = d; }
             pr[i] = jss_fast_exp(d);
             sum += pr[i];
+            if constexpr (ENT) x[i] = d;
         }
     }
     const uint32_t best = __reduce_max_sync(JSS_FULL, skey);
@@ -1230,9 +1265,15 @@ JSS_DEV int env_priority_sample_action(const JssLaunch &a, const InstView &iv, c
     for (int off = 16; off >= 1; off >>= 1) sum += __shfl_xor_sync(JSS_FULL, sum, off);   // the same sum in every lane
     const float da = __shfl_sync(JSS_FULL, sd, act / KJ);   // the drawn job's lane holds it as its best candidate
     logp = da - jss_fast_log(sum);
+    if constexpr (ENT) ent->h = jss_softmax_entropy<KJ>(x, pr, sum, jss_fast_log(sum));   // pr: still e_i
     const float inv = 1.0f / sum;
 #pragma unroll
     for (int i = 0; i < KJ; i++) pr[i] *= inv;
+    if constexpr (ENT) {
+        const float ls = jss_fast_log(sum);
+#pragma unroll
+        for (int i = 0; i < KJ; i++) ent->q[i] = pr[i] > 0.0f ? pr[i] * ((x[i] - ls) + ent->h) : 0.0f;
+    }
     return act;
 }
 
@@ -1322,7 +1363,7 @@ struct JssSmemLayout {
     int32_t off_scratch;    // step kernels: [mbarrier 16 B][state-in block][scratch][state-out block]; else 0
     int32_t off_logits;     // step kernels that take a row: [logits row, J + 1 floats] behind state-out; else 0
 };
-static_assert(sizeof(JssParams) == 248 && sizeof(JssLaunch) == 472 && sizeof(JssSmemLayout) == 32 &&
+static_assert(sizeof(JssParams) == 248 && sizeof(JssLaunch) == 496 && sizeof(JssSmemLayout) == 32 &&
               sizeof(JssTile) == 16 && sizeof(JssCtaRange) == 32,
               "ptxas allocates the kernels' registers by the parameter offsets (JssParams::pad0_): measure a change");
 // the same for the fields of JssLaunch that the fused step kernels read
@@ -1447,25 +1488,47 @@ JSS_DEV int env_undrawn(const EnvRegs<KJ> &s, int i) { return s.todo[i] + (s.tuf
 // the end (finish, +0 for a job never legal): one 4-byte access per decision, and the table of gradients is never read
 // but by the adds.  Every access to a job's row comes from the lane that owns the job, so program order orders them.
 // ADD (the replays of jss_sample_episodes_grad): a put adds w times the value; else it stores the value.
-template <int KJ, bool ADD>
+// ENT: the same for the episode's entropy beside it, in a second register per slot: hacc adds up the decisions' q_t(j)
+// = p_t(j) (lp_t(j) + H_t) (JssEnt), and G_H = 0 - hacc is put where G is.  ADD adds w G + v G_H (w G first, so that a
+// replay with v = 0 adds what the plain replay adds); else G goes to grad and G_H to hgrad, each skipped where NULL.
+template <int KJ, bool ADD, bool ENT = false>
 struct JssGradAcc {
     float *grad;
     int ms;
     float w;
     float acc[KJ];
-    JSS_DEV void put(int j, int k, float v) {
+    float *hgrad;            // ENT, stored form: the entropy's table
+    float v;                 // ENT, ADD: the entropy's weight
+    float hacc[KJ];
+    JSS_DEV bool on() const { return grad || (ENT && hgrad); }
+    JSS_DEV void put(int j, int k, float val, float hval = 0.0f) {
         float *q = grad + (size_t)j * ms + k;
-        if (ADD) *q += w * v;
-        else *q = v;
+        if (ADD) {
+            float t = *q + w * val;
+            if (ENT) t += v * hval;
+            *q = t;
+        } else {
+            if (!ENT || grad) *q = val;
+            if (ENT && hgrad) hgrad[(size_t)j * ms + k] = hval;
+        }
     }
-    // job `act` (< J) drawn, the owned slots' probabilities pr
-    JSS_DEV void draw(const EnvRegs<KJ> &s, int lane, int act, const float (&pr)[KJ]) {
+    JSS_DEV void clear() {
+#pragma unroll
+        for (int i = 0; i < KJ; i++) {
+            acc[i] = 0.0f;
+            if (ENT) hacc[i] = 0.0f;
+        }
+    }
+    // job `act` (< J) drawn, the owned slots' probabilities pr (ENT: and the decision's gradient terms ent->q)
+    JSS_DEV void draw(const EnvRegs<KJ> &s, int lane, int act, const float (&pr)[KJ], const JssEnt<KJ> *ent = nullptr) {
 #pragma unroll
         for (int i = 0; i < KJ; i++) {
             acc[i] += pr[i];
+            if constexpr (ENT) hacc[i] += ent->q[i];
             if (KJ * lane + i == act) {
-                put(act, s.todo[i], 1.0f - acc[i]);
+                put(act, s.todo[i], 1.0f - acc[i], ENT ? 0.0f - hacc[i] : 0.0f);
                 acc[i] = 0.0f;
+                if (ENT) hacc[i] = 0.0f;
             }
         }
     }
@@ -1473,7 +1536,7 @@ struct JssGradAcc {
 #pragma unroll
         for (int i = 0; i < KJ; i++) {
             const int j = KJ * lane + i, k0 = env_undrawn<KJ>(s, i);
-            if (j < J && k0 < M) put(j, k0, 0.0f - acc[i]);
+            if (j < J && k0 < M) put(j, k0, 0.0f - acc[i], ENT ? 0.0f - hacc[i] : 0.0f);
         }
     }
 };
@@ -1489,16 +1552,20 @@ struct JssGradAcc {
 // with grad_out, the gradient of that sum with respect to the env's table entries (JssGradAcc).  The operations drawn
 // before the call get 0, the first undrawn one at the end -acc and the later ones 0; an env that errs gets 0
 // everywhere, so that a caller who masks it out gets no NaN in a backward pass.
-template <int KJ, bool SAMPLE>
+// ENT (jss_rollout_priority_sample_entropy): also entropy_out[env], the fp32 sum of the decisions' entropies in
+// decision order (NaN where log_prob_out is), and, with entropy_grad_out, its gradient by the same rules (JssGradAcc).
+template <int KJ, bool SAMPLE, bool ENT = false>
 JSS_DEV void env_priority_rollout(const JssParams &p, const JssLaunch &a, const InstView &iv, EnvRegs<KJ> &s, int32_t *blk,
                                   int env, int lane, float *scratch) {
     const int J = jss_J(iv), M = jss_M(iv);
-    JssGradAcc<KJ, false> g{SAMPLE && a.grad_out ? a.grad_out + (size_t)env * p.jobs_max * p.machines_max : nullptr,
-                            p.machines_max, 1.0f, {}};
+    JssGradAcc<KJ, false, ENT> g{SAMPLE && a.grad_out ? a.grad_out + (size_t)env * p.jobs_max * p.machines_max : nullptr,
+                                 p.machines_max, 1.0f, {}};
+    if constexpr (ENT)
+        g.hgrad = a.entropy_grad_out ? a.entropy_grad_out + (size_t)env * p.jobs_max * p.machines_max : nullptr;
     const auto zero_ops = [&](int i, int k0, int k1) {   // operations k0 .. k1-1 of owned slot i
         for (int k = k0; k < k1; k++) g.put(KJ * lane + i, k, 0.0f);
     };
-    if (g.grad) {
+    if (g.on()) {
 #pragma unroll
         for (int i = 0; i < KJ; i++)
             if (KJ * lane + i < J) zero_ops(i, 0, (s.flags & JSS_FLAG_DONE) ? M : env_undrawn<KJ>(s, i));
@@ -1508,13 +1575,14 @@ JSS_DEV void env_priority_rollout(const JssParams &p, const JssLaunch &a, const 
     bool dirty = false;
     int raw = 0;                                         // the raw reward in the scalar record
     bool err = false;
-    float lp = 0.0f;
+    float lp = 0.0f, hs = 0.0f;
     for (int k = 0; k < a.n_steps && !(s.flags & JSS_FLAG_DONE); k++) {
         float logp = 0.0f, pr[KJ];
+        JssEnt<KJ> e;
         int act;
         if (SAMPLE) {
             const uint32_t h = jss_hash_env(jss_hash_key_folded(a.seed_folded, a.sample_counter + (uint64_t)k), genv);
-            act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
+            act = jss_uniform(env_priority_sample_action<KJ, ENT>(a, iv, s, env, lane, h, logp, pr, &e));
         } else {
             act = jss_uniform(env_priority_action<KJ>(a, iv, s, env, lane));
         }
@@ -1525,11 +1593,15 @@ JSS_DEV void env_priority_rollout(const JssParams &p, const JssLaunch &a, const 
         if (act == JSS_INF) {
             s.flags |= JSS_FLAG_ERROR;
         } else {
-            if (g.grad && act < J) g.draw(s, lane, act, pr);   // a job drawn (act == J, the no-op, has no p_t)
+            if (g.on() && act < J) g.draw(s, lane, act, pr, &e);   // a job drawn (act == J, the no-op, has no p_t)
             changed = env_step<KJ>(p, iv, s, env, lane, act, r, reinterpret_cast<int *>(scratch));
         }
         s.flags = jss_uniform(s.flags);
-        if (changed) { lp += logp; raw = r; dirty = true; continue; }
+        if (changed) {
+            lp += logp;
+            if (ENT) hs += e.h;
+            raw = r; dirty = true; continue;
+        }
         // unchanged, with the error bit (bad priorities, or a no-op without a pending event): every later decision
         // would find the same state.  A new bit comes with a zero-reward record (env_store_flags_only); the call's
         // log-probability is NaN.
@@ -1538,13 +1610,14 @@ JSS_DEV void env_priority_rollout(const JssParams &p, const JssLaunch &a, const 
         break;
     }
     if (SAMPLE) {
-        if (g.grad) {
+        if (g.on()) {
             if (!err) g.finish(s, lane, J, M);
 #pragma unroll
             for (int i = 0; i < KJ; i++)
                 if (KJ * lane + i < J) zero_ops(i, err ? 0 : env_undrawn<KJ>(s, i) + 1, M);
         }
         if (lane == 0) a.log_prob_out[env] = err ? JSS_F32_NAN : lp;
+        if (ENT && lane == 0) a.entropy_out[env] = err ? JSS_F32_NAN : hs;
     }
     env_store_rollout_end<KJ>(p, iv, blk, s, env, lane, scratch, dirty, raw, flags_in);
 }
@@ -1661,13 +1734,19 @@ JSS_DEV void env_lookahead(const JssParams &p, const JssLaunch &a, const InstVie
 //   the start time of each operation it starts into a.solution_out.
 // JSS_MODE_ORDER_LOG_PROB / _GRAD: the loop of JSS_MODE_SAMPLE_EPISODES / _GRAD with the decisions of env_order_action
 //   on order s of the env (a.order_in) in place of the draws; no RNG.
+// The _ENT forms of these modes also store each sample's or order's entropy (0 for an env done at entry, NaN where the
+// log-probability is NaN) at its column of a.entropy_out; their _GRAD replays add w_s G_s + v_s G_H,s, v_s from
+// a.entropy_weights, and skip a sample only where both weights are 0.
 JSS_HD constexpr bool jss_mode_samples(int mode) {
     return mode == JSS_MODE_SAMPLE_EPISODES || mode == JSS_MODE_SAMPLE_EPISODES_GRAD ||
            mode == JSS_MODE_SAMPLE_EPISODES_SOLUTION || mode == JSS_MODE_ORDER_LOG_PROB ||
-           mode == JSS_MODE_ORDER_LOG_PROB_GRAD;
+           mode == JSS_MODE_ORDER_LOG_PROB_GRAD || mode == JSS_MODE_SAMPLE_EPISODES_ENT ||
+           mode == JSS_MODE_SAMPLE_EPISODES_ENT_GRAD || mode == JSS_MODE_ORDER_LOG_PROB_ENT ||
+           mode == JSS_MODE_ORDER_LOG_PROB_ENT_GRAD;
 }
-template <int KJ, bool ROW = false>
-JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ]);
+template <int KJ, bool ROW = false, bool ENT = false>
+JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ],
+                            float *ent = nullptr);
 // Env `env`'s next decision under an operation order `ord` (row stride machines_max; jss_order_log_prob): that of
 // env_priority_action on the table -ord, the legal job whose current operation has the smallest entry, ties to the
 // lowest job.  Writes logp, its log-probability under the logit table a.table by env_table_logp (so that a beam's score
@@ -1676,13 +1755,16 @@ JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, i
 // JSS_INF for a bad table row; JSS_ACTION_SKIP when nothing is legal.
 // SWAP (jss_improve_orders): the entries at ord index sw.x and sw.y read as sw.z and sw.w (an index < 0 matches
 // nothing), and the decision is returned without reading a table (logp and p stay 0).
-template <int KJ, bool SWAP = false>
+// ENT: also the decision's entropy and gradient terms into *ent, as env_priority_sample_action<KJ, true> writes them.
+template <int KJ, bool SWAP = false, bool ENT = false>
 JSS_DEV int env_order_action(const JssLaunch &a, const InstView &iv, const EnvRegs<KJ> &s, int env, int lane,
-                             const int32_t *ord, int mstride, float &logp, float (&pr)[KJ], int4 sw = int4()) {
+                             const int32_t *ord, int mstride, float &logp, float (&pr)[KJ], int4 sw = int4(),
+                             JssEnt<KJ> *ent = nullptr) {
     constexpr uint32_t LM = jss_legal_mask<KJ>();
     logp = 0.0f;
 #pragma unroll
     for (int i = 0; i < KJ; i++) pr[i] = 0.0f;
+    if constexpr (ENT) jss_ent_clear<KJ>(ent);
     if (!__any_sync(JSS_FULL, (s.lb & LM) != 0u))
         return (s.flags & JSS_FLAG_NOOP_LEGAL) ? jss_J(iv) : JSS_ACTION_SKIP;
     int act = JSS_INF;
@@ -1695,12 +1777,13 @@ JSS_DEV int env_order_action(const JssLaunch &a, const InstView &iv, const EnvRe
     }, act);
     if (SWAP) return act;
     float lp[KJ];
-    if (!env_table_logp<KJ>(a, s, env, lane, lp)) return JSS_INF;
+    if (!env_table_logp<KJ, false, ENT>(a, s, env, lane, lp, ENT ? &ent->h : nullptr)) return JSS_INF;
     float la = 0.0f;
 #pragma unroll
     for (int i = 0; i < KJ; i++) {
         if ((s.lb >> i) & 1u) pr[i] = jss_fast_exp(lp[i]);
         if (KJ * lane + i == act) la = lp[i];
+        if constexpr (ENT) ent->q[i] = pr[i] > 0.0f ? pr[i] * (lp[i] + ent->h) : 0.0f;
     }
     logp = __shfl_sync(JSS_FULL, la, act / KJ);
     return act;
@@ -1708,8 +1791,12 @@ JSS_DEV int env_order_action(const JssLaunch &a, const InstView &iv, const EnvRe
 template <int KJ, int MODE>
 JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const InstView &iv, int env, int tile,
                                  int warp, int lane, int sp, float *scratch) {
-    constexpr bool ORD = MODE == JSS_MODE_ORDER_LOG_PROB || MODE == JSS_MODE_ORDER_LOG_PROB_GRAD;
-    constexpr bool GRAD = MODE == JSS_MODE_SAMPLE_EPISODES_GRAD || MODE == JSS_MODE_ORDER_LOG_PROB_GRAD;
+    constexpr bool ENT = MODE == JSS_MODE_SAMPLE_EPISODES_ENT || MODE == JSS_MODE_SAMPLE_EPISODES_ENT_GRAD ||
+                         MODE == JSS_MODE_ORDER_LOG_PROB_ENT || MODE == JSS_MODE_ORDER_LOG_PROB_ENT_GRAD;
+    constexpr bool ORD = MODE == JSS_MODE_ORDER_LOG_PROB || MODE == JSS_MODE_ORDER_LOG_PROB_GRAD ||
+                         MODE == JSS_MODE_ORDER_LOG_PROB_ENT || MODE == JSS_MODE_ORDER_LOG_PROB_ENT_GRAD;
+    constexpr bool GRAD = MODE == JSS_MODE_SAMPLE_EPISODES_GRAD || MODE == JSS_MODE_ORDER_LOG_PROB_GRAD ||
+                          MODE == JSS_MODE_SAMPLE_EPISODES_ENT_GRAD || MODE == JSS_MODE_ORDER_LOG_PROB_ENT_GRAD;
     constexpr bool SOL = MODE == JSS_MODE_SAMPLE_EPISODES_SOLUTION;
     const int32_t *blk = p.state + (size_t)jss_tile(p, a, p.uniform_inst >= 0, tile, warp).off16 * 4;
     const uint64_t genv = p.env_id_base + (uint64_t)env;
@@ -1727,11 +1814,15 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
     }
     if (s.flags & JSS_FLAG_DONE) {
         if (!GRAD && !SOL && lane == 0)
-            for (int k = first; k < end; k += stride) { a.makespan_out[row + k] = -1; a.log_prob_out[row + k] = 0.0f; }
+            for (int k = first; k < end; k += stride) {
+                a.makespan_out[row + k] = -1;
+                a.log_prob_out[row + k] = 0.0f;
+                if (ENT) a.entropy_out[row + k] = 0.0f;
+            }
         return;
     }
-    JssGradAcc<KJ, true> g{GRAD ? a.grad_out + ((size_t)sp * p.n_envs + env) * p.jobs_max * p.machines_max : nullptr,
-                           p.machines_max, 0.0f, {}};
+    JssGradAcc<KJ, true, ENT> g{GRAD ? a.grad_out + ((size_t)sp * p.n_envs + env) * p.jobs_max * p.machines_max
+                                     : nullptr, p.machines_max, 0.0f, {}};
     bool check = false;                                  // GRAD: a sample may err after an add
     if (GRAD) {
         const float *tab = jss_table_row(a.table, env);
@@ -1749,10 +1840,11 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
         check = __any_sync(JSS_FULL, !clean);
     }
     for (int smp = first; smp < end; smp += stride) {
-        float w = 0.0f;
+        float w = 0.0f, v = 0.0f;
         if (GRAD) {
             w = __int_as_float(jss_uniform(__float_as_int(a.weights[row + smp])));
-            if (w == 0.0f) continue;
+            if (ENT) v = __int_as_float(jss_uniform(__float_as_int(a.entropy_weights[row + smp])));
+            if (w == 0.0f && v == 0.0f) continue;
         }
         const uint64_t c0 = a.sample_counter + (uint64_t)smp * (uint64_t)bound;
         const int32_t *ord = ORD ? a.order_in + ((size_t)env * a.n_samples + smp) * p.jobs_max * p.machines_max : nullptr;
@@ -1762,33 +1854,37 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
             env_load<KJ>(iv, blk, lane, s);
             s.flags = jss_uniform(s.flags);
             g.w = w;
-#pragma unroll
-            for (int i = 0; i < KJ; i++) g.acc[i] = 0.0f;
+            g.v = v;
+            g.clear();
             bool err = false;
-            float lp = 0.0f;
+            float lp = 0.0f, hs = 0.0f;
             for (int d = 0; d < bound && !(s.flags & JSS_FLAG_DONE); d++) {
                 float logp, pr[KJ];
+                JssEnt<KJ> e;
                 int act;
                 if (ORD) {
-                    act = jss_uniform(env_order_action<KJ>(a, iv, s, env, lane, ord, p.machines_max, logp, pr));
+                    act = jss_uniform(env_order_action<KJ, false, ENT>(a, iv, s, env, lane, ord, p.machines_max, logp,
+                                                                       pr, int4(), &e));
                 } else {
                     const uint32_t h = jss_hash_env(jss_hash_key_folded(a.seed_folded, c0 + (uint64_t)d), genv);
-                    act = jss_uniform(env_priority_sample_action<KJ>(a, iv, s, env, lane, h, logp, pr));
+                    act = jss_uniform(env_priority_sample_action<KJ, ENT>(a, iv, s, env, lane, h, logp, pr, &e));
                 }
                 if (act == JSS_ACTION_SKIP) break;       // nothing legal: no decision changes the env
                 int r;
                 bool changed = false;
                 if (act != JSS_INF) {
-                    if (add && act < J) g.draw(s, lane, act, pr);   // a job drawn (the no-op has no p_t)
+                    if (add && act < J) g.draw(s, lane, act, pr, &e);   // a job drawn (the no-op has no p_t)
                     changed = env_step<KJ, false, false, SOL>(p, iv, s, env, lane, act, r, hz, a.solution_out);
                 }
                 s.flags = jss_uniform(s.flags);
                 if (!changed) { err = true; break; }
                 lp += logp;
+                if (ENT) hs += e.h;
             }
             if (!GRAD && !SOL && lane == 0) {
                 a.makespan_out[row + smp] = (s.flags & JSS_FLAG_DONE) ? s.t : -1;
                 a.log_prob_out[row + smp] = err ? JSS_F32_NAN : lp;
+                if (ENT) a.entropy_out[row + smp] = err ? JSS_F32_NAN : hs;
             }
             if (err) break;                              // GRAD: no adds, or none yet (decision 0 of pass 1)
             if (add) g.finish(s, lane, J, M);
@@ -1804,8 +1900,9 @@ JSS_DEV void env_sample_episodes(const JssParams &p, const JssLaunch &a, const I
 // At least one job must be legal; returns false for a bad row (the bad-table rule of env_priority_sample_action).
 // ROW (jss_beam_step): x_j is column j of env `env`'s logit row (a.rows) in place of the table entry of job j's current
 // operation; everything else is the same.
-template <int KJ, bool ROW>
-JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ]) {
+// ENT: also the decision's entropy into *ent (jss_softmax_entropy on the same d, exponentials, sum and log).
+template <int KJ, bool ROW, bool ENT>
+JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, int lane, float (&lp)[KJ], float *ent) {
     const float *row = ROW ? a.rows + (int64_t)env * a.rows_ld : jss_table_row(a.table, env);
     bool bad = false;                                    // a legal entry is NaN or +inf
     uint32_t xkey = 0u;                                  // 0: below every candidate's key
@@ -1821,15 +1918,20 @@ JSS_DEV bool env_table_logp(const JssLaunch &a, const EnvRegs<KJ> &s, int env, i
     }
     const float mx = jss_key_f32(__reduce_max_sync(JSS_FULL, xkey));
     if (__any_sync(JSS_FULL, bad) || mx == -JSS_F32_INF) return false;
-    float sum = 0.0f;
+    float sum = 0.0f, e[KJ];
 #pragma unroll
     for (int i = 0; i < KJ; i++) {
         x[i] -= mx;
-        if ((s.lb >> i) & 1u) sum += jss_fast_exp(x[i]);
+        e[i] = 0.0f;
+        if ((s.lb >> i) & 1u) {
+            e[i] = jss_fast_exp(x[i]);
+            sum += e[i];
+        }
     }
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) sum += __shfl_xor_sync(JSS_FULL, sum, off);   // the same sum in every lane
     const float ls = jss_fast_log(sum);
+    if constexpr (ENT) *ent = jss_softmax_entropy<KJ>(x, e, sum, ls);
 #pragma unroll
     for (int i = 0; i < KJ; i++) lp[i] = x[i] - ls;
     return true;
@@ -2448,8 +2550,9 @@ JSS_DEV void jss_process_env(const JssParams &p, const JssLaunch &a, const InstV
     if (mode == JSS_MODE_EXPORT) { env_export<KJ>(p, iv, s, env, lane); return; }
     if (mode == JSS_MODE_PACK) { env_pack<KJ>(a, iv, s, env, lane, scratch); return; }
     if (mode == JSS_MODE_REFRESH) { env_emit_obs<KJ>(p, jss_out_default(p), iv, s, env, lane, scratch); return; }
-    if (MODE == JSS_MODE_PRIORITY || MODE == JSS_MODE_PRIORITY_SAMPLE) {
-        env_priority_rollout<KJ, MODE == JSS_MODE_PRIORITY_SAMPLE>(p, a, iv, s, blk(), env, lane, scratch);
+    if (MODE == JSS_MODE_PRIORITY || MODE == JSS_MODE_PRIORITY_SAMPLE || MODE == JSS_MODE_PRIORITY_SAMPLE_ENT) {
+        constexpr bool ENT = MODE == JSS_MODE_PRIORITY_SAMPLE_ENT;
+        env_priority_rollout<KJ, MODE == JSS_MODE_PRIORITY_SAMPLE || ENT, ENT>(p, a, iv, s, blk(), env, lane, scratch);
         return;
     }
     if (mode == JSS_MODE_POLICY) {
@@ -2608,6 +2711,21 @@ constexpr JssMode JSS_MODES[] = {
     // is the SM's limit, and one CTA more spills with 4 and 8 jobs per lane
     {JSS_MODE_LOOKAHEAD_SAMPLE, {8, 8, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_JK, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
      JSS_REFRESH_NO},
+    // the entropy forms, each with its twin's items, grid, tables and layout.  Registers by class at these bounds, no
+    // stack: the rollout 80 / 80 / 80 / 119 (one CTA fewer than its twin with 1 and 4 jobs per lane, where the twin's
+    // count spills); the draws 48 / 48 / 48 / 76 (5 CTAs, not the twin's 8 / 8 / 6, with 1, 2 and 4: 6 spill); their
+    // replay 61 / 64 / 64 / 126, the twin's counts; the order likelihood 48 / 62 / 64 / 94 (5, not 6, with 1 job per
+    // lane); its gradient 64 / 72 / 89 / 140 (2, not 4, with 4 jobs per lane: 3 spill)
+    {JSS_MODE_PRIORITY_SAMPLE_ENT, {3, 3, 3, 2}, JSS_ITEM_WARP, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_YES},
+    {JSS_MODE_SAMPLE_EPISODES_ENT, {5, 5, 5, 3}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_K, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},
+    {JSS_MODE_SAMPLE_EPISODES_ENT_GRAD, {4, 4, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV,
+     false, JSS_REFRESH_NO},
+    {JSS_MODE_ORDER_LOG_PROB_ENT, {5, 4, 4, 2}, JSS_ITEM_SPLIT, JSS_GRID_SPREAD_K, JSS_STAGE_OPS, JSS_SMEM_ENV, false,
+     JSS_REFRESH_NO},
+    {JSS_MODE_ORDER_LOG_PROB_ENT_GRAD, {4, 3, 2, 1}, JSS_ITEM_SPLIT, JSS_GRID_RESIDENT, JSS_STAGE_OPS, JSS_SMEM_ENV,
+     false, JSS_REFRESH_NO},
 };
 static_assert(sizeof(JSS_MODES) / sizeof(JSS_MODES[0]) == JSS_NUM_MODES, "one row per JSS_MODE_*");
 // a mode that another mode's kernel runs has that kernel's loop, tables, layout and launch bound

@@ -233,6 +233,10 @@ struct JssLaunch {
     int32_t *parent_out;     // [N] each slot's parent slot: the beam steps
     int32_t *job_out;        // [N] each slot's job: the beam steps
     int32_t *bad_out;        // [N / W] each group's bad-row bit: the beam steps
+    float *entropy_out;      // the entropy of each episode, beside log_prob_out: the _ENT modes
+    float *entropy_grad_out; // [N][jobs_max][machines_max] d entropy / d table: jss_rollout_priority_sample_entropy
+                             // (may be NULL)
+    const float *entropy_weights;   // row i: each sample's weight of the entropy gradient: the _ENT_GRAD modes
 };
 
 #define JSS_MODE_RESET 0
@@ -272,6 +276,16 @@ struct JssLaunch {
                                          // (env, order) per CTA, the envs untouched (jss_improve_orders)
 #define JSS_MODE_LOOKAHEAD_SAMPLE 22     // each legal action's makespans under K episodes drawn from a logit table
                                          // after it, the envs untouched (jss_lookahead_sample)
-#define JSS_NUM_MODES 23                 // the rows of JSS_MODES (jss_device.cuh)
+// The entropy forms of the three differentiable log-probability producers: each also writes every episode's policy
+// entropy, the fp32 sum over its decisions of H_t = log S - T / S (jss_softmax_entropy), into a.entropy_out.
+#define JSS_MODE_PRIORITY_SAMPLE_ENT 23  // JSS_MODE_PRIORITY_SAMPLE, with d entropy / d table into a.entropy_grad_out
+                                         // (jss_rollout_priority_sample_entropy)
+#define JSS_MODE_SAMPLE_EPISODES_ENT 24  // JSS_MODE_SAMPLE_EPISODES (jss_sample_episodes_entropy)
+#define JSS_MODE_SAMPLE_EPISODES_ENT_GRAD 25   // its replay, adding w_s G_lp + v_s G_H with v_s from
+                                               // a.entropy_weights (jss_sample_episodes_entropy_grad)
+#define JSS_MODE_ORDER_LOG_PROB_ENT 26   // JSS_MODE_ORDER_LOG_PROB (jss_order_log_prob_entropy)
+#define JSS_MODE_ORDER_LOG_PROB_ENT_GRAD 27    // its gradient as JSS_MODE_SAMPLE_EPISODES_ENT_GRAD's
+                                               // (jss_order_log_prob_entropy_grad)
+#define JSS_NUM_MODES 28                 // the rows of JSS_MODES (jss_device.cuh)
 
 #define JSS_WARPS_PER_CTA 8

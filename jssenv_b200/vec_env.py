@@ -73,23 +73,29 @@ def _host_buffer(shape, dtype):
 def _sampled_log_prob():
     """The autograd Function of JssVecEnv.rollout_priority_sample's log_prob (made on first use: torch is imported
     lazily).  Forward runs the call with a gradient buffer; backward weights each env's gradient rows by the incoming
-    gradient and sums them over the table's broadcast dimensions."""
+    gradient and sums them over the table's broadcast dimensions.  With `entropy`, forward also returns the entropy and
+    stores its gradient rows, and backward adds those weighted by the entropy's incoming gradient."""
     import torch
 
     class SampledLogProb(torch.autograd.Function):
         @staticmethod
-        def forward(ctx, logits, env, n_steps):
+        def forward(ctx, logits, env, n_steps, entropy=False):
             # zero-filled: the kernel leaves the entries past J_i / M_i alone, and a broadcast table sums over them
-            grad = torch.zeros((env.num_envs, env.jobs, env.machines), dtype=torch.float32, device=env.device)
-            log_prob = env._rollout_priority_sample(logits, n_steps, grad)
-            ctx.save_for_backward(grad)
+            shape = (env.num_envs, env.jobs, env.machines)
+            grad = torch.zeros(shape, dtype=torch.float32, device=env.device)
+            hgrad = torch.zeros(shape, dtype=torch.float32, device=env.device) if entropy else None
+            out = env._rollout_priority_sample(logits, n_steps, grad, entropy, hgrad)
+            ctx.save_for_backward(grad, hgrad)
             ctx.shape, ctx.dtype = logits.shape, logits.dtype
-            return log_prob
+            return out
 
         @staticmethod
-        def backward(ctx, g):
-            (grad,) = ctx.saved_tensors
-            return (g[:, None, None] * grad).sum_to_size(ctx.shape).to(ctx.dtype), None, None
+        def backward(ctx, g, gh=None):
+            grad, hgrad = ctx.saved_tensors
+            total = g[:, None, None] * grad
+            if hgrad is not None:
+                total = total + gh[:, None, None] * hgrad
+            return total.sum_to_size(ctx.shape).to(ctx.dtype), None, None, None
 
     return SampledLogProb
 
@@ -99,25 +105,26 @@ def _episodes_log_prob():
     """The autograd Function of JssVecEnv.sample_episodes' log_prob (made on first use).  Forward draws the episodes and
     saves the table and the RNG counter; backward replays the draws (jss_sample_episodes_grad) with the incoming (N, k)
     gradient as weights, sums the chunks and then over the table's broadcast dimensions.  The replay starts from the
-    envs' state at backward time, which must still be their state at forward time."""
+    envs' state at backward time, which must still be their state at forward time.  With `entropy`, forward also
+    returns the (N, k) entropy, and the one replay takes its incoming gradient as the entropy weights."""
     import torch
 
     class EpisodesLogProb(torch.autograd.Function):
         @staticmethod
-        def forward(ctx, logits, env, k, step_index):
-            makespan, log_prob = env._sample_episodes(logits, k, step_index)
+        def forward(ctx, logits, env, k, step_index, entropy=False):
+            out = env._sample_episodes(logits, k, step_index, entropy)
             ctx.save_for_backward(logits)              # torch's version counter refuses a table changed in place
-            ctx.env, ctx.k, ctx.step_index = env, k, step_index
-            ctx.mark_non_differentiable(makespan)
-            return makespan, log_prob
+            ctx.env, ctx.k, ctx.step_index, ctx.entropy = env, k, step_index, entropy
+            ctx.mark_non_differentiable(out[0])
+            return out
 
         @staticmethod
-        def backward(ctx, _, g):
+        def backward(ctx, _, g, gh=None):
             (logits,) = ctx.saved_tensors
             env = ctx.env
             split = min(ctx.k, -(-env._warp_slots() // env.num_envs))
-            grad = env._sample_episodes_grad(logits, ctx.k, ctx.step_index, g, split)
-            return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None, None
+            grad = env._sample_episodes_grad(logits, ctx.k, ctx.step_index, g, split, gh)
+            return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None, None, None
 
     return EpisodesLogProb
 
@@ -129,26 +136,27 @@ def _order_log_prob_fn():
     orders last and any other outputs between, and saves the table and the orders; backward calls
     jss_order_log_prob_grad with the incoming (N, k) gradient as weights, sums the chunks and then over the table's
     broadcast dimensions.  The orders are replayed from the envs' state at backward time, which must still be their
-    state at forward time."""
+    state at forward time.  With `entropy`, `run` returns the (N, k) entropy second, differentiable too, and the one
+    replay takes its incoming gradient as the entropy weights."""
     import torch
 
     class OrderLogProb(torch.autograd.Function):
         @staticmethod
-        def forward(ctx, logits, env, run):
+        def forward(ctx, logits, env, run, entropy=False):
             outs = run(logits)
             ctx.save_for_backward(logits, outs[-1])    # torch's version counter refuses a table changed in place
-            ctx.env = env
-            ctx.mark_non_differentiable(*outs[1:])
+            ctx.env, ctx.entropy = env, entropy
+            ctx.mark_non_differentiable(*outs[2 if entropy else 1:])
             return outs
 
         @staticmethod
-        def backward(ctx, g, *_):
+        def backward(ctx, g, *rest):
             logits, order = ctx.saved_tensors
             env = ctx.env
             k = order.shape[1]
             split = min(k, -(-env._warp_slots() // env.num_envs))
-            grad = env._order_log_prob_grad(logits, order, g, split)
-            return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None
+            grad = env._order_log_prob_grad(logits, order, g, split, rest[0] if ctx.entropy else None)
+            return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None, None
 
     return OrderLogProb
 
@@ -495,7 +503,7 @@ class JssVecEnv:
         N.check(self._h, rc, "jss_rollout_priority")
         return self._obs(), self.reward, self.done, self._truncated, {}
 
-    def rollout_priority_sample(self, logits, n_steps: Optional[int] = None):
+    def rollout_priority_sample(self, logits, n_steps: Optional[int] = None, entropy: bool = False):
         """Run every env to the end of its episode in one launch per lane class, each decision drawn from the softmax
         over the legal jobs of the entries of their current operations (jss_rollout_priority_sample; the no-op only
         when no job is legal).  `logits` and `n_steps` are taken as rollout_priority's priorities and n_steps.  Decision
@@ -503,24 +511,39 @@ class JssVecEnv:
         the counter then advances by `n_steps`.  Returns the step tuple with ``{"log_prob": float32 (N,)}`` as info:
         each env's sum of its decisions' log-probabilities in this call (NaN for an env that got the error bit).  When
         `logits` requires grad (and grad mode is on), log_prob is differentiable with respect to it: the kernel also
-        writes d log_prob / d table, and broadcast tables such as (1, J, M) get the gradient summed over the envs."""
+        writes d log_prob / d table, and broadcast tables such as (1, J, M) get the gradient summed over the envs.
+        With `entropy`, info also holds ``"entropy"`` float32 (N,): each env's sum over its decisions in this call of
+        the policy's entropy at the decision, H_t = log S - T/S over the legal jobs (jss_rollout_priority_sample_entropy;
+        forced no-ops add 0, NaN where log_prob is NaN); everything else is bit for bit what the call without it gives.
+        With a table that requires grad, log_prob and entropy are then both differentiable from one stored forward."""
         import torch
         J, M = self.jobs, self.machines
         x = self._table_arg(logits, "rollout_priority_sample", "logits")
         n_steps = 2 * J * M + 1 if n_steps is None else int(n_steps)
         if x.requires_grad and torch.is_grad_enabled():
-            log_prob = _sampled_log_prob().apply(x, self, n_steps)
+            out = _sampled_log_prob().apply(x, self, n_steps, True) if entropy else \
+                _sampled_log_prob().apply(x, self, n_steps)
         else:
-            log_prob = self._rollout_priority_sample(x, n_steps, None)
-        return self._obs(), self.reward, self.done, self._truncated, {"log_prob": log_prob}
+            out = self._rollout_priority_sample(x, n_steps, None, entropy)
+        info = {"log_prob": out[0], "entropy": out[1]} if entropy else {"log_prob": out}
+        return self._obs(), self.reward, self.done, self._truncated, info
 
-    def _rollout_priority_sample(self, x, n_steps: int, grad_out):
+    def _rollout_priority_sample(self, x, n_steps: int, grad_out, entropy: bool = False, entropy_grad_out=None):
         """The native call of rollout_priority_sample on a checked table `x` (read through a detached float32 view,
         strides passed through); writes the gradient to `grad_out` ((N, J, M) float32, or None); advances the RNG
-        counter.  Returns log_prob."""
+        counter.  Returns log_prob, or with `entropy` (log_prob, entropy) and the entropy's gradient written to
+        `entropy_grad_out` (as grad_out)."""
         import torch
         v = self._table_view(x)
         log_prob = torch.empty(self.num_envs, dtype=torch.float32, device=self.device)
+        if entropy:
+            ent = torch.empty(self.num_envs, dtype=torch.float32, device=self.device)
+            rc = self._L.jss_rollout_priority_sample_entropy(self._h, *_table_args(v), self.seed, self._step_index,
+                                                             n_steps, log_prob.data_ptr(), ent.data_ptr(),
+                                                             _ptr(grad_out), _ptr(entropy_grad_out), self._stream())
+            N.check(self._h, rc, "jss_rollout_priority_sample_entropy")
+            self._step_index += n_steps
+            return log_prob, ent
         rc = self._L.jss_rollout_priority_sample(self._h, *_table_args(v), self.seed, self._step_index, n_steps,
                                                  log_prob.data_ptr(), _ptr(grad_out), self._stream())
         N.check(self._h, rc, "jss_rollout_priority_sample")
@@ -604,7 +627,7 @@ class JssVecEnv:
         best = torch.where(count > 0, best, -1)
         return {"makespan": out, "mean": mean, "min": best}
 
-    def sample_episodes(self, logits, k: int, solution: bool = False):
+    def sample_episodes(self, logits, k: int, solution: bool = False, entropy: bool = False):
         """Draw `k` whole episodes per env from the logit table `logits`, each from the env's current state, in one
         launch per lane class (jss_sample_episodes), leaving the envs untouched.  With B = 2*J*M + 1, sample s of env i
         is the episode rollout_priority_sample(logits) would draw from this state with the RNG counter at
@@ -615,7 +638,10 @@ class JssVecEnv:
         sample of smallest makespan, -1 if none ended; with `solution`, ``"solution"`` (N, J, M) int32, the start times
         of the best sample's operations over this env's solution so far (-1 without record_solution).  When `logits`
         requires grad (and grad mode is on), log_prob is differentiable with respect to it: the backward replays the
-        draws, so the envs must not be stepped or reset between this call and the backward."""
+        draws, so the envs must not be stepped or reset between this call and the backward.  With `entropy`, the dict
+        also holds ``"entropy"`` (N, k) float32, each sample's policy entropy as rollout_priority_sample(entropy=True)
+        reports it for the same episode (0 for an env done now); with a table that requires grad it is differentiable
+        too, and one replay gives the gradient of both."""
         import torch
         J, M = self.jobs, self.machines
         x = self._table_arg(logits, "sample_episodes", "logits")
@@ -623,12 +649,16 @@ class JssVecEnv:
             raise ValueError(f"sample_episodes: k must be at least 1, got {k!r}")
         k, step_index = int(k), self._step_index
         if x.requires_grad and torch.is_grad_enabled():
-            makespan, log_prob = _episodes_log_prob().apply(x, self, k, step_index)
+            res = _episodes_log_prob().apply(x, self, k, step_index, True) if entropy else \
+                _episodes_log_prob().apply(x, self, k, step_index)
         else:
-            makespan, log_prob = self._sample_episodes(x, k, step_index)
+            res = self._sample_episodes(x, k, step_index, entropy)
+        makespan, log_prob = res[0], res[1]
         self._step_index += k * (2 * J * M + 1)
         best = _best_slot(makespan)
         out = {"makespan": makespan, "log_prob": log_prob, "best": best}
+        if entropy:
+            out["entropy"] = res[2]
         if solution:
             sol = (self.solution.clone() if self.solution is not None
                    else torch.full((self.num_envs, J, M), -1, dtype=torch.int32, device=self.device))
@@ -788,7 +818,7 @@ class JssVecEnv:
         N.check(self._h, rc, "jss_sample_without_replacement")
         return log_prob, makespan, key, ord_
 
-    def order_log_prob(self, logits, order):
+    def order_log_prob(self, logits, order, entropy: bool = False):
         """The log-likelihood under the logit table `logits` of given operation orders, each from the env's current
         state, in one launch per lane class (jss_order_log_prob), leaving the envs untouched.  `order` is (N, J, M) or
         (N, k, J, M) integer: order s of env i stands for the episode rollout_priority(-order[i, s]) runs from this
@@ -797,10 +827,21 @@ class JssVecEnv:
         of the decisions' log-probabilities computed as rollout_priority_sample() computes them (forced no-ops add 0;
         NaN where a decision meets a bad entry; 0 for an env done now), makespan int32, the end time (-1 unless the
         episode ends done).  When `logits` requires grad (and grad mode is on), log_prob is differentiable with respect
-        to it (jss_order_log_prob_grad); the envs must not be stepped or reset between this call and the backward."""
+        to it (jss_order_log_prob_grad); the envs must not be stepped or reset between this call and the backward.
+        With `entropy`, returns ``(log_prob, makespan, entropy)``: entropy float32 like log_prob, the sum over the
+        episode's decisions of the policy's entropy, bit for bit what rollout_priority_sample(entropy=True) reports for
+        an episode drawing the same jobs from this state (0 for an env done now, NaN where log_prob is NaN); with a
+        table that requires grad both log_prob and entropy are differentiable, through one replay."""
         import torch
         x = self._table_arg(logits, "order_log_prob", "logits")
         o, single = self._orders_arg(order, "order_log_prob")
+        if entropy:
+            run = functools.partial(self._order_log_prob, order=o, entropy=True)
+            if x.requires_grad and torch.is_grad_enabled():
+                log_prob, ent, makespan, _ = _order_log_prob_fn().apply(x, self, run, True)
+            else:
+                log_prob, ent, makespan, _ = run(x)
+            return (log_prob[:, 0], makespan[:, 0], ent[:, 0]) if single else (log_prob, makespan, ent)
         run = functools.partial(self._order_log_prob, order=o)
         if x.requires_grad and torch.is_grad_enabled():
             log_prob, makespan, _ = _order_log_prob_fn().apply(x, self, run)
@@ -844,51 +885,79 @@ class JssVecEnv:
         out["best"] = _best_slot(out["makespan"])
         return out
 
-    def _order_log_prob(self, x, order):
+    def _order_log_prob(self, x, order, entropy: bool = False):
         """The native call of order_log_prob on a checked table `x` and (N, k, J, M) contiguous int32 orders:
-        (log_prob, makespan, order)."""
+        (log_prob, makespan, order), with `entropy` (log_prob, entropy, makespan, order)."""
         import torch
         v = self._table_view(x)
         k = order.shape[1]
         makespan = torch.empty((self.num_envs, k), dtype=torch.int32, device=self.device)
         log_prob = torch.empty((self.num_envs, k), dtype=torch.float32, device=self.device)
+        if entropy:
+            ent = torch.empty((self.num_envs, k), dtype=torch.float32, device=self.device)
+            rc = self._L.jss_order_log_prob_entropy(self._h, *_table_args(v), order.data_ptr(), k, makespan.data_ptr(),
+                                                    log_prob.data_ptr(), ent.data_ptr(), k, self._stream())
+            N.check(self._h, rc, "jss_order_log_prob_entropy")
+            return log_prob, ent, makespan, order
         rc = self._L.jss_order_log_prob(self._h, *_table_args(v), order.data_ptr(), k, makespan.data_ptr(),
                                         log_prob.data_ptr(), k, self._stream())
         N.check(self._h, rc, "jss_order_log_prob")
         return log_prob, makespan, order
 
-    def _order_log_prob_grad(self, x, order, weights, split: int):
+    def _order_log_prob_grad(self, x, order, weights, split: int, entropy_weights=None):
         """The native backward of order_log_prob: the (split, N, J, M) float32 chunks of sum_s weights[:, s] *
-        d log_prob[:, s] / d table for the (N, k, J, M) int32 orders, replayed from the current state."""
+        d log_prob[:, s] / d table for the (N, k, J, M) int32 orders, replayed from the current state; with
+        `entropy_weights`, plus entropy_weights[:, s] * d entropy[:, s] / d table, in the same replay."""
         import torch
         v = self._table_view(x)
         k = order.shape[1]
         w = weights.detach().to(torch.float32).contiguous()
         grad = torch.zeros((split, self.num_envs, self.jobs, self.machines), dtype=torch.float32, device=self.device)
+        if entropy_weights is not None:
+            u = entropy_weights.detach().to(torch.float32).contiguous()
+            rc = self._L.jss_order_log_prob_entropy_grad(self._h, *_table_args(v), order.data_ptr(), k, w.data_ptr(),
+                                                         u.data_ptr(), k, int(split), grad.data_ptr(), self._stream())
+            N.check(self._h, rc, "jss_order_log_prob_entropy_grad")
+            return grad
         rc = self._L.jss_order_log_prob_grad(self._h, *_table_args(v), order.data_ptr(), k, w.data_ptr(), k, int(split),
                                              grad.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_order_log_prob_grad")
         return grad
 
-    def _sample_episodes(self, x, k: int, step_index: int):
+    def _sample_episodes(self, x, k: int, step_index: int, entropy: bool = False):
         """The native call of sample_episodes on a checked table `x` at RNG counter `step_index`: (makespan, log_prob),
-        each (N, k)."""
+        each (N, k); with `entropy` (makespan, log_prob, entropy)."""
         import torch
         v = self._table_view(x)
         makespan = torch.empty((self.num_envs, k), dtype=torch.int32, device=self.device)
         log_prob = torch.empty((self.num_envs, k), dtype=torch.float32, device=self.device)
+        if entropy:
+            ent = torch.empty((self.num_envs, k), dtype=torch.float32, device=self.device)
+            rc = self._L.jss_sample_episodes_entropy(self._h, *_table_args(v), self.seed, step_index, k,
+                                                     makespan.data_ptr(), log_prob.data_ptr(), ent.data_ptr(), k,
+                                                     self._stream())
+            N.check(self._h, rc, "jss_sample_episodes_entropy")
+            return makespan, log_prob, ent
         rc = self._L.jss_sample_episodes(self._h, *_table_args(v), self.seed, step_index, k, makespan.data_ptr(),
                                          log_prob.data_ptr(), k, self._stream())
         N.check(self._h, rc, "jss_sample_episodes")
         return makespan, log_prob
 
-    def _sample_episodes_grad(self, x, k: int, step_index: int, weights, split: int):
+    def _sample_episodes_grad(self, x, k: int, step_index: int, weights, split: int, entropy_weights=None):
         """The native backward of sample_episodes: the (split, N, J, M) float32 chunks of sum_s weights[:, s] *
-        d log_prob[:, s] / d table, replayed from the current state at RNG counter `step_index`."""
+        d log_prob[:, s] / d table, replayed from the current state at RNG counter `step_index`; with
+        `entropy_weights`, plus entropy_weights[:, s] * d entropy[:, s] / d table, in the same replay."""
         import torch
         v = self._table_view(x)
         w = weights.detach().to(torch.float32).contiguous()
         grad = torch.zeros((split, self.num_envs, self.jobs, self.machines), dtype=torch.float32, device=self.device)
+        if entropy_weights is not None:
+            u = entropy_weights.detach().to(torch.float32).contiguous()
+            rc = self._L.jss_sample_episodes_entropy_grad(self._h, *_table_args(v), self.seed, step_index, k,
+                                                          w.data_ptr(), u.data_ptr(), k, int(split), grad.data_ptr(),
+                                                          self._stream())
+            N.check(self._h, rc, "jss_sample_episodes_entropy_grad")
+            return grad
         rc = self._L.jss_sample_episodes_grad(self._h, *_table_args(v), self.seed, step_index, k, w.data_ptr(), k,
                                               int(split), grad.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_sample_episodes_grad")
