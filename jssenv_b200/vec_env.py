@@ -10,6 +10,11 @@ not validated beyond setting a per-env error bit, and ``truncated`` is always Fa
 One exception to the live alias: after ``step_logits_record()`` or ``step_greedy_record()``, which write the
 observation into the caller's rollout slot instead, ``real_obs`` is stale until the next non-recording call or
 ``refresh_obs()``.
+
+The gradients of sample_episodes(), order_log_prob() and sample_without_replacement() are replayed from the envs' state
+at backward time.  Every call that may change an env's state (reset, the steps and their _record forms, the rollouts,
+beam_step, stochastic_beam_step, import_state and the host-buffer steps) counts as a change, whether or not it changed
+one in the end, and a backward of such an output made before it raises RuntimeError; so does a backward after close().
 """
 import ctypes
 import functools
@@ -103,10 +108,11 @@ def _sampled_log_prob():
 @functools.lru_cache(maxsize=None)
 def _episodes_log_prob():
     """The autograd Function of JssVecEnv.sample_episodes' log_prob (made on first use).  Forward draws the episodes and
-    saves the table and the RNG counter; backward replays the draws (jss_sample_episodes_grad) with the incoming (N, k)
-    gradient as weights, sums the chunks and then over the table's broadcast dimensions.  The replay starts from the
-    envs' state at backward time, which must still be their state at forward time.  With `entropy`, forward also
-    returns the (N, k) entropy, and the one replay takes its incoming gradient as the entropy weights."""
+    saves the table, the RNG counter and the envs' state epoch; backward replays the draws (jss_sample_episodes_grad)
+    with the incoming (N, k) gradient as weights, sums the chunks and then over the table's broadcast dimensions.  The
+    replay starts from the envs' state at backward time, so backward raises RuntimeError, before any launch, if a call
+    that may change that state ran after forward, or if the env was closed.  With `entropy`, forward also returns the
+    (N, k) entropy, and the one replay takes its incoming gradient as the entropy weights."""
     import torch
 
     class EpisodesLogProb(torch.autograd.Function):
@@ -115,6 +121,7 @@ def _episodes_log_prob():
             out = env._sample_episodes(logits, k, step_index, entropy)
             ctx.save_for_backward(logits)              # torch's version counter refuses a table changed in place
             ctx.env, ctx.k, ctx.step_index, ctx.entropy = env, k, step_index, entropy
+            ctx.epoch = env._state_epoch
             ctx.mark_non_differentiable(out[0])
             return out
 
@@ -122,6 +129,7 @@ def _episodes_log_prob():
         def backward(ctx, _, g, gh=None):
             (logits,) = ctx.saved_tensors
             env = ctx.env
+            env._check_replay(ctx.epoch, "sample_episodes")
             split = min(ctx.k, -(-env._warp_slots() // env.num_envs))
             grad = env._sample_episodes_grad(logits, ctx.k, ctx.step_index, g, split, gh)
             return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None, None, None
@@ -132,20 +140,21 @@ def _episodes_log_prob():
 @functools.lru_cache(maxsize=None)
 def _order_log_prob_fn():
     """The autograd Function of the log_prob of JssVecEnv.order_log_prob and JssVecEnv.sample_without_replacement
-    (made on first use).  Forward runs `run(logits)`, which returns the (N, k) log_prob first, the (N, k, J, M) int32
-    orders last and any other outputs between, and saves the table and the orders; backward calls
-    jss_order_log_prob_grad with the incoming (N, k) gradient as weights, sums the chunks and then over the table's
-    broadcast dimensions.  The orders are replayed from the envs' state at backward time, which must still be their
-    state at forward time.  With `entropy`, `run` returns the (N, k) entropy second, differentiable too, and the one
-    replay takes its incoming gradient as the entropy weights."""
+    (made on first use; `who` names the call).  Forward runs `run(logits)`, which returns the (N, k) log_prob first,
+    the (N, k, J, M) int32 orders last and any other outputs between, and saves the table, the orders and the envs'
+    state epoch; backward calls jss_order_log_prob_grad with the incoming (N, k) gradient as weights, sums the chunks
+    and then over the table's broadcast dimensions.  The orders are replayed from the envs' state at backward time, so
+    backward raises RuntimeError, before any launch, if a call that may change that state ran after forward, or if the
+    env was closed.  With `entropy`, `run` returns the (N, k) entropy second, differentiable too, and the one replay
+    takes its incoming gradient as the entropy weights."""
     import torch
 
     class OrderLogProb(torch.autograd.Function):
         @staticmethod
-        def forward(ctx, logits, env, run, entropy=False):
+        def forward(ctx, logits, env, run, who, entropy=False):
             outs = run(logits)
             ctx.save_for_backward(logits, outs[-1])    # torch's version counter refuses a table changed in place
-            ctx.env, ctx.entropy = env, entropy
+            ctx.env, ctx.who, ctx.entropy, ctx.epoch = env, who, entropy, env._state_epoch
             ctx.mark_non_differentiable(*outs[2 if entropy else 1:])
             return outs
 
@@ -153,10 +162,11 @@ def _order_log_prob_fn():
         def backward(ctx, g, *rest):
             logits, order = ctx.saved_tensors
             env = ctx.env
+            env._check_replay(ctx.epoch, ctx.who)
             k = order.shape[1]
             split = min(k, -(-env._warp_slots() // env.num_envs))
             grad = env._order_log_prob_grad(logits, order, g, split, rest[0] if ctx.entropy else None)
-            return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None, None
+            return grad.sum(0).sum_to_size(logits.shape).to(logits.dtype), None, None, None, None
 
     return OrderLogProb
 
@@ -181,6 +191,8 @@ class JssVecEnv:
         self.env_id_base = int(env_id_base)
         self.auto_reset = bool(auto_reset)
         self._step_index = 0
+        # bumped by every call that may change an env's state: a replayed gradient refuses to run across a bump
+        self._state_epoch = 0
         insts, env_to_inst = _instance_list(env_config)
         self.instances = insts
         flags = ((N.CREATE_AUTO_RESET if auto_reset else 0) | (N.CREATE_RECORD_SOLUTION if record_solution else 0) |
@@ -259,6 +271,18 @@ class JssVecEnv:
             self._L.jss_destroy(self._h)
             self._h = ctypes.c_void_p()
 
+    def _check_replay(self, epoch: int, who: str):
+        """Refuses the replayed backward of an output of `who` made at state epoch `epoch` once the handle is closed or
+        a call that may change an env's state ran since: the replay would call into a destroyed handle, or walk other
+        episodes than the ones the output describes."""
+        if not self._h.value:
+            raise RuntimeError(f"{who}: backward after close(): the gradient is replayed on the envs, so take it before "
+                               f"closing them")
+        if self._state_epoch != epoch:
+            raise RuntimeError(f"{who}: backward after a call that may have changed the envs' state (a step, reset, "
+                               f"rollout, beam step or import_state): the gradient is replayed from the current state, "
+                               f"so run {who} again from the new state")
+
     def __del__(self):
         try:
             self.close()
@@ -290,12 +314,14 @@ class JssVecEnv:
     def reset(self, mask=None):
         """reset() of every env (or of the envs where `mask` is nonzero) -> obs (jss_env.py:145-181)."""
         m = self._env_mask(mask)
+        self._state_epoch += 1
         N.check(self._h, self._L.jss_reset(self._h, _ptr(m), self._stream()), "jss_reset")
         return self._obs()
 
     def step(self, actions):
         """actions: int32[N] on the env's device (torch) or anything torch.as_tensor accepts."""
         a = self._device_i32(actions)
+        self._state_epoch += 1
         N.check(self._h, self._L.jss_step(self._h, a.data_ptr(), self._stream()), "jss_step")
         return self._obs(), self.reward, self.done, self._truncated, {}
 
@@ -303,6 +329,7 @@ class JssVecEnv:
         """Host-mirror batches (the single-env facade): apply the actions written to ``self.host["actions"]`` and decode
         the new state into the x_* arrays in ONE launch (jss_step_export), then wait; afterwards every array of
         ``self.host`` is current.  No per-transition copies: the kernels write straight into the pinned block."""
+        self._state_epoch += 1
         rc = self._L.jss_step_export(self._h, self._mirror_actions.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_step_export")
         N.backend.synchronize(self.device_index)
@@ -312,6 +339,7 @@ class JssVecEnv:
         step tuple plus the int32[N] tensor of next actions (`out`, default: in place of `actions`)."""
         a = self._device_i32(actions)
         out = a if out is None else out
+        self._state_epoch += 1
         rc = self._L.jss_step_sample(self._h, a.data_ptr(), _rule_id(rule), _coin_id(coin), self.seed,
                                      self._step_index, out.data_ptr(), self._stream())
         N.check(self._h, rc, "jss_step_sample")
@@ -341,6 +369,7 @@ class JssVecEnv:
         """The native call of the steps that take their action from a row (`what` = step_logits, step_greedy or their
         _record forms): jss_<what>(h, row, ld, *pre, seed, step_index, actions_out, log_prob_out, *slot, stream); then
         the RNG counter advances."""
+        self._state_epoch += 1
         rc = getattr(self._L, "jss_" + what)(self._h, x.data_ptr(), int(ld), *pre, self.seed, self._step_index,
                                              acts.data_ptr(), logp.data_ptr(), *slot, self._stream())
         N.check(self._h, rc, "jss_" + what)
@@ -480,6 +509,7 @@ class JssVecEnv:
 
     def rollout(self, rule: Union[str, int], n_steps: int, write_obs: bool = True):
         """n_steps x (policy -> step) fused on device (DispatchingRule.run_episode, dispatching.py:55-75)."""
+        self._state_epoch += 1
         rc = self._L.jss_rollout(self._h, _rule_id(rule), self.seed, self._step_index, int(n_steps),
                                  int(bool(write_obs)), self._stream())
         N.check(self._h, rc, "jss_rollout")
@@ -499,6 +529,7 @@ class JssVecEnv:
         v = self._table_view(self._table_arg(priorities, "rollout_priority", "priorities"))
         if n_steps is None:
             n_steps = 2 * J * M + 1
+        self._state_epoch += 1
         rc = self._L.jss_rollout_priority(self._h, *_table_args(v), int(n_steps), self._stream())
         N.check(self._h, rc, "jss_rollout_priority")
         return self._obs(), self.reward, self.done, self._truncated, {}
@@ -536,6 +567,7 @@ class JssVecEnv:
         import torch
         v = self._table_view(x)
         log_prob = torch.empty(self.num_envs, dtype=torch.float32, device=self.device)
+        self._state_epoch += 1
         if entropy:
             ent = torch.empty(self.num_envs, dtype=torch.float32, device=self.device)
             rc = self._L.jss_rollout_priority_sample_entropy(self._h, *_table_args(v), self.seed, self._step_index,
@@ -638,7 +670,8 @@ class JssVecEnv:
         sample of smallest makespan, -1 if none ended; with `solution`, ``"solution"`` (N, J, M) int32, the start times
         of the best sample's operations over this env's solution so far (-1 without record_solution).  When `logits`
         requires grad (and grad mode is on), log_prob is differentiable with respect to it: the backward replays the
-        draws, so the envs must not be stepped or reset between this call and the backward.  With `entropy`, the dict
+        draws from the envs' state, so it raises RuntimeError after a call that may change that state (a step, reset,
+        rollout, beam step or import_state) or after close(); draw again instead.  With `entropy`, the dict
         also holds ``"entropy"`` (N, k) float32, each sample's policy entropy as rollout_priority_sample(entropy=True)
         reports it for the same episode (0 for an env done now); with a table that requires grad it is differentiable
         too, and one replay gives the gradient of both."""
@@ -757,6 +790,7 @@ class JssVecEnv:
                     or t.device != x.device):
                 raise ValueError(f"{who}: {name} must be a contiguous {dt} tensor of shape ({n},) on {x.device}")
         bad = torch.empty(n // width, dtype=torch.int32, device=self.device)
+        self._state_epoch += 1
         if key is None:
             rc = self._L.jss_beam_step(self._h, x.data_ptr(), int(ld), width, score.data_ptr(), parent_out.data_ptr(),
                                        action_out.data_ptr(), bad.data_ptr(), self._stream())
@@ -781,9 +815,9 @@ class JssVecEnv:
         -1 if none; with `order`, ``"order"`` (N, k, J, M) int32, every slot's allocation round of each operation in
         beam_search()'s format (-1 for operations started before the call, and everywhere in a slot without a complete
         beam).  When `logits` requires grad (and grad mode is on), log_prob is differentiable with respect to it: the
-        backward replays the slots' orders (order_log_prob()), so the envs must not be stepped or reset between this
-        call and the backward.  With k + 1 draws, ``key[:, k]`` is the threshold of the priority-sampling estimator
-        (INTEGRATION.md)."""
+        backward replays the slots' orders (order_log_prob()) from the envs' state, so it raises RuntimeError after a
+        call that may change that state, as sample_episodes()' does.  With k + 1 draws, ``key[:, k]`` is the threshold
+        of the priority-sampling estimator (INTEGRATION.md)."""
         import torch
         x = self._table_arg(logits, "sample_without_replacement", "logits")
         if not 1 <= int(k) <= N.MAX_BEAM_WIDTH:
@@ -792,7 +826,7 @@ class JssVecEnv:
         grad = x.requires_grad and torch.is_grad_enabled()
         run = functools.partial(self._sample_without_replacement, k=k, step_index=step_index, order=order or grad)
         if grad:
-            log_prob, makespan, key, ord_ = _order_log_prob_fn().apply(x, self, run)
+            log_prob, makespan, key, ord_ = _order_log_prob_fn().apply(x, self, run, "sample_without_replacement")
         else:
             log_prob, makespan, key, ord_ = run(x)
         self._step_index += self.jobs * self.machines
@@ -827,7 +861,8 @@ class JssVecEnv:
         of the decisions' log-probabilities computed as rollout_priority_sample() computes them (forced no-ops add 0;
         NaN where a decision meets a bad entry; 0 for an env done now), makespan int32, the end time (-1 unless the
         episode ends done).  When `logits` requires grad (and grad mode is on), log_prob is differentiable with respect
-        to it (jss_order_log_prob_grad); the envs must not be stepped or reset between this call and the backward.
+        to it (jss_order_log_prob_grad): the backward replays the orders from the envs' state, so it raises
+        RuntimeError after a call that may change that state, as sample_episodes()' does.
         With `entropy`, returns ``(log_prob, makespan, entropy)``: entropy float32 like log_prob, the sum over the
         episode's decisions of the policy's entropy, bit for bit what rollout_priority_sample(entropy=True) reports for
         an episode drawing the same jobs from this state (0 for an env done now, NaN where log_prob is NaN); with a
@@ -838,13 +873,13 @@ class JssVecEnv:
         if entropy:
             run = functools.partial(self._order_log_prob, order=o, entropy=True)
             if x.requires_grad and torch.is_grad_enabled():
-                log_prob, ent, makespan, _ = _order_log_prob_fn().apply(x, self, run, True)
+                log_prob, ent, makespan, _ = _order_log_prob_fn().apply(x, self, run, "order_log_prob", True)
             else:
                 log_prob, ent, makespan, _ = run(x)
             return (log_prob[:, 0], makespan[:, 0], ent[:, 0]) if single else (log_prob, makespan, ent)
         run = functools.partial(self._order_log_prob, order=o)
         if x.requires_grad and torch.is_grad_enabled():
-            log_prob, makespan, _ = _order_log_prob_fn().apply(x, self, run)
+            log_prob, makespan, _ = _order_log_prob_fn().apply(x, self, run, "order_log_prob")
         else:
             log_prob, makespan, _ = run(x)
         return (log_prob[:, 0], makespan[:, 0]) if single else (log_prob, makespan)
@@ -1031,6 +1066,7 @@ class JssVecEnv:
             out["reward"] = out["_scalars"][:, :, 0].view(torch.float32)
             out["reward_raw"] = out["_scalars"][:, :, 1]
             out["time"] = out["_scalars"][:, :, 2]
+        self._state_epoch += 1
         rc = self._L.jss_rollout_traj(self._h, r, self.seed, self._step_index, K, _ptr(out["_obs"]), _ptr(out["_mask"]),
                                       _ptr(out["_scalars"]), _ptr(out["actions"]), self._stream())
         N.check(self._h, rc, "jss_rollout_traj")
@@ -1052,6 +1088,7 @@ class JssVecEnv:
                 "mask": self._host["mask"].numpy()[:, : J + 1].view(np.bool_), "obs": self._host["obs"].numpy(),
                 "reward": sc.view(np.float32)[:, 0], "done": sc.view(np.uint8)[:, 12].view(np.bool_)}
         hb, hv = self._host, self._host_views
+        self._state_epoch += 1
         rc = self._L.jss_step_host(self._h, ctypes.c_void_p(a.ctypes.data), _ptr(hb["mask"]),
                                    _ptr(hb["obs"]) if want_obs else None, _ptr(hb["scalars"]), self._stream())
         N.check(self._h, rc, "jss_step_host")
@@ -1095,6 +1132,7 @@ class JssVecEnv:
         b["packed"] = bool(packed)
         b["expanded"] = not packed
         b["n_dma"] = 0
+        self._state_epoch += 1
         if packed and dma_fraction > 0.0:
             g = 256 if n >= 4096 else 1
             b["n_dma"] = min(n, int(dma_fraction * n) // g * g)
@@ -1171,6 +1209,7 @@ class JssVecEnv:
 
     def import_state(self, state: Dict[str, Any], mask=None):
         """Restore a snapshot taken with export_state() (tensors are copied into the library's buffers)."""
+        self._state_epoch += 1
         if getattr(self, "_pipe_inflight", 0):
             # the copies below are torch ops, which the library cannot order after a host_step_begin still writing
             # the time and flags; its own entry points can
