@@ -526,43 +526,52 @@ JSS_DEV void env_prioritize(const InstView &iv, EnvRegs<KJ> &s, int lane) {
 
 // ---- _check_no_op (jss_env.py:256-401); returns legal_actions[J] -----------------
 // `hz` is a 32-int per-warp shared scratch (aliases the observation staging area).
+//
+// Pass 1 visits the legal jobs one by one in ascending order, but nothing it decides depends on that order, so it runs
+// once per legal machine (<= 3) with every lane taking its own jobs on the machine, one REDUX.MIN for the machine's
+// shortest legal job:
+// - it returns "not legal" iff some legal job ends before the next event, t + d < t + mn;
+// - max_horizon_machine[m] ends as t + min(max_time_op, min d) over the legal jobs on m; pass 2 reads it only where
+//   machine_legal[m], so elsewhere the table holds INT_MIN;
+// - max_horizon, the largest value a running minimum takes at a visit, is t + the first legal job's d on some machine,
+//   and can exceed H = the largest final minimum.  It only bounds pass 2's walks, and a walk step at a time >= H adds
+//   nothing (that needs max_horizon_machine[m] > time for a legal m) while the time only grows: walking to H instead
+//   gives the same machine_next in fewer steps.
+// Pass 2 is order-free as well: machine_next only collects legal machines and only grows, so "it reached
+// nb_machine_legal at some point" is "it equals machine_legal at the end", and each walk reads only the final table,
+// the bound and its job's state.  Its early exits after a job slot whose walks cover every legal machine only save work
+// (they end 43 % of the ta80 checks that reach pass 2 before the last slot, DESIGN.md §4).  Times are relative to t.
 template <int KJ>
 JSS_DEV bool env_check_no_op(const InstView &iv, const EnvRegs<KJ> &s, int lane, uint32_t ML, int nlegal,
                              int *hz) {
     const unsigned mn = __reduce_min_sync(JSS_FULL, (unsigned)(s.tuam > 0 ? s.tuam : JSS_INF));
     if (mn == (unsigned)JSS_INF || __popc(ML) > 3 || nlegal > 4) return false;   // gate :284-288
-    const int next_event = s.t + (int)mn;                                        // :293
-    int maxh = s.t;                                                              // :296
-    int lm0 = -1, lm1 = -1, lm2 = -1;                   // the <= 3 legal machines and their horizons
-    const int hinit = s.t + iv.si->max_time_op;             // :300-302
-    int h0 = hinit, h1 = hinit, h2 = hinit;
-    // pass 1 (:305-321): legal jobs in ascending job index = ascending lane, then slot
-    uint32_t lanes = __ballot_sync(JSS_FULL, (s.lb & jss_legal_mask<KJ>()) != 0u);
-    while (lanes) {
-        const int l = __ffs((int)lanes) - 1;
-        lanes &= lanes - 1u;
-        // KJ = 1: the lane's only job is the legal one (no need to fetch its bits, no inner loop)
-        uint32_t bits = (KJ == 1) ? 1u : (__shfl_sync(JSS_FULL, s.lb, l) & jss_legal_mask<KJ>());
+    const uint32_t lg = s.lb & jss_legal_mask<KJ>();
+    const int mto = iv.si->max_time_op;                 // :300-302
+    int maxh = 0;                                       // H - t
+    int lm0 = -1, lm1 = -1, lm2 = -1, h0 = 0, h1 = 0, h2 = 0;   // the legal machines and their horizons - t
+    uint32_t rest = ML;
 #pragma unroll 1
-        while (bits) {                                  // warp-uniform: the legal jobs of lane l, ascending
-            const int i = (KJ == 1) ? 0 : __ffs((int)bits) - 1;
-            bits = (KJ == 1) ? 0u : (bits & (bits - 1u));
-            const uint32_t o = __shfl_sync(JSS_FULL, jss_sel<KJ>(s.op, i), l);
-            const int m = (int)jss_op_m(o);
-            const int end = s.t + jss_op_d(o);
-            if (end < next_event) return false;         // :314-315
-            int cur;
-            if (lm0 == m || lm0 < 0) { lm0 = m; h0 = min(h0, end); cur = h0; }
-            else if (lm1 == m || lm1 < 0) { lm1 = m; h1 = min(h1, end); cur = h1; }
-            else { lm2 = m; h2 = min(h2, end); cur = h2; }
-            maxh = max(maxh, cur);                      // :321
+    while (rest) {                                      // :305-321, warp-uniform
+        const int m = __ffs((int)rest) - 1;
+        rest &= rest - 1u;
+        int d = JSS_INF;
+#pragma unroll
+        for (int i = 0; i < KJ; i++) {
+            const bool on = ((lg >> i) & 1u) && (int)jss_op_m(s.op[i]) == m;
+            // two spellings of one minimum: with these, ptxas (CUDA 12.9) keeps every kernel that inlines the check at
+            // its launch bound without spills but jss_step_mixed_kernel<0, false> (DESIGN.md §4)
+            d = KJ == 8 ? min(d, on ? jss_op_d(s.op[i]) : JSS_INF) : (on ? min(d, jss_op_d(s.op[i])) : d);
         }
+        d = (int)__reduce_min_sync(JSS_FULL, (unsigned)d);
+        if (d < (int)mn) return false;                  // :314-315
+        d = min(mto, d);
+        if (lm0 < 0) { lm0 = m; h0 = d; } else if (lm1 < 0) { lm1 = m; h1 = d; } else { lm2 = m; h2 = d; }
+        maxh = max(maxh, d);
     }
-    const int last = jss_M(iv) - 1;
-    // per-machine horizon table: finite only for machines that have a legal job, so the
-    // walk's test `max_horizon_machine[m] > time and machine_legal[m]` is one compare
     hz[lane] = (lane == lm0) ? h0 : (lane == lm1) ? h1 : (lane == lm2) ? h2 : (int)0x80000000;
     __syncwarp();
+    const int last = jss_M(iv) - 1;
     // pass 2 (:324-401): jobs that are not legal now but may need a legal machine soon
     uint32_t want = 0u;
     const int row = KJ * lane * jss_M(iv);
@@ -572,8 +581,8 @@ JSS_DEV bool env_check_no_op(const InstView &iv, const EnvRegs<KJ> &s, int lane,
         const int tq = __shfl_sync(JSS_FULL, s.tuam, (int)(jss_op_m(s.op[i]) & 31u));
         if (!(s.lb & (1u << i)) && s.todo[i] < jss_M(iv)) {
             int ts, tm;
-            if (s.tufco[i] > 0) { ts = s.todo[i] + 1; tm = s.t + s.tufco[i]; }      // case 1 (:327-337); a running
-            else if (!(s.lb & ((1u << jss_bs<KJ>()) << i))) { ts = s.todo[i]; tm = s.t + tq; }       // last op walks nothing either way
+            if (s.tufco[i] > 0) { ts = s.todo[i] + 1; tm = s.tufco[i]; }            // case 1 (:327-337); a running
+            else if (!(s.lb & ((1u << jss_bs<KJ>()) << i))) { ts = s.todo[i]; tm = tq; }   // last op walks nothing either way
             else { ts = jss_M(iv); tm = 0; }                                         // case 2 (:366-377) / blocked
             const uint16_t *o_ptr = iv.ops + row + i * jss_M(iv);
             while (ts < last && maxh > tm) {                                        // :340-342 / :380-382
@@ -583,8 +592,7 @@ JSS_DEV bool env_check_no_op(const InstView &iv, const EnvRegs<KJ> &s, int lane,
                 ts += 1;
             }
         }
-        // the reference returns as soon as machine_next covers every legal machine (:357 / :395);
-        // about half of the pass-2 runs end "legal", most of them after the first job slot
+        // the reference returns as soon as machine_next covers every legal machine (:357 / :395)
         if (i + 1 < KJ && ML != 0u && __reduce_or_sync(JSS_FULL, want) == ML) {
             __syncwarp();                               // hz aliases the obs staging buffer
             return true;
